@@ -4,7 +4,7 @@ synthetic 24 kHz audio per GPU (125 frames of 80 ms each, one frame of every str
 sequence), seeded synthetic weights.  Metric: codec frames/s (one frame = 1920 samples encoded to
 8 tokens and decoded back); real-time streams = frames/s / 12.5.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 A "step" = one pass over the whole batch: 125 streaming frames x 256 streams (encode + decode).
 `value` is measured with the 10 s inputs already resident in HBM; `e2e` copies every 80 ms chunk
@@ -12,11 +12,16 @@ from pinned host memory and reads tokens + waveform back each frame.  Multi-GPU:
 across ranks with no data-path collective (weak scaling); timing = max over ranks.
 `--impl reference` times the reference's CPU implementation of the same path (the oracle port, torch
 CPU fp32 with all host threads) on a bounded sample.
+`--dump-outputs DIR` writes what the last timed step computed (rank 0; collected by an untimed replay of that step, whose
+last frame is checked bit for bit against the timed one): DIR/codes.npy, every stream's tokens of the 125
+frames [256, 8, 125], and DIR/wav.npy, the decoded 10 s waveforms of a fixed seeded sample of 32 streams [32, 240000]
+(stream indices in DIR/wav_streams.npy), all float32.  Inputs are seeded, so two builds can be compared output for output.
 
 Next to the headline (N = 1 only, extra keys, each its own unit of work and outside the headline's timed region):
   steady_state        the same pass with the codec transformers' rings already full (context 250), i.e. what a long-running
                       server sees; the headline's 10 s streams start cold;
-  lm_decode           BASELINE configs[2]: one 7B decode step, B = 64, KV ring 2048 (wrapped);
+  lm_decode           BASELINE configs[2]: one 7B decode step, B = 32, KV ring 2048 (wrapped; 64 streams' rings would not
+                      fit next to the weights in 80 GB);
   cfg4_infer          BASELINE configs[3]: Mimi encode -> InferenceImp (prefill + 1000 generated frames) -> Mimi decode, B = 32;
   cfg5_duplex         BASELINE configs[4] on one GPU: batched real-time loop (codec encode -> LM frame -> codec decode per 80 ms
                       tick, rstnet_b200.serve.DuplexEngine), per-tick latency p50 / p99 and the streams that sustain real time;
@@ -51,11 +56,12 @@ def _peaks():
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"], "bf16_tflops_sustained": d["bf16_tflops_sustained"],
                 "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    # NVIDIA's H100 SXM data sheet (700 W card, dense BF16): an upper bound, not a measured rate
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "H100 SXM data sheet"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
 
     def __init__(self, index: int):
         self.index, self.rows, self._stop = index, [], threading.Event()
@@ -195,6 +201,11 @@ def run_ours(args):
     out_codes_host = torch.empty(B, 8, 1, dtype=torch.int64).pin_memory()
 
     state = {"entered": False}
+    # --dump-outputs: what every frame of a step returned (tokens of every stream, the waveform of a fixed seeded sample
+    # of streams), collected by an untimed replay of the last timed step (see run_ours), never inside the timed region
+    dump = {"on": False, "codes": [], "wav": []}
+    wav_rows = torch.randperm(B, generator=torch.Generator().manual_seed(0))[:32].sort().values
+    wav_rows_dev = wav_rows.to(dev)
 
     def step(resident: bool, cold: bool = True):
         """125 streaming frames for all streams: encode chunk -> decode tokens.  One streaming scope is
@@ -210,6 +221,10 @@ def run_ours(args):
                 chunk = host_frames[i].to(dev, non_blocking=True)
             codes = m.encode(chunk)
             wav = m.decode(codes)
+            state["last"] = (codes, wav)
+            if dump["on"]:
+                dump["codes"].append(codes.clone())
+                dump["wav"].append(wav.index_select(0, wav_rows_dev))
             if not resident:
                 out_codes_host.copy_(codes, non_blocking=True)
                 out_wav_host.copy_(wav, non_blocking=True)
@@ -249,6 +264,24 @@ def run_ours(args):
     with ClockSampler(local) as cs:
         ms, _ = timed(True, args.steps)
     clocks = cs.summary()
+    if args.dump_outputs and rank == 0:
+        # Every timed step is a cold pass over the same inputs, so an untimed replay of one computes what the last timed
+        # step computed; the replay's last frame is checked bit for bit against the last frame the timed run returned.
+        import numpy as np
+        last_codes, last_wav = (t.clone() for t in state["last"])
+        dump["on"] = True
+        step(True)
+        dump["on"] = False
+        assert torch.equal(dump["codes"][-1], last_codes) and torch.equal(dump["wav"][-1], last_wav.index_select(0, wav_rows_dev)), \
+            "the untimed replay differs from the last timed step"
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        codes_all = torch.stack(dump["codes"]).reshape(FRAMES, B, 8).permute(1, 2, 0)             # [B, 8, FRAMES]
+        wav_all = torch.stack(dump["wav"]).reshape(FRAMES, len(wav_rows), FRAME).permute(1, 0, 2)  # [32, FRAMES, 1920]
+        np.save(os.path.join(args.dump_outputs, "codes.npy"), codes_all.float().cpu().numpy())
+        np.save(os.path.join(args.dump_outputs, "wav.npy"), wav_all.reshape(len(wav_rows), -1).float().cpu().numpy())
+        np.save(os.path.join(args.dump_outputs, "wav_streams.npy"), wav_rows.float().numpy())
+        dump["codes"].clear()
+        dump["wav"].clear()
     for _ in range(1):
         step(False)
     ms_e2e, _ = timed(False, args.steps)
@@ -325,7 +358,7 @@ def run_ours(args):
 
 
 def roofline_pass(m, x_dev, B, dev):
-    """Dominant kernel = gemm_tc_ts_kernel (persistent tcgen05 3xTF32 GEMM; every conv / transposed conv /
+    """Dominant kernel = gemm_tc_kernel (persistent wgmma 3xTF32 GEMM; every conv / transposed conv /
     linear of a frame).  Per-launch CUDA-event timing of each launch over a few eager streaming frames
     (events on the launching stream).  Each frame is queued behind a ~10 ms spin kernel so the host stays
     ahead of the device and the event pairs bracket device time, not host launch latency.
@@ -375,22 +408,11 @@ def roofline_pass(m, x_dev, B, dev):
     achieved = flops / (t_ms * 1e-3) / 1e12
     peak = peaks["bf16_tflops_sustained"]
     alg_bytes = sum(b for b in rec_bytes) / max(1, len(rec_bytes))     # per launch, like `traffic`
-    traffic, traffic_src = None, None
-    tp = os.path.join(ROOT, "profiles", "r2_traffic.json")              # summary of the committed ncu pass (scripts/ncu_traffic.py)
-    if os.path.exists(tp):
-        try:
-            tj = json.load(open(tp))
-            k = tj["kernels"].get("gemm_tc_ts_kernel")
-            if k:
-                traffic, traffic_src = k["dram_bytes_per_launch"], tj.get("source")
-        except Exception:
-            pass
-    return {"bound": "tensor", "kernel": "gemm_tc_ts_kernel (persistent tcgen05 kind::tf32 GEMM, A from TMEM, 3xTF32 split = fp32-equivalent; all conv/linear launches of a frame)",
-            "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak, "traffic": traffic,
-            "traffic_source": traffic_src, "algorithmic_bytes_per_launch": alg_bytes,
-            "traffic_over_algorithmic": (traffic / alg_bytes) if traffic else None,
+    return {"bound": "tensor", "kernel": "gemm_tc_kernel (persistent wgmma tf32 GEMM, A fragments in registers, 3xTF32 split = fp32-equivalent; all conv/linear launches of a frame)",
+            "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
+            "algorithmic_bytes_per_launch": alg_bytes,
             "frac_of_3xtf32_ceiling": achieved / (peak / 6.0),
-            "peak_source": f"{peaks['source']} bf16 sustained (TF32 dense peak is half of it; 3xTF32 issues 3 MMAs per product, so the ceiling of this metric is peak/6)",
+            "peak_source": f"{peaks['source']} dense bf16 (TF32 dense peak is half of it; 3xTF32 issues 3 MMAs per product, so the ceiling of this metric is peak/6)",
             "launches": len(rec) // nframes, "avg_launch_us": 1e3 * t_ms / max(1, len(rec)),
             "share_of_frame_time": t_ms / frame_ms, "eager_frame_ms": frame_ms / nframes,
             "gflop_per_frame_batch": flops / nframes / 1e9}
@@ -398,14 +420,15 @@ def roofline_pass(m, x_dev, B, dev):
 
 def lm_decode_bench(dev, steps: int, warmup: int):
     """BASELINE.json configs[2]: one decode step (temporal 32-layer 7B + 8 depth steps + sampling) of the
-    speech-text LM, random-init bf16 weights, batch 64 streams, KV ring pre-filled to 2048 positions.
+    speech-text LM, random-init bf16 weights, batch 32 streams, KV ring pre-filled to 2048 positions (a stream's 7B MHA ring
+    costs 1.07 GB: 64 of them would not fit next to the 17 GB of weights in 80 GB).
     Reported next to the codec headline (it is a different unit of work, not part of `value`)."""
     import torch
     from rstnet_b200 import _lib, ops
     from rstnet_b200 import lm as LMmod
     from rstnet_b200.lm import GPT, Config
     peaks = _peaks()
-    B, KV = 64, 2048
+    B, KV = 32, 2048
     cfg = Config(block_size=4096, n_layer=32, n_embd=4096, n_head=32, head_size=128, intermediate_size=11008,
                  padded_vocab_size=152064, audio_card=2050, n_q=8, dep_q=8, codecformer_dim=1024, codecformer_heads=16,
                  codecformer_layers=6, codecformer_dim_feedforward=4224, context=KV)
@@ -499,7 +522,7 @@ def lm_decode_bench(dev, steps: int, warmup: int):
     w_bytes = 2.0 * n_params - 2.0 * (152064 * 4096 + 8 * 2051 * 4096 + 152064 * 1024 + 7 * 2051 * 1024)  # embeddings are gathered, not streamed
     kv_bytes = 32 * 2.0 * B * 32 * (KV - 1) * 128 * 2
     step_bytes = w_bytes + kv_bytes
-    out = {"workload": "gpt7b_decode_step_B64_kv2048 (32-layer temporal + 8x6-layer depth + sampling)", "dtype": "bf16",
+    out = {"workload": f"gpt7b_decode_step_B{B}_kv{KV} (32-layer temporal + 8x6-layer depth + sampling)", "dtype": "bf16",
            "params": n_params, "ms_per_step": ms, "frames_per_s": B / (ms * 1e-3), "tokens_per_s": B * 9 / (ms * 1e-3),
            "e2e_ms_per_step": ms_e2e, "e2e_tokens_per_s": B * 9 / (ms_e2e * 1e-3),
            "algorithmic_gbytes_per_step": step_bytes / 1e9,
@@ -650,14 +673,16 @@ def cfg5_duplex_bench(dev, S, ticks: int = 40):
     tick: H2D of every stream's 1920-sample chunk, codec encode, one 7B LM frame (temporal + depth + sampling), codec
     decode, D2H of tokens + PCM (the loop of moshi/server.py:108-144 for a batch).  Reports the wall-clock latency of a
     tick (p50 / p99 over `ticks` ticks after warm-up) and which batch sizes stay under the 80 ms real-time budget.  The
-    7B MHA KV ring (context 2048, bf16) costs 1.07 GB per stream, which is what bounds streams per GPU (SURVEY.md H4)."""
+    7B MHA KV ring (context 2048, bf16) costs 1.07 GB per stream, which is what bounds streams per GPU (SURVEY.md H4):
+    with the 17 GB of weights roughly 55 streams' rings fit in 80 GB; the batches tried stay below that, so the reported
+    streams per GPU is a lower bound."""
     import torch
     from rstnet_b200.serve import DuplexEngine, FrameScheduler
     codec = _mimi(dev, S)
     lm = _gpt7b(dev, context=2048)
     res = {"tick_budget_ms": 80.0, "runs": []}
     audio = S.synthetic_audio(8, FRAME * 8, seed=12)
-    for B in (64, 128):
+    for B in (32, 48):
         try:
             eng = DuplexEngine(codec, lm, B)
             sch = FrameScheduler(eng, B)
@@ -692,8 +717,8 @@ def cfg5_duplex_bench(dev, S, ticks: int = 40):
     ok = [r["streams"] for r in res["runs"] if r.get("realtime")]
     res["realtime_streams_per_gpu"] = max(ok) if ok else 0
     res["state"] = "steady: LM KV rings full (2048-key window, wrapped), codec transformer rings full (250 tokens)"
-    res["note"] = ("codec + 7B LM per stream at an 80 ms cadence; the largest batch tried that keeps p99 < 80 ms "
-                   "(128 = one weight-streaming GEMM pass and ~137 GB of MHA KV rings)")
+    res["note"] = ("codec + 7B LM per stream at an 80 ms cadence; the largest batch tried that keeps p99 < 80 ms (a lower bound) "
+                   "(48 streams = ~51 GB of MHA KV rings next to the weights)")
     del lm, codec
     return res
 
@@ -706,8 +731,10 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-lm", dest="no_lm", action="store_true", help="skip the secondary LM decode-step measurement")
+    ap.add_argument("--dump-outputs", dest="dump_outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32)")
     ap.add_argument("--frames", type=int, default=FRAMES,
-                    help="frames per stream per step (profiling aid: ncu runs use a short pass; the default 125 is the bench)")
+                    help="frames per stream per step (profiling aid: a short pass; the default 125 is the bench)")
     args = ap.parse_args()
     if args.frames != FRAMES:
         FRAMES = args.frames

@@ -1,8 +1,8 @@
-/* rstnet_b200 — C ABI of the B200 (sm_100a) kernels behind RSTnet's real-time inference hot path.
+/* rstnet_b200 — C ABI of the H100 (sm_90a) kernels behind RSTnet's real-time inference hot path.
  *
  * The reference (yangdongchao/RSTnet) is pure Python/PyTorch and has no FFI of its own; the
  * drop-in boundary is its Python class surface (SURVEY.md §8b).  Each entry point below replaces
- * the ATen call cluster of one reference method (cited as file:line under /root/reference) and is
+ * the ATen call cluster of one reference method (cited as file:line of the reference repository) and is
  * what a replacement library must export.  Conventions:
  *   - plain C: raw DEVICE pointers, explicit sizes/strides in ELEMENTS, no torch types;
  *   - the caller owns every buffer (activations, KV rings, conv carry rows, scratch);
@@ -70,21 +70,20 @@ typedef struct {
 } rstnet_gemm_rows_args;
 int rstnet_gemm_rows_f32(const rstnet_gemm_rows_args* args, rstnet_stream_t stream);
 
-/* ---- the same contraction on the 5th-gen tensor cores (tcgen05.mma, accumulator in TMEM, operands
- * staged by TMA), as a plan bound to fixed buffers (the library owns only the TMA descriptors and
+/* ---- the same contraction on the tensor cores (warpgroup MMA, wgmma, with operands staged by TMA), as a plan bound
+ * to fixed buffers (the library owns only the TMA descriptors and
  * tile configuration; the caller owns all tensors):
  *   D[(i,o), n] = sum_tap sum_c A[c, i + tap*tap_di, o*o_mul + tap*tap_do] * W[n, tap*Kc + c]
  * A is the activation buffer viewed as a 3-D tensor (c, i, o) with element strides
  * (1, a_i_stride, a_o_stride); W is [N][taps*Kc] (K contiguous).  Output element (i, o, n) goes to
  * C + o*c_o_stride + i*c_i_stride + n, or, when n_split > 0 (transposed conv: n = j*n_split + co),
  * to C + o*c_o_stride + i*c_i_stride + j*c_split_stride + co; R (optional residual) likewise.
- * Epilogue: post(R + scale*(acc + bias)); pre_act is applied to A in shared memory.
+ * Epilogue: post(R + scale*(acc + bias)); pre_act (RSTNET_ACT_NONE or RSTNET_ACT_ELU; others are rejected by
+ * rstnet_tc_gemm_create) is applied to A in registers as the operand fragments are built.
  * precision 0 = 3xTF32 split (fp32-equivalent, for RVQ-index exactness; W must already be rounded to
  * TF32 and W_lo = tf32(w - W) supplied -- see rstnet_tf32_split_f32), 1 = single TF32 pass.
- * Precision 0 runs the persistent kernel (one CTA per SM walking the tiles, A operand through TMEM, TMA-store
- * epilogue) when W_lo lies at a positive 16-byte-aligned distance after W, so that one 3-D descriptor reaches both --
- * allocate them as one [2][N][K] tensor, as rstnet_b200/ops.py:tf32_split does; otherwise (and for precision 1) the
- * one-CTA-per-tile kernel is used.  ELU in the persistent kernel's epilogue is evaluated with ex2.approx.
+ * The kernel is persistent (at most one CTA per SM walking the 128 x 32 or 128 x 64 output tiles).  ELU, as pre- and
+ * post-activation, is evaluated with ex2.approx.
  * Same reference call sites as rstnet_gemm_rows_f32. */
 typedef struct rstnet_tc_plan rstnet_tc_plan;
 typedef struct {
@@ -110,10 +109,7 @@ typedef struct {
 int rstnet_tc_gemm_create(const rstnet_tc_gemm_desc* desc, rstnet_tc_plan** out);
 int rstnet_tc_gemm_run(const rstnet_tc_plan* plan, rstnet_stream_t stream);
 void rstnet_tc_gemm_destroy(rstnet_tc_plan* plan);
-/* profiling aid: CTA 0 writes clock64 stamps per k iteration of one tile to trace[>= padded taps*Kc/32][8]
- * (0 producer, 1 operands landed, 2 transformed, 3 MMA start, 4 MMA issued, 5/6 drain begin/end, column 7: epilogue);
- * cta_times[max(grid.x, SM count)][4] globaltimer ns per CTA.  rstnet_tc_gemm_grid reports the tile grid (M x N tiles). */
-void rstnet_tc_gemm_set_trace(rstnet_tc_plan* plan, int64_t* trace, int64_t* cta_times);
+/* the plan's tile grid: M tiles (I tiles x O_out), N tiles, tile width */
 int rstnet_tc_gemm_grid(const rstnet_tc_plan* plan, int32_t* grid_x, int32_t* grid_y, int32_t* tile_n);
 /* hi[i] = tf32_rna(x[i]); lo[i] = tf32_rna(x[i] - hi[i])  (one-time weight preparation for precision 0) */
 int rstnet_tf32_split_f32(const float* x, float* hi, float* lo, int64_t n, rstnet_stream_t stream);
@@ -226,8 +222,8 @@ int rstnet_rvq_decode_gather_f32(const int64_t* codes, const float* E, float* q,
  * ====================================================================================== */
 
 /* ---- weight-streaming GEMM  out[m,n] = sum_k X[m,k] * W[n,k] (+ R[m,n]), all bf16, W exactly as
- * nn.Linear stores it.  tcgen05 (kind::f16) with W as the 128-row MMA operand, TMA-staged, fp32
- * accumulator in TMEM, optional split-K (fp32 partials in `partial_ws` + finalize).  Replaces F.linear
+ * nn.Linear stores it.  wgmma with W as the 128-row MMA operand (two m64 halves), TMA-staged, fp32
+ * accumulator in registers, optional split-K (fp32 partials in `partial_ws` + finalize).  Replaces F.linear
  * in LoRAQKVLinear/LoRALinear after merge (llama_streaming.py:113-143, 368-406), LLaMAMLP
  * (lit_model.py:399-403), lm_head (:691), codecformer_in / multi_linear / gating / audio_linears
  * (llama_streaming.py:727-749, modules/transformer.py:155-179, modules/gating.py:12-21).

@@ -1,6 +1,6 @@
 """Generate tests/golden/lm_small.npz by running the UNMODIFIED reference GPT (streaming decode) here.
 
-Run:  python -m oracle.gen_golden_lm      (needs /root/reference)
+Run:  python -m oracle.gen_golden_lm      (needs a checkout of the reference repository at REF)
 
 The reference `models.llama_streaming.GPT` (small config, seeded synthetic weights from
 oracle/lm_oracle.synthetic_weights) is stepped for a few frames under `with gpt.streaming(B)` with
@@ -24,6 +24,25 @@ from . import lm_oracle as L
 from .gen_golden import weights_digest
 
 GOLDEN = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden")
+# Every fixture stays under 1 MB: logits are stored for a fixed seeded sample of LOGIT_SAMPLE vocabulary columns (indices in
+# "logit_cols", the argmax over the whole vocabulary beside each as "<name>_argmax"), merged LoRA weights for a seeded
+# sample of LORA_ROWS rows (indices in "lora_merged_<i>_rows").
+LOGIT_SAMPLE, LORA_ROWS = 448, 128
+
+
+def shrink(save: dict) -> dict:
+    out = dict(save)
+    for k, a in save.items():
+        if k.endswith("_logits"):
+            cols = np.sort(np.random.default_rng(0).choice(a.shape[-1], LOGIT_SAMPLE, replace=False))
+            out["logit_cols"] = cols
+            out[k] = np.ascontiguousarray(a[..., cols])
+            out[k[:-len("_logits")] + "_argmax"] = a.argmax(-1)
+        elif k.startswith("lora_merged_") and not k.endswith("_rows"):
+            rows = np.sort(np.random.default_rng(1).choice(a.shape[0], LORA_ROWS, replace=False))
+            out[k] = np.ascontiguousarray(a[rows])
+            out[k + "_rows"] = rows
+    return out
 
 
 def reference_frames(w, cfg, seqs, dtype):
@@ -141,7 +160,8 @@ def gen_variant(save):
         print(f"gqa/partial-rope {tag}: oracle == reference on {frames} streaming frames")
         keep = (0, 1, 15, 16, 19)
         save[f"gqa_{tag}_out"] = torch.stack([ref[f][0].float() for f in keep]).numpy()
-        save[f"gqa_{tag}_audio_logits"] = torch.stack([ref[f][2].float() for f in keep]).numpy()
+        if tag == "bf16":   # the GPU tests compare bf16 audio logits; the fp32 ones are covered by the tokens above
+            save[f"gqa_{tag}_audio_logits"] = torch.stack([ref[f][2].float() for f in keep]).numpy()
         save[f"gqa_{tag}_tokens"] = torch.stack([ref[f][3] for f in range(frames)]).numpy()
         save["gqa_keep"] = np.array(keep)
         # non-streaming forms on the first T frames (T < context: equal to T streaming steps up to rounding)
@@ -201,12 +221,13 @@ def gen_lora(save):
 def main():
     torch.set_num_threads(min(8, os.cpu_count() or 1))
     os.makedirs(GOLDEN, exist_ok=True)
-    extra = {}
+    extra, lora = {}, {}
     gen_infer(extra)
     gen_variant(extra)
-    gen_lora(extra)
-    np.savez_compressed(os.path.join(GOLDEN, "lm_round2.npz"), **extra)
-    print("wrote", os.path.join(GOLDEN, "lm_round2.npz"))
+    gen_lora(lora)
+    np.savez_compressed(os.path.join(GOLDEN, "lm_round2.npz"), **shrink(extra))
+    np.savez_compressed(os.path.join(GOLDEN, "lm_lora.npz"), **shrink(lora))
+    print("wrote", os.path.join(GOLDEN, "lm_round2.npz"), os.path.join(GOLDEN, "lm_lora.npz"))
     cfg = L.SMALL
     B, frames = 3, 20  # 20 > context (16): the ring wraps
     g = torch.Generator().manual_seed(99)
@@ -241,7 +262,7 @@ def main():
         if tag == "f32":
             save["weights_sha256"] = np.array(weights_digest(w))
     save["seqs"] = torch.stack(seqs).numpy()
-    np.savez_compressed(os.path.join(GOLDEN, "lm_small.npz"), **save)
+    np.savez_compressed(os.path.join(GOLDEN, "lm_small.npz"), **shrink(save))
     print("wrote", os.path.join(GOLDEN, "lm_small.npz"))
 
 

@@ -1,7 +1,7 @@
 """ctypes binding of librstnet_b200.so (the C ABI declared in include/rstnet_b200.h).
 
 There is no CPU fallback: if the shared library is missing, or an entry point fails, this module
-raises.  Build with ``python -m rstnet_b200.build`` (nvcc, sm_100a).
+raises.  Build with ``python -m rstnet_b200.build`` (nvcc, sm_90a).
 """
 from __future__ import annotations
 
@@ -16,7 +16,7 @@ ACT_NONE, ACT_ELU, ACT_GELU = 0, 1, 2
 # every symbol include/rstnet_b200.h declares (tests assert the .so exports all of them)
 SYMBOLS = [
     "rstnet_version", "rstnet_last_error", "rstnet_launch_count", "rstnet_device_error_flags",
-    "rstnet_gemm_rows_f32", "rstnet_tc_gemm_create", "rstnet_tc_gemm_run", "rstnet_tc_gemm_destroy", "rstnet_tc_gemm_set_trace", "rstnet_tc_gemm_grid", "rstnet_tf32_split_f32", "rstnet_conv1d_cin1_f32", "rstnet_conv1d_cout1_f32",
+    "rstnet_gemm_rows_f32", "rstnet_tc_gemm_create", "rstnet_tc_gemm_run", "rstnet_tc_gemm_destroy", "rstnet_tc_gemm_grid", "rstnet_tf32_split_f32", "rstnet_conv1d_cin1_f32", "rstnet_conv1d_cout1_f32",
     "rstnet_convtr1d_depthwise_f32", "rstnet_rows_fill_f32", "rstnet_rows_copy_table_f32",
     "rstnet_counter_add", "rstnet_layer_norm_f32", "rstnet_rope_kv_append_f32",
     "rstnet_ring_attention_f32", "rstnet_rope_ring_attention_f32", "rstnet_rvq_encode_workspace", "rstnet_rvq_encode_f32",
@@ -101,9 +101,7 @@ def lib() -> C.CDLL:
     L.rstnet_tc_gemm_run.argtypes = [vp, vp]
     L.rstnet_tc_gemm_destroy.argtypes = [vp]
     L.rstnet_tc_gemm_destroy.restype = None
-    L.rstnet_tc_gemm_set_trace.argtypes = [vp, vp, vp]
     L.rstnet_tc_gemm_grid.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)]
-    L.rstnet_tc_gemm_set_trace.restype = None
     L.rstnet_tf32_split_f32.argtypes = [vp, vp, vp, i64, vp]
     L.rstnet_conv1d_cin1_f32.argtypes = [vp, i64, i64, vp, vp, vp, vp, i64, i64, i32, i32, i32, i32, i32, i32, vp]
     L.rstnet_conv1d_cout1_f32.argtypes = [vp, i64, i64, vp, vp, vp, i64, i32, i32, i32, i32, vp]

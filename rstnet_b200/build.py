@@ -1,7 +1,7 @@
-"""In-tree build of librstnet_b200.so (nvcc, sm_100a only).
+"""In-tree build of librstnet_b200.so (nvcc, sm_90a: H100).
 
 `python -m rstnet_b200.build` or `__graft_entry__.build()`.  nvcc cross-compiles without a GPU.
-The .so is git-ignored but travels to the GPU box with the gpurun snapshot.
+The library and its objects land in rstnet_b200/lib/ (git-ignored build products).
 """
 from __future__ import annotations
 
@@ -16,7 +16,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "librstnet_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 

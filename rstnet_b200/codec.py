@@ -1,4 +1,4 @@
-"""B200-native Mimi codec behind the reference's Python API.
+"""H100-native Mimi codec behind the reference's Python API.
 
 Mirrors (names, signatures, tensor layouts, state_dict keys):
   * ``MimiCodec.encode(audio[B,1,L]) -> codes[B,n_q,ceil(L/1920)] int64`` and
@@ -10,7 +10,7 @@ Mirrors (names, signatures, tensor layouts, state_dict keys):
     ring KV caches kept in device buffers;
   * ``MimiTokenizer.tokenize / detokenize`` (tools/tokenizer/MimiCodec/mimi_tokenizer.py:56-82).
 
-All arithmetic runs in librstnet_b200.so (hand-written sm_100a CUDA); this file only lays out
+All arithmetic runs in librstnet_b200.so (hand-written sm_90a CUDA); this file only lays out
 buffers in HBM and sequences launches.  Internal activation layout is [B, T, C] (channels last)
 so that every conv is a GEMM over overlapping contiguous rows; each layer's input buffer carries
 its own left context rows (`k - stride`), which double as the streaming carry.
@@ -166,22 +166,22 @@ class MimiCodec(nn.Module):
         self._engine: Optional["_Engine"] = None
         self._stream_state: Optional["_StreamState"] = None
         self.use_cuda_graphs = True
-        # streaming steps run their GEMMs on the tensor cores (tcgen05, 3xTF32 = fp32-equivalent products,
+        # streaming steps run their GEMMs on the tensor cores (wgmma, 3xTF32 = fp32-equivalent products,
         # fp32 accumulation); False selects the fp32 FFMA kernels (bit-faithful fp32 arithmetic) there too.
         self.streaming_tensor_cores = True
         # 0 = 3xTF32 (fp32-equivalent; the default on both sides: RVQ indices must match the fp32 reference and the
-        # measured waveform error stays at 4e-6).  decoder_precision = 1 opts the decoder into single-pass TF32 (the
-        # precision of PyTorch's own cuDNN convolutions on GPUs): +8 % frames/s, waveform error 1.3e-3 of a 0.57 peak.
+        # waveform stays within fp32 rounding of it).  decoder_precision = 1 opts the decoder into single-pass TF32 (the
+        # precision of PyTorch's own cuDNN convolutions on GPUs): fewer MMAs, waveform error of order 1e-3 of the peak.
         self.tc_precision = 0
         self.decoder_precision = 0
         # resblock convs (k=3 C->C/2, 1x1 C/2->C) on the tensor cores too; False keeps them on the CUDA-core kernel
         self.resblock_tensor_cores = True
         # non-streaming encode / decode of a batch (offline tokenization, SURVEY.md §8f-3): batches of at least this many
-        # clips run the tcgen05 path (a 128-row tile = 128 clips at one time step), smaller ones the fp32 CUDA-core path
+        # clips run the tensor-core path (a 128-row tile = 128 clips at one time step), smaller ones the fp32 CUDA-core path
         self.batch_tensor_cores_min = 96
         self.fused_rope_attention = True     # streaming steps: RoPE + KV append inside the attention launch
         # resblocks up to this width read the raw tensor and apply ELU in the operand transform (_Plan.elu_in_transform).
-        # 0 = never (default): measured 3.16 / 3.20 ms per 256-stream frame step at 128 / 64 vs 3.11 ms with the ELU'd copy
+        # 0 = never (default): the ELU'd copy was the faster form where both were timed (scripts/codec_ab.py)
         self.elu_in_transform_max_channels = 0
 
     # ------------------------------------------------------------------ parameters
@@ -212,7 +212,7 @@ class MimiCodec(nn.Module):
     def _eng(self) -> "_Engine":
         dev = self.device
         if dev.type != "cuda":
-            raise RstnetError("MimiCodec runs on CUDA only (sm_100a kernels; the CPU path is the reference itself)")
+            raise RstnetError("MimiCodec runs on CUDA only (sm_90a kernels; the CPU path is the reference itself)")
         if self._engine is None or self._engine.device != dev:
             self._engine = _Engine(self, dev)
         return self._engine
@@ -397,7 +397,7 @@ class _Engine:
         D = self.D
 
         def conv_w(prefix):
-            """[Cout,Cin,k] -> Wt[(tap,ci), co] for the FFMA kernel and W[co, (tap,ci)] for tcgen05."""
+            """[Cout,Cin,k] -> Wt[(tap,ci), co] for the FFMA kernel and W[co, (tap,ci)] for the tensor-core GEMM."""
             w = sd[f"{prefix}.weight"]
             cout, cin, k = w.shape
             wk = w.permute(0, 2, 1).reshape(cout, k * cin).contiguous()
@@ -538,7 +538,7 @@ class _Plan:
     """Common machinery: a plan is a list of launch closures over static buffers.
 
     tensor_cores=False: [B, rows, C] buffers + the fp32 FFMA strided-row GEMM (exact fp32 arithmetic;
-    any batch / clip length).  tensor_cores=True: [rows, B, C] buffers + tcgen05 3xTF32 GEMM plans
+    any batch / clip length).  tensor_cores=True: [rows, B, C] buffers + wgmma 3xTF32 GEMM plans
     (streaming steps: every 128-row tile is 128 streams at one time step)."""
 
     def __init__(self, eng: _Engine, B: int, streaming: bool, tensor_cores: bool, active: Optional[torch.Tensor] = None):
@@ -555,9 +555,9 @@ class _Plan:
         """Tensor-core plans: does the resblock conv of a C-channel level apply its input ELU in the GEMM's operand transform
         (reading the raw tensor) instead of reading an ELU'd copy written by the producer?  Same values either way (one
         ELU implementation, bit-identical results).  The idea: at the wide, shallow levels (24 kHz C = 64, 6 kHz C = 128)
-        the copy is a second 126 / 63 MB tensor per 256-stream frame.  Measured (scripts/codec_ab.py, same box): it does NOT
-        pay -- the 32 extra ex2 per thread and stage on the transform warps cost more than the saved stores (3.16 vs 3.11 ms
-        per frame step), so MimiCodec.elu_in_transform_max_channels defaults to 0."""
+        the copy is a second 126 / 63 MB tensor per 256-stream frame.  Where it was timed (scripts/codec_ab.py) it did not
+        pay -- the extra ex2 per operand element cost more than the saved stores -- so
+        MimiCodec.elu_in_transform_max_channels defaults to 0; time it with scripts/codec_ab.py before changing that."""
         return self.tc and C <= self.eng.m.elu_in_transform_max_channels and self.precision == 0 and self.eng.m.resblock_tensor_cores
 
     @staticmethod

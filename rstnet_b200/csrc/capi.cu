@@ -23,7 +23,7 @@ bool pdl_enabled() {
   static int v = -1;
   if (v < 0) {
     const char* e = getenv("RSTNET_PDL");
-    v = (e && e[0] == '1') ? 1 : 0;     // opt-in: measured SLOWER inside CUDA graphs (LM frame 24.1 ms vs 20.0 ms, B200, driver 580)
+    v = (e && e[0] == '1') ? 1 : 0;     // opt-in (common.cuh)
   }
   return v != 0;
 }

@@ -10,6 +10,10 @@
 namespace rstnet {
 extern void count_launch();
 
+// cos / sin of a RoPE angle, out of line: the separate append kernel and the fused attention kernel must rotate bit for
+// bit alike, and inlined copies of cosf / sinf may be contracted or share their range reduction differently per call site
+__device__ __noinline__ float2 rope_cos_sin(float ang) { return make_float2(cosf(ang), sinf(ang)); }
+
 // one warp per (b, t, h); lanes stride over the D/2 rotation pairs
 __global__ void rope_kv_append_kernel(float* __restrict__ qkv, long long qbs, long long qts, float* __restrict__ kv,
                                       const long long* __restrict__ offset, int ostride, const float* __restrict__ freqs,
@@ -33,8 +37,8 @@ __global__ void rope_kv_append_kernel(float* __restrict__ qkv, long long qbs, lo
   // ts = offset.float() + arange(T) in fp32 (rope.py:39)
   const float ts = __fadd_rn((float)off, (float)t);
   for (int pr = lane; pr < D / 2; pr += 32) {
-    const float ang = __fmul_rn(freqs[pr], ts);
-    const float c = cosf(ang), s = sinf(ang);
+    const float2 cs = rope_cos_sin(__fmul_rn(freqs[pr], ts));
+    const float c = cs.x, s = cs.y;
     const float qr = q[2 * pr], qi = q[2 * pr + 1];
     const float kr = k[2 * pr], ki = k[2 * pr + 1];
     // separate mul / sub / add (no FMA contraction) as the eager reference evaluates them
@@ -224,18 +228,18 @@ __global__ void ring_attention_pair_kernel(const float* __restrict__ qkv, long l
 // of the 64 dims, its two query slices live in registers), so a 128-bit load instruction covers four whole rows
 // instead of 32 different lines; the partial dots are reduced with three shuffles.  V: sixteen lanes cover one row with
 // 128-bit loads (two rows per instruction), the two half-warps accumulate alternate keys and are added at the end.
-// Ring slots advance incrementally (no per-key modulo).  At a 200-token context this kernel is 16 x 136 us of a
-// 256-stream frame in the one-row-per-lane form (launch list profiles/r1_codec_late_frame_launches_rowperlane_attn.csv).
+// Ring slots advance incrementally (no per-key modulo).  The one-row-per-lane form read 32 different lines per load
+// instruction and was the slowest launch of a late streaming frame.
 // ROPE: the streaming step (T == 2: one warp owns both new tokens of its (stream, head)) rotates q in registers, rotates and
 // appends k, copies v into the ring itself -- arithmetic of rope_kv_append_kernel above -- and then attends; the separate
-// RoPE / append launch (16 per frame) disappears.  The ring is then read with plain loads (the warp reads rows it wrote).
-template <bool ROPE>
+// RoPE / append launch (16 per frame) disappears.  The ring is read with plain loads (the warp may read rows it wrote).
+// The fused form (freqs != nullptr) is a runtime branch of ONE compiled kernel, not a second instantiation: both forms then
+// run the same attention instructions, so they agree bit for bit whatever FMA contraction the compiler chooses.
 __global__ void __launch_bounds__(128, 4) ring_attention_pair64_kernel(const float* __restrict__ qkv, long long qbs, long long qts,
                                              float* kv, const long long* __restrict__ offset, int ostride,
                                              float* __restrict__ out, long long obs, long long ots, int B, int T, int H,
                                              int cap, int context, int linear, const float* __restrict__ freqs) {
   constexpr int D = 64;
-  auto ldk = [](const float4* p) { return ROPE ? *p : __ldg(p); };
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   const int P = (T + 1) / 2;
   const long long wid = (long long)blockIdx.x * (blockDim.x / 32) + warp;
@@ -258,13 +262,13 @@ __global__ void __launch_bounds__(128, 4) ring_attention_pair64_kernel(const flo
   const long long off = offset[(long long)b * ostride];
   const long long end = off + T;
   const long long pos0 = off + t0, pos1 = has1 ? pos0 + 1 : pos0;
-  if (ROPE) {
+  if (freqs) {
     // ts = offset.float() + arange(T) in fp32 (rope.py:39); separate mul / sub / add as the eager reference evaluates them
     auto rotate8 = [&](float* x, float ts) {
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
-        const float ang = __fmul_rn(freqs[4 * sub + i], ts);
-        const float c = cosf(ang), s = sinf(ang);
+        const float2 cs = rope_cos_sin(__fmul_rn(freqs[4 * sub + i], ts));
+        const float c = cs.x, s = cs.y;
         const float xr = x[2 * i], xi = x[2 * i + 1];
         x[2 * i] = __fsub_rn(__fmul_rn(xr, c), __fmul_rn(xi, s));
         x[2 * i + 1] = __fadd_rn(__fmul_rn(xr, s), __fmul_rn(xi, c));
@@ -310,7 +314,7 @@ __global__ void __launch_bounds__(128, 4) ring_attention_pair64_kernel(const flo
     // ---- scores of the 32 keys of the block: lane holds keys 4 it + grp, it = 0..7
     // All 16 K loads of the block are issued before the first use (branch-free slot arithmetic keeps the unrolled loop
     // one basic block): with a `while (slot >= cap)` wrap per key the compiler could keep only two loads in flight per
-    // warp and the kernel ran at memory LATENCY, not bandwidth (99 us per layer at a 200-token context, round 1).
+    // warp and the kernel ran at memory LATENCY, not bandwidth.
     float s0[8], s1[8];
     {
       float4 kq[8][2];
@@ -320,8 +324,8 @@ __global__ void __launch_bounds__(128, 4) ring_attention_pair64_kernel(const flo
         slot = small_ring ? slot % cap : (slot >= cap ? slot - cap : slot);
         const bool in = p0 + 4 * it + grp <= pos1;
         const float* kr = Kb + (long long)(in ? slot : slot_last) * D + 8 * sub;
-        kq[it][0] = ldk(reinterpret_cast<const float4*>(kr));
-        kq[it][1] = ldk(reinterpret_cast<const float4*>(kr + 4));
+        kq[it][0] = *reinterpret_cast<const float4*>(kr);
+        kq[it][1] = *reinterpret_cast<const float4*>(kr + 4);
       }
 #pragma unroll
       for (int it = 0; it < 8; ++it) {
@@ -366,7 +370,7 @@ __global__ void __launch_bounds__(128, 4) ring_attention_pair64_kernel(const flo
       const int j = 2 * i + half;
       int slot = base + j;
       slot = small_ring ? slot % cap : (slot >= cap ? slot - cap : slot);
-      vq[i] = ldk(reinterpret_cast<const float4*>(Vb + (long long)(j < nk ? slot : slot_last) * D + 4 * vl));
+      vq[i] = *reinterpret_cast<const float4*>(Vb + (long long)(j < nk ? slot : slot_last) * D + 4 * vl);
     }
 #pragma unroll
     for (int i = 0; i < 16; ++i) {
@@ -419,7 +423,7 @@ extern "C" int rstnet_rope_ring_attention_f32(const float* qkv, int64_t q_batch_
                  "rope_ring_attention: buffers and strides must be 16-byte aligned");
   const int warps = 4;
   const long long total = (long long)batch * H;
-  ring_attention_pair64_kernel<true><<<ceil_div(total, warps), warps * 32, 0, (cudaStream_t)stream>>>(
+  ring_attention_pair64_kernel<<<ceil_div(total, warps), warps * 32, 0, (cudaStream_t)stream>>>(
       qkv, q_batch_stride, q_time_stride, kv, (const long long*)offset, offset_stride ? 1 : 0, out, o_batch_stride, o_time_stride, batch, T, H,
       cap, context, 0, freqs);
   count_launch();
@@ -439,7 +443,7 @@ extern "C" int rstnet_ring_attention_f32(const float* qkv, int64_t q_batch_strid
                          q_time_stride % 4 == 0 && o_batch_stride % 4 == 0 && o_time_stride % 4 == 0;
   if (T >= 2 && D == 64 && aligned16) {
     const long long total = (long long)batch * ((T + 1) / 2) * H;
-    ring_attention_pair64_kernel<false><<<ceil_div(total, warps), warps * 32, 0, (cudaStream_t)stream>>>(
+    ring_attention_pair64_kernel<<<ceil_div(total, warps), warps * 32, 0, (cudaStream_t)stream>>>(
         qkv, q_batch_stride, q_time_stride, const_cast<float*>(kv), (const long long*)offset, ostride, out, o_batch_stride, o_time_stride,
         batch, T, H, cap, context, linear, nullptr);
   } else if (T >= 2) {

@@ -59,7 +59,7 @@ __global__ void conv_cout1_kernel(const float* __restrict__ x, long long xbs, lo
     const int total = nrows * Cin;
     if ((Cin & 3) == 0 && (xts & 3) == 0 && ((uintptr_t)xb & 15) == 0) {
       // 16-byte loads, four row pieces per lane in flight: the kernel is a pure stream over the input (126 MB per 256-stream
-      // frame at 24 kHz) and scalar loads left it at 1.8 TB/s
+      // frame at 24 kHz) and scalar loads left it far below HBM bandwidth
       const int c4n = Cin >> 2, total4 = nrows * c4n;
       for (int i0 = lane; i0 < total4; i0 += 128) {
         float4 v[4];
@@ -195,7 +195,7 @@ __global__ void layer_norm_kernel(const float* __restrict__ x, long long xbs, co
 }
 
 // Same arithmetic, but the row lives in registers: ONE pass over memory instead of three dependent ones (the 25 Hz
-// transformer launches this 32 times per frame on 512 rows: it ran at memory latency, 7.9 us for 2 MB).
+// transformer launches this 32 times per frame on 512 rows: the three-pass form ran at memory latency).
 template <int NPL>
 __global__ void layer_norm_reg_kernel(const float* __restrict__ x, long long xbs, const float* __restrict__ w,
                                       const float* __restrict__ bias, float* __restrict__ y, long long rows, int rows_per_batch,

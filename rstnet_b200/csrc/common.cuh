@@ -1,4 +1,4 @@
-// Shared helpers for the rstnet_b200 CUDA library (sm_100a only).
+// Shared helpers for the rstnet_b200 CUDA library (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
@@ -76,14 +76,22 @@ __device__ __forceinline__ float warp_max(float v) {
 
 inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }
 
+// SMs of the current device (grid sizing of persistent and grid-stride kernels)
+inline int sm_count() {
+  int dev = 0, n = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+  return n > 0 ? n : 1;
+}
+
 // ---- programmatic dependent launch (PDL), opt-in with RSTNET_PDL=1.  The LM frame is a chain of ~800 small dependent
 // kernels; with the launch attribute below the next kernel's CTAs are scheduled while the previous grid drains and run their
-// prologue (barrier / TMEM set-up, descriptor prefetch) up to `pdl_wait()`, which returns once the previous grid has
+// prologue (barrier set-up, descriptor prefetch) up to `pdl_wait()`, which returns once the previous grid has
 // completed and flushed.  Every kernel launched through launch_pdl() calls pdl_launch_dependents() and then pdl_wait()
 // before its first global access, so the ordering guarantees are those of plain stream order (also inside a captured CUDA
-// graph).  MEASURED (scripts/lm_frame_timing.py, 7B frame, B = 64, graph replay): 24.1 ms with PDL vs 20.0 ms without --
-// programmatic edges between graph kernel nodes cost ~5 us per launch more than plain edges on this driver, which outweighs
-// the hidden prologues; hence off by default.  Without the attribute griddepcontrol.* are no-ops.
+// graph).  Off by default: inside a replayed CUDA graph, programmatic edges between kernel nodes can cost more per launch
+// than plain edges, which outweighs the hidden prologues (time the frame with scripts/lm_frame_timing.py before enabling
+// it).  Without the attribute griddepcontrol.* are no-ops.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 bool pdl_enabled();   // env RSTNET_PDL=1 (default off); capi.cu

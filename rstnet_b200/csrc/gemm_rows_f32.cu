@@ -235,9 +235,9 @@ extern "C" int rstnet_gemm_rows_f32(const rstnet_gemm_rows_args* args, rstnet_st
   cudaStream_t st = (cudaStream_t)stream;
   const long long M = (long long)a.batch * a.rows;
   const int N = a.N;
-  // Tile choice: widest tile that still gives >= 2 CTAs per SM (148 SMs); narrow N gets narrow BN.
+  // Tile choice: widest tile that still gives >= 2 CTAs per SM; narrow N gets narrow BN.
   auto ctas = [&](int bm, int bn) { return (long long)ceil_div(M, bm) * ceil_div(N, bn); };
-  const long long want = 2 * 148;
+  const long long want = 2 * sm_count();
   if (N <= 32) {
     if (ctas(128, 32) >= want) return launch_cfg<TileCfg<128, 32, 4, 4>>(a, st);
     return launch_cfg<TileCfg<32, 32, 2, 4>>(a, st);

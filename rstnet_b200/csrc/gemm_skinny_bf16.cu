@@ -1,9 +1,9 @@
-// Weight-streaming skinny GEMM for the LM decode step (tcgen05 kind::f16 / bf16, fp32 accumulate in
-// TMEM):   out[m, n] = sum_k X[m, k] * W[n, k]  (+ R[m, n]),   M = concurrent streams (<= 256).
+// Weight-streaming skinny GEMM for the LM decode step (wgmma, bf16 operands, fp32 accumulate in
+// registers):   out[m, n] = sum_k X[m, k] * W[n, k]  (+ R[m, n]),   M = concurrent streams (<= 128).
 //
 // The step is HBM-bound (each bf16 weight is used for M MACs), so the design goal is to keep
-// 148 SMs pulling weight tiles at full rate: the weight matrix is the MMA "A" operand (128 rows of
-// W per CTA = UMMA M), the activations are the "B" operand (UMMA N = M rounded up to 16), both
+// every SM pulling weight tiles at full rate: the weight matrix is the MMA "A" operand (128 rows of
+// W per CTA = two m64 wgmmas), the activations are the "B" operand (wgmma N = M rounded up to 16, 32, 64 or 128), both
 // K-major exactly as nn.Linear stores them, 4-stage TMA ring of 128x64 bf16 weight tiles, two CTAs per SM, and
 // split-K across CTAs when N/128 alone cannot fill the machine (fp32 partials + finalize kernel).
 // Replaces F.linear in CausalSelfAttention / LLaMAMLP / lm_head (models/llama_streaming.py:935-998,
@@ -21,16 +21,23 @@ namespace rstnet {
 extern void count_launch();
 using namespace tc;
 
-constexpr int SK_BN = 128;      // weight rows per CTA (UMMA M)
+constexpr int SK_BN = 128;      // weight rows per CTA (two m64 wgmmas)
 constexpr int SK_BK = 64;       // bf16 elements per 128-byte swizzle row
 constexpr int SK_W_BYTES = SK_BN * 128;
-constexpr int SK_THREADS = 192; // TMA, MMA, 4 epilogue warps
+constexpr int SK_THREADS = 160; // one consumer warpgroup + the TMA warp
+constexpr int SK_STAGES = 4;
+
+template <int NB>   // wgmma N: streams rounded up to 16, 32, 64 or 128
+struct SkCfg {
+  static constexpr int STAGE_BYTES = SK_W_BYTES + ((NB * 128 + 1023) & ~1023);
+  static constexpr int SMEM_BYTES = SK_STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+};
 
 struct SkParams {
   __nv_bfloat16* out;        // [M][N] bf16 (splits == 1)
   float* partial;            // [splits][M][N] fp32 (splits > 1)
   const __nv_bfloat16* R;    // optional residual [M][N]
-  int M, N, K, MB;           // MB = M rounded up to 16 (UMMA N)
+  int M, N, K;
   int splits, k_iters;       // k_iters = 64-element chunks per split
   int force_partial;         // write fp32 partials even with one split (a fused finalize kernel consumes them)
   // ---- in-kernel finalize ("tail"): once the `splits` CTAs of an N tile have all arrived on tail_cnt[tile], each of them
@@ -163,20 +170,21 @@ __device__ __forceinline__ void skinny_tail(const SkParams& p, int tile, int par
   }
 }
 
-template <int STAGES>
+// Thread roles (160 threads): warpgroup 0 = consumers (wgmma issue + epilogue), warp 4 = TMA producer.  A consumer
+// thread (warp wq, lane = 4 gq + tq) ends with the accumulators of weight rows n0 + 64 h + 16 wq + gq (+ 8), streams
+// 8 b + 2 tq (+ 1) for both 64-row halves h.
+template <int NB>
 __global__ void __launch_bounds__(SK_THREADS, 2)
 gemm_skinny_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX, const SkParams p) {
+  constexpr int STAGES = SK_STAGES;
+  constexpr int STAGE_BYTES = SkCfg<NB>::STAGE_BYTES;
+  constexpr int NR = NB / 2;   // accumulator registers per thread of one 64 x NB wgmma
   extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment as pointer arithmetic on the __shared__ array (an integer round trip would demote every later
-  // access through `smem` to generic LD / ST)
+  // 1024-byte alignment (128-byte swizzle atoms) as pointer arithmetic on the __shared__ array (an integer round trip
+  // would demote every later access through `smem` to generic LD / ST)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  const int x_bytes = p.MB * 128;
-  const int stage_bytes = SK_W_BYTES + ((x_bytes + 1023) & ~1023);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * stage_bytes);
-  uint64_t* full = bars;
-  uint64_t* empty = bars + STAGES;
-  uint64_t* tmem_full = bars + 2 * STAGES;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 1);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
+  uint64_t* empty = full + STAGES;
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   const int n0 = blockIdx.x * SK_BN;
   const int split = blockIdx.y;
@@ -184,90 +192,82 @@ gemm_skinny_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
   int k_count = p.K / SK_BK - k_begin;
   if (k_count > p.k_iters) k_count = p.k_iters;
 
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmW);
-    tma_prefetch_desc(&tmX);
+  if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], 4);   // one arrival per consumer warp
     }
-    mbar_init(tmem_full, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<256>(tmem_ptr);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  // everything above touched only this CTA's shared memory / TMEM: it overlaps the tail of the previous kernel (PDL)
+  // everything above touched only this CTA's shared memory: it overlaps the tail of the previous kernel (PDL)
   pdl_launch_dependents();
   pdl_wait();
 
-  if (warp == 0) {
-    for (int kit = 0; kit < k_count; ++kit) {
-      const int s = kit % STAGES;
-      const uint32_t ph = (kit / STAGES) & 1;
-      mbar_wait(&empty[s], ph ^ 1);
-      if (elect_one()) {
-        uint8_t* st = smem + s * stage_bytes;
-        mbar_arrive_expect_tx(&full[s], SK_W_BYTES + x_bytes);
+  if (warp == 4) {
+    if (elect_one()) {
+      tma_prefetch_desc(&tmW);
+      tma_prefetch_desc(&tmX);
+      for (int kit = 0; kit < k_count; ++kit) {
+        const int s = kit % STAGES;
+        mbar_wait(&empty[s], ((kit / STAGES) & 1) ^ 1);
+        uint8_t* st = smem + s * STAGE_BYTES;
+        mbar_arrive_expect_tx(&full[s], SK_W_BYTES + NB * 128);
         tma_load_2d(st, &tmW, &full[s], (k_begin + kit) * SK_BK, n0);
         tma_load_2d(st + SK_W_BYTES, &tmX, &full[s], (k_begin + kit) * SK_BK, 0);
       }
-      __syncwarp();
     }
-  } else if (warp == 1) {
-    const uint32_t idesc = instr_desc(1u, SK_BN, (uint32_t)p.MB);
-    for (int kit = 0; kit < k_count; ++kit) {
-      const int s = kit % STAGES;
-      const uint32_t ph = (kit / STAGES) & 1;
-      mbar_wait(&full[s], ph);
-      tc_fence_after();
-      if (elect_one()) {
-        uint8_t* st = smem + s * stage_bytes;
-        const uint64_t dw = smem_desc_sw128(smem_u32(st)), dx = smem_desc_sw128(smem_u32(st + SK_W_BYTES));
+    return;
+  }
+
+  float c0[NR], c1[NR];   // weight rows [0, 64) and [64, 128) of the tile
 #pragma unroll
-        for (int k = 0; k < 4; ++k)  // 4 x (K = 16 bf16 = 32 bytes)
-          mma_f16(tmem_base, dw + (uint64_t)(2 * k), dx + (uint64_t)(2 * k), idesc, (kit > 0 || k > 0) ? 1u : 0u);
-        tc_commit(&empty[s]);
-        if (kit == k_count - 1) tc_commit(tmem_full);
-      }
-      __syncwarp();
+  for (int j = 0; j < NR; ++j) c0[j] = c1[j] = 0.f;
+  const uint32_t smem0 = smem_u32(smem);
+  for (int kit = 0; kit < k_count; ++kit) {
+    const int s = kit % STAGES;
+    mbar_wait(&full[s], (kit / STAGES) & 1);
+    const uint32_t st = smem0 + (uint32_t)(s * STAGE_BYTES);
+    const uint64_t dw0 = gmma_desc_sw128(st), dw1 = gmma_desc_sw128(st + 64 * 128), dx = gmma_desc_sw128(st + SK_W_BYTES);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {  // 4 x (K = 16 bf16 = 32 bytes)
+      const uint32_t acc_in = (kit > 0 || k > 0) ? 1u : 0u;
+      wgmma_bf16_ss<NB>(c0, dw0 + (uint64_t)(2 * k), dx + (uint64_t)(2 * k), acc_in);
+      wgmma_bf16_ss<NB>(c1, dw1 + (uint64_t)(2 * k), dx + (uint64_t)(2 * k), acc_in);
     }
-  } else {
-    // epilogue: thread = one weight row n; TMEM columns = streams m
-    mbar_wait(tmem_full, 0);
-    tc_fence_after();
-    const int q = warp % 4;
-    const int n = n0 + q * 32 + lane;
-    const bool nv = n < p.N;
-    for (int c0 = 0; c0 < p.MB; c0 += 32) {
-      uint32_t r[32];
-      tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, r);
-      tmem_ld_wait();
-      if (p.tail == 4) {
-        // rows 2j / 2j+1 of the interleaved weight are a_j / b_j: neighbouring lanes hold the gate and the value of
-        // output column j, so SiLU gating needs one shuffle and no fp32 partials (gating.py:12-21; lit_model.py:399-403)
-        const int I = p.N / 2;
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_acc(c0);
+    fence_acc(c1);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[s]);
+  }
+
+  // epilogue: weight rows n, streams m
+  const int gq = lane / 4, tq = lane % 4;
+  auto store = [&](const float (&c)[NR], int half) {
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const float v = __uint_as_float(r[j]);
-          const float o = __shfl_xor_sync(0xffffffffu, v, 1);
-          const int m = c0 + j;
-          if (!(lane & 1) && nv && m < p.M) {
-            const float a = __bfloat162float(__float2bfloat16(v)), b = __bfloat162float(__float2bfloat16(o));
-            const float sl = __bfloat162float(__float2bfloat16(a / (1.0f + expf(-a))));
-            p.aux[(long long)m * I + (n >> 1)] = __float2bfloat16(sl * b);
-          }
-        }
-        continue;
-      }
-      if (nv) {
+    for (int e = 0; e < 2; ++e) {
+      const int n = n0 + 64 * half + 16 * warp + gq + 8 * e;
+      const bool nv = n < p.N;
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const int m = c0 + j;
-          if (m < p.M) {
-            float v = __uint_as_float(r[j]);
+      for (int b = 0; b < NB / 8; ++b) {
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+          const int m = 8 * b + 2 * tq + u;
+          float v = c[4 * b + 2 * e + u];
+          if (p.tail == 4) {
+            // rows 2j / 2j+1 of the interleaved weight are a_j / b_j: lanes 4 apart hold the gate and the value of
+            // output column j, so SiLU gating needs one shuffle and no fp32 partials (gating.py:12-21; lit_model.py:399-403)
+            const float o = __shfl_xor_sync(0xffffffffu, v, 4);
+            if (!(gq & 1) && nv && m < p.M) {
+              const int I = p.N / 2;
+              const float a = __bfloat162float(__float2bfloat16(v)), bb = __bfloat162float(__float2bfloat16(o));
+              const float sl = __bfloat162float(__float2bfloat16(a / (1.0f + expf(-a))));
+              p.aux[(long long)m * I + (n >> 1)] = __float2bfloat16(sl * bb);
+            }
+          } else if (nv && m < p.M) {
             if (p.splits > 1 || p.force_partial) {
               p.partial[((long long)split * p.M + m) * p.N + n] = v;
             } else {
@@ -278,31 +278,30 @@ gemm_skinny_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
         }
       }
     }
-    if (p.tail && p.tail != 4) {
-      const int t = threadIdx.x - 64;
-      const int n_tiles = (int)gridDim.x, half = n_tiles / 2;
-      const bool gate = p.tail == 3;             // SiLU: the a and b tiles of a column block are finalized together
-      const int cnt = gate ? (int)blockIdx.x % half : (int)blockIdx.x;
-      const int nparts = gate ? 2 * p.splits : p.splits;
-      const int part = gate ? 2 * (int)blockIdx.y + ((int)blockIdx.x >= half ? 1 : 0) : (int)blockIdx.y;
-      int* arrive = p.tail_cnt + cnt;
-      int* seen = p.tail_cnt + n_tiles + cnt;
-      __threadfence();                 // this CTA's partials are visible before its arrival is counted
-      named_bar_sync(1, 128);
-      if (t == 0) {
-        atomicAdd(arrive, 1);
-        while (*reinterpret_cast<volatile int*>(arrive) < nparts) __nanosleep(32);
-        // the last CTA to have seen the full count re-arms the pair of counters for the next launch
-        if (atomicAdd(seen, 1) == nparts - 1) { *arrive = 0; *seen = 0; }
-        __threadfence();
-      }
-      named_bar_sync(1, 128);
-      skinny_tail(p, cnt, part, nparts, t);
+  };
+  store(c0, 0);
+  store(c1, 1);
+  if (p.tail && p.tail != 4) {
+    const int t = threadIdx.x;
+    const int n_tiles = (int)gridDim.x, half = n_tiles / 2;
+    const bool gate = p.tail == 3;             // SiLU: the a and b tiles of a column block are finalized together
+    const int cnt = gate ? (int)blockIdx.x % half : (int)blockIdx.x;
+    const int nparts = gate ? 2 * p.splits : p.splits;
+    const int part = gate ? 2 * (int)blockIdx.y + ((int)blockIdx.x >= half ? 1 : 0) : (int)blockIdx.y;
+    int* arrive = p.tail_cnt + cnt;
+    int* seen = p.tail_cnt + n_tiles + cnt;
+    __threadfence();                 // this CTA's partials are visible before its arrival is counted
+    named_bar_sync(1, 128);
+    if (t == 0) {
+      atomicAdd(arrive, 1);
+      while (*reinterpret_cast<volatile int*>(arrive) < nparts) __nanosleep(32);
+      // the last CTA to have seen the full count re-arms the pair of counters for the next launch
+      if (atomicAdd(seen, 1) == nparts - 1) { *arrive = 0; *seen = 0; }
+      __threadfence();
     }
+    named_bar_sync(1, 128);
+    skinny_tail(p, cnt, part, nparts, t);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<256>(tmem_base);
 }
 
 // plain finalize: out = bf16(sum_s partial[s] + R), 4 elements per thread (N % 4 == 0)
@@ -430,6 +429,30 @@ static EncodeTiledFn2 get_encode_fn2() {
   }
   return fn;
 }
+
+typedef void (*SkinnyKernel)(const CUtensorMap, const CUtensorMap, const SkParams);
+static SkinnyKernel skinny_kernel(int nb) {
+  switch (nb) {
+    case 16: return gemm_skinny_kernel<16>;
+    case 32: return gemm_skinny_kernel<32>;
+    case 64: return gemm_skinny_kernel<64>;
+    default: return gemm_skinny_kernel<128>;
+  }
+}
+static int skinny_smem(int nb) {
+  switch (nb) {
+    case 16: return SkCfg<16>::SMEM_BYTES;
+    case 32: return SkCfg<32>::SMEM_BYTES;
+    case 64: return SkCfg<64>::SMEM_BYTES;
+    default: return SkCfg<128>::SMEM_BYTES;
+  }
+}
+// one-time opt-in to the instantiation's dynamic shared memory (per device, like smem_optin)
+static void skinny_optin(int nb) {
+  static unsigned long long done[4] = {0, 0, 0, 0};
+  const int idx = nb == 16 ? 0 : nb == 32 ? 1 : nb == 64 ? 2 : 3;
+  smem_optin(skinny_kernel(nb), skinny_smem(nb), done[idx]);
+}
 }  // namespace rstnet
 using namespace rstnet;
 
@@ -438,6 +461,7 @@ struct rstnet_skinny_plan {
   SkParams p;
   dim3 grid;
   size_t smem;
+  int nb;        // wgmma N (streams rounded up)
   int fin_mode;  // 0 plain, 1 finalize + residual + RMSNorm -> aux, 2 finalize + SiLU gating -> aux
   const __nv_bfloat16* norm_w;
   __nv_bfloat16* aux;
@@ -475,18 +499,17 @@ extern "C" int rstnet_skinny_gemm_create_fused(const void* X, const void* W, con
   EncodeTiledFn2 enc = get_encode_fn2();
   RSTNET_REQUIRE(enc != nullptr, "skinny_gemm_create: cuTensorMapEncodeTiled unavailable");
   rstnet_skinny_plan* pl = new rstnet_skinny_plan();
-  const int MB = ((M + 15) / 16) * 16;
+  const int NB = M <= 16 ? 16 : M <= 32 ? 32 : M <= 64 ? 64 : 128;
   const int n_tiles = ceil_div(N, SK_BN);
   const int kchunks = K / SK_BK;
   int splits = 1;
   RSTNET_REQUIRE(!(partial_ws && max_splits > 1) || N % 4 == 0, "skinny_gemm_create: split-K needs N %% 4 == 0");
   if (partial_ws && max_splits > 1) {
-    // Enough CTAs to keep ~1.5 per SM streaming, no more: every split adds an fp32 partial round trip.  Measured on
-    // the 7B shapes (scripts/skinny_sweep.py, GEMM + finalize, us): qkv 96 tiles {1: 30.7, 2: 28.9, 4: 36.7},
-    // fc 172 tiles {1: 48.1, 2: 53.4}, proj 32 tiles {2: 22.7, 4: 20.4, 8: 19.4}, mlp proj {4: 30.9, 6: 28.8, 8: 29.0}.
+    // Enough CTAs to keep ~1.5 per SM streaming, no more: every split adds an fp32 partial round trip
+    // (scripts/skinny_sweep.py times GEMM + finalize per split factor and layer shape).
     {
       const int cand[6] = {1, 2, 3, 4, 6, 8};
-      const float want = 224.0f / (float)n_tiles;
+      const float want = 1.5f * (float)sm_count() / (float)n_tiles;
       float best = 1e30f;
       for (int c : cand) {
         if (c > max_splits || (c > 1 && kchunks / c < 8)) continue;
@@ -509,7 +532,7 @@ extern "C" int rstnet_skinny_gemm_create_fused(const void* X, const void* W, con
     CUresult r = enc(&pl->tmW, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (void*)W, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     cuuint64_t gdx[2] = {(cuuint64_t)K, (cuuint64_t)M};
-    cuuint32_t bx[2] = {SK_BK, (cuuint32_t)MB};
+    cuuint32_t bx[2] = {SK_BK, (cuuint32_t)NB};
     if (r == CUDA_SUCCESS)
       r = enc(&pl->tmX, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (void*)X, gdx, gstr, bx, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
               CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -521,34 +544,31 @@ extern "C" int rstnet_skinny_gemm_create_fused(const void* X, const void* W, con
   }
   SkParams& p = pl->p;
   p.out = (__nv_bfloat16*)out; p.partial = partial_ws; p.R = (const __nv_bfloat16*)R;
-  p.M = M; p.N = N; p.K = K; p.MB = MB; p.splits = splits;
+  p.M = M; p.N = N; p.K = K; p.splits = splits;
+  pl->nb = NB;
   pl->fin_mode = fin_mode; pl->norm_w = (const __nv_bfloat16*)norm_w; pl->aux = (__nv_bfloat16*)aux_out; pl->eps = eps; pl->kyutai = kyutai;
   // a fused finalize always reads fp32 partials, so the main kernel takes the split path even with one split
   p.force_partial = fin_mode == 1 || fin_mode == 2;
   p.k_iters = ceil_div(kchunks, splits);
   pl->grid = dim3((unsigned)n_tiles, (unsigned)splits);
-  const int stage_bytes = SK_W_BYTES + ((MB * 128 + 1023) & ~1023);
-  // 4 stages (<= 98 KB with M <= 64): two CTAs fit per SM, so a GEMM whose tile count is not a multiple of 148
+  // 4 stages (<= 98 KB with M <= 64): two CTAs fit per SM, so a GEMM whose tile count is not a multiple of the SM count
   // still keeps every SM streaming (bandwidth-bound CTAs progress at equal rates) and prologues overlap main loops
-  pl->smem = (size_t)4 * stage_bytes + 1024 + 256;
+  pl->smem = (size_t)skinny_smem(NB);
   // In-kernel finalize instead of a second launch: possible whenever fp32 partials are written, the grid is co-resident
   // (every CTA waits for the other K slices of its tile, the RMSNorm tail for the whole grid) and, for SiLU, the a / b
   // column blocks are whole tiles.  OPT-IN (RSTNET_SKINNY_TAIL=1), parity-tested, because it does not pay: the tail is a
   // chain of ~6-8 dependent L2 round trips (release fence, arrival atomic, poll, partial loads, sums-of-squares exchange,
-  // stores) = 5-8 us, as much as the launch boundary it removes.  Measured on the 7B frame at B = 64: temporal part
-  // 14.47 ms with the tail vs 14.48 ms with 96 finalize launches; depth part (192 small GEMMs) 4.5 ms vs 3.0 ms.
+  // stores), as long as the launch boundary it removes; on the small depth GEMMs it sits on every CTA's critical path.
   p.tail = 0; p.tail_cnt = nullptr; p.tail_ssq = nullptr; pl->tail_mem = nullptr;
   p.norm_w = pl->norm_w; p.aux = pl->aux; p.eps = eps; p.kyutai = kyutai;
   {
     static const bool tail_on = []() { const char* e = getenv("RSTNET_SKINNY_TAIL"); return e && e[0] == '1'; }();
     const bool partials = splits > 1 || p.force_partial;
     // every CTA waits for the other K slices of its tile (and, for RMSNorm, for the whole grid): the grid must be co-resident
-    int sms = 148, dev = 0, per_sm = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    static unsigned long long attr = 0;
-    smem_optin(gemm_skinny_kernel<4>, 200 * 1024, attr);
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gemm_skinny_kernel<4>, SK_THREADS, pl->smem) != cudaSuccess) {
+    const int sms = sm_count();
+    int per_sm = 0;
+    skinny_optin(NB);
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, skinny_kernel(NB), SK_THREADS, pl->smem) != cudaSuccess) {
       cudaGetLastError();
       per_sm = 0;
     }
@@ -576,10 +596,9 @@ extern "C" int rstnet_skinny_gemm_create_fused(const void* X, const void* W, con
 
 extern "C" int rstnet_skinny_gemm_run(const rstnet_skinny_plan* pl, rstnet_stream_t stream) {
   RSTNET_REQUIRE(pl != nullptr, "skinny_gemm_run: null plan");
-  static unsigned long long attr = 0;
-  smem_optin(gemm_skinny_kernel<4>, 200 * 1024, attr);
+  skinny_optin(pl->nb);
   cudaStream_t st = (cudaStream_t)stream;
-  launch_pdl(gemm_skinny_kernel<4>, pl->grid, dim3(SK_THREADS), pl->smem, st, pl->tmW, pl->tmX, pl->p);
+  launch_pdl(skinny_kernel(pl->nb), pl->grid, dim3(SK_THREADS), pl->smem, st, pl->tmW, pl->tmX, pl->p);
   count_launch();
   if (int e = check_launch("gemm_skinny")) return e;
   if (pl->p.tail) return 0;          // finalized inside the kernel
@@ -592,14 +611,14 @@ extern "C" int rstnet_skinny_gemm_run(const rstnet_skinny_plan* pl, rstnet_strea
   }
   if (pl->fin_mode == 2) {
     int g = ceil_div(MN / 2, 256);
-    if (g > 148 * 8) g = 148 * 8;
+    if (g > sm_count() * 8) g = sm_count() * 8;
     launch_pdl(skinny_finalize_silu_kernel, dim3(g), dim3(256), 0, st, (const float*)pl->p.partial, pl->aux, pl->p.M, pl->p.N, pl->p.splits);
     count_launch();
     return check_launch("skinny_finalize_silu");
   }
   if (pl->p.splits > 1) {
     int g = ceil_div(MN / 4, 256);
-    if (g > 148 * 4) g = 148 * 4;
+    if (g > sm_count() * 4) g = sm_count() * 4;
     launch_pdl(skinny_finalize_kernel, dim3(g), dim3(256), 0, st, (const float*)pl->p.partial, pl->p.R, pl->p.out, MN, pl->p.splits);
     count_launch();
     return check_launch("skinny_finalize");

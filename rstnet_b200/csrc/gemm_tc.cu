@@ -1,21 +1,22 @@
-// tcgen05 / TMEM / TMA GEMM for the codec's convs, transposed convs and linears.
+// Warpgroup-MMA (wgmma) / TMA GEMM for the codec's convs, transposed convs and linears.
 //
 //   D[(i,o), n] = sum_{tap} sum_{c} A[c, i + tap*tap_di, o*o_mul + tap*tap_do] * W[n, tap*Kc + c]
 //
 // A is a 3-D TMA tensor (c, i, o): the activation buffer itself (no im2col), so a causal conv is a
-// K loop over taps.  One CTA owns a 128 x BN output tile with the fp32 accumulator in TMEM.
-// Warp roles (448 threads): warp 0 = TMA producer, warp 1 = TMEM allocator + single-thread
-// tcgen05.mma issuer, warps 2..9 = activation transform (pre-activation, TF32 hi/lo split of the A
-// tile in shared memory; weights arrive pre-split), warps 10..13 = promote the TMEM chunk
-// accumulators into fp32 registers, then run the epilogue.
+// K loop over taps.  A CTA computes 128 x BN output tiles, persistently: tiles blockIdx.x, +gridDim.x, ... with the N tile
+// fastest, so CTAs running together share A rows in L2, and the TMA warp fetches the next tile's stages while the
+// consumers run the epilogue of the current one.  Warp roles (288 threads): warpgroups 0 and 1 = consumers, each owning
+// 64 rows of the tile; warp 8 = TMA producer filling an S-stage ring of [A fp32 128 x 32 | W_hi BN x 32 | W_lo BN x 32].
 //
-// Precision 0 ("3xTF32"): fp32-equivalent products for the encoder side, where RVQ indices must
-// match the fp32 reference (SURVEY.md H1).  Each fp32 operand x is split in shared memory into
-// hi = rna_tf32(x) and lo = rna_tf32(x - hi) (both exactly representable in TF32), and three TF32
-// MMAs accumulate a_lo*b_hi + a_hi*b_lo + a_hi*b_hi in fp32 (dropping the 2^-22 lo*lo term).
-// Precision 1: one TF32 MMA (hi only).  The transform warps also apply a fused pre-activation (ELU).
+// Precision 0 ("3xTF32"): fp32-equivalent products for the encoder side, where RVQ indices must match the fp32 reference
+// (SURVEY.md H1).  A consumer reads its A fragment out of the swizzled fp32 tile into registers, applies the fused
+// pre-activation and splits each value x into hi = rna_tf32(x) and lo = rna_tf32(x - hi) (both exactly representable in
+// TF32); the weights arrive pre-split.  Register-A wgmmas accumulate a_hi*b_hi into one accumulator and a_lo*b_hi +
+// a_hi*b_lo into a second (the small terms kept apart; the 2^-22 lo*lo term is dropped).  Precision 1: one TF32 wgmma
+// (hi only; the tensor core reads the top 19 bits of the fp32 weights).
+// Every chunk of TC_CHUNK_STAGES stages (K = 128) starts fresh wgmma accumulators that are then added into fp32 registers
+// with round-to-nearest, so the error of the tensor core's internal accumulation is bounded by one chunk, whatever K is.
 #include <cstdlib>
-#include <type_traits>
 
 #include "common.cuh"
 #include "tc_common.cuh"
@@ -28,10 +29,9 @@ using namespace tc;
 constexpr int TC_BM = 128;
 constexpr int TC_BKE = 32;                 // fp32 elements per 128-byte swizzle row
 constexpr int TC_A_BYTES = TC_BM * 128;    // 16 KB
-constexpr int TC_THREADS = 448;          // TMA, MMA, 8 transform, 4 drain/epilogue warps
-constexpr int TC_XF_THREADS = 256;       // transform threads (warps 2..9)
-constexpr int TC_CHUNK_STAGES = 4;       // K elements accumulated in TMEM before promotion = 4 * 32
-constexpr int TC_NACC = 2;               // independent TMEM accumulators per buffer (consecutive MMAs alternate: no RAW chain)
+constexpr int TC_CONSUMER_WARPS = 8;       // two warpgroups of 64 tile rows each
+constexpr int TC_THREADS = 32 * TC_CONSUMER_WARPS + 32;   // + the TMA warp
+constexpr int TC_CHUNK_STAGES = 4;         // K stages accumulated by the tensor core before promotion = 4 * 32
 
 struct TcParams {
   float* C;
@@ -46,21 +46,16 @@ struct TcParams {
   int I_out, O_out, N, Kc;
   int taps, tap_di, tap_do, o_mul, kchunks;
   int pre_act, post_act, i_tiles;
-  int tma_store, c_tr;   // .ts kernel: epilogue through TMA tile stores (no residual); c_tr = output rows per o for n_split
-  int m_tiles, n_tiles;  // (I tiles x O_out) and N tiles: the persistent .ts kernel walks m_tiles * n_tiles
-  int ksplit;            // .ts kernel: K slices per tile = CTAs per cluster (1, or 2 for the few-tile long-K linears)
-  long long* trace;  // optional [total_k][8] clock64 stamps of CTA 0 (debug / profiling)
-  long long* cta_times;  // optional [grid.x][4] %globaltimer: entry, setup done, mainloop+epilogue done, exit (blockIdx.y == 0)
+  int m_tiles, n_tiles;  // (I tiles x O_out) and N tiles
 };
 
 template <int BN, int PREC>
 struct TcCfg {
   static constexpr bool SPLIT = PREC == 0;
   static constexpr int B_BYTES = BN * 128;
-  static constexpr int STAGE_BYTES = (TC_A_BYTES + B_BYTES) * (SPLIT ? 2 : 1);
-  static constexpr int STAGES = (200 * 1024 / STAGE_BYTES) > 6 ? 6 : (200 * 1024 / STAGE_BYTES);
+  static constexpr int STAGE_BYTES = TC_A_BYTES + B_BYTES * (SPLIT ? 2 : 1);
+  static constexpr int STAGES = (200 * 1024 / STAGE_BYTES) > 8 ? 8 : (200 * 1024 / STAGE_BYTES);
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
-  static constexpr int TMEM_COLS = 2 * TC_NACC * BN;  // two buffers x TC_NACC interleaved accumulators
 };
 
 // round-to-nearest (ties away) TF32 on the integer pipe: add half an ulp of the 10-bit mantissa to
@@ -68,736 +63,174 @@ struct TcCfg {
 // the slow conversion rate).  |x - hi| <= 2^-12 |x|, so with lo = rna(x - hi) the split
 // x ~ hi + lo is good to 2^-24 |x|: fp32-equivalent products.
 __device__ __forceinline__ float tf32_rna(float x) { return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u); }
-__device__ __forceinline__ float4 tf32_hi(float4 v) {
-  return make_float4(tf32_rna(v.x), tf32_rna(v.y), tf32_rna(v.z), tf32_rna(v.w));
+
+// fused activation of the tensor-core path (ELU through ex2.approx, common.cuh)
+__device__ __forceinline__ float act_tc(float x, int act) {
+  if (act == ACT_ELU) return elu_fast(x);
+  if (act == ACT_GELU) return gelu_f(x);
+  return x;
 }
 
-template <int BN, int PREC>
+// PRE_ELU: the fused pre-activation (ELU or none) is a template parameter and evaluated branch-free, so the consumer
+// path from one wgmma group to the next has no data-dependent divergence (ptxas would otherwise serialise the wgmmas
+// behind compiler-inserted warpgroup arrives).
+template <int BN, int PREC, bool PRE_ELU>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
                const __grid_constant__ CUtensorMap tmWlo, const TcParams p) {
   using Cfg = TcCfg<BN, PREC>;
   constexpr int S = Cfg::STAGES;
   constexpr int CH = TC_CHUNK_STAGES;
+  constexpr int NR = BN / 2;   // accumulator registers per thread of a 64 x BN wgmma
   extern __shared__ uint8_t smem_raw[];
-  auto gtime = []() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return (long long)t; };
-  const bool timed = p.cta_times && blockIdx.y == 0 && threadIdx.x == 0;
-  if (timed) p.cta_times[blockIdx.x * 4 + 0] = gtime();
-  // 1024-byte alignment as pointer arithmetic on the __shared__ array (an integer round trip would demote every later
-  // access through `smem` to generic LD / ST)
+  // 1024-byte alignment (128-byte swizzle atoms) as pointer arithmetic on the __shared__ array (an integer round trip
+  // would demote every later access through `smem` to generic LD / ST)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S * Cfg::STAGE_BYTES);
-  uint64_t* full = bars;               // [S] TMA landed
-  uint64_t* ready = bars + S;          // [S] operands transformed (128 arrivals)
-  uint64_t* empty = bars + 2 * S;      // [S] MMAs reading the stage retired
-  uint64_t* acc_full = bars + 3 * S;   // [2] a K chunk has been accumulated into TMEM buffer b
-  uint64_t* acc_empty = bars + 3 * S + 2;  // [2] buffer b drained into registers (128 arrivals)
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 3 * S + 4);
-
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + S * Cfg::STAGE_BYTES);   // [S] TMA landed
+  uint64_t* empty = full + S;                                                  // [S] every consumer warp is done with it
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
-  const int it = blockIdx.x % p.i_tiles, ot = blockIdx.x / p.i_tiles;
-  const int i0 = it * TC_BM, n0 = blockIdx.y * BN;
   const int total_k = p.taps * p.kchunks;
-  const int nchunks = (total_k + CH - 1) / CH;
-  // single-pass TF32 without a pre-activation needs no operand transform: the tensor core reads the top 19 bits
-  // of the fp32 words TMA delivered (truncation), so the MMA warp consumes the TMA barrier directly
-  const bool xf = Cfg::SPLIT || p.pre_act != ACT_NONE;
+  const int total_tiles = p.m_tiles * p.n_tiles;
 
-  auto a_hi = [&](int s) { return smem + s * Cfg::STAGE_BYTES; };
-  auto b_hi = [&](int s) { return smem + s * Cfg::STAGE_BYTES + TC_A_BYTES; };
-  auto a_lo = [&](int s) { return smem + s * Cfg::STAGE_BYTES + TC_A_BYTES + Cfg::B_BYTES; };
-  auto b_lo = [&](int s) { return smem + s * Cfg::STAGE_BYTES + 2 * TC_A_BYTES + Cfg::B_BYTES; };
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmW);
+  if (threadIdx.x == 0) {
     for (int s = 0; s < S; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&ready[s], TC_XF_THREADS);
-      mbar_init(&empty[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&acc_full[b], 1);
-      mbar_init(&acc_empty[b], 128);
+      mbar_init(&empty[s], TC_CONSUMER_WARPS);
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<Cfg::TMEM_COLS>(tmem_ptr);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  if (timed) p.cta_times[blockIdx.x * 4 + 1] = gtime();
 
-  if (warp == 0) {
-    // ================= TMA producer (whole warp runs the loop; one elected lane issues)
-    for (int kit = 0; kit < total_k; ++kit) {
-      const int s = kit % S;
-      const uint32_t ph = (kit / S) & 1;
-      mbar_wait(&empty[s], ph ^ 1);
-      const int tap = kit / p.kchunks, kc = kit % p.kchunks;
-      if (elect_one()) {
-        if (p.trace && blockIdx.x == 0 && blockIdx.y == 0) p.trace[kit * 8 + 0] = clock64();
-        mbar_arrive_expect_tx(&full[s], TC_A_BYTES + Cfg::B_BYTES * (Cfg::SPLIT ? 2 : 1));
-        tma_load_3d(a_hi(s), &tmA, &full[s], kc * TC_BKE, i0 + tap * p.tap_di, ot * p.o_mul + tap * p.tap_do);
-        tma_load_2d(b_hi(s), &tmW, &full[s], tap * p.Kc + kc * TC_BKE, n0);
-        if (Cfg::SPLIT) tma_load_2d(b_lo(s), &tmWlo, &full[s], tap * p.Kc + kc * TC_BKE, n0);
-      }
-      __syncwarp();
-    }
-  } else if (warp == 1) {
-    // ================= MMA issuer (one thread).  The tensor core adds into its fp32 accumulator with
-    // truncation, a bias that grows linearly with the number of accumulation steps; each chunk of CH
-    // stages therefore starts a fresh TMEM accumulator (two buffers, ping-pong) that the drain warps add
-    // into fp32 registers with round-to-nearest (same idea as FP8 GEMM accumulator promotion).
-    constexpr uint32_t idesc = instr_desc(2u, TC_BM, BN);
-    for (int kit = 0; kit < total_k; ++kit) {
-      const int s = kit % S;
-      const uint32_t ph = (kit / S) & 1;
-      const int chunk = kit / CH, pos = kit % CH, buf = chunk & 1;
-      if (pos == 0) mbar_wait(&acc_empty[buf], ((chunk >> 1) & 1) ^ 1);
-      mbar_wait(xf ? &ready[s] : &full[s], ph);
-      tc_fence_after();
-      if (elect_one()) {
-        if (p.trace && blockIdx.x == 0 && blockIdx.y == 0) p.trace[kit * 8 + 3] = clock64();
-        const uint32_t d0 = tmem_base + (uint32_t)(buf * TC_NACC * BN);  // accumulator 0 of this buffer
-        const uint32_t d1 = d0 + (uint32_t)BN;                            // accumulator 1
-        const uint64_t da = smem_desc_sw128(smem_u32(a_hi(s))), db = smem_desc_sw128(smem_u32(b_hi(s)));
-        uint64_t dal = 0, dbl = 0;
-        if (Cfg::SPLIT) {
-          dal = smem_desc_sw128(smem_u32(a_lo(s)));
-          dbl = smem_desc_sw128(smem_u32(b_lo(s)));
+  if (warp == TC_CONSUMER_WARPS) {
+    // ================= TMA producer: one elected lane walks this CTA's stages (all its tiles back to back)
+    if (elect_one()) {
+      tma_prefetch_desc(&tmA);
+      tma_prefetch_desc(&tmW);
+      if (Cfg::SPLIT) tma_prefetch_desc(&tmWlo);
+      int g = 0;
+      for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+        const int nt = t % p.n_tiles, mt = t / p.n_tiles;
+        const int i0 = (mt % p.i_tiles) * TC_BM, ot = mt / p.i_tiles, n0 = nt * BN;
+        for (int kit = 0; kit < total_k; ++kit, ++g) {
+          const int s = g % S;
+          mbar_wait(&empty[s], ((g / S) & 1) ^ 1);
+          const int tap = kit / p.kchunks, kc = kit % p.kchunks;
+          uint8_t* st = smem + s * Cfg::STAGE_BYTES;
+          mbar_arrive_expect_tx(&full[s], Cfg::STAGE_BYTES);
+          tma_load_3d(st, &tmA, &full[s], kc * TC_BKE, i0 + tap * p.tap_di, ot * p.o_mul + tap * p.tap_do);
+          tma_load_2d(st + TC_A_BYTES, &tmW, &full[s], kit * TC_BKE, n0);   // tap * Kc + kc * 32 == kit * 32
+          if (Cfg::SPLIT) tma_load_2d(st + TC_A_BYTES + Cfg::B_BYTES, &tmWlo, &full[s], kit * TC_BKE, n0);
         }
+      }
+    }
+    return;
+  }
+
+  // ================= consumers.  Thread (warp wq of warpgroup wg, lane = 4 gq + tq) holds A rows r0 and r0 + 8 of the
+  // tile, columns tq and tq + 4 of every 8-wide K step (the wgmma register fragment); the accumulator fragment covers the
+  // same two rows, columns 8 b + 2 tq and 8 b + 2 tq + 1 of every 8-column block b.
+  const int wg = warp / 4, wq = warp % 4, gq = lane / 4, tq = lane % 4;
+  const int r0 = wg * 64 + wq * 16 + gq;
+  // element (r, c) of a stage's swizzled [128][32] fp32 A tile sits at byte r * 128 + ((c / 4) ^ (r % 8)) * 16 + (c % 4) * 4;
+  // rows r0 and r0 + 8 share r % 8
+  const uint32_t a_row = (uint32_t)r0 * 128u + (uint32_t)tq * 4u, a_sw = (uint32_t)(r0 & 7);
+  const uint32_t smem0 = smem_u32(smem);
+  float acc[NR], d0[NR], d1[NR];
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {  // 4 x (K = 8 tf32 = 32 bytes) per 128-byte row
-          const uint64_t adv = (uint64_t)(k * 2);  // +32 bytes in 16-byte units
-          const uint32_t fresh = (pos == 0 && k == 0) ? 0u : 1u;
-          if (Cfg::SPLIT) {
-            mma_tf32(d0, da + adv, db + adv, idesc, fresh);    // a_hi * b_hi
-            mma_tf32(d1, dal + adv, db + adv, idesc, fresh);   // a_lo * b_hi   (small terms kept apart)
-            mma_tf32(d1, da + adv, dbl + adv, idesc, 1u);      // a_hi * b_lo
-          } else {
-            mma_tf32((k & 1) ? d1 : d0, da + adv, db + adv, idesc, (pos == 0 && k < 2) ? 0u : 1u);
+  for (int j = 0; j < NR; ++j) d0[j] = d1[j] = 0.f;
+  int g = 0;
+  for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+    const int nt = t % p.n_tiles, mt = t / p.n_tiles;
+    const int i0 = (mt % p.i_tiles) * TC_BM, ot = mt / p.i_tiles, n0 = nt * BN;
+#pragma unroll
+    for (int j = 0; j < NR; ++j) acc[j] = 0.f;
+    // K in chunks of up to CH stages, each chunk's accumulators promoted after it.  Every wgmma wait sits outside any
+    // branch, so ptxas needs no serialising warpgroup waits of its own.  The two consumer warpgroups overlap each other:
+    // one builds fragments while the other's wgmmas run.
+    for (int k0 = 0; k0 < total_k; k0 += CH) {
+      const int nst = total_k - k0 < CH ? total_k - k0 : CH;
+      for (int u = 0; u < nst; ++u, ++g) {
+        const int s = g % S;
+        mbar_wait(&full[s], (g / S) & 1);
+        const uint32_t st = smem0 + (uint32_t)(s * Cfg::STAGE_BYTES);
+        uint32_t ah[4][4], al[4][4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {   // a[e]: row r0 + 8 (e & 1), column 8 k + tq + 4 (e >> 1)
+            const uint32_t chunk = (uint32_t)(2 * k + (e >> 1));
+            float v;
+            asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(st + a_row + (e & 1) * 1024u + ((chunk ^ a_sw) << 4)));
+            if (PRE_ELU) {   // elu_fast, as a select: x > 0 ? x : exp(x) - 1
+              const float e = __expf(v) - 1.f;
+              v = v > 0.f ? v : e;
+            }
+            const float h = tf32_rna(v);
+            ah[k][e] = __float_as_uint(h);
+            al[k][e] = __float_as_uint(tf32_rna(v - h));
           }
         }
-        tc_commit(&empty[s]);  // frees the stage once these MMAs have read it
-        if (pos == CH - 1 || kit == total_k - 1) tc_commit(&acc_full[buf]);
-        if (p.trace && blockIdx.x == 0 && blockIdx.y == 0) p.trace[kit * 8 + 4] = clock64();
-      }
-      __syncwarp();
-    }
-  } else if (warp < 10) {
-    // ================= transform warps (2..9): pre-activation + TF32 hi/lo split of the A tile, in place.
-    // Weights were rounded / split once on the host side of the plan (W_hi, W_lo arrive by TMA).
-    const int tid = threadIdx.x - 64;  // 0..255
-    for (int kit = 0; xf && kit < total_k; ++kit) {
-      const int s = kit % S;
-      const uint32_t ph = (kit / S) & 1;
-      mbar_wait(&full[s], ph);
-      if (p.trace && blockIdx.x == 0 && blockIdx.y == 0 && tid == 0) p.trace[kit * 8 + 1] = clock64();
-      float4* ah = reinterpret_cast<float4*>(a_hi(s));
-      float4* al = reinterpret_cast<float4*>(a_lo(s));
+        const uint64_t db = gmma_desc_sw128(st + TC_A_BYTES);
+        const uint64_t dbl = gmma_desc_sw128(st + TC_A_BYTES + Cfg::B_BYTES);
+        wgmma_fence();
 #pragma unroll
-      for (int j = 0; j < TC_A_BYTES / 16 / TC_XF_THREADS; ++j) {
-        float4 v = ah[j * TC_XF_THREADS + tid];
-        if (p.pre_act != ACT_NONE) {
-          v.x = apply_act(v.x, p.pre_act); v.y = apply_act(v.y, p.pre_act);
-          v.z = apply_act(v.z, p.pre_act); v.w = apply_act(v.w, p.pre_act);
+        for (int k = 0; k < 4; ++k) {   // 4 x (K = 8 tf32 = 32 bytes) per 128-byte row
+          const uint32_t acc_in = (u == 0 && k == 0) ? 0u : 1u;   // a chunk starts fresh accumulators
+          wgmma_tf32_rs<BN>(d0, ah[k], db + (uint64_t)(2 * k), acc_in);                 // a_hi * b_hi
+          if (Cfg::SPLIT) {
+            wgmma_tf32_rs<BN>(d1, al[k], db + (uint64_t)(2 * k), acc_in);               // a_lo * b_hi
+            wgmma_tf32_rs<BN>(d1, ah[k], dbl + (uint64_t)(2 * k), 1u);                  // a_hi * b_lo
+          }
         }
-        const float4 h = tf32_hi(v);
-        ah[j * TC_XF_THREADS + tid] = h;
-        if (Cfg::SPLIT) al[j * TC_XF_THREADS + tid] = tf32_hi(make_float4(v.x - h.x, v.y - h.y, v.z - h.z, v.w - h.w));
+        wgmma_commit();
+        // the group's A operand is registers the next stage's fragments would overwrite: it must retire first
+        wgmma_wait<0>();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[s]);   // this warp's wgmmas have read the stage
       }
-      fence_proxy_async_smem();
-      if (p.trace && blockIdx.x == 0 && blockIdx.y == 0 && tid == 0) p.trace[kit * 8 + 2] = clock64();
-      mbar_arrive(&ready[s]);
+      fence_acc(d0);
+      if (Cfg::SPLIT) fence_acc(d1);
+#pragma unroll
+      for (int j = 0; j < NR; ++j) acc[j] += Cfg::SPLIT ? d0[j] + d1[j] : d0[j];
     }
-  } else {
-    // ================= drain + epilogue warps (10..13): TMEM chunk accumulators -> fp32 registers
-    const int q = warp % 4;  // TMEM lane quarter this warp may read
-    float acc[BN];
+    // ---- epilogue: bias, LayerScale, residual, activation -> global (8-byte stores: 4 lanes = one 32-byte sector)
 #pragma unroll
-    for (int j = 0; j < BN; ++j) acc[j] = 0.f;
-    for (int chunk = 0; chunk < nchunks; ++chunk) {
-      const int buf = chunk & 1;
-      mbar_wait(&acc_full[buf], (chunk >> 1) & 1);
-      tc_fence_after();
-      if (p.trace && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 320) p.trace[chunk * 8 + 5] = clock64();
-#pragma unroll
-      for (int c0 = 0; c0 < BN; c0 += 32) {
-        uint32_t r[32];
-        uint32_t r2[32];
-        const uint32_t col = (uint32_t)(buf * TC_NACC * BN + c0);
-        tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + col, r);
-        tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + col + (uint32_t)BN, r2);
-        tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 32; ++j) acc[c0 + j] += __uint_as_float(r[j]) + __uint_as_float(r2[j]);
-      }
-      tc_fence_before();
-      if (p.trace && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 320) p.trace[chunk * 8 + 6] = clock64();
-      mbar_arrive(&acc_empty[buf]);
-    }
-    // ---- epilogue: bias, LayerScale, residual, activation -> global
-    const int row = q * 32 + lane;
-    const int i = i0 + row;
-    if (i < p.I_out) {
+    for (int h = 0; h < 2; ++h) {
+      const int i = i0 + r0 + 8 * h;
+      if (i >= p.I_out) continue;
       float* crow = p.C + (long long)ot * p.c_o_stride + (long long)i * p.c_i_stride;
       float* crow2 = p.C2 ? p.C2 + (long long)ot * p.c_o_stride + (long long)i * p.c_i_stride : nullptr;
       const float* rrow = p.R ? p.R + (long long)ot * p.r_o_stride + (long long)i * p.r_i_stride : nullptr;
 #pragma unroll
-      for (int g = 0; g < BN / 4; ++g) {
-        const int n = n0 + 4 * g;
-        if (n < p.N) {
-          float4 v = make_float4(acc[4 * g], acc[4 * g + 1], acc[4 * g + 2], acc[4 * g + 3]);
+      for (int b = 0; b < BN / 8; ++b) {
+        const int n = n0 + 8 * b + 2 * tq;
+        if (n < p.N) {   // N % 4 == 0: n + 1 < N as well
+          float2 v = make_float2(acc[4 * b + 2 * h], acc[4 * b + 2 * h + 1]);
           if (p.bias) {
-            const float4 bb = *reinterpret_cast<const float4*>(p.bias + n);
-            v.x += bb.x; v.y += bb.y; v.z += bb.z; v.w += bb.w;
+            const float2 bb = *reinterpret_cast<const float2*>(p.bias + n);
+            v.x += bb.x; v.y += bb.y;
           }
           if (p.scale) {
-            const float4 ss = *reinterpret_cast<const float4*>(p.scale + n);
-            v.x *= ss.x; v.y *= ss.y; v.z *= ss.z; v.w *= ss.w;
+            const float2 ss = *reinterpret_cast<const float2*>(p.scale + n);
+            v.x *= ss.x; v.y *= ss.y;
           }
           long long coff = n, roff = n;
-          if (p.n_split > 0) {
+          if (p.n_split > 0) {   // n_split % 4 == 0: n and n + 1 fall in the same split
             const int j = n / p.n_split, co = n % p.n_split;
             coff = (long long)j * p.c_split_stride + co;
             roff = (long long)j * p.r_split_stride + co;
           }
           if (rrow) {
-            const float4 rr = *reinterpret_cast<const float4*>(rrow + roff);
-            v.x += rr.x; v.y += rr.y; v.z += rr.z; v.w += rr.w;
+            const float2 rr = *reinterpret_cast<const float2*>(rrow + roff);
+            v.x += rr.x; v.y += rr.y;
           }
-          if (crow2) {  // e.g. the ELU'd copy a resblock's first conv consumes while the skip reads the raw one
-            *reinterpret_cast<float4*>(crow2 + coff) = make_float4(apply_act(v.x, p.act2), apply_act(v.y, p.act2),
-                                                                   apply_act(v.z, p.act2), apply_act(v.w, p.act2));
-          }
-          if (p.post_act != ACT_NONE) {
-            v.x = apply_act(v.x, p.post_act); v.y = apply_act(v.y, p.post_act);
-            v.z = apply_act(v.z, p.post_act); v.w = apply_act(v.w, p.post_act);
-          }
-          *reinterpret_cast<float4*>(crow + coff) = v;
+          if (crow2)   // e.g. the ELU'd copy a resblock's first conv consumes while the skip reads the raw one
+            *reinterpret_cast<float2*>(crow2 + coff) = make_float2(act_tc(v.x, p.act2), act_tc(v.y, p.act2));
+          *reinterpret_cast<float2*>(crow + coff) = make_float2(act_tc(v.x, p.post_act), act_tc(v.y, p.post_act));
         }
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (timed) p.cta_times[blockIdx.x * 4 + 2] = gtime();
-  if (warp == 1) tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
-  if (timed) p.cta_times[blockIdx.x * 4 + 3] = gtime();
-}
-
-// ---------------------------------------------------------------- ".ts" variant: A operand from TMEM, persistent CTAs
-// The SS kernel above is shared-memory-bandwidth bound: per 32-element K stage the hi/lo split writes 32 KB back to
-// shared memory and the three MMAs re-read the A tile three times (~150 KB of smem traffic per 384 clk of MMA work).
-// Here the transform warps read the TMA-landed fp32 A tile ONCE (un-swizzling the 128-byte rows) and write hi / lo
-// straight into TMEM (tcgen05.st), from where tcgen05.mma takes its A operand; only the pre-split weight tiles are
-// read from shared memory by the tensor core.  TMEM: columns [0, 4*BN) two ping-pong buffers of two accumulators,
-// then TS_NA stages of (32 hi + 32 lo) A columns.
-// One CTA per SM walks tiles t = blockIdx.x, +gridDim.x, ... (N tile fastest, so CTAs running together share A rows
-// in L2); the barrier phases run on across tiles, and because the drain warps keep the promoted sums in registers
-// the epilogue of tile t overlaps the MMAs of tile t+1.
-constexpr int TS_NA = 4;
-
-template <int BN>
-struct TsCfg {
-  static constexpr int B_BYTES = BN * 128;
-  static constexpr int STAGE_BYTES = TC_A_BYTES + 2 * B_BYTES;
-  static constexpr int STAGES = BN == 64 ? 5 : 8;
-  static constexpr int OUT_LD = BN + 4;                       // padded row of the epilogue staging tile (floats)
-  static constexpr int BOXSET_BYTES = (BN / 32) * TC_BM * 128;   // [BN/32] swizzled [128 x 32] fp32 boxes of the TMA-store epilogue
-  static constexpr int OUT_BYTES = 2 * BOXSET_BYTES;          // two box sets (residual layers alternate per tile); the fallback transpose (4*32*OUT_LD*4) fits inside
-  static constexpr int CTRL_BYTES = 2048;                     // barriers (512) + bias/scale x2 (<= 1024), keeps the staging area 1024-aligned
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + CTRL_BYTES + OUT_BYTES;
-  static constexpr int ACC_COLS = 2 * TC_NACC * BN;
-};
-
-// DW = drain / epilogue warps: 4 (each thread finishes a whole BN-wide row; also the non-TMA-store fallback) or 8 (two
-// warps share a TMEM lane quarter and split the columns; 576 threads, 96 registers).  A short-K tile (the 24 kHz / 6 kHz
-// resblock convs: 1..8 stages) is bound by its epilogue -- promotion adds, bias, residual, ELU, swizzled staging of 128 x BN
-// outputs -- which four warps run at ~4 650 clk per 128x64 tile against <= 2 000 clk of main loop; eight warps halve it.
-template <int BN, int DW>
-__global__ void __launch_bounds__(320 + 32 * DW, 1)
-gemm_tc_ts_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW3,
-                  const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmC2,
-                  const __grid_constant__ CUtensorMap tmR, const TcParams p) {
-  using Cfg = TsCfg<BN>;
-  constexpr int S = Cfg::STAGES;
-  constexpr int CH = TC_CHUNK_STAGES;
-  static_assert(CH == 4 && TS_NA == 4, "a chunk is at most 4 stages = the 4 TMEM A stages");
-  // Stage g of this CTA's stream (all its tiles back to back, NO padding: a tile contributes exactly taps * kchunks
-  // stages, its last chunk may be short) uses smem slot g % S and TMEM A slot g % 4; parities follow from g.  Round 1
-  // padded every tile to whole 4-stage chunks, which made a K = 32 tile (the 24 kHz 1x1 convs) pay four A loads,
-  // four transforms and 32 MMAs for one stage of work.
-  extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment as pointer arithmetic on the __shared__ array (an integer round trip would demote every later
-  // access through `smem` to generic LD / ST)
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S * Cfg::STAGE_BYTES);
-  uint64_t* full = bars;                         // [S] TMA landed (A fp32, [B_hi; B_lo])
-  uint64_t* empty = bars + S;                    // [S] MMAs reading B of the stage retired (A smem was consumed earlier)
-  uint64_t* a_ready = bars + 2 * S;              // [NA] hi/lo of the A tile are in TMEM (128 arrivals)
-  uint64_t* a_free = bars + 2 * S + TS_NA;       // [NA] MMAs reading that TMEM stage retired
-  uint64_t* acc_full = bars + 2 * S + 2 * TS_NA; // [2]
-  uint64_t* acc_empty = acc_full + 2;            // [2] (128 arrivals)
-  uint64_t* r_full = acc_empty + 2;              // [2] residual tile landed in the epilogue boxes (even / odd tiles of this CTA)
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(r_full + 2);
-  float* sbs = reinterpret_cast<float*>(smem + S * Cfg::STAGE_BYTES + 512);  // [2][2*BN] bias | scale of the drain's tile
-  float* out_stage = reinterpret_cast<float*>(smem + S * Cfg::STAGE_BYTES + Cfg::CTRL_BYTES);   // epilogue staging (1024-aligned)
-
-  auto gtime = []() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return (long long)t; };
-  const bool timed = p.cta_times && threadIdx.x == 0;
-  const bool tr = p.trace && blockIdx.x == 0;
-  if (timed) p.cta_times[blockIdx.x * 4 + 0] = gtime();
-  const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
-  // A tile's K loop = taps * kchunks stages of 32 elements, in chunks of up to 4 stages (one accumulator promotion each).
-  // K split over a 2-CTA cluster (ksplit == 2; linears whose tile count leaves half the SMs idle: a CTA's long K loop is
-  // bound by the ~58 B/clk its SM ingests from L2, two SMs ingest twice that): rank r runs stages [r, r + 1) * total_k of
-  // the tile, rank 1 hands its promoted fp32 accumulators to rank 0 through distributed shared memory, rank 0 adds them
-  // (rank order: deterministic) and runs the epilogue.  One tile per cluster.
-  const int ks = p.ksplit;
-  uint32_t crank = 0;
-  if (ks > 1) asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(crank));
-  const int cid = (int)blockIdx.x / ks, ncl = (int)gridDim.x / ks;   // tile walker: cluster index / count
-  const int total_k = p.taps * p.kchunks / ks;
-  const int koff = (int)crank * total_k;
-  const int nchunks = (total_k + CH - 1) / CH;
-  const int total_tiles = p.m_tiles * p.n_tiles;
-  const int my_tiles = (cid < total_tiles) ? (total_tiles - cid + ncl - 1) / ncl : 0;
-  const int tr_ti = my_tiles > 3 ? 3 : 0;   // the traced tile: steady state when the CTA has several
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmW3);
-    if (p.tma_store) { tma_prefetch_desc(&tmC); if (p.C2) tma_prefetch_desc(&tmC2); if (p.R) tma_prefetch_desc(&tmR); }
-    for (int s = 0; s < S; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int s = 0; s < TS_NA; ++s) { mbar_init(&a_ready[s], 128); mbar_init(&a_free[s], 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&acc_full[b], 1); mbar_init(&acc_empty[b], 32 * DW); }
-    mbar_init(&r_full[0], 1);
-    mbar_init(&r_full[1], 1);
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc<512>(tmem_ptr);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  const uint32_t a_tmem0 = tmem_base + (uint32_t)Cfg::ACC_COLS;
-  if (ks > 1) {   // distributed shared memory may only be written once the peer CTA is known to have started
-    asm volatile("barrier.cluster.arrive.release;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire;" ::: "memory");
-  }
-  if (timed) p.cta_times[blockIdx.x * 4 + 1] = gtime();
-
-  if (warp == 0) {
-    // ---- TMA producer: one elected thread per chunk
-    int kc = 0, ci = 0, co = 0, n0 = 0;
-    int s = 0;            // smem slot of the next stage (g % S, kept as a running counter: no division on this thread's path)
-    uint32_t sph = 0;     // (g / S) & 1
-    const bool leader = elect_one();   // ONE election: the running counters live in this lane's registers
-    for (int ti = 0; ti < my_tiles; ++ti) {
-      const int t = cid + ti * ncl;
-      const int nt = t % p.n_tiles, mt = t / p.n_tiles;
-      n0 = nt * BN; ci = (mt % p.i_tiles) * TC_BM; co = (mt / p.i_tiles) * p.o_mul; kc = koff;   // koff != 0 only with taps == 1
-      const bool first_tile = ti == tr_ti;
-      if (leader) {
-        // Two stages per trip, the independent steps of both grouped (slot waits, then transaction counts, then the four
-        // loads): this thread shares its scheduler with four ALU-heavy warps and loses its issue slot at every dependent
-        // stall, so fewer, longer independent runs set the pace (stamps: ~350 clk per stage one stage at a time).
-        int kit = 0;
-        for (; kit + 1 < total_k; kit += 2) {
-          const int s0 = s;
-          const uint32_t ph0 = sph;
-          int s1 = s + 1;
-          uint32_t ph1 = sph;
-          if (s1 == S) { s1 = 0; ph1 ^= 1u; }
-          const int kc0 = kc, ci0 = ci, co0 = co;
-          if (++kc == p.kchunks) { kc = 0; ci += p.tap_di; co += p.tap_do; }
-          const int kc1 = kc, ci1 = ci, co1 = co;
-          if (++kc == p.kchunks) { kc = 0; ci += p.tap_di; co += p.tap_do; }
-          mbar_wait(&empty[s0], ph0 ^ 1u);
-          mbar_wait(&empty[s1], ph1 ^ 1u);
-          if (tr && first_tile) { const long long c = clock64(); p.trace[kit * 8 + 0] = c; p.trace[(kit + 1) * 8 + 0] = c; }
-          uint8_t* st0 = smem + s0 * Cfg::STAGE_BYTES;
-          uint8_t* st1 = smem + s1 * Cfg::STAGE_BYTES;
-          mbar_arrive_expect_tx(&full[s0], TC_A_BYTES + 2 * Cfg::B_BYTES);
-          mbar_arrive_expect_tx(&full[s1], TC_A_BYTES + 2 * Cfg::B_BYTES);
-          tma_load_3d(st0, &tmA, &full[s0], kc0 * TC_BKE, ci0, co0);
-          tma_load_3d(st0 + TC_A_BYTES, &tmW3, &full[s0], (koff + kit) * TC_BKE, n0, 0);   // tap * Kc + kc * 32 == kit * 32
-          tma_load_3d(st1, &tmA, &full[s1], kc1 * TC_BKE, ci1, co1);
-          tma_load_3d(st1 + TC_A_BYTES, &tmW3, &full[s1], (koff + kit + 1) * TC_BKE, n0, 0);
-          s = s1 + 1;
-          sph = ph1;
-          if (s == S) { s = 0; sph ^= 1u; }
-        }
-        if (kit < total_k) {   // odd stage count: the last stage alone
-          mbar_wait(&empty[s], sph ^ 1u);
-          if (tr && first_tile) p.trace[kit * 8 + 0] = clock64();
-          uint8_t* st = smem + s * Cfg::STAGE_BYTES;
-          mbar_arrive_expect_tx(&full[s], TC_A_BYTES + 2 * Cfg::B_BYTES);
-          tma_load_3d(st, &tmA, &full[s], kc * TC_BKE, ci, co);
-          tma_load_3d(st + TC_A_BYTES, &tmW3, &full[s], (koff + kit) * TC_BKE, n0, 0);
-          if (++kc == p.kchunks) { kc = 0; ci += p.tap_di; co += p.tap_do; }
-          if (++s == S) { s = 0; sph ^= 1u; }
-        }
-      }
-      __syncwarp();
-    }
-  } else if (warp == 1) {
-    // ---- MMA issue: per k-step  D[hh | hl] (+)= A_hi x [B_hi; B_lo]  (one N = 2*BN MMA), then  D[hl] += A_lo x B_hi
-    constexpr uint32_t idesc2 = instr_desc(2u, TC_BM, 2 * BN), idesc1 = instr_desc(2u, TC_BM, BN);
-    const uint64_t desc0 = smem_desc_sw128(smem_u32(smem));   // stage s adds s * STAGE_BYTES / 16 to the address field
-    int cc = 0;
-    int s = 0;                  // g % S as a running counter
-    uint32_t ga = 0;            // g % 8: TMEM A slot = ga & 3, its phase bit = ga >> 2
-    uint64_t db = desc0 + (uint64_t)(TC_A_BYTES >> 4);   // weight-tile descriptor of smem slot s
-    const bool leader = elect_one();
-    for (int ti = 0; ti < my_tiles; ++ti) {
-      const bool first_tile = ti == tr_ti;
-      if (leader) {
-        for (int kit = 0; kit < total_k; kit += CH, ++cc) {
-          const int nst = total_k - kit < CH ? total_k - kit : CH;
-          const int buf = cc & 1;
-          mbar_wait(&acc_empty[buf], (uint32_t)(((cc >> 1) & 1) ^ 1));
-          const uint32_t d0 = tmem_base + (uint32_t)(buf * TC_NACC * BN), d1 = d0 + (uint32_t)BN;
-          auto stage = [&](int u, bool first, bool last) {
-            const uint32_t sa = ga & 3u;
-            mbar_wait(&a_ready[sa], ga >> 2);   // implies full[s]: the transform waited for it
-            tc_fence_after();
-            if (tr && first_tile) p.trace[(kit + u) * 8 + 3] = clock64();
-            const uint32_t ah = a_tmem0 + sa * 64u, al = ah + 32u;
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              mma_tf32_ts(d0, ah + (uint32_t)(8 * k), db + (uint64_t)(2 * k), idesc2, (first && k == 0) ? 0u : 1u);
-              mma_tf32_ts(d1, al + (uint32_t)(8 * k), db + (uint64_t)(2 * k), idesc1, 1u);
-            }
-            tc_commit(&empty[s]);
-            tc_commit(&a_free[sa]);
-            if (last) tc_commit(&acc_full[buf]);
-            if (tr && first_tile) p.trace[(kit + u) * 8 + 4] = clock64();
-            ga = (ga + 1u) & 7u;
-            db += (uint64_t)(Cfg::STAGE_BYTES >> 4);
-            if (++s == S) { s = 0; db = desc0 + (uint64_t)(TC_A_BYTES >> 4); }
-          };
-          if (nst == CH) {
-            stage(0, true, false); stage(1, false, false); stage(2, false, false); stage(3, false, true);
-          } else {
-            for (int u = 0; u < nst; ++u) stage(u, u == 0, u == nst - 1);
-          }
-        }
-      }
-      __syncwarp();
-    }
-  } else if (warp < 10) {
-    // transform: two groups of 4 warps alternate stages; thread = one A row (TMEM lane).  It never looks at tile
-    // boundaries: stage g of this CTA's stream is stage g, whatever tile it belongs to.
-    const int grp = (warp - 2) / 4, q = warp % 4;
-    const int row = q * 32 + lane;
-    const uint32_t rowoff = (uint32_t)(row * 128 + ((row & 7) << 4));   // chunk j of the swizzled row: rowoff ^ (j << 4)
-    const uint32_t smem0 = smem_u32(smem);
-    const uint32_t ta0 = a_tmem0 + ((uint32_t)(q * 32) << 16);
-    const int my_total = my_tiles * total_k;
-    auto run = [&](auto act_tag) {
-      constexpr bool ACT = decltype(act_tag)::value;
-      for (int g = grp; g < my_total; g += 2) {
-        const int s = g % S, sa = g % TS_NA;
-        // Order matters.  With an odd stage count the previous fill of slot s (stage g - S) belongs to the OTHER transform
-        // group, so this thread may get here before that fill has even landed; a parity wait on full[s] would then be
-        // satisfied by the phase before it and the tile would be read while the TMA for stage g is still in flight (seen as
-        // a rare wrong output tile on cold GPUs).  a_free of stage g - 4 implies the MMAs of stage g - S have retired, i.e.
-        // full[s] is in this stage's phase, so waiting for it second is exact.
-        mbar_wait(&a_free[sa], ((g / TS_NA) & 1) ^ 1);
-        mbar_wait(&full[s], (g / S) & 1);
-        if (tr && q == 0 && lane == 0 && g >= tr_ti * total_k && g < (tr_ti + 1) * total_k) p.trace[(g - tr_ti * total_k) * 8 + 1] = clock64();
-        tc_fence_after();
-        const uint32_t base = smem0 + (uint32_t)(s * Cfg::STAGE_BYTES) + rowoff;
-        uint32_t hi[32], lo[32];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          float4 v = lds128(base ^ (uint32_t)(j << 4));
-          // pre-activation with the epilogues' ELU (ex2.approx): ELU(x) here == the ELU'd copy a producer epilogue would
-          // have stored, bit for bit, so a consumer may read the raw tensor instead of a second, activated one
-          if (ACT) v = apply_act4_tc(v, p.pre_act);
-          const float e[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            const uint32_t h = (__float_as_uint(e[c]) + 0x1000u) & 0xFFFFE000u;
-            hi[4 * j + c] = h;
-            // the tensor core ignores the low 13 bits of a tf32 operand: adding half an ulp is the whole rounding
-            lo[4 * j + c] = __float_as_uint(e[c] - __uint_as_float(h)) + 0x1000u;
-          }
-        }
-        tmem_st32(ta0 + (uint32_t)(sa * 64), hi);
-        tmem_st32(ta0 + (uint32_t)(sa * 64) + 32u, lo);
-        tmem_st_wait();
-        tc_fence_before();
-        mbar_arrive(&a_ready[sa]);
-        if (tr && q == 0 && lane == 0 && g >= tr_ti * total_k && g < (tr_ti + 1) * total_k) p.trace[(g - tr_ti * total_k) * 8 + 2] = clock64();
-      }
-    };
-    if (p.pre_act != ACT_NONE) run(std::true_type{}); else run(std::false_type{});
-  } else {
-    const int q = warp % 4, dt = threadIdx.x - 320;
-    const int row = q * 32 + lane;
-    constexpr int NDT = 32 * DW;             // drain threads
-    constexpr int CW = BN / (DW / 4);        // columns finished by one drain thread
-    const int cbeg = ((warp - 10) / 4) * CW; // this warp's column range [cbeg, cbeg + CW) of the tile
-    int cc = 0;
-    for (int ti = 0; ti < my_tiles; ++ti) {
-      const int t = cid + ti * ncl;
-      const int nt = t % p.n_tiles, mt = t / p.n_tiles;
-      const int i0 = (mt % p.i_tiles) * TC_BM, ot = mt / p.i_tiles, n0 = nt * BN;
-      // bias | scale of the tile's columns -> smem (double buffered); with a single N tile they are the same for every tile
-      const bool sb_fixed = p.n_tiles == 1;
-      float* sb = sbs + (sb_fixed ? 0 : (ti & 1)) * 2 * BN;
-      if (!sb_fixed || ti == 0) {
-        if (dt < BN) sb[dt] = (p.bias && n0 + dt < p.N) ? p.bias[n0 + dt] : 0.f;
-        else if (dt < 2 * BN) sb[dt] = (p.scale && n0 + dt - BN < p.N) ? p.scale[n0 + dt - BN] : 1.f;
-      }
-      // Residual tile -> epilogue boxes by TMA.  Residual layers alternate between two box sets (and two mbarriers): the
-      // residual of tile t+1 is requested from the epilogue of tile t, as soon as the store of tile t-1 has been read out of
-      // the set it is going to land in, so its latency overlaps the staging and the store of tile t.  (A load landing in
-      // boxes a store is still reading corrupted the tail rows of a tile -- seen rarely, on cold GPUs, on the 64->128 1x1
-      // conv of the 6 kHz decoder level, scripts/diag_rows.py -- hence the read-out wait in front of every request.)
-      auto request_residual = [&](int tix) {
-        const int t2 = cid + tix * ncl;
-        const int nt2 = t2 % p.n_tiles, mt2 = t2 / p.n_tiles;
-        const int i2 = (mt2 % p.i_tiles) * TC_BM, ot2 = mt2 / p.i_tiles, n2 = nt2 * BN;
-        uint8_t* boxes = reinterpret_cast<uint8_t*>(out_stage) + (tix & 1) * Cfg::BOXSET_BYTES;
-        int nb = 0;
-        for (int g8 = 0; g8 < BN / 32; ++g8) nb += (n2 + g8 * 32 < p.N) ? 1 : 0;
-        mbar_arrive_expect_tx(&r_full[tix & 1], (uint32_t)(nb * TC_BM * 128));
-        for (int g8 = 0; g8 < BN / 32; ++g8) {
-          const int n = n2 + g8 * 32;
-          if (n < p.N) {
-            int c0 = n, c2 = ot2;
-            if (p.n_split > 0) { c0 = n % p.n_split; c2 = ot2 * p.c_tr + n / p.n_split; }
-            tma_load_3d(boxes + g8 * (TC_BM * 128), &tmR, &r_full[tix & 1], c0, i2, c2);
-          }
-        }
-      };
-      if (p.tma_store && p.R && crank == 0) {
-        if (dt == 0 && ti == 0) request_residual(0);
-        // The NEXT tile's residual is requested at the top of this tile, by the owner of the other box set, as soon as its
-        // store of tile ti-1 has been read out: the residual is the block input, long evicted from L2, and takes ~3 000 clk
-        // under load -- most of a tile period.  (Requested after this tile's store instead: 68 -> 81 us on the 24 kHz 1x1 conv.)
-        if (dt == 32 * ((ti + 1) & 1) && ti + 1 < my_tiles) {
-          bulk_wait_read0();
-          request_residual(ti + 1);
-        }
-      }
-      float acc[CW];
-#pragma unroll
-      for (int j = 0; j < CW; ++j) acc[j] = 0.f;
-      for (int chunk = 0; chunk < nchunks; ++chunk, ++cc) {
-        const int buf = cc & 1;
-        mbar_wait(&acc_full[buf], (cc >> 1) & 1);
-        tc_fence_after();
-        if (tr && ti == tr_ti && threadIdx.x == 320) p.trace[chunk * 8 + 5] = clock64();
-        if (tr && ti == tr_ti + 1 && chunk == 0 && threadIdx.x == 320) p.trace[7 * 8 + 7] = clock64();   // next tile's drain start: the tile period
-#pragma unroll
-        for (int c0 = 0; c0 < CW; c0 += 16) {
-          uint32_t r[16], r2[16];
-          const uint32_t col = (uint32_t)(buf * TC_NACC * BN + cbeg + c0);
-          tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + col, r);
-          tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + col + (uint32_t)BN, r2);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 16; ++j) acc[c0 + j] += __uint_as_float(r[j]) + __uint_as_float(r2[j]);
-        }
-        tc_fence_before();
-        mbar_arrive(&acc_empty[buf]);
-        if (tr && ti == tr_ti && threadIdx.x == 320) p.trace[chunk * 8 + 6] = clock64();
-      }
-      if (ks > 1) {
-        // exchange buffer = box set 1 of rank 0 (unused: one tile per cluster), [BN / 4][128 rows] float4
-        const uint32_t xbuf = smem_u32(reinterpret_cast<uint8_t*>(out_stage) + Cfg::BOXSET_BYTES);
-        if (crank == 1) {
-          uint32_t rbuf;
-          asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rbuf) : "r"(xbuf), "r"(0));
-#pragma unroll
-          for (int lc = 0; lc < CW; lc += 4) {
-            const uint32_t a = rbuf + (uint32_t)((((cbeg + lc) >> 2) * TC_BM + row) * 16);
-            asm volatile("st.shared::cluster.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(a), "f"(acc[lc]), "f"(acc[lc + 1]), "f"(acc[lc + 2]),
-                         "f"(acc[lc + 3]) : "memory");
-          }
-        }
-        asm volatile("barrier.cluster.arrive.release;" ::: "memory");
-        asm volatile("barrier.cluster.wait.acquire;" ::: "memory");
-        if (crank == 1) break;          // rank 0 finishes the tile
-#pragma unroll
-        for (int lc = 0; lc < CW; lc += 4) {
-          const float4 o = lds128(xbuf + (uint32_t)((((cbeg + lc) >> 2) * TC_BM + row) * 16));
-          acc[lc] += o.x; acc[lc + 1] += o.y; acc[lc + 2] += o.z; acc[lc + 3] += o.w;
-        }
-      }
-      const bool etr = tr && ti == tr_ti && threadIdx.x == 320;
-      if (etr) p.trace[1 * 8 + 7] = clock64();
-      named_bar_sync(1, NDT);   // bias/scale of this tile are in smem (written before the chunk loop)
-      if (etr) p.trace[2 * 8 + 7] = clock64();
-      if (p.tma_store) {
-        // Epilogue without per-thread global stores: the row (thread = TMEM lane) is finished in registers, written
-        // into 128-byte-swizzled [128 x 32] boxes in shared memory and one thread issues TMA tile stores.  Two
-        // outputs (raw + ELU'd copy for the next layer) go through the two box sets, so neither store's source is rewritten
-        // within the tile.
-        const uint32_t rsw = (uint32_t)(row * 128), rx = (uint32_t)(row & 7);
-        const int nout = p.C2 ? 2 : 1;
-        for (int oi = 0; oi < nout; ++oi) {
-          const bool second = (nout == 2) && oi == 0;   // C2 first, C last
-          const int act = second ? p.act2 : p.post_act;
-          // [BN/32][128 rows][128 B] boxes, 1024-aligned; set 1 = odd tiles of residual layers / the second output of dual-output layers
-          // single-output layers alternate the two box sets per tile, dual-output layers per output: either way the set
-          // staged next was last read by the store before the most recent one, so ONE store may stay in flight
-          // Box set k is OWNED by drain thread 32 k (lane 0 of drain warp k): it issues every TMA store that reads the
-          // set, waits for its own stores' read-out before the set is rewritten, and requests the residual tiles that land
-          // in it -- so the two sets' serial duties (store issue ~450 clk, read-out wait + residual request ~1 000 clk) run on
-          // two threads instead of queueing on one.
-          const int set = (p.R || nout == 1) ? (ti & 1) : oi;
-          const bool owner = dt == 32 * set;
-          uint8_t* boxes = reinterpret_cast<uint8_t*>(out_stage) + (set ? Cfg::BOXSET_BYTES : 0);
-          if (!p.R) {
-            if (owner) bulk_wait_read0();          // this thread's previous store from the set
-            named_bar_sync(2, NDT);
-          }
-          if (etr) p.trace[3 * 8 + 7] = clock64();
-          auto stage_rows = [&](auto act_c, auto res_c) {   // one instantiation per activation: only the executed one is fetched
-            constexpr int ACTC = decltype(act_c)::value;
-            constexpr bool RES = decltype(res_c)::value;
-            // The operands of column group lc + 4 (bias, scale, residual) are loaded BEFORE the result of group lc is
-            // stored: the compiler cannot tell the box stores from the bias / scale loads (all shared memory) and would
-            // otherwise serialise load -> math -> store per group (255 clk per group, 2 000 clk per 128 x 64 tile).
-            auto slot_of = [&](int lc) {
-              const int c = cbeg + lc;
-              return reinterpret_cast<float4*>(boxes + (c >> 5) * (TC_BM * 128) + rsw + ((((uint32_t)((c & 31) >> 2)) ^ rx) << 4));
-            };
-            float4* slot = slot_of(0);
-            float4 bb = *reinterpret_cast<const float4*>(sb + cbeg), ss = *reinterpret_cast<const float4*>(sb + BN + cbeg);
-            float4 rr = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (RES) rr = *slot;
-#pragma unroll
-            for (int lc = 0; lc < CW; lc += 4) {          // register index static, box / slot from the runtime column
-              float4* slot_n = slot;
-              float4 bbn = bb, ssn = ss, rrn = rr;
-              if (lc + 4 < CW) {
-                slot_n = slot_of(lc + 4);
-                bbn = *reinterpret_cast<const float4*>(sb + cbeg + lc + 4);
-                ssn = *reinterpret_cast<const float4*>(sb + BN + cbeg + lc + 4);
-                if (RES) rrn = *slot_n;
-              }
-              float4 v = make_float4((acc[lc] + bb.x) * ss.x, (acc[lc + 1] + bb.y) * ss.y, (acc[lc + 2] + bb.z) * ss.z, (acc[lc + 3] + bb.w) * ss.w);
-              if (RES) { v.x += rr.x; v.y += rr.y; v.z += rr.z; v.w += rr.w; }
-              *slot = apply_act4_tc<ACTC>(v);
-              slot = slot_n; bb = bbn; ss = ssn; rr = rrn;
-            }
-          };
-          if (p.R) {
-            mbar_wait(&r_full[ti & 1], (uint32_t)((ti >> 1) & 1));   // one residual load per tile
-            if (etr) p.trace[3 * 8 + 7] = clock64();
-            if (act == ACT_ELU) stage_rows(std::integral_constant<int, ACT_ELU>{}, std::true_type{});
-            else stage_rows(std::integral_constant<int, ACT_NONE>{}, std::true_type{});
-          } else if (act == ACT_ELU) stage_rows(std::integral_constant<int, ACT_ELU>{}, std::false_type{});
-          else if (act == ACT_GELU) stage_rows(std::integral_constant<int, ACT_GELU>{}, std::false_type{});
-          else stage_rows(std::integral_constant<int, ACT_NONE>{}, std::false_type{});
-          if (etr) p.trace[4 * 8 + 7] = clock64();
-          fence_proxy_async_smem();
-          if (etr) p.trace[5 * 8 + 7] = clock64();
-          named_bar_sync(3, NDT);
-          if (etr) p.trace[6 * 8 + 7] = clock64();
-          if (owner) {
-            const CUtensorMap* tm = second ? &tmC2 : &tmC;
-            for (int g8 = 0; g8 < BN / 32; ++g8) {
-              const int n = n0 + g8 * 32;
-              if (n < p.N) {
-                int c0 = n, c2 = ot;
-                if (p.n_split > 0) { c0 = n % p.n_split; c2 = ot * p.c_tr + n / p.n_split; }
-                tma_store_3d(tm, boxes + g8 * (TC_BM * 128), c0, i0, c2);
-              }
-            }
-            bulk_commit();
-          }
-        }
-        if (tr && ti == tr_ti && threadIdx.x == 320) p.trace[7] = clock64();
-        continue;
-      }
-      if constexpr (DW == 4) {
-      // transpose through shared memory: thread = row while draining TMEM, 8 lanes = one 128-byte row segment when
-      // storing, so every global access is a full line (plans whose output cannot be a TMA tile store; DW == 4 only)
-      constexpr int LD = Cfg::OUT_LD;
-      float* stg = out_stage + q * 32 * LD;
-      __syncwarp();
-#pragma unroll
-      for (int g4 = 0; g4 < BN / 4; ++g4)
-        *reinterpret_cast<float4*>(stg + lane * LD + 4 * g4) = make_float4(acc[4 * g4], acc[4 * g4 + 1], acc[4 * g4 + 2], acc[4 * g4 + 3]);
-      __syncwarp();
-      if (etr) p.trace[3 * 8 + 7] = clock64();
-      const int cg = lane & 7, rsub = lane >> 3;
-      const long long c_base = (long long)ot * p.c_o_stride, r_base = (long long)ot * p.r_o_stride;
-      const int irow0 = i0 + q * 32 + rsub;
-      // The store loop stays rolled: the activations are long inline sequences and an unrolled epilogue (thousands of
-      // instructions) thrashed the instruction cache -- it cost more than the tile's MMAs.
-#pragma unroll 1
-      for (int pass = 0; pass < BN / 32; ++pass) {
-        const int nl = pass * 32 + cg * 4, n = n0 + nl;
-        if (n < p.N) {
-          const float4 bb = *reinterpret_cast<const float4*>(sb + nl);
-          const float4 ss = *reinterpret_cast<const float4*>(sb + BN + nl);
-          long long coff = n, roff = n;
-          if (p.n_split > 0) {
-            const int j = n / p.n_split, co = n % p.n_split;
-            coff = (long long)j * p.c_split_stride + co;
-            roff = (long long)j * p.r_split_stride + co;
-          }
-          float* srow = stg + rsub * LD + nl;
-          if (p.R) {   // (acc + bias) * scale + residual, residual rows fetched as one batch of eight loads
-            float4 rr[8];
-#pragma unroll
-            for (int it = 0; it < 8; ++it) {
-              const int i = irow0 + 4 * it;
-              rr[it] = i < p.I_out ? __ldg(reinterpret_cast<const float4*>(p.R + r_base + (long long)i * p.r_i_stride + roff)) : make_float4(0.f, 0.f, 0.f, 0.f);
-            }
-#pragma unroll
-            for (int it = 0; it < 8; ++it) {
-              float4 v = *reinterpret_cast<const float4*>(srow + 4 * it * LD);
-              v.x = (v.x + bb.x) * ss.x + rr[it].x; v.y = (v.y + bb.y) * ss.y + rr[it].y;
-              v.z = (v.z + bb.z) * ss.z + rr[it].z; v.w = (v.w + bb.w) * ss.w + rr[it].w;
-              *reinterpret_cast<float4*>(srow + 4 * it * LD) = v;
-            }
-          } else {
-#pragma unroll
-            for (int it = 0; it < 8; ++it) {
-              float4 v = *reinterpret_cast<const float4*>(srow + 4 * it * LD);
-              v.x = (v.x + bb.x) * ss.x; v.y = (v.y + bb.y) * ss.y; v.z = (v.z + bb.z) * ss.z; v.w = (v.w + bb.w) * ss.w;
-              *reinterpret_cast<float4*>(srow + 4 * it * LD) = v;
-            }
-          }
-          if (etr) p.trace[(4 + 2 * pass) * 8 + 7] = clock64();
-          long long off = c_base + (long long)irow0 * p.c_i_stride + coff;
-#pragma unroll 1
-          for (int it = 0; it < 8; ++it, off += 4 * p.c_i_stride) {
-            if (irow0 + 4 * it < p.I_out) {
-              const float4 v = *reinterpret_cast<const float4*>(srow + 4 * it * LD);
-              if (p.C2) *reinterpret_cast<float4*>(p.C2 + off) = apply_act4_tc(v, p.act2);
-              *reinterpret_cast<float4*>(p.C + off) = apply_act4_tc(v, p.post_act);
-            }
-          }
-          if (etr) p.trace[(5 + 2 * pass) * 8 + 7] = clock64();
-        }
-      }
-      if (tr && ti == tr_ti && threadIdx.x == 320) p.trace[7] = clock64();
-      }  // DW == 4
-    }
-  }
-  if (ks > 1 && warp < 10) {   // the producer / MMA / transform warps' side of the hand-over barrier (all threads of both CTAs)
-    asm volatile("barrier.cluster.arrive.release;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire;" ::: "memory");
-  }
-  if (threadIdx.x == 320 || threadIdx.x == 352) bulk_wait0();   // the issuing threads' TMA stores are complete before the CTA (and its smem) goes away
-  if (timed) p.cta_times[blockIdx.x * 4 + 2] = gtime();
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<512>(tmem_base);
-  if (timed) p.cta_times[blockIdx.x * 4 + 3] = gtime();
 }
 
 // ---------------------------------------------------------------- host side
@@ -820,47 +253,17 @@ using namespace rstnet;
 
 struct rstnet_tc_plan {
   CUtensorMap tmA, tmW, tmWlo;
-  CUtensorMap tmC, tmC2, tmR;  // output (and residual) tiles of the .ts kernel's TMA-store epilogue
-  CUtensorMap tmW3;  // [2 (hi, lo)][N][K] when W_lo follows W at a 16-byte-aligned distance (.ts kernel)
-  bool ts_ok;
   TcParams p;
-  dim3 grid;     // one CTA per tile (SS kernel)
-  dim3 grid_ts;  // persistent .ts kernel: min(tiles, SMs)
+  dim3 grid;     // persistent CTAs: min(tiles, SMs)
   int bn, prec;
 };
 
-template <int BN, int DW>
-static int tc_launch_ts(const rstnet_tc_plan* pl, cudaStream_t st) {
-  using Cfg = TsCfg<BN>;
-  static unsigned long long attr = 0;
-  smem_optin(gemm_tc_ts_kernel<BN, DW>, Cfg::SMEM_BYTES, attr);
-  if (pl->p.ksplit > 1) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = pl->grid_ts;
-    cfg.blockDim = dim3(320 + 32 * DW);
-    cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-    cfg.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = (unsigned)pl->p.ksplit;
-    at[0].val.clusterDim.y = 1;
-    at[0].val.clusterDim.z = 1;
-    cfg.attrs = at;
-    cfg.numAttrs = 1;
-    cudaLaunchKernelEx(&cfg, gemm_tc_ts_kernel<BN, DW>, pl->tmA, pl->tmW3, pl->tmC, pl->tmC2, pl->tmR, pl->p);
-  } else {
-    gemm_tc_ts_kernel<BN, DW><<<pl->grid_ts, 320 + 32 * DW, Cfg::SMEM_BYTES, st>>>(pl->tmA, pl->tmW3, pl->tmC, pl->tmC2, pl->tmR, pl->p);
-  }
-  count_launch();
-  return check_launch("gemm_tc_ts");
-}
-
-template <int BN, int PREC>
+template <int BN, int PREC, bool PRE_ELU>
 static int tc_launch(const rstnet_tc_plan* pl, cudaStream_t st) {
   using Cfg = TcCfg<BN, PREC>;
   static unsigned long long attr = 0;
-  smem_optin(gemm_tc_kernel<BN, PREC>, Cfg::SMEM_BYTES, attr);
-  gemm_tc_kernel<BN, PREC><<<pl->grid, TC_THREADS, Cfg::SMEM_BYTES, st>>>(pl->tmA, pl->tmW, pl->tmWlo, pl->p);
+  smem_optin(gemm_tc_kernel<BN, PREC, PRE_ELU>, Cfg::SMEM_BYTES, attr);
+  gemm_tc_kernel<BN, PREC, PRE_ELU><<<pl->grid, TC_THREADS, Cfg::SMEM_BYTES, st>>>(pl->tmA, pl->tmW, pl->tmWlo, pl->p);
   count_launch();
   return check_launch("gemm_tc");
 }
@@ -873,6 +276,7 @@ extern "C" int rstnet_tc_gemm_create(const rstnet_tc_gemm_desc* d, rstnet_tc_pla
   RSTNET_REQUIRE(d->N > 0 && d->N % 4 == 0, "tc_gemm_create: N (%d) must be a multiple of 4", d->N);
   RSTNET_REQUIRE(d->taps >= 1 && d->I_out > 0 && d->O_out > 0, "tc_gemm_create: bad shape");
   RSTNET_REQUIRE(d->precision == 0 || d->precision == 1, "tc_gemm_create: precision must be 0 (3xTF32) or 1 (TF32)");
+  RSTNET_REQUIRE(d->pre_act == ACT_NONE || d->pre_act == ACT_ELU, "tc_gemm_create: pre_act must be NONE or ELU (got %d)", d->pre_act);
   RSTNET_REQUIRE((uintptr_t)d->A % 16 == 0 && (uintptr_t)d->W % 16 == 0 && (uintptr_t)d->C % 16 == 0 &&
                      d->a_i_stride % 4 == 0 && d->a_o_stride % 4 == 0 && d->c_i_stride % 4 == 0 && d->c_o_stride % 4 == 0 &&
                      d->c_split_stride % 4 == 0 && d->n_split % 4 == 0,
@@ -881,17 +285,15 @@ extern "C" int rstnet_tc_gemm_create(const rstnet_tc_gemm_desc* d, rstnet_tc_pla
   RSTNET_REQUIRE(enc != nullptr, "tc_gemm_create: cuTensorMapEncodeTiled unavailable (no CUDA driver?)");
   rstnet_tc_plan* pl = new rstnet_tc_plan();
   const int N = d->N;
+  const int sms = sm_count();
   pl->bn = N >= 64 ? 64 : 32;
-  // narrow the tile when the grid would leave most of the 148 SMs idle
   const int i_tiles = ceil_div(d->I_out, TC_BM);
   {
-    // persistent CTAs: rounds x per-tile cost (a BN=64 tile costs ~1.5x a BN=32 tile: same A transform, twice the MMAs)
+    // narrow the tile when that takes fewer rounds of the SMs (a BN=64 tile costs ~1.5x a BN=32 tile: same A fragment
+    // loads and splits, twice the MMAs)
     const long long mt = (long long)i_tiles * d->O_out;
     const long long t64 = mt * ceil_div(N, 64), t32 = mt * ceil_div(N, 32);
-    if (pl->bn == 64 && ((t32 + 147) / 148) * 2 <= ((t64 + 147) / 148) * 3) pl->bn = 32;
-    static const int force_bn = []() { const char* e = getenv("RSTNET_TC_BN"); return e ? atoi(e) : 0; }();   // tuning aid
-    if (force_bn == 64 && N >= 64) pl->bn = 64;
-    if (force_bn == 32) pl->bn = 32;
+    if (pl->bn == 64 && ((t32 + sms - 1) / sms) * 2 <= ((t64 + sms - 1) / sms) * 3) pl->bn = 32;
   }
   pl->prec = d->precision;
   {
@@ -924,46 +326,6 @@ extern "C" int rstnet_tc_gemm_create(const rstnet_tc_gemm_desc* d, rstnet_tc_pla
       set_error("tc_gemm_create: cuTensorMapEncodeTiled(W) failed with %d", (int)r);
       return 3;
     }
-    // persistent .ts kernel: 3xTF32 with hi/lo weights reachable through one descriptor
-    pl->ts_ok = false;
-    const long long wdiff = d->W_lo ? (const char*)d->W_lo - (const char*)d->W : 0;
-    if (pl->prec == 0 && wdiff > 0 && wdiff % 16 == 0) {
-      cuuint64_t gdim3[3] = {(cuuint64_t)d->taps * d->Kc, (cuuint64_t)N, 2};
-      cuuint64_t gstr3[2] = {(cuuint64_t)d->taps * d->Kc * 4, (cuuint64_t)wdiff};
-      cuuint32_t box3[3] = {TC_BKE, (cuuint32_t)pl->bn, 2};
-      cuuint32_t estr3[3] = {1, 1, 1};
-      r = enc(&pl->tmW3, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, (void*)d->W, gdim3, gstr3, box3, estr3, CU_TENSOR_MAP_INTERLEAVE_NONE,
-              CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      pl->ts_ok = r == CUDA_SUCCESS;
-    }
-    // TMA-store epilogue: no residual, 32-column boxes, 16-byte aligned rows
-    pl->p.tma_store = 0; pl->p.c_tr = 1;
-    const bool split = d->n_split > 0, split0 = split;
-    const bool res_ok = !d->R || (!d->C2 && (d->post_act == ACT_NONE || d->post_act == ACT_ELU) && d->r_i_stride % 4 == 0 && d->r_o_stride % 4 == 0 &&
-                                  ((uintptr_t)d->R % 16) == 0 && (!split0 || (d->r_split_stride > 0 && d->r_o_stride % d->r_split_stride == 0 &&
-                                                                                  d->r_o_stride / d->r_split_stride == d->c_o_stride / (d->c_split_stride > 0 ? d->c_split_stride : 1))));
-    if (pl->ts_ok && res_ok && N % 32 == 0 && (!split || (d->n_split % 32 == 0 && d->c_split_stride > 0 && d->c_o_stride % d->c_split_stride == 0)) &&
-        d->c_i_stride % 4 == 0 && d->c_o_stride % 4 == 0 && ((uintptr_t)d->C % 16) == 0 && (!d->C2 || ((uintptr_t)d->C2 % 16) == 0)) {
-      const long long tr_rows = split ? d->c_o_stride / d->c_split_stride : 1;
-      cuuint64_t cdim[3] = {(cuuint64_t)(split ? d->n_split : N), (cuuint64_t)d->I_out, (cuuint64_t)(d->O_out * tr_rows)};
-      cuuint64_t cstr[2] = {(cuuint64_t)d->c_i_stride * 4, (cuuint64_t)(split ? d->c_split_stride : (d->O_out > 1 ? d->c_o_stride : d->c_i_stride * d->I_out)) * 4};
-      cuuint32_t cbox[3] = {32, TC_BM, 1};
-      cuuint32_t cest[3] = {1, 1, 1};
-      CUresult rc = enc(&pl->tmC, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, (void*)d->C, cdim, cstr, cbox, cest, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                        CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      if (rc == CUDA_SUCCESS && d->C2)
-        rc = enc(&pl->tmC2, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, (void*)d->C2, cdim, cstr, cbox, cest, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                 CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      else if (rc == CUDA_SUCCESS)
-        pl->tmC2 = pl->tmC;
-      pl->tmR = pl->tmC;
-      if (rc == CUDA_SUCCESS && d->R) {
-        cuuint64_t rstr[2] = {(cuuint64_t)d->r_i_stride * 4, (cuuint64_t)(split ? d->r_split_stride : (d->O_out > 1 ? d->r_o_stride : d->r_i_stride * d->I_out)) * 4};
-        rc = enc(&pl->tmR, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, (void*)d->R, cdim, rstr, cbox, cest, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                 CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      }
-      if (rc == CUDA_SUCCESS) { pl->p.tma_store = 1; pl->p.c_tr = (int)tr_rows; }
-    }
   }
   TcParams& p = pl->p;
   p.C2 = d->C2; p.act2 = d->act2;
@@ -973,25 +335,10 @@ extern "C" int rstnet_tc_gemm_create(const rstnet_tc_gemm_desc* d, rstnet_tc_pla
   p.I_out = d->I_out; p.O_out = d->O_out; p.N = N; p.Kc = d->Kc;
   p.taps = d->taps; p.tap_di = d->tap_di; p.tap_do = d->tap_do; p.o_mul = d->o_mul; p.kchunks = d->Kc / TC_BKE;
   p.pre_act = d->pre_act; p.post_act = d->post_act; p.i_tiles = i_tiles;
-  p.trace = nullptr;
-  p.cta_times = nullptr;
-  pl->grid = dim3((unsigned)(i_tiles * d->O_out), (unsigned)ceil_div(N, pl->bn));
-  p.m_tiles = (int)pl->grid.x; p.n_tiles = (int)pl->grid.y;
-  {
-    static int sms = 0;
-    if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 148; }
-    const long long tiles = (long long)p.m_tiles * p.n_tiles;
-    pl->grid_ts = dim3((unsigned)(tiles < sms ? tiles : sms));
-    // K split over 2-CTA clusters: plain linears (one tap) with a TMA-store epilogue, a single output, an even stage count
-    // of >= 8 per half... and few enough tiles that both halves get an SM of their own (RSTNET_TC_KSPLIT=0 turns it off)
-    static const bool ksplit_on = []() { const char* e = getenv("RSTNET_TC_KSPLIT"); return !(e && e[0] == '0'); }();
-    p.ksplit = 1;
-    if (ksplit_on && pl->ts_ok && p.tma_store && d->precision == 0 && p.taps == 1 && !p.C2 && p.n_split == 0 && p.kchunks % 2 == 0 &&
-        p.kchunks >= 16 && 2 * tiles <= sms) {
-      p.ksplit = 2;
-      pl->grid_ts = dim3((unsigned)(2 * tiles));
-    }
-  }
+  p.m_tiles = i_tiles * d->O_out;
+  p.n_tiles = ceil_div(N, pl->bn);
+  const long long tiles = (long long)p.m_tiles * p.n_tiles;
+  pl->grid = dim3((unsigned)(tiles < sms ? tiles : sms));
   *out = pl;
   return 0;
 }
@@ -999,33 +346,19 @@ extern "C" int rstnet_tc_gemm_create(const rstnet_tc_gemm_desc* d, rstnet_tc_pla
 extern "C" int rstnet_tc_gemm_run(const rstnet_tc_plan* pl, rstnet_stream_t stream) {
   RSTNET_REQUIRE(pl != nullptr, "tc_gemm_run: null plan");
   cudaStream_t st = (cudaStream_t)stream;
+  const bool elu = pl->p.pre_act == ACT_ELU;
   if (pl->prec == 0) {
-    static const bool use_ts = []() { const char* e = getenv("RSTNET_TC_SS"); return !(e && e[0] == '1'); }();
-    if (use_ts && pl->ts_ok) {
-      // eight drain warps whenever the epilogue is a TMA tile store (measured on the 256-stream codec pass: 63.6 k frames/s
-      // with four drain warps everywhere, 64.9 k with eight on tiles of <= 8 stages only, 68.5 k with eight everywhere:
-      // the drain of a long-K tile also gains more from twice the warps than it loses to 96 registers);
-      // RSTNET_TC_DW=4 restores the four-warp kernel
-      static const int force_dw = []() { const char* e = getenv("RSTNET_TC_DW"); return e ? atoi(e) : 0; }();
-      const bool dw8 = pl->p.tma_store && force_dw != 4;
-      if (dw8) return pl->bn == 64 ? tc_launch_ts<64, 8>(pl, st) : tc_launch_ts<32, 8>(pl, st);
-      return pl->bn == 64 ? tc_launch_ts<64, 4>(pl, st) : tc_launch_ts<32, 4>(pl, st);
-    }
-    if (pl->bn == 64) return tc_launch<64, 0>(pl, st);
-    return tc_launch<32, 0>(pl, st);
+    if (pl->bn == 64) return elu ? tc_launch<64, 0, true>(pl, st) : tc_launch<64, 0, false>(pl, st);
+    return elu ? tc_launch<32, 0, true>(pl, st) : tc_launch<32, 0, false>(pl, st);
   }
-  if (pl->bn == 64) return tc_launch<64, 1>(pl, st);
-  return tc_launch<32, 1>(pl, st);
+  if (pl->bn == 64) return elu ? tc_launch<64, 1, true>(pl, st) : tc_launch<64, 1, false>(pl, st);
+  return elu ? tc_launch<32, 1, true>(pl, st) : tc_launch<32, 1, false>(pl, st);
 }
 
 extern "C" void rstnet_tc_gemm_destroy(rstnet_tc_plan* pl) { delete pl; }
-/* debug: CTA (0,0) records clock64 stamps per k iteration into trace[total_k][8] (device int64) */
-extern "C" void rstnet_tc_gemm_set_trace(rstnet_tc_plan* pl, int64_t* trace, int64_t* cta_times) {
-  if (pl) { pl->p.trace = (long long*)trace; pl->p.cta_times = (long long*)cta_times; }
-}
 extern "C" int rstnet_tc_gemm_grid(const rstnet_tc_plan* pl, int32_t* gx, int32_t* gy, int32_t* bn) {
   if (!pl) return 1;
-  *gx = (int)pl->grid.x; *gy = (int)pl->grid.y; *bn = pl->bn;
+  *gx = pl->p.m_tiles; *gy = pl->p.n_tiles; *bn = pl->bn;
   return 0;
 }
 
@@ -1043,7 +376,7 @@ extern "C" int rstnet_tf32_split_f32(const float* x, float* hi, float* lo, int64
   RSTNET_REQUIRE(x && hi && lo, "tf32_split: null pointer");
   if (n <= 0) return 0;
   int g = ceil_div(n, 256);
-  if (g > 148 * 8) g = 148 * 8;
+  if (g > sm_count() * 8) g = sm_count() * 8;
   rstnet::tf32_split_kernel<<<g, 256, 0, (cudaStream_t)stream>>>(x, hi, lo, n);
   count_launch();
   return check_launch("tf32_split");

@@ -5,12 +5,12 @@
 // StreamingTransformer with weights_per_step (modules/transformer.py:155-179, 375-419, 518-577), ActivationGating
 // (modules/gating.py:12-21), sample_token* (utils/sampling.py:85-154).
 //
-// Why this shape: a step streams only 2-11 MB of weights per GEMM (1.27 GB per frame = 0.19 ms at HBM speed) and the
+// Why this shape: a step streams only 2-11 MB of weights per GEMM (1.27 GB per frame = 0.38 ms at the H100 data-sheet 3.35 TB/s) and the
 // eight steps are sequentially dependent, so the frame is bound by per-launch fixed costs, not by bandwidth or math.
 // Here every SM stays resident; a GEMM phase gives each CTA a few 16-row blocks of the weight matrix, which it streams
 // once through a 3-stage cp.async ring while the (tiny) activation panel [M <= 128 streams][K] comes from L2; the
 // contraction runs on mma.sync (bf16, fp32 accumulate) -- the tensor pipe is idle either way at M <= 128 and a
-// register-operand MMA needs no TMEM / descriptor set-up per phase.  Phases are separated by a grid-wide barrier
+// register-operand MMA needs no shared-memory descriptor set-up per phase.  Phases are separated by a grid-wide barrier
 // (one atomic per CTA).  RMSNorm is folded into the consumer: the producer's epilogue leaves per-block sums of squares,
 // the consumer scales the activation fragments on the fly (same fp32 arithmetic as modules/transformer.py:34-48).
 // bf16 roundings follow the eager reference: a linear's output is rounded before the residual / embedding add.
@@ -33,8 +33,8 @@ __device__ __forceinline__ bf16 f2b(float v) { return __float2bfloat16(v); }
 constexpr int DF_THREADS = 256;
 constexpr int DF_KC = 128;                // K elements per pipeline stage
 constexpr int DF_PITCH = DF_KC * 2 + 16;  // shared-memory row pitch in bytes: 8 consecutive rows hit distinct banks (ldmatrix)
-// pipeline depth: per chunk a CTA has only ~30 KB in flight, and a chunk costs a full DRAM round trip (~1 us measured with
-// 3 stages: the phases ran at memory latency); 6 stages for <= 64 streams, 4 for <= 128 (shared-memory budget)
+// pipeline depth: per chunk a CTA has only ~30 KB in flight, and a chunk costs a full DRAM round trip (with 3 stages the
+// phases ran at memory latency); 6 stages for <= 64 streams, 4 for <= 128 (shared-memory budget)
 constexpr int DF_MAXU = 3;                // 16-row weight blocks per CTA per round
 constexpr int DF_MAXQ = 8, DF_MAXL = 8;
 constexpr int DF_SMEM_MAX = 201 * 1024;   // dynamic; the sampler's static arrays (25 KB) come on top: 227 KB per CTA in all
@@ -178,7 +178,7 @@ __device__ void gemm_phase(const DepthFrameParams& p, uint8_t* smem, const bf16*
 
   if (norm_alpha) {
     // r[m] from the producer's per-block sums of squares.  The nb partials of a row are spread over `nsub` threads, each
-    // issuing its loads in independent batches of 8 (a plain dependent loop cost nb L2 round trips: 40 us per phase),
+    // issuing its loads in independent batches of 8 (a plain dependent loop costs nb L2 round trips per phase),
     // then added in a fixed order.
     const int nb = K / 16;
     const int mc = Mpad <= 64 ? 64 : 128, nsub = DF_THREADS / mc;

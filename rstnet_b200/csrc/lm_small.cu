@@ -552,7 +552,7 @@ extern "C" int rstnet_lm_ring_decode_attention_bf16(const void* q, const void* k
   const int q_per_kv = n_head / n_kv;
   const int G = q_per_kv % 2 == 0 ? 2 : 1;   // query heads per CTA sharing the K/V rows (the rest of a group hits L2)
   cudaStream_t st = (cudaStream_t)stream;
-  static const int sms = []() { int d = 0, n = 148; cudaGetDevice(&d); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, d); return n; }();
+  const int sms = sm_count();
   const int n_jobs = rows * (n_head / G);
   int* arrive = (int*)split_ws;
   float* ws = split_ws ? (float*)((char*)split_ws + (size_t)rows * n_head * 4) : nullptr;
@@ -590,7 +590,7 @@ extern "C" int rstnet_lm_silu_mul_bf16(const void* ab, void* out, int32_t M, int
   RSTNET_REQUIRE(ab && out && M > 0 && I > 0, "lm_silu_mul: bad argument");
   const long long total = (long long)M * I;
   int g = ceil_div(total, 256);
-  if (g > 148 * 8) g = 148 * 8;
+  if (g > sm_count() * 8) g = sm_count() * 8;
   launch_pdl(silu_mul_kernel, dim3(g), dim3(256), 0, (cudaStream_t)stream, (const bf16*)ab, (bf16*)out, M, I);
   count_launch();
   return check_launch("lm_silu_mul");

@@ -7,7 +7,7 @@
 // residual of its 32 frames from the previous level's winners (reducing that level's per-chunk
 // partial minima), then scores them against a 128-centroid chunk with an fp32 FFMA GEMM
 // (K = dim, centroids streamed k-major through a 3-stage cp.async pipeline), and writes one
-// (distance, index) partial per frame.  Splitting bins across CTAs is what keeps 148 SMs busy in
+// (distance, index) partial per frame.  Splitting bins across CTAs is what keeps every SM busy in
 // the streaming regime (N = concurrent streams, e.g. 256 frames per step); codebooks (16 MiB)
 // stay L2-resident.  Distances use torch.cdist's matmul form so near-ties resolve the same way:
 // d = sqrt(max(|x|^2 + |e|^2 - 2 x.e, 0)).
@@ -327,7 +327,7 @@ extern "C" int rstnet_rvq_decode_gather_f32(const int64_t* codes, const float* E
   RSTNET_REQUIRE(N > 0 && T > 0 && N % T == 0 && dim % 4 == 0, "rvq_decode_gather: bad shape");
   const long long total = (long long)N * (dim / 4);
   int gx = ceil_div(total, 256);
-  if (gx > 148 * 16) gx = 148 * 16;
+  if (gx > sm_count() * 16) gx = sm_count() * 16;
   rvq_gather_kernel<<<gx, 256, 0, (cudaStream_t)stream>>>((const long long*)codes, E, q, N, T, n_q, ns, dim, bins, time_major);
   count_launch();
   return check_launch("rvq_decode_gather");

@@ -1,4 +1,4 @@
-"""B200-native decode path of the speech-text LM behind the reference's Python API.
+"""H100-native decode path of the speech-text LM behind the reference's Python API.
 
 Mirrors ``models.llama_streaming.GPT`` (MLLM_v2/models/llama_streaming.py:520-766):
   * streaming (`with gpt.streaming(B):`): ``forward_global(seq[B,9,T]) -> (transformer_out[B,T,E], text_logits[B,T,V])``
@@ -14,7 +14,7 @@ Mirrors ``models.llama_streaming.GPT`` (MLLM_v2/models/llama_streaming.py:520-76
 plus ``forward_step`` -- the whole frame (temporal step, text sampling, 8 depth steps with sampling) as one CUDA-graph
 replay; BASELINE.json names it although no such symbol exists upstream.
 
-All arithmetic runs in librstnet_b200.so: tcgen05 weight-streaming GEMMs, ring decode attention, fused
+All arithmetic runs in librstnet_b200.so: wgmma weight-streaming GEMMs, ring decode attention, fused
 norm / RoPE / gating / sampling kernels.  bf16 weights and activations, fp32 accumulation, exactly the
 dtype recipe of `GPT(config).to(device, bfloat16)` (infer_no_streaming.py:104-105).
 """
@@ -96,7 +96,7 @@ _GATE_INTERLEAVE = os.environ.get("RSTNET_LM_GATE_INTERLEAVE", "1") != "0"
 
 def interleave_gate_rows(w_gate: torch.Tensor, w_value: torch.Tensor) -> torch.Tensor:
     """[gate row 0, value row 0, gate row 1, value row 1, ...]: the packing the GEMM's in-epilogue SiLU gating expects (the
-    two rows of an output column sit in neighbouring lanes of the tcgen05 epilogue; fc_1 / fc_2 of LLaMAMLP,
+    two rows of an output column sit in neighbouring lanes of the GEMM epilogue; fc_1 / fc_2 of LLaMAMLP,
     lit_model.py:399-403, or the halves of ActivationGating.linear_in, modules/gating.py:12-21)."""
     return torch.stack([w_gate, w_value], dim=1).reshape(2 * w_gate.shape[0], w_gate.shape[1]).contiguous()
 
@@ -248,13 +248,13 @@ class GPT(nn.Module):
         self._ns_state: Optional["_LMState"] = None      # scratch scope of the non-streaming forward_global
         self.use_cuda_graphs = True
         # True: the depth transformer of a frame as ONE persistent cooperative kernel (csrc/lm_depth_frame.cu) instead of one
-        # launch per GEMM / attention / sampler.  Parity-tested, but measured SLOWER on B200 at the 7B shapes (5.3 ms vs
-        # 3.7 ms per frame at B = 64: the per-CTA activation-panel reads from L2 and the mma.sync dependency chains do not
-        # overlap, and 264 grid barriers cost 0.55 ms by themselves -- DESIGN.md §6), so it is opt-in.
+        # launch per GEMM / attention / sampler.  Parity-tested but opt-in: the per-CTA activation-panel reads from L2,
+        # the mma.sync dependency chains and the 264 grid barriers of a frame do not overlap (time it with
+        # scripts/depth_timing.py before enabling it).
         self.use_depth_frame_kernel = False
         # True: the temporal attention cuts every (stream, head) job's keys in three chunks walked by persistent CTAs
-        # (csrc/lm_small.cu).  Removes the under-filled last wave but pays the per-job prologue/combine three times:
-        # measured 491 us vs 430 us per layer at B = 64 x 32 heads x 2047 keys, so it is opt-in.
+        # (csrc/lm_small.cu).  Removes the under-filled last wave but pays the per-job prologue/combine three times, which
+        # made it slower where it was timed (scripts/lm_attn_bench.py), so it is opt-in.
         self.attention_key_split = False
 
     # parameter names of the depth transformer (the Moshi-style LMModel of rstnet_b200/moshi.py has the same structure under
@@ -371,7 +371,7 @@ class GPT(nn.Module):
     def _check_runnable(self):
         dev = self.device
         if dev.type != "cuda":
-            raise RstnetError("GPT decode runs on CUDA only (sm_100a kernels; the CPU path is the reference itself)")
+            raise RstnetError("GPT decode runs on CUDA only (sm_90a kernels; the CPU path is the reference itself)")
         if next(self.parameters()).dtype != torch.bfloat16:
             raise RstnetError("GPT decode runs in bfloat16: call .to(device, torch.bfloat16) as infer_no_streaming.py:104-105 does")
 
@@ -560,8 +560,8 @@ class _LMState:
         if m._packed is None:
             pk = self._pack_temporal(P)
             # depth gating weights: K padded to the GEMM granularity.  They keep the stacked [gate; value] form + finalize
-            # kernel: with 44 column tiles the GEMM wants two K slices (13.4 us vs 14.5 us for one, scripts/skinny_sweep.py),
-            # which the in-epilogue gating cannot have -- measured 3.3 ms vs 3.0 ms for the depth part of a frame.
+            # kernel: with 44 column tiles the GEMM wants two K slices (scripts/skinny_sweep.py times the choices), which
+            # the in-epilogue gating cannot have.
             for l in range(c.codecformer_layers if (Hp != H or self.frame_kernel) else 0):
                 for k in range(c.dep_q):
                     w_in = P[m._DN["dlayer"].format(l) + f".gating.{k}.linear_in.weight"]

@@ -1,4 +1,4 @@
-"""B200-native streaming decode path of the Moshi-style `LMModel` / `LMGen` twin of the reference.
+"""H100-native streaming decode path of the Moshi-style `LMModel` / `LMGen` twin of the reference.
 
 Mirrors ``models.model.LMModel`` (MLLM_v2/models/model.py:98-428) and ``LMGen`` (:440-597) -- the model
 `moshi/server.py:44-166` drives: a Kyutai `StreamingTransformer` backbone (rms_norm_f32, pair-RoPE, SiLU gating,
@@ -11,7 +11,7 @@ embedding, a text head, and the depth transformer with per-codebook-step weights
   * ``LMGen(lm, use_sampling, temp, temp_text, top_k, top_k_text).step(input_tokens[B, K_in, 1]) -> [B, dep_q+1, 1] | None``
     with the delay cache of :490-562 (acoustic delays, initial tokens, `max_delay` warm-up frames returning None).
 
-The kernels are the GPT path's (rstnet_b200/lm.py): weight-streaming tcgen05 GEMMs with fused Kyutai RMSNorm / SiLU gating
+The kernels are the GPT path's (rstnet_b200/lm.py): weight-streaming wgmma GEMMs with fused Kyutai RMSNorm / SiLU gating
 finalizes, ring decode attention, the depth transformer, device-side sampling; plus the bf16 pair-RoPE kernel.  One
 `LMGen.step` is one CUDA-graph replay.
 """
@@ -274,7 +274,7 @@ class LMModel(nn.Module):
     @on_own_device
     def streaming_forever(self, batch_size: int):
         if self.device.type != "cuda":
-            raise RstnetError("LMModel decode runs on CUDA only (sm_100a kernels; the CPU path is the reference itself)")
+            raise RstnetError("LMModel decode runs on CUDA only (sm_90a kernels; the CPU path is the reference itself)")
         if next(self.parameters()).dtype != torch.bfloat16:
             raise RstnetError("LMModel decode runs in bfloat16: call .to(device, torch.bfloat16)")
         self._state = _MoshiState(self, batch_size)

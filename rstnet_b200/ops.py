@@ -62,7 +62,7 @@ def tf32_split(w: torch.Tensor):
 
 
 class TcGemm:
-    """A tcgen05 GEMM plan bound to fixed buffers (rstnet_tc_gemm_create / run / destroy).
+    """A tensor-core (wgmma) GEMM plan bound to fixed buffers (rstnet_tc_gemm_create / run / destroy).
 
     D[(i,o), n] = sum_tap sum_c A[c, i + tap*tap_di, o*o_mul + tap*tap_do] * W[n, tap*Kc + c];
     offsets / strides in elements; see include/rstnet_b200.h."""

@@ -1,4 +1,4 @@
-"""Per-shape table of the codec's tcgen05 GEMM launches over one streaming frame (256 streams): time, FLOP/s, bytes/s."""
+"""Per-shape table of the codec's tensor-core GEMM launches over one streaming frame (256 streams): time, FLOP/s, bytes/s."""
 import sys, json
 import torch
 sys.path.insert(0, ".")

@@ -70,7 +70,7 @@ def one(B):
         json.dump(res, open("gpurun_out/r2_depth_timing.json", "w"), indent=1)
 
 
-for B in (64, 128):
+for B in (32, 48):
     try:
         one(B)
     except torch.cuda.OutOfMemoryError as e:

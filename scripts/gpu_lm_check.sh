@@ -8,9 +8,9 @@ import json, sys, torch
 sys.path.insert(0, '.')
 import bench
 dev = torch.device('cuda', 0)
-# depth-transformer kernel alone (7B shapes, B = 64)
+# depth-transformer kernel alone (7B shapes, B = 32)
 m = bench._gpt7b(dev, context=2048)
-with m.streaming(64):
+with m.streaming(32):
     st = m._state
     st.tout.normal_()
     st.tokens.random_(0, 2048)
@@ -22,7 +22,7 @@ with m.streaming(64):
     for _ in range(50):
         st._depth_frame(0, 8, True, True, 30, 0.8, [2048] * 8)
     e1.record(); torch.cuda.synchronize()
-    print("depth frame kernel (8 steps x 6 layers + sampling), B=64: %.3f ms" % (e0.elapsed_time(e1) / 50))
+    print("depth frame kernel (8 steps x 6 layers + sampling), B=32: %.3f ms" % (e0.elapsed_time(e1) / 50))
     m.check_device_errors()
 del m; torch.cuda.empty_cache()
 r = bench.lm_decode_bench(dev, steps=10, warmup=3)

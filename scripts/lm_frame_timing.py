@@ -1,4 +1,4 @@
-"""Time one LM frame (7B shapes, B = 64, full 2048-key ring): temporal graph and whole-frame graph.  RSTNET_PDL=0/1."""
+"""Time one LM frame (7B shapes, B = 32, full 2048-key ring): temporal graph and whole-frame graph.  RSTNET_PDL=0/1."""
 import json
 import os
 import sys
@@ -10,7 +10,7 @@ import bench
 
 dev = torch.device("cuda", 0)
 m = bench._gpt7b(dev, context=2048)
-B = int(os.environ.get("LM_B", "64"))
+B = int(os.environ.get("LM_B", "32"))
 
 
 def timeit(fn, n=20):

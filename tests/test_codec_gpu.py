@@ -323,7 +323,7 @@ def test_empty_input(codec):
 def test_streaming_vs_reference_golden_and_batch(golden_dir, codec, graphs, tc):
     """MimiModel streaming (compression.py:368-423) golden + the reference property streaming == batch.
     tc=False: fp32 FFMA kernels (same arithmetic as the batch path -> identical results);
-    tc=True: tcgen05 3xTF32 GEMMs (fp32-equivalent; indices may differ only on near-ties)."""
+    tc=True: wgmma 3xTF32 GEMMs (fp32-equivalent; indices may differ only on near-ties)."""
     g = np.load(os.path.join(golden_dir, "mimi_stream6.npz"))
     x = S.synthetic_audio(2, 1920 * 6, seed=int(g["audio_seed"])).to(DEV)
     codec.use_cuda_graphs, codec.streaming_tensor_cores = graphs, tc

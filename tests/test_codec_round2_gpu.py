@@ -234,7 +234,7 @@ def test_frame_scheduler_with_duplex_engine(codec):
 def test_offline_tokenization_and_batch_tensor_core_path(official_weights, codec, tmp_path):
     """rstnet_b200.offline (offline_codec_tokenization.py / inference.py drivers): equal-length clips are batched, the dict
     `utt -> int16 [8, T]` equals per-clip MimiTokenizer.tokenize and survives torch.save; a batch of >= 96 clips runs the
-    non-streaming tcgen05 path and must agree with the oracle wherever the margins allow; wav directory round trip."""
+    non-streaming tensor-core path and must agree with the oracle wherever the margins allow; wav directory round trip."""
     from rstnet_b200 import offline
     tok = MimiTokenizer(codec, device=torch.device(DEV))
     lens = [4000, 9600, 9600, 1920, 9600, 5000]

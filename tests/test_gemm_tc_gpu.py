@@ -1,4 +1,4 @@
-"""tcgen05 GEMM (rstnet_tc_gemm_*) vs the CPU oracle: linear, strided causal conv and transposed
+"""Tensor-core wgmma GEMM (rstnet_tc_gemm_*) vs the CPU oracle: linear, strided causal conv and transposed
 conv in the time-major/batch-inner layout used by the streaming plans.  Precision 0 (3xTF32) must
 be fp32-equivalent (<= 3e-6 relative to the fp32 result scale); precision 1 (TF32) ~1e-3."""
 import pytest

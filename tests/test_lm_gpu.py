@@ -207,6 +207,7 @@ def test_streaming_decode_vs_reference_golden(golden_dir, small_lm, graphs):
     gold = np.load(os.path.join(golden_dir, "lm_small.npz"))
     seqs = torch.from_numpy(gold["seqs"])
     keep = list(gold["bf16_keep"])
+    cols = torch.from_numpy(gold["logit_cols"])
     m.use_cuda_graphs = graphs
     tok_ok, n_tok = 0, 0
     # fp32 evaluation of the same bf16-valued weights: the yardstick for "bf16 noise"
@@ -240,11 +241,13 @@ def test_streaming_decode_vs_reference_golden(golden_dir, small_lm, graphs):
             n_tok += ref_tokens.numel()
             if f in keep:
                 i = keep.index(f)
+                # the stored logits are a seeded sample of the vocabulary columns (gold["logit_cols"])
                 ro, ra = torch.from_numpy(gold["bf16_out"][i]), torch.from_numpy(gold["bf16_audio_logits"][i])
-                assert _cos(out, ro) >= 0.999 and _cos(al, ra) >= 0.999, (f, _cos(out, ro), _cos(al, ra))
+                al_s, t_al_s = al[..., cols], t_al[..., cols]
+                assert _cos(out, ro) >= 0.999 and _cos(al_s, ra) >= 0.999, (f, _cos(out, ro), _cos(al_s, ra))
                 # our deviation from the fp32 evaluation must be of the same size as the reference's own bf16 deviation
                 e_mine, e_ref = _rel(out, t_out), _rel(ro, t_out)
-                a_mine, a_ref = _rel(al, t_al), _rel(ra, t_al)
+                a_mine, a_ref = _rel(al_s, t_al_s), _rel(ra, t_al_s)
                 worst = max(worst, e_mine / max(e_ref, 1e-3), a_mine / max(a_ref, 1e-3))
                 assert e_mine <= 2.0 * e_ref + 1e-2 and a_mine <= 2.0 * a_ref + 1e-2, (f, e_mine, e_ref, a_mine, a_ref)
                 top = tl.float().topk(8, dim=-1).values.cpu()
@@ -407,8 +410,9 @@ def test_gqa_partial_rope_streaming_vs_reference_golden(gqa_lm):
             if f in keep:
                 i = keep.index(f)
                 ro, ra = torch.from_numpy(gold["gqa_bf16_out"][i]), torch.from_numpy(gold["gqa_bf16_audio_logits"][i])
-                assert _cos(out, ro) >= 0.999 and _cos(al, ra) >= 0.999, (f, _cos(out, ro), _cos(al, ra))
-                assert _rel(out, ro) <= 5e-2 and _rel(al, ra) <= 5e-2
+                al_s = al[..., torch.from_numpy(gold["logit_cols"]).to(DEV)]   # the stored seeded sample of the vocabulary
+                assert _cos(out, ro) >= 0.999 and _cos(al_s, ra) >= 0.999, (f, _cos(out, ro), _cos(al_s, ra))
+                assert _rel(out, ro) <= 5e-2 and _rel(al_s, ra) <= 5e-2
     print(f"gqa greedy token agreement with the reference: {tok_ok}/{n_tok}")
     assert tok_ok / n_tok >= 0.9
 
@@ -467,10 +471,11 @@ def test_forward_local_vs_reference_golden(gqa_lm):
     t_out = torch.from_numpy(gold["gqa_bf16_full_out"]).to(DEV, BF)
     start = m.codecformer_text_emb(toks[:, 0, :])
     lg = m.forward_local(local_start_token=start, sequence=toks[:, 1:, :], transformer_out=t_out)
-    ref = torch.from_numpy(gold["gqa_bf16_local_logits"])
-    assert lg.shape == ref.shape
-    assert _cos(lg, ref) >= 0.999 and _rel(lg, ref) <= 5e-2, (_cos(lg, ref), _rel(lg, ref))
-    agree = float((lg.float().argmax(-1).cpu() == ref.argmax(-1)).float().mean())
+    ref = torch.from_numpy(gold["gqa_bf16_local_logits"])              # a seeded sample of the vocabulary columns
+    assert lg.shape[:-1] == ref.shape[:-1] and lg.shape[-1] == cfg.audio_card
+    lg_s = lg[..., torch.from_numpy(gold["logit_cols"]).to(DEV)]
+    assert _cos(lg_s, ref) >= 0.999 and _rel(lg_s, ref) <= 5e-2, (_cos(lg_s, ref), _rel(lg_s, ref))
+    agree = float((lg.float().argmax(-1).cpu() == torch.from_numpy(gold["gqa_bf16_local_argmax"])).float().mean())
     print(f"forward_local argmax agreement with the reference: {agree:.3f}")
     assert agree >= 0.9
 

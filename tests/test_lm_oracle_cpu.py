@@ -27,7 +27,8 @@ def test_lm_oracle_matches_reference_golden(golden_dir, tag, dtype):
             if f in keep:
                 i = keep.index(f)
                 assert np.array_equal(out.float().numpy(), g[f"{tag}_out"][i])
-                assert np.array_equal(al.float().numpy(), g[f"{tag}_audio_logits"][i])
+                assert np.array_equal(al.float().numpy()[..., g["logit_cols"]], g[f"{tag}_audio_logits"][i])
+                assert np.array_equal(al.float().argmax(-1).numpy(), g[f"{tag}_audio_argmax"][i])
 
 
 def test_ring_labels_oldest_slot_as_end_offset():

@@ -281,14 +281,10 @@ int rstnet_lm_rope_pair_kv_append_bf16(const void* qkv, const int64_t* offset, i
 /* ---- one query position per row over the ring with RingKVCache.complete's position labels and the
  * (pos_k>=0)&(delta>=0)&(delta<context) mask (llama_streaming.py:983-992), fp32 softmax. HBM-bound.  Rows as above;
  * every position of the launch must already be in the ring and no slot a query needs may have been overwritten
- * (callers keep *offset + Tn <= cap for Tn > 1).
- * split_ws (optional, rstnet_lm_attention_split_workspace bytes, its first rows*n_head int32 zeroed ONCE by the caller): lets
- * the kernel cut every job's keys in three chunks walked by persistent CTAs when rows * heads would otherwise leave a badly
- * filled last wave; partials are combined in chunk order (deterministic). */
-int64_t rstnet_lm_attention_split_workspace(int32_t rows, int32_t n_head, int32_t hs);
+ * (callers keep *offset + Tn <= cap for Tn > 1). */
 int rstnet_lm_ring_decode_attention_bf16(const void* q, const void* kv, const int64_t* offset, int32_t offset_stride,
                                          void* out, int32_t rows, int32_t B, int32_t n_head, int32_t n_kv, int32_t hs,
-                                         int32_t cap, int32_t context, void* split_ws, rstnet_stream_t stream);
+                                         int32_t cap, int32_t context, rstnet_stream_t stream);
 /* out[m][c] = silu(ab[m][c]) * ab[m][I + c]   (LLaMAMLP / ActivationGating) */
 int rstnet_lm_silu_mul_bf16(const void* ab, void* out, int32_t M, int32_t I, rstnet_stream_t stream);
 /* ---- depth transformer attention at codebook step `step` (keys 0..step, capacity dep_q <= 8, no RoPE):
@@ -297,33 +293,6 @@ int rstnet_lm_silu_mul_bf16(const void* ab, void* out, int32_t M, int32_t I, rst
  * on the last step; 0: non-streaming form (forward_local, :694-725; KVCacheResult.from_kv keeps every key). */
 int rstnet_lm_depth_attention_bf16(const void* qkv, void* kvd, void* out, int32_t B, int32_t H, int32_t hd, int32_t cap,
                                    int32_t step, int32_t ring_quirk, rstnet_stream_t stream);
-/* ---- the depth transformer of a frame as ONE persistent (cooperative) kernel: steps [k_begin, k_end) of
- * GPT.forward_codecformer (llama_streaming.py:727-749; per-step weights modules/transformer.py:155-179, 518-577; gating
- * modules/gating.py:12-21), each = codecformer_in[k](transformer_out) + embedding of the step's input token, L layers
- * (RMSNorm-f32, per-step in/out projections, attention over the <= dep_q keys of this frame, SiLU gating), audio_linears[k]
- * -> logits[k][M][card], and (do_sample) sample_token_audio on the device: tokens[m][k + 1] feeds step k + 1.
- * tokens[m][k] is the INPUT token of step k (column 0: the text token).  All buffers are the caller's; `barrier` is two
- * uint32 words (arrival counter, zeroed by run; sticky error word: bit 0 token id outside its table, bit 2 barrier
- * watchdog).  w_gin[l*Q + k]: gating linear_in with its rows interleaved in 8-row groups [a_8u..8u+7; b_8u..8u+7] and the
- * hidden width zero-padded to Hp (a multiple of 128); w_gout[l*Q + k]: linear_out [D][Hp].  Requires M <= 128,
- * D, E, Hp multiples of 128, D <= 2048.  step0_embedding (optional, [M][D]) replaces the token lookup of step 0
- * (forward_local passes features there, llama_streaming.py:700-705); ring_quirk as in rstnet_lm_depth_attention_bf16. */
-typedef struct rstnet_depth_plan rstnet_depth_plan;
-typedef struct {
-  int32_t M, D, E, Hp, H, hd, Q, L, card, tok_stride;
-  const void* tout; void* x; void* qkv; void* att; void* dh; void* logits; void* dkv; float* ss_part; int64_t* tokens; void* barrier;
-  const void* w_in[8]; const void* emb[8]; int64_t emb_rows[8]; const void* w_head[8];
-  const void* w_qkv[8]; const void* w_out[8]; const void* a1[8]; const void* a2[8];
-  const void* w_gin[64]; const void* w_gout[64];
-} rstnet_depth_frame_desc;
-int rstnet_lm_depth_frame_create(const rstnet_depth_frame_desc* desc, rstnet_depth_plan** plan);
-int rstnet_lm_depth_frame_run(const rstnet_depth_plan* plan, int32_t k_begin, int32_t k_end, int32_t ring_quirk, int32_t do_sample,
-                              int32_t top_k, float temp, uint32_t seed, const int64_t* frame_counter, const int32_t* n_valid,
-                              const void* step0_embedding, rstnet_stream_t stream);
-void rstnet_lm_depth_frame_destroy(rstnet_depth_plan* plan);
-/* profiling aid: CTA 0 writes clock64 stamps (start, then after every phase and after every barrier) to trace[>= 1024] */
-void rstnet_lm_depth_frame_set_trace(rstnet_depth_plan* plan, int64_t* trace);
-
 /* ---- sample_token / sample_token_audio[_2048] (utils/sampling.py:85-154): ids restricted to [0, n_valid);
  * top_k == 0 -> argmax (first maximum; use_sampling False); 1 <= top_k <= 1024 -> top-k + temperature +
  * exponential-noise multinomial (sample_top_k, :49-60); top_k < 0 -> temperature multinomial over all n_valid ids

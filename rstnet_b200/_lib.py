@@ -24,8 +24,7 @@ SYMBOLS = [
     "rstnet_skinny_gemm_workspace", "rstnet_skinny_gemm_create", "rstnet_skinny_gemm_create_fused", "rstnet_skinny_gemm_run", "rstnet_skinny_gemm_destroy",
     "rstnet_lm_embed_sum_bf16", "rstnet_lm_embed_rows_bf16", "rstnet_lm_rms_norm_bf16", "rstnet_lm_rope_kv_append_bf16",
     "rstnet_lm_rope_pair_kv_append_bf16",
-    "rstnet_lm_ring_decode_attention_bf16", "rstnet_lm_attention_split_workspace", "rstnet_lm_silu_mul_bf16", "rstnet_lm_depth_attention_bf16", "rstnet_lm_sample_bf16",
-    "rstnet_lm_depth_frame_create", "rstnet_lm_depth_frame_run", "rstnet_lm_depth_frame_destroy", "rstnet_lm_depth_frame_set_trace",
+    "rstnet_lm_ring_decode_attention_bf16", "rstnet_lm_silu_mul_bf16", "rstnet_lm_depth_attention_bf16", "rstnet_lm_sample_bf16",
 ]
 
 
@@ -57,14 +56,6 @@ class TcGemmDesc(C.Structure):
 class RowCopy(C.Structure):
     _fields_ = [("buf", C.c_void_p), ("batch_stride", C.c_int64), ("C", C.c_int32), ("src_row", C.c_int32),
                 ("dst_row", C.c_int32), ("nrows", C.c_int32), ("cps", C.c_int32), ("reserved", C.c_int32)]
-
-
-class DepthFrameDesc(C.Structure):
-    _fields_ = [(n, C.c_int32) for n in ("M", "D", "E", "Hp", "H", "hd", "Q", "L", "card", "tok_stride")] + \
-               [(n, C.c_void_p) for n in ("tout", "x", "qkv", "att", "dh", "logits", "dkv", "ss_part", "tokens", "barrier")] + \
-               [("w_in", C.c_void_p * 8), ("emb", C.c_void_p * 8), ("emb_rows", C.c_int64 * 8), ("w_head", C.c_void_p * 8),
-                ("w_qkv", C.c_void_p * 8), ("w_out", C.c_void_p * 8), ("a1", C.c_void_p * 8), ("a2", C.c_void_p * 8),
-                ("w_gin", C.c_void_p * 64), ("w_gout", C.c_void_p * 64)]
 
 
 class RstnetError(RuntimeError):
@@ -131,18 +122,10 @@ def lib() -> C.CDLL:
     L.rstnet_lm_rms_norm_bf16.argtypes = [vp, vp, vp, i32, i32, f32, i32, vp]
     L.rstnet_lm_rope_kv_append_bf16.argtypes = [vp, vp, vp, i64, i32, vp, i32, vp, vp, i32, i32, i32, i32, i32, i32, vp]
     L.rstnet_lm_rope_pair_kv_append_bf16.argtypes = [vp, vp, i32, vp, vp, i32, i32, i32, i32, i32, vp, vp]
-    L.rstnet_lm_ring_decode_attention_bf16.argtypes = [vp, vp, vp, i32, vp, i32, i32, i32, i32, i32, i32, i32, vp, vp]
-    L.rstnet_lm_attention_split_workspace.argtypes = [i32, i32, i32]
-    L.rstnet_lm_attention_split_workspace.restype = i64
+    L.rstnet_lm_ring_decode_attention_bf16.argtypes = [vp, vp, vp, i32, vp, i32, i32, i32, i32, i32, i32, i32, vp]
     L.rstnet_lm_silu_mul_bf16.argtypes = [vp, vp, i32, i32, vp]
     L.rstnet_lm_depth_attention_bf16.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]
     L.rstnet_lm_sample_bf16.argtypes = [vp, i32, i32, i32, i32, f32, C.c_uint32, vp, vp, i32, vp]
-    L.rstnet_lm_depth_frame_create.argtypes = [C.POINTER(DepthFrameDesc), C.POINTER(C.c_void_p)]
-    L.rstnet_lm_depth_frame_run.argtypes = [vp, i32, i32, i32, i32, i32, f32, C.c_uint32, vp, vp, vp, vp]
-    L.rstnet_lm_depth_frame_destroy.argtypes = [vp]
-    L.rstnet_lm_depth_frame_destroy.restype = None
-    L.rstnet_lm_depth_frame_set_trace.argtypes = [vp, vp]
-    L.rstnet_lm_depth_frame_set_trace.restype = None
     for name in SYMBOLS:
         fn = getattr(L, name)
         if fn.restype is C.c_int and name not in ("rstnet_version",):

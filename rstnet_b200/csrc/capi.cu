@@ -3,7 +3,6 @@
 #include "../../include/rstnet_b200.h"
 #include <atomic>
 #include <cstdarg>
-#include <cstdlib>
 
 namespace rstnet {
 
@@ -18,15 +17,6 @@ void set_error(const char* fmt, ...) {
 }
 
 void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
-
-bool pdl_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("RSTNET_PDL");
-    v = (e && e[0] == '1') ? 1 : 0;     // opt-in (common.cuh)
-  }
-  return v != 0;
-}
 
 // Launch-configuration errors only (cudaGetLastError does not synchronise, and is legal during
 // stream capture); asynchronous faults surface at the caller's next synchronisation.
@@ -46,7 +36,7 @@ unsigned int lm_read_errors(bool clear);
 unsigned int rvq_read_errors(bool clear);
 }
 
-extern "C" int rstnet_version(void) { return 200; }
+extern "C" int rstnet_version(void) { return 201; }
 // Sticky device-side error bits of the CURRENT device (synchronises it): 1 = token / code id outside its table,
 // 2 = RoPE position beyond the cos/sin tables.  Kernels cannot raise; they poison their output (NaN) and set a bit.
 extern "C" uint32_t rstnet_device_error_flags(int clear) {

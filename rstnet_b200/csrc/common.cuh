@@ -84,33 +84,6 @@ inline int sm_count() {
   return n > 0 ? n : 1;
 }
 
-// ---- programmatic dependent launch (PDL), opt-in with RSTNET_PDL=1.  The LM frame is a chain of ~800 small dependent
-// kernels; with the launch attribute below the next kernel's CTAs are scheduled while the previous grid drains and run their
-// prologue (barrier set-up, descriptor prefetch) up to `pdl_wait()`, which returns once the previous grid has
-// completed and flushed.  Every kernel launched through launch_pdl() calls pdl_launch_dependents() and then pdl_wait()
-// before its first global access, so the ordering guarantees are those of plain stream order (also inside a captured CUDA
-// graph).  Off by default: inside a replayed CUDA graph, programmatic edges between kernel nodes can cost more per launch
-// than plain edges, which outweighs the hidden prologues (time the frame with scripts/lm_frame_timing.py before enabling
-// it).  Without the attribute griddepcontrol.* are no-ops.
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-bool pdl_enabled();   // env RSTNET_PDL=1 (default off); capi.cu
-
-template <typename... KArgs, typename... Args>
-inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
-}
-
 // One-time opt-in to more than 48 KB of dynamic shared memory.  The attribute belongs to the (function, device) pair, so
 // the "done" mask is keyed by the CURRENT device ordinal: a second GPU in the same process gets its own opt-in.
 template <typename Kernel>

@@ -11,7 +11,6 @@
 #include <cuda_bf16.h>
 
 #include <cooperative_groups.h>
-#include <cstdlib>
 
 #include "common.cuh"
 #include "tc_common.cuh"
@@ -40,135 +39,9 @@ struct SkParams {
   int M, N, K;
   int splits, k_iters;       // k_iters = 64-element chunks per split
   int force_partial;         // write fp32 partials even with one split (a fused finalize kernel consumes them)
-  // ---- in-kernel finalize ("tail"): once the `splits` CTAs of an N tile have all arrived on tail_cnt[tile], each of them
-  // sums the partials (in split order) of its share of the rows and applies the epilogue: no finalize kernel is launched
-  int tail;                  // 0 off; 1 plain (+R) -> out; 2 (+R) -> out, RMSNorm(out) * norm_w -> aux; 3 SiLU gating -> aux;
-                             // 4: SiLU gating in the epilogue itself (one split, weight rows interleaved a_0 b_0 a_1 b_1 ...)
-  int* tail_cnt;             // [n_tiles] arrivals per tile (per tile pair for SiLU) | [n_tiles] "seen" | done | passed; self-resetting
-  float* tail_ssq;           // [n_tiles][M] per-tile sums of squares of the stored bf16 row pieces (mode 2)
-  const __nv_bfloat16* norm_w;
-  __nv_bfloat16* aux;
-  float eps;
-  int kyutai;
+  int gate_interleaved;      // SiLU gating in the epilogue itself (one split, weight rows interleaved a_0 b_0 a_1 b_1 ...)
+  __nv_bfloat16* aux;        // [M][N/2] gated output (gate_interleaved)
 };
-
-// In-kernel finalize of one N tile, shared by the CTAs that computed its K slices: once all of them have arrived, CTA
-// `part` of `nparts` finalizes rows part, part + nparts, ... with its 128 epilogue threads (t = 0..127).  A warp takes one
-// row at a time: 32 lanes x 4 columns = the tile's 128 columns, so a row's sum of squares is one warp reduction; RB rows
-// and all splits are loaded before the first add (one L2 latency per batch, not per row).  Arithmetic as the stand-alone
-// finalize kernels below (partials added in split order, bf16 roundings in the same places).
-constexpr int SK_RB = 4;
-__device__ __forceinline__ void skinny_tail(const SkParams& p, int tile, int part, int nparts, int t) {
-  const int n_tiles = (int)gridDim.x;
-  const long long MN = (long long)p.M * p.N;
-  const int lane = t & 31, w = t >> 5;
-  const int I = p.N / 2;
-  const int n = tile * SK_BN + 4 * lane;
-  const bool nv = p.tail == 3 ? n < I : n < p.N;
-  auto row_of = [&](int j) { return part + nparts * (w + 4 * j); };
-  for (int j0 = 0; row_of(j0) < p.M; j0 += SK_RB) {
-    float4 v[SK_RB], u[SK_RB];
-#pragma unroll
-    for (int r = 0; r < SK_RB; ++r) v[r] = u[r] = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (nv) {
-#pragma unroll
-      for (int s = 0; s < 8; ++s) {
-        if (s < p.splits) {
-#pragma unroll
-          for (int r = 0; r < SK_RB; ++r) {
-            const int m = row_of(j0 + r);
-            if (m < p.M) {
-              const float* src = p.partial + (long long)s * MN + (long long)m * p.N + n;
-              const float4 a = __ldcg(reinterpret_cast<const float4*>(src));
-              v[r].x += a.x; v[r].y += a.y; v[r].z += a.z; v[r].w += a.w;
-              if (p.tail == 3) {
-                const float4 b = __ldcg(reinterpret_cast<const float4*>(src + I));
-                u[r].x += b.x; u[r].y += b.y; u[r].z += b.z; u[r].w += b.w;
-              }
-            }
-          }
-        }
-      }
-    }
-#pragma unroll
-    for (int r = 0; r < SK_RB; ++r) {
-      const int m = row_of(j0 + r);
-      if (m >= p.M) break;
-      if (p.tail == 3) {
-        if (nv) {
-          auto gate = [](float av, float bv) {
-            av = __bfloat162float(__float2bfloat16(av));
-            bv = __bfloat162float(__float2bfloat16(bv));
-            const float sl = __bfloat162float(__float2bfloat16(av / (1.0f + expf(-av))));
-            return sl * bv;
-          };
-          __nv_bfloat162* o2 = reinterpret_cast<__nv_bfloat162*>(p.aux + (long long)m * I + n);
-          o2[0] = __floats2bfloat162_rn(gate(v[r].x, u[r].x), gate(v[r].y, u[r].y));
-          o2[1] = __floats2bfloat162_rn(gate(v[r].z, u[r].z), gate(v[r].w, u[r].w));
-        }
-        continue;
-      }
-      float ss = 0.f;
-      if (nv) {
-        const long long i = (long long)m * p.N + n;
-        float4 x = v[r];
-        if (p.R) {
-          const __nv_bfloat162* r2 = reinterpret_cast<const __nv_bfloat162*>(p.R + i);
-          const float2 a = __bfloat1622float2(r2[0]), b = __bfloat1622float2(r2[1]);
-          x.x += a.x; x.y += a.y; x.z += b.x; x.w += b.y;
-        }
-        const __nv_bfloat162 lo = __floats2bfloat162_rn(x.x, x.y), hi = __floats2bfloat162_rn(x.z, x.w);
-        __nv_bfloat162* o2 = reinterpret_cast<__nv_bfloat162*>(p.out + i);
-        o2[0] = lo; o2[1] = hi;
-        const float2 fa = __bfloat1622float2(lo), fb = __bfloat1622float2(hi);  // the norm sees the stored bf16 values
-        ss = fmaf(fa.x, fa.x, ss); ss = fmaf(fa.y, fa.y, ss); ss = fmaf(fb.x, fb.x, ss); ss = fmaf(fb.y, fb.y, ss);
-      }
-      if (p.tail == 2) {
-        ss = warp_sum(ss);
-        if (lane == 0) p.tail_ssq[(long long)tile * p.M + m] = ss;
-      }
-    }
-  }
-  if (p.tail != 2) return;
-  // ---- RMSNorm needs whole rows: publish this CTA's sums, wait for every CTA of the grid (all co-resident: the plan
-  // takes this path only when n_tiles * splits <= 2 CTAs x SMs)
-  const int n_ctas = n_tiles * (int)gridDim.y;
-  int* done = p.tail_cnt + 2 * n_tiles;
-  int* passed = done + 1;
-  __threadfence();
-  named_bar_sync(1, 128);
-  if (t == 0) {
-    atomicAdd(done, 1);
-    while (*reinterpret_cast<volatile int*>(done) < n_ctas) __nanosleep(32);
-    __threadfence();
-  }
-  named_bar_sync(1, 128);
-  for (int j = 0; row_of(j) < p.M; ++j) {
-    const int m = row_of(j);
-    float tot = 0.f;
-    for (int tt = lane; tt < n_tiles; tt += 32) tot += __ldcg(p.tail_ssq + (long long)tt * p.M + m);
-    tot = warp_sum(tot);
-    const float mean = tot / (float)p.N;
-    const float r = p.kyutai ? rsqrtf(p.eps + mean) : rsqrtf(mean + p.eps);
-    if (nv) {
-      const long long i = (long long)m * p.N + n;
-      const __nv_bfloat162* x2 = reinterpret_cast<const __nv_bfloat162*>(p.out + i);
-      const __nv_bfloat162* w2 = reinterpret_cast<const __nv_bfloat162*>(p.norm_w + n);
-      const float2 xa = __bfloat1622float2(x2[0]), xb = __bfloat1622float2(x2[1]);
-      const float2 wa = __bfloat1622float2(w2[0]), wb = __bfloat1622float2(w2[1]);
-      float4 o;
-      if (p.kyutai) { o.x = xa.x * (wa.x * r); o.y = xa.y * (wa.y * r); o.z = xb.x * (wb.x * r); o.w = xb.y * (wb.y * r); }
-      else          { o.x = (xa.x * r) * wa.x; o.y = (xa.y * r) * wa.y; o.z = (xb.x * r) * wb.x; o.w = (xb.y * r) * wb.y; }
-      __nv_bfloat162* a2 = reinterpret_cast<__nv_bfloat162*>(p.aux + i);
-      a2[0] = __floats2bfloat162_rn(o.x, o.y);
-      a2[1] = __floats2bfloat162_rn(o.z, o.w);
-    }
-  }
-  if (t == 0) {
-    // every CTA has seen done == n_ctas before it counts itself here: the last one re-arms both counters
-    if (atomicAdd(passed, 1) == n_ctas - 1) { *done = 0; *passed = 0; }
-  }
-}
 
 // Thread roles (160 threads): warpgroup 0 = consumers (wgmma issue + epilogue), warp 4 = TMA producer.  A consumer
 // thread (warp wq, lane = 4 gq + tq) ends with the accumulators of weight rows n0 + 64 h + 16 wq + gq (+ 8), streams
@@ -200,9 +73,6 @@ gemm_skinny_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
     fence_barrier_init();
   }
   __syncthreads();
-  // everything above touched only this CTA's shared memory: it overlaps the tail of the previous kernel (PDL)
-  pdl_launch_dependents();
-  pdl_wait();
 
   if (warp == 4) {
     if (elect_one()) {
@@ -257,7 +127,7 @@ gemm_skinny_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
         for (int u = 0; u < 2; ++u) {
           const int m = 8 * b + 2 * tq + u;
           float v = c[4 * b + 2 * e + u];
-          if (p.tail == 4) {
+          if (p.gate_interleaved) {
             // rows 2j / 2j+1 of the interleaved weight are a_j / b_j: lanes 4 apart hold the gate and the value of
             // output column j, so SiLU gating needs one shuffle and no fp32 partials (gating.py:12-21; lit_model.py:399-403)
             const float o = __shfl_xor_sync(0xffffffffu, v, 4);
@@ -281,34 +151,11 @@ gemm_skinny_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
   };
   store(c0, 0);
   store(c1, 1);
-  if (p.tail && p.tail != 4) {
-    const int t = threadIdx.x;
-    const int n_tiles = (int)gridDim.x, half = n_tiles / 2;
-    const bool gate = p.tail == 3;             // SiLU: the a and b tiles of a column block are finalized together
-    const int cnt = gate ? (int)blockIdx.x % half : (int)blockIdx.x;
-    const int nparts = gate ? 2 * p.splits : p.splits;
-    const int part = gate ? 2 * (int)blockIdx.y + ((int)blockIdx.x >= half ? 1 : 0) : (int)blockIdx.y;
-    int* arrive = p.tail_cnt + cnt;
-    int* seen = p.tail_cnt + n_tiles + cnt;
-    __threadfence();                 // this CTA's partials are visible before its arrival is counted
-    named_bar_sync(1, 128);
-    if (t == 0) {
-      atomicAdd(arrive, 1);
-      while (*reinterpret_cast<volatile int*>(arrive) < nparts) __nanosleep(32);
-      // the last CTA to have seen the full count re-arms the pair of counters for the next launch
-      if (atomicAdd(seen, 1) == nparts - 1) { *arrive = 0; *seen = 0; }
-      __threadfence();
-    }
-    named_bar_sync(1, 128);
-    skinny_tail(p, cnt, part, nparts, t);
-  }
 }
 
 // plain finalize: out = bf16(sum_s partial[s] + R), 4 elements per thread (N % 4 == 0)
 __global__ void skinny_finalize_kernel(const float* __restrict__ partial, const __nv_bfloat16* __restrict__ R,
                                        __nv_bfloat16* __restrict__ out, long long MN, int splits) {
-  pdl_launch_dependents();
-  pdl_wait();
   const long long n4 = MN / 4;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
     float4 v = *reinterpret_cast<const float4*>(partial + 4 * i);
@@ -342,8 +189,6 @@ skinny_finalize_norm_kernel(const float* __restrict__ partial, const __nv_bfloat
   cg::cluster_group cluster = cg::this_cluster();
   __shared__ float red[32];
   __shared__ float slice_ss;
-  pdl_launch_dependents();
-  pdl_wait();
   const int m = blockIdx.x / FIN_CL, slice = (int)cluster.block_rank();
   const int n_lo = slice * (N / FIN_CL), n_hi = n_lo + N / FIN_CL;
   const long long MN = (long long)M * N;
@@ -399,8 +244,6 @@ skinny_finalize_norm_kernel(const float* __restrict__ partial, const __nv_bfloat
 // finalize + SiLU gating: aux[m][c] = bf16(silu(bf16(a)) ) * bf16(b) with a = cols [0,I), b = cols [I,2I) of the GEMM result
 __global__ void skinny_finalize_silu_kernel(const float* __restrict__ partial, __nv_bfloat16* __restrict__ aux, int M, int N,
                                             int splits) {
-  pdl_launch_dependents();
-  pdl_wait();
   const int I = N / 2;
   const long long MN = (long long)M * N, total = (long long)M * I;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
@@ -462,12 +305,11 @@ struct rstnet_skinny_plan {
   dim3 grid;
   size_t smem;
   int nb;        // wgmma N (streams rounded up)
-  int fin_mode;  // 0 plain, 1 finalize + residual + RMSNorm -> aux, 2 finalize + SiLU gating -> aux
+  int fin_mode;  // 0 plain, 1 finalize + residual + RMSNorm -> aux, 2 finalize + SiLU gating -> aux, 3 gating in the epilogue
   const __nv_bfloat16* norm_w;
   __nv_bfloat16* aux;
   float eps;
   int kyutai;
-  void* tail_mem;   // counters + per-tile sums of the in-kernel finalize (owned)
 };
 
 extern "C" int rstnet_skinny_gemm_create_fused(const void* X, const void* W, const void* R, void* out, float* partial_ws,
@@ -505,21 +347,14 @@ extern "C" int rstnet_skinny_gemm_create_fused(const void* X, const void* W, con
   int splits = 1;
   RSTNET_REQUIRE(!(partial_ws && max_splits > 1) || N % 4 == 0, "skinny_gemm_create: split-K needs N %% 4 == 0");
   if (partial_ws && max_splits > 1) {
-    // Enough CTAs to keep ~1.5 per SM streaming, no more: every split adds an fp32 partial round trip
-    // (scripts/skinny_sweep.py times GEMM + finalize per split factor and layer shape).
-    {
-      const int cand[6] = {1, 2, 3, 4, 6, 8};
-      const float want = 1.5f * (float)sm_count() / (float)n_tiles;
-      float best = 1e30f;
-      for (int c : cand) {
-        if (c > max_splits || (c > 1 && kchunks / c < 8)) continue;
-        const float r = (float)c > want ? (float)c / want : want / (float)c;
-        if (r < best) { best = r; splits = c; }
-      }
-    }
-    if (const char* e = getenv("RSTNET_SKINNY_SPLITS")) {   // tuning aid (scripts/skinny_sweep.py)
-      const int v = atoi(e);
-      if (v >= 1 && v <= max_splits) splits = v;
+    // Enough CTAs to keep ~1.5 per SM streaming, no more: every split adds an fp32 partial round trip.
+    const int cand[6] = {1, 2, 3, 4, 6, 8};
+    const float want = 1.5f * (float)sm_count() / (float)n_tiles;
+    float best = 1e30f;
+    for (int c : cand) {
+      if (c > max_splits || (c > 1 && kchunks / c < 8)) continue;
+      const float r = (float)c > want ? (float)c / want : want / (float)c;
+      if (r < best) { best = r; splits = c; }
     }
     // every split must own at least one K chunk (a CTA without work would never signal its accumulator)
     while (splits > 1 && (splits - 1) * ceil_div(kchunks, splits) >= kchunks) --splits;
@@ -545,6 +380,7 @@ extern "C" int rstnet_skinny_gemm_create_fused(const void* X, const void* W, con
   SkParams& p = pl->p;
   p.out = (__nv_bfloat16*)out; p.partial = partial_ws; p.R = (const __nv_bfloat16*)R;
   p.M = M; p.N = N; p.K = K; p.splits = splits;
+  p.gate_interleaved = fin_mode == 3; p.aux = (__nv_bfloat16*)aux_out;
   pl->nb = NB;
   pl->fin_mode = fin_mode; pl->norm_w = (const __nv_bfloat16*)norm_w; pl->aux = (__nv_bfloat16*)aux_out; pl->eps = eps; pl->kyutai = kyutai;
   // a fused finalize always reads fp32 partials, so the main kernel takes the split path even with one split
@@ -554,42 +390,6 @@ extern "C" int rstnet_skinny_gemm_create_fused(const void* X, const void* W, con
   // 4 stages (<= 98 KB with M <= 64): two CTAs fit per SM, so a GEMM whose tile count is not a multiple of the SM count
   // still keeps every SM streaming (bandwidth-bound CTAs progress at equal rates) and prologues overlap main loops
   pl->smem = (size_t)skinny_smem(NB);
-  // In-kernel finalize instead of a second launch: possible whenever fp32 partials are written, the grid is co-resident
-  // (every CTA waits for the other K slices of its tile, the RMSNorm tail for the whole grid) and, for SiLU, the a / b
-  // column blocks are whole tiles.  OPT-IN (RSTNET_SKINNY_TAIL=1), parity-tested, because it does not pay: the tail is a
-  // chain of ~6-8 dependent L2 round trips (release fence, arrival atomic, poll, partial loads, sums-of-squares exchange,
-  // stores), as long as the launch boundary it removes; on the small depth GEMMs it sits on every CTA's critical path.
-  p.tail = 0; p.tail_cnt = nullptr; p.tail_ssq = nullptr; pl->tail_mem = nullptr;
-  p.norm_w = pl->norm_w; p.aux = pl->aux; p.eps = eps; p.kyutai = kyutai;
-  {
-    static const bool tail_on = []() { const char* e = getenv("RSTNET_SKINNY_TAIL"); return e && e[0] == '1'; }();
-    const bool partials = splits > 1 || p.force_partial;
-    // every CTA waits for the other K slices of its tile (and, for RMSNorm, for the whole grid): the grid must be co-resident
-    const int sms = sm_count();
-    int per_sm = 0;
-    skinny_optin(NB);
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, skinny_kernel(NB), SK_THREADS, pl->smem) != cudaSuccess) {
-      cudaGetLastError();
-      per_sm = 0;
-    }
-    const bool resident = (long long)n_tiles * splits <= (long long)per_sm * sms;
-    const bool silu_ok = fin_mode != 2 || ((N / 2) % SK_BN == 0 && n_tiles % 2 == 0);
-    if (tail_on && partials && partial_ws && N % 4 == 0 && silu_ok && resident && splits <= 8) {
-      const size_t cnt_bytes = ((size_t)(2 * n_tiles + 2) * sizeof(int) + 15) & ~(size_t)15;
-      const size_t bytes = cnt_bytes + (size_t)n_tiles * M * sizeof(float);
-      if (cudaMalloc(&pl->tail_mem, bytes) != cudaSuccess || cudaMemset(pl->tail_mem, 0, bytes) != cudaSuccess) {
-        cudaGetLastError();
-        if (pl->tail_mem) cudaFree(pl->tail_mem);
-        delete pl;
-        set_error("skinny_gemm_create: could not allocate the finalize counters (%zu bytes)", bytes);
-        return 3;
-      }
-      p.tail = fin_mode == 1 ? 2 : (fin_mode == 2 ? 3 : 1);
-      p.tail_cnt = (int*)pl->tail_mem;
-      p.tail_ssq = (float*)((char*)pl->tail_mem + cnt_bytes);
-    }
-  }
-  if (fin_mode == 3) p.tail = 4;
   *outp = pl;
   return 0;
 }
@@ -598,28 +398,27 @@ extern "C" int rstnet_skinny_gemm_run(const rstnet_skinny_plan* pl, rstnet_strea
   RSTNET_REQUIRE(pl != nullptr, "skinny_gemm_run: null plan");
   skinny_optin(pl->nb);
   cudaStream_t st = (cudaStream_t)stream;
-  launch_pdl(skinny_kernel(pl->nb), pl->grid, dim3(SK_THREADS), pl->smem, st, pl->tmW, pl->tmX, pl->p);
+  skinny_kernel(pl->nb)<<<pl->grid, dim3(SK_THREADS), pl->smem, st>>>(pl->tmW, pl->tmX, pl->p);
   count_launch();
   if (int e = check_launch("gemm_skinny")) return e;
-  if (pl->p.tail) return 0;          // finalized inside the kernel
   const long long MN = (long long)pl->p.M * pl->p.N;
   if (pl->fin_mode == 1) {
-    launch_pdl(skinny_finalize_norm_kernel, dim3(pl->p.M * FIN_CL), dim3(256), 0, st, (const float*)pl->p.partial, pl->p.R, pl->p.out, pl->norm_w,
-               pl->aux, pl->p.M, pl->p.N, pl->p.splits, pl->eps, pl->kyutai);
+    skinny_finalize_norm_kernel<<<dim3(pl->p.M * FIN_CL), dim3(256), 0, st>>>((const float*)pl->p.partial, pl->p.R, pl->p.out, pl->norm_w,
+                                                                              pl->aux, pl->p.M, pl->p.N, pl->p.splits, pl->eps, pl->kyutai);
     count_launch();
     return check_launch("skinny_finalize_norm");
   }
   if (pl->fin_mode == 2) {
     int g = ceil_div(MN / 2, 256);
     if (g > sm_count() * 8) g = sm_count() * 8;
-    launch_pdl(skinny_finalize_silu_kernel, dim3(g), dim3(256), 0, st, (const float*)pl->p.partial, pl->aux, pl->p.M, pl->p.N, pl->p.splits);
+    skinny_finalize_silu_kernel<<<dim3(g), dim3(256), 0, st>>>((const float*)pl->p.partial, pl->aux, pl->p.M, pl->p.N, pl->p.splits);
     count_launch();
     return check_launch("skinny_finalize_silu");
   }
   if (pl->p.splits > 1) {
     int g = ceil_div(MN / 4, 256);
     if (g > sm_count() * 4) g = sm_count() * 4;
-    launch_pdl(skinny_finalize_kernel, dim3(g), dim3(256), 0, st, (const float*)pl->p.partial, pl->p.R, pl->p.out, MN, pl->p.splits);
+    skinny_finalize_kernel<<<dim3(g), dim3(256), 0, st>>>((const float*)pl->p.partial, pl->p.R, pl->p.out, MN, pl->p.splits);
     count_launch();
     return check_launch("skinny_finalize");
   }
@@ -627,7 +426,6 @@ extern "C" int rstnet_skinny_gemm_run(const rstnet_skinny_plan* pl, rstnet_strea
 }
 
 extern "C" void rstnet_skinny_gemm_destroy(rstnet_skinny_plan* pl) {
-  if (pl && pl->tail_mem) cudaFree(pl->tail_mem);
   delete pl;
 }
 extern "C" int64_t rstnet_skinny_gemm_workspace(int32_t M, int32_t N, int32_t max_splits) {

@@ -3,7 +3,6 @@
 // embedding gather, greedy / top-k sampling.  One token per stream (T == 1): rows are streams.
 #include <cuda_bf16.h>
 
-#include <cstdlib>
 #include "common.cuh"
 #include "../../include/rstnet_b200.h"
 
@@ -32,8 +31,6 @@ __device__ __forceinline__ bf16 f2b(float v) { return __float2bfloat16(v); }
 __global__ void embed_sum_kernel(const long long* __restrict__ seq, int seq_stride, const bf16* __restrict__ wte,
                                  const bf16* const* __restrict__ tables, int n_q, int E, bf16* __restrict__ x,
                                  long long wte_rows, long long table_rows) {
-  pdl_launch_dependents();
-  pdl_wait();
   const int b = blockIdx.x;
   const long long* ids = seq + (long long)b * seq_stride;
   bool bad = ids[0] < -1 || ids[0] >= wte_rows;
@@ -59,8 +56,6 @@ __global__ void embed_sum_kernel(const long long* __restrict__ seq, int seq_stri
 // out[b] = table[id[b]] (zero row for id < 0): depth-transformer token embeddings (llama_streaming.py:738-742)
 __global__ void embed_rows_kernel(const long long* __restrict__ ids, int id_stride, const bf16* __restrict__ table, int D,
                                   bf16* __restrict__ out, long long rows) {
-  pdl_launch_dependents();
-  pdl_wait();
   const int b = blockIdx.x;
   const long long id = ids[(long long)b * id_stride];
   const bool bad = id < -1 || id >= rows;
@@ -73,8 +68,6 @@ __global__ void embed_rows_kernel(const long long* __restrict__ ids, int id_stri
 // kyutai variant modules/transformer.py:34-48: var = eps + mean(x^2); y = x * (alpha * rsqrt(var)))
 __global__ void rms_norm_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w, bf16* __restrict__ y, int dim, float eps,
                                 int kyutai) {
-  pdl_launch_dependents();
-  pdl_wait();
   __shared__ float red[32];
   const int b = blockIdx.x;
   const bf16* xr = x + (long long)b * dim;
@@ -110,8 +103,6 @@ __global__ void rope_kv_append_bf16_kernel(const bf16* __restrict__ qkv, const b
                                            const long long* __restrict__ offset, bf16* __restrict__ q_out, bf16* __restrict__ kv,
                                            int ostride, int B, int n_kv, int q_per_kv, int hs, int cap, int rope_n,
                                            long long rope_rows) {
-  pdl_launch_dependents();
-  pdl_wait();
   const int row = blockIdx.x / n_kv, g = blockIdx.x % n_kv;
   const int b = row % B;
   const long long pos = offset[(long long)b * ostride] + row / B;   // per-stream counters (ostride 1) or one shared (0)
@@ -153,8 +144,6 @@ __global__ void rope_kv_append_bf16_kernel(const bf16* __restrict__ qkv, const b
 __global__ void rope_pair_kv_append_bf16_kernel(const bf16* __restrict__ qkv, const long long* __restrict__ offset, int ostride,
                                                 bf16* __restrict__ q_out, bf16* __restrict__ kv, int B, int H, int hd, int cap,
                                                 const float* __restrict__ freqs) {
-  pdl_launch_dependents();
-  pdl_wait();
   const int row = blockIdx.x / H, h = blockIdx.x % H;
   const int b = row % B;
   const long long off = offset[(long long)b * ostride];
@@ -188,45 +177,32 @@ __global__ void rope_pair_kv_append_bf16_kernel(const bf16* __restrict__ qkv, co
 // Mask = RingKVCache.complete + (pos_k>=0)&(delta>=0)&(delta<context) (llama_streaming.py:983-992).
 // Row r = tl*B + b queries stream b at position *offset + tl; all positions of the launch are already in the ring
 // (the caller guarantees no slot a query still needs has been overwritten: see GPT.forward_global's prefill path).
-// NS > 1 (key-split form): the work items are (row, head group, key chunk) triples walked by persistent CTAs
-// (item = blockIdx.x + i * gridDim.x), so the 2048 equal (stream, head) jobs of the 7B step no longer run as 4.6 waves of 444
-// resident CTAs (8 % of the kernel was an under-filled last wave) but as 13.8 rounds of thirds.  A chunk's unnormalised
-// (max, sum, acc[HS]) goes to `ws`; the CTA that completes a (row, head group) -- found with one atomic counter, reset for
-// the next launch -- combines the NS partials in chunk order, so the result does not depend on which CTA came last.
-// ST > 0: the K/V rows travel through a per-lane cp.async ring in shared memory, ST - 1 sweeps (of 32 keys per CTA) in
-// flight per warp instead of the one a register double buffer affords -- every lane copies and reads back only its own
-// 16-byte pieces, so cp.async.wait_group is the only synchronisation.
-template <int HS, int G, int NS, int ST>
-__global__ void __launch_bounds__(256, (G == 1 ? 3 : 2)) ring_decode_attention_kernel(const bf16* __restrict__ q, const bf16* __restrict__ kv,
+// The K/V rows travel through a per-lane cp.async ring in shared memory, ATT_STAGES - 1 sweeps (of 32 keys per CTA) in
+// flight per warp -- every lane copies and reads back only its own 16-byte pieces, so cp.async.wait_group is the only
+// synchronisation.
+constexpr int ATT_STAGES = 4;
+constexpr int ATT_WARPS = 8;
+template <int HS, int G>
+__global__ void __launch_bounds__(ATT_WARPS * 32, (G == 1 ? 3 : 2)) ring_decode_attention_kernel(const bf16* __restrict__ q, const bf16* __restrict__ kv,
                                                                     const long long* __restrict__ offset, bf16* __restrict__ out,
                                                                     int ostride, int B, int nh, int n_kv, int cap, int context,
-                                                                    float scale, int rows, float* __restrict__ ws, int* __restrict__ arrive) {
-  pdl_launch_dependents();
-  pdl_wait();
+                                                                    float scale) {
+  constexpr int ST = ATT_STAGES;
   constexpr int DPL = HS / 8;  // dims per lane
-  constexpr int PW = HS + 2;   // floats per partial: acc[HS], max, sum
-  __shared__ float sm_m[G][8], sm_l[G][8], sm_acc[G][8][HS];
-  __shared__ int sm_last;
+  __shared__ float sm_m[G][ATT_WARPS], sm_l[G][ATT_WARPS], sm_acc[G][ATT_WARPS][HS];
   const int nhg = nh / G;
-  const int n_items = rows * nhg * NS;
-  for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-  const int split = item % NS, hg = (item / NS) % nhg, row = item / (NS * nhg);
+  const int hg = blockIdx.x % nhg, row = blockIdx.x / nhg;
   const int h0 = hg * G;
   const int b = row % B;
   const int g = h0 / (nh / n_kv);
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   const int grp = lane / 8, sub = lane % 8;
-  const int nwarps = blockDim.x / 32;
+  constexpr int nwarps = ATT_WARPS;
   const long long pos = offset[(long long)b * ostride] + row / B;  // position of the query; its key/value were appended just before
   long long lo = pos - context + 1;
   if (lo < 0) lo = 0;
   if (lo < pos + 2 - cap) lo = pos + 2 - cap;  // ring quirk: the oldest slot is labelled end_offset and masked
-  const long long nkeys_all = pos - lo + 1;
-  const long long csz = NS == 1 ? nkeys_all : ((nkeys_all + NS - 1) / NS + 31) / 32 * 32;   // keys per chunk (whole 32-key sweeps)
-  lo += (long long)split * csz;
-  long long nkeys = nkeys_all - (long long)split * csz;
-  if (nkeys > csz) nkeys = csz;
-  if (nkeys < 0) nkeys = 0;
+  const long long nkeys = pos - lo + 1;
   const bf16* Kb = kv + ((long long)b * n_kv + g) * cap * HS;
   const bf16* Vb = Kb + (long long)B * n_kv * cap * HS;
   float qf[G][DPL];
@@ -245,11 +221,11 @@ __global__ void __launch_bounds__(256, (G == 1 ? 3 : 2)) ring_decode_attention_k
 #pragma unroll
     for (int i = 0; i < DPL; ++i) acc[u][i] = 0.f;
   }
-  // software pipeline: the K/V rows of the next iteration(s) are in flight while this one is reduced
+  // software pipeline: the K/V rows of the next iterations are in flight while this one is reduced
   constexpr int CH = DPL / 8;          // 16-byte pieces of a K (or V) row per lane
-  uint4 kr[CH], vr[CH], kn[ST > 0 ? 1 : CH], vn[ST > 0 ? 1 : CH];
+  uint4 kr[CH], vr[CH];
   extern __shared__ __align__(16) unsigned char attn_ring[];
-  uint4* ring = reinterpret_cast<uint4*>(attn_ring) + (ST > 0 ? warp * (ST * 2 * CH * 32) : 0);   // [stage][K pieces, V pieces][lane]
+  uint4* ring = reinterpret_cast<uint4*>(attn_ring) + warp * (ST * 2 * CH * 32);   // [stage][K pieces, V pieces][lane]
   auto issue_rows = [&](long long j0, int s) {
     const long long j = j0 + grp;
     const int slot = (int)((lo + (j < nkeys ? j : 0)) % cap);
@@ -261,42 +237,25 @@ __global__ void __launch_bounds__(256, (G == 1 ? 3 : 2)) ring_decode_attention_k
       cp_async16(&ring[(s * 2 * CH + CH + i) * 32 + lane], vp + i * 8, 16);
     }
   };
-  auto load_rows = [&](long long j0, uint4* kd, uint4* vd) {
-    const long long j = j0 + grp;
-    const int slot = (int)((lo + (j < nkeys ? j : 0)) % cap);
-    const uint4* kp = reinterpret_cast<const uint4*>(Kb + (long long)slot * HS) + sub;
-    const uint4* vp = reinterpret_cast<const uint4*>(Vb + (long long)slot * HS) + sub;
-#pragma unroll
-    for (int i = 0; i < DPL / 8; ++i) { kd[i] = __ldg(kp + i * 8); vd[i] = __ldg(vp + i * 8); }
-  };
   const long long jstep = (long long)nwarps * 4;
   long long j0 = (long long)warp * 4;
   int stage = 0;
-  if constexpr (ST > 0) {
 #pragma unroll
-    for (int s = 0; s < ST - 1; ++s) {
-      if (j0 + s * jstep < nkeys) issue_rows(j0 + s * jstep, s);
-      cp_async_commit();
-    }
-  } else {
-    if (j0 < nkeys) load_rows(j0, kr, vr);
+  for (int s = 0; s < ST - 1; ++s) {
+    if (j0 + s * jstep < nkeys) issue_rows(j0 + s * jstep, s);
+    cp_async_commit();
   }
   for (; j0 < nkeys; j0 += jstep) {
-    const bool more = j0 + jstep < nkeys;
-    if constexpr (ST > 0) {
-      const int sn = stage == 0 ? ST - 1 : stage - 1;       // the stage consumed in the previous iteration
-      if (j0 + (ST - 1) * jstep < nkeys) issue_rows(j0 + (ST - 1) * jstep, sn);
-      cp_async_commit();
-      cp_async_wait<ST - 1>();
+    const int sn = stage == 0 ? ST - 1 : stage - 1;       // the stage consumed in the previous iteration
+    if (j0 + (ST - 1) * jstep < nkeys) issue_rows(j0 + (ST - 1) * jstep, sn);
+    cp_async_commit();
+    cp_async_wait<ST - 1>();
 #pragma unroll
-      for (int i = 0; i < CH; ++i) {
-        kr[i] = ring[(stage * 2 * CH + i) * 32 + lane];
-        vr[i] = ring[(stage * 2 * CH + CH + i) * 32 + lane];
-      }
-      stage = stage + 1 == ST ? 0 : stage + 1;
-    } else {
-      if (more) load_rows(j0 + jstep, kn, vn);
+    for (int i = 0; i < CH; ++i) {
+      kr[i] = ring[(stage * 2 * CH + i) * 32 + lane];
+      vr[i] = ring[(stage * 2 * CH + CH + i) * 32 + lane];
     }
+    stage = stage + 1 == ST ? 0 : stage + 1;
     const bool valid = j0 + grp < nkeys;
     float dot[G];
 #pragma unroll
@@ -333,14 +292,8 @@ __global__ void __launch_bounds__(256, (G == 1 ? 3 : 2)) ring_decode_attention_k
         m[u] = m_new;
       }
     }
-    if constexpr (ST == 0) {
-      if (more) {
-#pragma unroll
-        for (int i = 0; i < DPL / 8; ++i) { kr[i] = kn[i]; vr[i] = vn[i]; }
-      }
-    }
   }
-  if constexpr (ST > 0) cp_async_wait<0>();
+  cp_async_wait<0>();
 #pragma unroll
   for (int u = 0; u < G; ++u) {
     // combine the 4 key groups of the warp (lanes sub, sub+8, sub+16, sub+24 hold the same dims)
@@ -372,53 +325,23 @@ __global__ void __launch_bounds__(256, (G == 1 ? 3 : 2)) ring_decode_attention_k
       ll += sm_l[u][w] * c;
       a += sm_acc[u][w][d] * c;
     }
-    if (NS == 1) {
-      out[((long long)row * nh + h0 + u) * HS + d] = f2b(a / ll);
-    } else {
-      float* pw = ws + ((long long)item * G + u) * PW;
-      pw[d] = a;
-      if (d == 0) { pw[HS] = mm; pw[HS + 1] = ll; }
-    }
+    out[((long long)row * nh + h0 + u) * HS + d] = f2b(a / ll);
   }
-  if (NS > 1) {
-    __threadfence();                 // this chunk's partial is visible before the arrival is counted
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      const int old = atomicAdd(&arrive[row * nhg + hg], 1);
-      sm_last = old == NS - 1;
-      if (sm_last) arrive[row * nhg + hg] = 0;      // ready for the next launch (all NS arrivals of this one are in)
-    }
-    __syncthreads();
-    if (sm_last) {
-      __threadfence();
-      const long long first = ((long long)(row * nhg + hg) * NS) * G;   // the NS partials of this (row, head group) are adjacent items
-      for (int idx = threadIdx.x; idx < G * HS; idx += blockDim.x) {
-        const int u = idx / HS, d = idx % HS;
-        float mm = -INFINITY;
-#pragma unroll
-        for (int sp = 0; sp < NS; ++sp) mm = fmaxf(mm, __ldcg(ws + (first + (long long)sp * G + u) * PW + HS));
-        float ll = 0.f, a = 0.f;
-#pragma unroll
-        for (int sp = 0; sp < NS; ++sp) {
-          const float* pw = ws + (first + (long long)sp * G + u) * PW;
-          const float ms = __ldcg(pw + HS);
-          const float c = ms == -INFINITY ? 0.f : __expf(ms - mm);
-          ll += __ldcg(pw + HS + 1) * c;
-          a += __ldcg(pw + d) * c;
-        }
-        out[((long long)row * nh + h0 + u) * HS + d] = f2b(a / ll);
-      }
-    }
-  }
-  __syncthreads();                   // the shared combine buffers are reused by the next item
-  }
+}
+
+// one CTA per (row, head group); the dynamic shared memory is the cp.async ring: stages x warps x lanes x (K, V pieces) x 16 B
+template <int HS, int G>
+void launch_ring_decode_attention(cudaStream_t st, const bf16* q, const bf16* kv, const long long* offset, bf16* out, int ostride,
+                                  int rows, int B, int nh, int n_kv, int cap, int context, float scale) {
+  constexpr int smem = ATT_STAGES * ATT_WARPS * 32 * (HS / 64) * 2 * 16;
+  static unsigned long long attr = 0;
+  smem_optin(ring_decode_attention_kernel<HS, G>, smem, attr);
+  ring_decode_attention_kernel<HS, G><<<rows * (nh / G), ATT_WARPS * 32, smem, st>>>(q, kv, offset, out, ostride, B, nh, n_kv, cap, context, scale);
 }
 
 // ---------------------------------------------------------------- SiLU gating: out = silu(a) * b  (bf16 roundings as eager)
 // ab [M][2*I] with a = cols [0,I), b = cols [I,2I) (fused fc_1|fc_2, or gating's view(B,T,2,-1), gating.py:16-19)
 __global__ void silu_mul_kernel(const bf16* __restrict__ ab, bf16* __restrict__ out, int M, int I) {
-  pdl_launch_dependents();
-  pdl_wait();
   const long long total = (long long)M * I;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const long long m = i / I, c = i % I;
@@ -434,8 +357,6 @@ __global__ void silu_mul_kernel(const bf16* __restrict__ ab, bf16* __restrict__ 
 // (forward_codecformer); 0: the non-streaming form (forward_local: KVCacheResult.from_kv keeps every key).
 __global__ void depth_attention_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ kvd, bf16* __restrict__ out, int B, int H,
                                        int hd, int cap, int step, int ring_quirk) {
-  pdl_launch_dependents();
-  pdl_wait();
   const int b = blockIdx.x / H, h = blockIdx.x % H;
   const int lane = threadIdx.x;
   const int HD = H * hd;
@@ -469,12 +390,221 @@ __global__ void depth_attention_kernel(const bf16* __restrict__ qkv, bf16* __res
   }
 }
 
-#include "lm_sample.cuh"
+// ---------------------------------------------------------------- sampling (utils/sampling.py:85-154)
+__device__ __forceinline__ uint32_t hash_u32(uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
+  uint32_t h = a * 0x9E3779B1u ^ (b + 0x7F4A7C15u) * 0x85EBCA77u ^ (c + 0x165667B1u) * 0xC2B2AE3Du ^ (d * 0x27D4EB2Fu);
+  h ^= h >> 16; h *= 0x7FEB352Du; h ^= h >> 15; h *= 0x846CA68Bu; h ^= h >> 16;
+  return h;
+}
+
+// logits [rows][V] bf16, candidates restricted to ids < n_valid.  top_k <= 0: argmax (first maximum).
+// top_k > 0: the top_k largest logits, weights exp((l - max)/temp), token = argmax_i w_i / Exp(1)_i
+// (= torch's exponential-noise multinomial over the top-k probabilities, sampling.py:43-46, 57-59).
+//
+// Large vocabularies (the 152k text head) first shrink the row to a candidate list: bf16 has 16 key bits, so two
+// 256-bin histogram passes give the exact key of the top_k-th largest logit; every logit with key >= that threshold
+// (top_k of them plus ties) is compacted into shared memory and the ordered selection below runs on the list instead
+// of re-scanning the row top_k times.  Same result as the full scan: (value desc, index asc) order.
+constexpr int SAMPLE_CAND = 1024;
+constexpr int SAMPLE_HISTS = 16;
+
+__device__ __forceinline__ uint32_t bf16_order_key(bf16 v) {
+  const uint32_t u = (uint32_t)__bfloat16_as_ushort(v);
+  return (u & 0x8000u) ? (~u & 0xFFFFu) : (u | 0x8000u);
+}
+
+// block-wide argmax in the order (value desc, index asc); every thread returns the winner
+__device__ __forceinline__ void block_argmax(float& bv, int& bi, float* s_val, int* s_idx) {
+  const int tid = threadIdx.x, nthr = blockDim.x;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+    if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+  }
+  __syncthreads();   // the previous round's readers are done with s_val / s_idx
+  if (tid % 32 == 0) { s_val[tid / 32] = bv; s_idx[tid / 32] = bi; }
+  __syncthreads();
+  if (tid < 32) {
+    bv = tid < nthr / 32 ? s_val[tid] : -INFINITY;
+    bi = tid < nthr / 32 ? s_idx[tid] : 0x7fffffff;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+      if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+    }
+    if (tid == 0) { s_val[0] = bv; s_idx[0] = bi; }
+  }
+  __syncthreads();
+  bv = s_val[0];
+  bi = s_idx[0];
+}
+
+__device__ __forceinline__ float gumbel_of(uint32_t seed, uint32_t stepc, uint32_t row, uint32_t id) {
+  const uint32_t u = hash_u32(seed, stepc, row, id);
+  const float uni = ((float)(u >> 8) + 0.5f) * (1.0f / 16777216.0f);  // (0,1)
+  return -logf(-logf(uni));   // argmax_i (l_i/temp + G_i)  ==  argmax_i softmax(l/temp)_i / Exp(1)_i
+}
+
+// top_k == 0: argmax.  1..64: ordered selection of the top-k (below), noise keyed by rank.  65..SAMPLE_CAND: threshold
+// select (the k largest by (value desc, index asc), found with the histogram + candidate list), noise keyed by token id.
+// top_k < 0: multinomial over all n_valid ids (sample_token with top_k == 0, utils/sampling.py:97-101).
+// All threads of the block call it (any block size that is a multiple of 32, <= 1024); writes *token_out.
+__device__ __noinline__ void sample_row(const bf16* __restrict__ lr, int n_valid, int top_k, float temp, uint32_t seed, uint32_t stepc,
+                                        int row, long long* __restrict__ token_out) {
+  __shared__ float s_val[32];
+  __shared__ int s_idx[32];
+  __shared__ float top_v[64];
+  __shared__ int top_i[64];
+  __shared__ int hist[SAMPLE_HISTS][256];
+  __shared__ float cand_v[SAMPLE_CAND];
+  __shared__ int cand_i[SAMPLE_CAND];
+  __shared__ int s_sel[5];   // [0] high-byte bin, [1] count above the threshold key, [2] threshold key, [3] candidate count, [4] ties taken
+  const int tid = threadIdx.x, nthr = blockDim.x;
+
+  if (top_k < 0) {   // full multinomial
+    float bv = -INFINITY;
+    int bi = 0x7fffffff;
+    const float inv_t = 1.0f / temp;
+    for (int i = tid; i < n_valid; i += nthr) {
+      const float sc = b2f(lr[i]) * inv_t + gumbel_of(seed, stepc, (uint32_t)row, (uint32_t)i);
+      if (sc > bv) { bv = sc; bi = i; }
+    }
+    block_argmax(bv, bi, s_val, s_idx);
+    if (tid == 0) *token_out = bi;
+    return;
+  }
+
+  const bool big = top_k > 64;
+  const int kk = top_k <= 0 ? 1 : (big ? top_k : top_k);
+  int n_items = n_valid;
+  bool from_list = false;
+  if (big || (kk > 1 && n_valid > 4 * SAMPLE_CAND)) {
+    int* myh = hist[(tid / 32) % SAMPLE_HISTS];
+    for (int pass = 0; pass < 2; ++pass) {
+      for (int i = tid; i < SAMPLE_HISTS * 256; i += nthr) (&hist[0][0])[i] = 0;
+      __syncthreads();
+      const int b1 = pass ? s_sel[0] : 0;
+      for (int i = tid; i < n_valid; i += nthr) {
+        const uint32_t k = bf16_order_key(lr[i]);
+        if (pass == 0) atomicAdd(&myh[k >> 8], 1);
+        else if ((int)(k >> 8) == b1) atomicAdd(&myh[k & 255u], 1);
+      }
+      __syncthreads();
+      if (tid < 256) {
+        int c = 0;
+#pragma unroll
+        for (int h = 0; h < SAMPLE_HISTS; ++h) c += hist[h][tid];
+        hist[0][tid] = c;
+      }
+      __syncthreads();
+      if (tid == 0) {
+        int above = pass ? s_sel[1] : 0, b = 255;
+        while (b > 0 && above + hist[0][b] < kk) { above += hist[0][b]; --b; }
+        if (pass == 0) { s_sel[0] = b; s_sel[1] = above; }
+        else { s_sel[2] = (s_sel[0] << 8) | b; s_sel[1] = above; s_sel[3] = 0; s_sel[4] = 0; }
+      }
+      __syncthreads();
+    }
+    const uint32_t thr = (uint32_t)s_sel[2];
+    for (int i = tid; i < n_valid; i += nthr) {
+      const bf16 v = lr[i];
+      if (bf16_order_key(v) >= thr) {
+        const int slot = atomicAdd(&s_sel[3], 1);
+        if (slot < SAMPLE_CAND) { cand_v[slot] = b2f(v); cand_i[slot] = i; }
+      }
+    }
+    __syncthreads();
+    if (s_sel[3] <= SAMPLE_CAND) { from_list = true; n_items = s_sel[3]; }   // else: massive ties at the threshold
+  }
+
+  if (big) {
+    const uint32_t thr = (uint32_t)s_sel[2];
+    const int above = s_sel[1];
+    const int need = kk - above;          // ties at the threshold to take, lowest ids first
+    const float inv_t = 1.0f / temp;
+    float bv = -INFINITY;
+    int bi = 0x7fffffff;
+    if (from_list) {
+      for (int t = tid; t < n_items; t += nthr) {
+        const float v = cand_v[t];
+        const int id = cand_i[t];
+        bool in = bf16_order_key(f2b(v)) > thr;
+        if (!in) {
+          int rank = 0;
+          for (int j = 0; j < n_items; ++j) rank += (cand_v[j] == v && cand_i[j] < id) ? 1 : 0;
+          in = rank < need;
+        }
+        if (in) {
+          const float sc = v * inv_t + gumbel_of(seed, stepc, (uint32_t)row, (uint32_t)id);
+          if (sc > bv || (sc == bv && id < bi)) { bv = sc; bi = id; }
+        }
+      }
+    } else {
+      // more than SAMPLE_CAND logits share the threshold value: walk the row in index order, counting ties
+      for (int base = 0; base < n_valid; base += nthr) {
+        const int i = base + tid;
+        const uint32_t k = i < n_valid ? bf16_order_key(lr[i]) : 0u;
+        const bool tie = i < n_valid && k == thr;
+        const unsigned bal = __ballot_sync(0xffffffffu, tie);
+        const int wpre = __popc(bal & ((1u << (tid % 32)) - 1u));
+        __syncthreads();
+        if (tid % 32 == 0) s_idx[tid / 32] = __popc(bal);
+        __syncthreads();
+        int before = s_sel[4];
+        for (int w = 0; w < tid / 32; ++w) before += s_idx[w];
+        const bool in = i < n_valid && (k > thr || (tie && before + wpre < need));
+        if (in) {
+          const float sc = b2f(lr[i]) * inv_t + gumbel_of(seed, stepc, (uint32_t)row, (uint32_t)i);
+          if (sc > bv || (sc == bv && i < bi)) { bv = sc; bi = i; }
+        }
+        __syncthreads();
+        if (tid == 0) { int t = 0; for (int w = 0; w < nthr / 32; ++w) t += s_idx[w]; s_sel[4] += t; }
+        __syncthreads();
+      }
+    }
+    block_argmax(bv, bi, s_val, s_idx);
+    if (tid == 0) *token_out = bi;
+    return;
+  }
+
+  float last_v = INFINITY;
+  int last_i = -1;
+  for (int r = 0; r < kk; ++r) {
+    // largest (value, lowest index) strictly after (last_v, last_i) in the order (value desc, index asc)
+    float bv = -INFINITY;
+    int bi = 0x7fffffff;
+    for (int i = tid; i < n_items; i += nthr) {
+      const float v = from_list ? cand_v[i] : b2f(lr[i]);
+      const int id = from_list ? cand_i[i] : i;
+      const bool after = v < last_v || (v == last_v && id > last_i);
+      if (after && (v > bv || (v == bv && id < bi))) { bv = v; bi = id; }
+    }
+    block_argmax(bv, bi, s_val, s_idx);
+    if (tid == 0) { top_v[r] = bv; top_i[r] = bi; }
+    last_v = bv;
+    last_i = bi;
+  }
+  if (tid == 0) {
+    int pick = top_i[0];
+    if (top_k > 0) {
+      float best = -INFINITY;
+      for (int r = 0; r < kk; ++r) {
+        const float w = expf((top_v[r] - top_v[0]) / temp);
+        const uint32_t u = hash_u32(seed, stepc, (uint32_t)row, (uint32_t)r);
+        const float uni = ((float)(u >> 8) + 0.5f) * (1.0f / 16777216.0f);  // (0,1)
+        const float e = -logf(uni);                                        // Exp(1)
+        const float score = w / e;
+        if (score > best) { best = score; pick = top_i[r]; }
+      }
+    }
+    *token_out = pick;
+  }
+}
 
 __global__ void sample_kernel(const bf16* __restrict__ logits, int V, int n_valid, int top_k, float temp, uint32_t seed,
                               const long long* __restrict__ step_counter, long long* __restrict__ tokens, int tok_stride) {
-  pdl_launch_dependents();
-  pdl_wait();
   const int row = blockIdx.x;
   const uint32_t stepc = step_counter ? (uint32_t)(*step_counter) : 0u;
   sample_row(logits + (long long)row * V, n_valid, top_k, temp, seed, stepc, row, tokens + (long long)row * tok_stride);
@@ -487,7 +617,7 @@ extern "C" int rstnet_lm_embed_sum_bf16(const int64_t* seq, int32_t seq_stride, 
                                         const void* const* tables_dev, int64_t table_rows, int32_t n_q, int32_t E, void* x,
                                         int32_t rows, rstnet_stream_t stream) {
   RSTNET_REQUIRE(seq && wte && tables_dev && x && rows > 0 && wte_rows > 0 && table_rows > 0, "lm_embed_sum: bad argument");
-  launch_pdl(embed_sum_kernel, dim3(rows), dim3(256), 0, (cudaStream_t)stream, (const long long*)seq, seq_stride, (const bf16*)wte,
+  embed_sum_kernel<<<dim3(rows), dim3(256), 0, (cudaStream_t)stream>>>((const long long*)seq, seq_stride, (const bf16*)wte,
              (const bf16* const*)tables_dev, n_q, E, (bf16*)x, (long long)wte_rows, (long long)table_rows);
   count_launch();
   return check_launch("lm_embed_sum");
@@ -496,7 +626,7 @@ extern "C" int rstnet_lm_embed_sum_bf16(const int64_t* seq, int32_t seq_stride, 
 extern "C" int rstnet_lm_embed_rows_bf16(const int64_t* ids, int32_t id_stride, const void* table, int64_t table_rows, int32_t D,
                                          void* out, int32_t rows, rstnet_stream_t stream) {
   RSTNET_REQUIRE(ids && table && out && rows > 0 && table_rows > 0, "lm_embed_rows: bad argument");
-  launch_pdl(embed_rows_kernel, dim3(rows), dim3(128), 0, (cudaStream_t)stream, (const long long*)ids, id_stride, (const bf16*)table, D,
+  embed_rows_kernel<<<dim3(rows), dim3(128), 0, (cudaStream_t)stream>>>((const long long*)ids, id_stride, (const bf16*)table, D,
              (bf16*)out, (long long)table_rows);
   count_launch();
   return check_launch("lm_embed_rows");
@@ -505,7 +635,7 @@ extern "C" int rstnet_lm_embed_rows_bf16(const int64_t* ids, int32_t id_stride, 
 extern "C" int rstnet_lm_rms_norm_bf16(const void* x, const void* w, void* y, int32_t rows, int32_t dim, float eps, int32_t kyutai,
                                        rstnet_stream_t stream) {
   RSTNET_REQUIRE(x && w && y && rows > 0 && dim > 0, "lm_rms_norm: bad argument");
-  launch_pdl(rms_norm_kernel, dim3(rows), dim3(256), 0, (cudaStream_t)stream, (const bf16*)x, (const bf16*)w, (bf16*)y, dim, eps, kyutai);
+  rms_norm_kernel<<<dim3(rows), dim3(256), 0, (cudaStream_t)stream>>>((const bf16*)x, (const bf16*)w, (bf16*)y, dim, eps, kyutai);
   count_launch();
   return check_launch("lm_rms_norm");
 }
@@ -518,7 +648,7 @@ extern "C" int rstnet_lm_rope_kv_append_bf16(const void* qkv, const void* cos_ta
   RSTNET_REQUIRE(rows > 0 && B > 0 && rows % B == 0, "lm_rope_kv_append: rows (%d) must be a multiple of the stream count (%d)", rows, B);
   RSTNET_REQUIRE(n_kv > 0 && n_head % n_kv == 0, "lm_rope_kv_append: n_head (%d) must be a multiple of n_kv (%d)", n_head, n_kv);
   RSTNET_REQUIRE(rope_n >= 0 && rope_n <= hs && rope_n % 2 == 0 && rope_rows > 0, "lm_rope_kv_append: bad rope table (%d of %d dims)", rope_n, hs);
-  launch_pdl(rope_kv_append_bf16_kernel, dim3(rows * n_kv), dim3(64), 0, (cudaStream_t)stream, (const bf16*)qkv, (const bf16*)cos_tab,
+  rope_kv_append_bf16_kernel<<<dim3(rows * n_kv), dim3(64), 0, (cudaStream_t)stream>>>((const bf16*)qkv, (const bf16*)cos_tab,
              (const bf16*)sin_tab, (const long long*)offset, (bf16*)q_out, (bf16*)kv, offset_stride ? 1 : 0, B, n_kv, n_head / n_kv, hs,
              cap, rope_n, (long long)rope_rows);
   count_launch();
@@ -530,20 +660,15 @@ extern "C" int rstnet_lm_rope_pair_kv_append_bf16(const void* qkv, const int64_t
                                                   rstnet_stream_t stream) {
   RSTNET_REQUIRE(qkv && offset && q_out && kv && freqs, "lm_rope_pair_kv_append: null pointer");
   RSTNET_REQUIRE(rows > 0 && B > 0 && rows % B == 0 && H > 0 && hd > 0 && hd % 2 == 0 && cap > 0, "lm_rope_pair_kv_append: bad shape");
-  launch_pdl(rope_pair_kv_append_bf16_kernel, dim3(rows * H), dim3(64), 0, (cudaStream_t)stream, (const bf16*)qkv,
+  rope_pair_kv_append_bf16_kernel<<<dim3(rows * H), dim3(64), 0, (cudaStream_t)stream>>>((const bf16*)qkv,
              (const long long*)offset, offset_stride ? 1 : 0, (bf16*)q_out, (bf16*)kv, B, H, hd, cap, freqs);
   count_launch();
   return check_launch("lm_rope_pair_kv_append");
 }
 
-extern "C" int64_t rstnet_lm_attention_split_workspace(int32_t rows, int32_t n_head, int32_t hs) {
-  // [rows * n_head] int32 arrival counters (zeroed by the caller once), then 3 partials of (hs + 2) floats per (row, head)
-  return (int64_t)rows * n_head * 4 + (int64_t)rows * n_head * 3 * (hs + 2) * 4;
-}
-
 extern "C" int rstnet_lm_ring_decode_attention_bf16(const void* q, const void* kv, const int64_t* offset, int32_t offset_stride,
                                                     void* out, int32_t rows, int32_t B, int32_t n_head, int32_t n_kv, int32_t hs,
-                                                    int32_t cap, int32_t context, void* split_ws, rstnet_stream_t stream) {
+                                                    int32_t cap, int32_t context, rstnet_stream_t stream) {
   RSTNET_REQUIRE(q && kv && offset && out, "lm_ring_decode_attention: null pointer");
   RSTNET_REQUIRE(hs == 128 || hs == 64, "lm_ring_decode_attention: head_size must be 64 or 128 (got %d)", hs);
   RSTNET_REQUIRE(rows > 0 && B > 0 && rows % B == 0, "lm_ring_decode_attention: rows (%d) must be a multiple of the stream count (%d)", rows, B);
@@ -551,37 +676,10 @@ extern "C" int rstnet_lm_ring_decode_attention_bf16(const void* q, const void* k
   const float scale = 1.0f / sqrtf((float)hs);
   const int q_per_kv = n_head / n_kv;
   const int G = q_per_kv % 2 == 0 ? 2 : 1;   // query heads per CTA sharing the K/V rows (the rest of a group hits L2)
-  cudaStream_t st = (cudaStream_t)stream;
-  const int sms = sm_count();
-  const int n_jobs = rows * (n_head / G);
-  int* arrive = (int*)split_ws;
-  float* ws = split_ws ? (float*)((char*)split_ws + (size_t)rows * n_head * 4) : nullptr;
-  // split the keys only when the jobs would leave a badly filled last wave of resident CTAs
-  const int resident = sms * (G == 1 ? 3 : 2);
-  // opt-in by passing split_ws (measured slower than one CTA per job at the 7B shapes, DESIGN.md): only when the jobs exceed one wave
-  const bool split = split_ws != nullptr && n_jobs > resident;
-  static const int ring_stages = []() { const char* e = getenv("RSTNET_ATTN_STAGES"); return e ? atoi(e) : 4; }();   // 0: register double buffer
-  const bool ring = ring_stages == 4 && !split;
-  const int ring_bytes = ring ? 4 * 8 * 32 * (hs / 64) * 2 * 16 : 0;   // stages x warps x lanes x (K, V pieces) x 16 B
-#define RSTNET_ATTN(HS_, G_)                                                                                                       \
-  do {                                                                                                                             \
-    if (split)                                                                                                                     \
-      launch_pdl(ring_decode_attention_kernel<HS_, G_, 3, 0>, dim3(resident), dim3(256), 0, st, (const bf16*)q, (const bf16*)kv,   \
-                 (const long long*)offset, (bf16*)out, offset_stride ? 1 : 0, B, n_head, n_kv, cap, context, scale, rows, ws, arrive); \
-    else if (ring) {                                                                                                               \
-      static unsigned long long attr = 0;                                                                                          \
-      smem_optin(ring_decode_attention_kernel<HS_, G_, 1, 4>, ring_bytes, attr);                                                   \
-      launch_pdl(ring_decode_attention_kernel<HS_, G_, 1, 4>, dim3(n_jobs), dim3(256), ring_bytes, st, (const bf16*)q,             \
-                 (const bf16*)kv, (const long long*)offset, (bf16*)out, offset_stride ? 1 : 0, B, n_head, n_kv, cap, context,      \
-                 scale, rows, (float*)nullptr, (int*)nullptr);                                                                     \
-    } else                                                                                                                         \
-      launch_pdl(ring_decode_attention_kernel<HS_, G_, 1, 0>, dim3(n_jobs), dim3(256), 0, st, (const bf16*)q, (const bf16*)kv,     \
-                 (const long long*)offset, (bf16*)out, offset_stride ? 1 : 0, B, n_head, n_kv, cap, context, scale, rows,          \
-                 (float*)nullptr, (int*)nullptr);                                                                                  \
-  } while (0)
-  if (hs == 128) { if (G == 2) RSTNET_ATTN(128, 2); else RSTNET_ATTN(128, 1); }
-  else           { if (G == 2) RSTNET_ATTN(64, 2); else RSTNET_ATTN(64, 1); }
-#undef RSTNET_ATTN
+  const auto launch = hs == 128 ? (G == 2 ? launch_ring_decode_attention<128, 2> : launch_ring_decode_attention<128, 1>)
+                                : (G == 2 ? launch_ring_decode_attention<64, 2> : launch_ring_decode_attention<64, 1>);
+  launch((cudaStream_t)stream, (const bf16*)q, (const bf16*)kv, (const long long*)offset, (bf16*)out, offset_stride ? 1 : 0, rows, B,
+         n_head, n_kv, cap, context, scale);
   count_launch();
   return check_launch("lm_ring_decode_attention");
 }
@@ -591,7 +689,7 @@ extern "C" int rstnet_lm_silu_mul_bf16(const void* ab, void* out, int32_t M, int
   const long long total = (long long)M * I;
   int g = ceil_div(total, 256);
   if (g > sm_count() * 8) g = sm_count() * 8;
-  launch_pdl(silu_mul_kernel, dim3(g), dim3(256), 0, (cudaStream_t)stream, (const bf16*)ab, (bf16*)out, M, I);
+  silu_mul_kernel<<<dim3(g), dim3(256), 0, (cudaStream_t)stream>>>((const bf16*)ab, (bf16*)out, M, I);
   count_launch();
   return check_launch("lm_silu_mul");
 }
@@ -600,7 +698,7 @@ extern "C" int rstnet_lm_depth_attention_bf16(const void* qkv, void* kvd, void* 
                                               int32_t step, int32_t ring_quirk, rstnet_stream_t stream) {
   RSTNET_REQUIRE(qkv && kvd && out, "lm_depth_attention: null pointer");
   RSTNET_REQUIRE(step >= 0 && step < cap && cap <= 8, "lm_depth_attention: step %d / capacity %d (<= 8) out of range", step, cap);
-  launch_pdl(depth_attention_kernel, dim3(B * H), dim3(32), 0, (cudaStream_t)stream, (const bf16*)qkv, (bf16*)kvd, (bf16*)out, B, H, hd, cap,
+  depth_attention_kernel<<<dim3(B * H), dim3(32), 0, (cudaStream_t)stream>>>((const bf16*)qkv, (bf16*)kvd, (bf16*)out, B, H, hd, cap,
              step, ring_quirk);
   count_launch();
   return check_launch("lm_depth_attention");
@@ -613,7 +711,7 @@ extern "C" int rstnet_lm_sample_bf16(const void* logits, int32_t rows, int32_t V
   RSTNET_REQUIRE(top_k <= SAMPLE_CAND && (top_k == 0 || temp > 0.f), "lm_sample: top_k <= %d and temp > 0 required (top_k=%d)", SAMPLE_CAND, top_k);
   if (n_valid <= 0 || n_valid > V) n_valid = V;
   if (top_k > n_valid) top_k = n_valid;   // torch.topk would raise; the whole support is the natural reading
-  launch_pdl(sample_kernel, dim3(rows), dim3(1024), 0, (cudaStream_t)stream, (const bf16*)logits, V, n_valid, top_k, temp, (uint32_t)seed,
+  sample_kernel<<<dim3(rows), dim3(1024), 0, (cudaStream_t)stream>>>((const bf16*)logits, V, n_valid, top_k, temp, (uint32_t)seed,
              (const long long*)step_counter, (long long*)tokens, tok_stride);
   count_launch();
   return check_launch("lm_sample");

@@ -21,7 +21,6 @@ dtype recipe of `GPT(config).to(device, bfloat16)` (infer_no_streaming.py:104-10
 from __future__ import annotations
 
 import ctypes as C
-import os
 from contextlib import contextmanager
 from dataclasses import dataclass
 from typing import Dict, Optional
@@ -88,10 +87,6 @@ class Config:
     def ff_hidden(self) -> int:  # modules/gating.py:40-43
         d, ff = self.codecformer_dim, self.codecformer_dim_feedforward
         return (21 * d) // 8 if ff == 4 * d else (2 * ff) // 3
-
-
-# A/B switch (tuning aid): RSTNET_LM_GATE_INTERLEAVE=0 packs fc_1 | fc_2 stacked and gates in a finalize kernel
-_GATE_INTERLEAVE = os.environ.get("RSTNET_LM_GATE_INTERLEAVE", "1") != "0"
 
 
 def interleave_gate_rows(w_gate: torch.Tensor, w_value: torch.Tensor) -> torch.Tensor:
@@ -247,15 +242,6 @@ class GPT(nn.Module):
         self._local_states: Dict[int, "_LMState"] = {}
         self._ns_state: Optional["_LMState"] = None      # scratch scope of the non-streaming forward_global
         self.use_cuda_graphs = True
-        # True: the depth transformer of a frame as ONE persistent cooperative kernel (csrc/lm_depth_frame.cu) instead of one
-        # launch per GEMM / attention / sampler.  Parity-tested but opt-in: the per-CTA activation-panel reads from L2,
-        # the mma.sync dependency chains and the 264 grid barriers of a frame do not overlap (time it with
-        # scripts/depth_timing.py before enabling it).
-        self.use_depth_frame_kernel = False
-        # True: the temporal attention cuts every (stream, head) job's keys in three chunks walked by persistent CTAs
-        # (csrc/lm_small.cu).  Removes the under-filled last wave but pays the per-job prologue/combine three times, which
-        # made it slower where it was timed (scripts/lm_attn_bench.py), so it is opt-in.
-        self.attention_key_split = False
 
     # parameter names of the depth transformer (the Moshi-style LMModel of rstnet_b200/moshi.py has the same structure under
     # other names, models/model.py:188-224)
@@ -427,14 +413,6 @@ class GPT(nn.Module):
         block_size): device code cannot raise, it poisons its output and sets a sticky flag (synchronises)."""
         with torch.cuda.device(self.device):
             flags = int(_lib.lib().rstnet_device_error_flags(int(clear)))
-            for st in [self._state] + list(self._local_states.values()):
-                if st is not None and getattr(st, "df", None) is not None:
-                    w = int(st.df_sync[1])
-                    flags |= (w & 1) | (8 if w & 4 else 0)
-                    if clear and w:
-                        st.df_sync[1] = 0
-        if flags & 8:
-            raise RuntimeError("the persistent depth-transformer kernel lost a CTA at its grid barrier (watchdog fired)")
         if flags & 1:
             raise IndexError("a token id was outside its embedding table (index out of range in self)")
         if flags & 2:
@@ -524,12 +502,6 @@ class GPT(nn.Module):
         raise NotImplementedError("training / teacher-forcing forward is out of scope; use forward_global / forward_local")
 
 
-def _attention_split_workspace(rows: int, n_head: int, hs: int, dev) -> torch.Tensor:
-    """Scratch of the key-split attention form (include/rstnet_b200.h): arrival counters (zero between launches) + partials."""
-    n = _lib.lib().rstnet_lm_attention_split_workspace(rows, n_head, hs)
-    return torch.zeros(n, dtype=torch.uint8, device=dev)
-
-
 class _LMState:
     """Buffers, KV rings, GEMM plans of one `streaming(B)` scope.  Rows of every activation buffer are (position,
     stream) pairs, position-major: row = tl * B + b.  The decode state has tn == 1; a prefill chunk state (`parent` set)
@@ -547,11 +519,7 @@ class _LMState:
         E, V, I, D, H = c.n_embd, c.padded_vocab_size, c.intermediate_size, c.codecformer_dim, c.ff_hidden
         nh, nkv, hs = c.n_head, c.n_query_groups, c.head_size
         self.cap = c.context
-        # the whole depth transformer of a frame as one persistent kernel (csrc/lm_depth_frame.cu) when the shapes allow
-        self.frame_kernel = (m.use_depth_frame_kernel and D % 128 == 0 and E % 128 == 0 and D <= 2048 and c.dep_q <= 8
-                             and c.codecformer_layers <= 8 and D % c.codecformer_heads == 0 and D // c.codecformer_heads <= 128)
-        gran = 128 if self.frame_kernel else 64
-        Hp = -(-H // gran) * gran  # the GEMMs' K granularity: pad the gating hidden size with zero weights
+        Hp = -(-H // 64) * 64  # the GEMMs' K granularity: pad the gating hidden size with zero weights
         self.Hp = Hp
 
         def z(*shape, dtype=bf):
@@ -560,27 +528,18 @@ class _LMState:
         if m._packed is None:
             pk = self._pack_temporal(P)
             # depth gating weights: K padded to the GEMM granularity.  They keep the stacked [gate; value] form + finalize
-            # kernel: with 44 column tiles the GEMM wants two K slices (scripts/skinny_sweep.py times the choices), which
-            # the in-epilogue gating cannot have.
-            for l in range(c.codecformer_layers if (Hp != H or self.frame_kernel) else 0):
+            # kernel: with 44 column tiles the GEMM's split-K heuristic picks two K slices, which the in-epilogue gating
+            # cannot have.
+            for l in range(c.codecformer_layers if Hp != H else 0):
                 for k in range(c.dep_q):
                     w_in = P[m._DN["dlayer"].format(l) + f".gating.{k}.linear_in.weight"]
                     w_out = P[m._DN["dlayer"].format(l) + f".gating.{k}.linear_out.weight"]
                     gi = z(2 * Hp, D)
                     gi[:H], gi[Hp:Hp + H] = w_in[:H], w_in[H:]
-                    if self.frame_kernel:
-                        # rows interleaved in 8-row groups [a_8u..8u+7 ; b_8u..8u+7]: one mma row block then holds a
-                        # gate / value pair per thread and SiLU gating happens in the GEMM's epilogue
-                        gi = torch.stack([gi[:Hp].view(Hp // 8, 8, D), gi[Hp:].view(Hp // 8, 8, D)], 1).reshape(2 * Hp, D).contiguous()
-                    go = w_out
-                    if Hp != H:
-                        go = z(D, Hp)
-                        go[:, :H] = w_out
+                    go = z(D, Hp)
+                    go[:, :H] = w_out
                     pk[f"gin.{l}.{k}"], pk[f"gout.{l}.{k}"] = gi, go
-            pk["frame_kernel"] = self.frame_kernel
             m._packed = pk
-        elif m._packed.get("frame_kernel") != self.frame_kernel:
-            raise RstnetError("use_depth_frame_kernel changed after the weights were packed; reload or move the model to repack")
         wsmax = max((nh + 2 * nkv) * hs, 2 * I, 4096, 3 * D, 2 * Hp)
         self.ws = parent.ws if parent is not None and parent.M >= M else torch.empty(8 * M * wsmax, dtype=torch.float32, device=dev)
         G = lambda X, W, out, R=None, **kw: SkinnyGemm(X, W, out, R, self.ws if W.shape[0] <= wsmax else None, **kw)
@@ -604,7 +563,6 @@ class _LMState:
             hd = D // c.codecformer_heads
             self.dkv_all = z(c.codecformer_layers, 2, M, c.codecformer_heads, c.dep_q, hd)
             self.dkv = [self.dkv_all[l] for l in range(c.codecformer_layers)]
-            self.df = None
             # depth transformer: per-codebook-step weight slabs
             DN = m._DN
             self.text_emb = P[DN["dtext"]]
@@ -613,7 +571,7 @@ class _LMState:
             a1 = [P[DN["dlayer"].format(l) + ".norm1.alpha"].view(-1) for l in range(Ld)]
             a2 = [P[DN["dlayer"].format(l) + ".norm2.alpha"].view(-1) for l in range(Ld)]
             self.dsteps = []
-            for k in range(c.dep_q if not self.frame_kernel else 0):
+            for k in range(c.dep_q):
                 layers = []
                 for l in range(Ld):
                     p = DN["dlayer"].format(l)
@@ -630,15 +588,10 @@ class _LMState:
                 self.dsteps.append(dict(
                     inp=G(self.tout, P[DN["din"].format(k)], self.dx, self.demb, norm_w=a1[0], aux=self.dn, eps=1e-8, kyutai=True),
                     layers=layers, head=G(self.dx, P[DN["dhead"].format(k)], self.dlogits)))
-            if self.frame_kernel:
-                self._build_depth_frame(P)
 
     def _pack_temporal(self, P):
-        """one-time repacked weights of the temporal transformer (fc_1 | fc_2 as one GEMM)"""
+        """one-time repacked weights of the temporal transformer (fc_1 and fc_2 interleaved as one GEMM)"""
         c = self.c
-        if not _GATE_INTERLEAVE:
-            return {f"fc12.{l}": torch.cat([P[f"transformer.h.{l}.mlp.fc_1.linear.weight"],
-                                            P[f"transformer.h.{l}.mlp.fc_2.linear.weight"]], 0).contiguous() for l in range(c.n_layer)}
         return {f"fc12.{l}": interleave_gate_rows(P[f"transformer.h.{l}.mlp.fc_1.linear.weight"],
                                                   P[f"transformer.h.{l}.mlp.fc_2.linear.weight"])
                 for l in range(c.n_layer)}
@@ -650,7 +603,6 @@ class _LMState:
         nh, nkv, hs = c.n_head, c.n_query_groups, c.head_size
         self.seq = z(M, c.n_q + 1, dtype=torch.int64)
         self.x, self.xn, self.q, self.att = z(M, E), z(M, E), z(M, nh * hs), z(M, nh * hs)
-        self.att_ws = _attention_split_workspace(M, nh, hs, dev) if m.attention_key_split else None
         self.qkv, self.hmid = z(M, (nh + 2 * nkv) * hs), z(M, I)
         self.out, self.logits = z(M, E), z(M, V)
         if parent is None:
@@ -694,62 +646,11 @@ class _LMState:
                 # x = attn + x ; xn = norm_2(x)   (Block.forward, llama_streaming.py:846-849) in the GEMM's finalize
                 proj=G(self.att, P[f"{p}.attn.proj.linear.weight"], self.x, self.x, norm_w=n2[l], aux=self.xn, eps=c.norm_eps),
                 # hmid = silu(fc_1 x) * fc_2 x   (LLaMAMLP, lit_model.py:399-403)
-                fc=G(self.xn, m._packed[f"fc12.{l}"], None, silu_out=self.hmid, interleaved=_GATE_INTERLEAVE),
+                fc=G(self.xn, m._packed[f"fc12.{l}"], None, silu_out=self.hmid, interleaved=True),
                 # x = mlp + x ; xn = norm_1 of the next block (or ln_f -> transformer_out)
                 down=G(self.hmid, P[f"{p}.mlp.proj.linear.weight"], self.x, self.x, norm_w=self.ln_f if last else n1[l + 1],
                        aux=self.out if last else self.xn, eps=c.norm_eps)))
         self.head = G(self.out, P["lm_head.linear.weight"], self.logits)
-
-    def _build_depth_frame(self, P):
-        c, M = self.c, self.M
-        D, E = c.codecformer_dim, c.n_embd
-        dev = self.tout.device
-        self.df_logits = torch.zeros(c.dep_q, M, c.audio_card, dtype=torch.bfloat16, device=dev)
-        self.df_ss = torch.zeros(D // 16, M, dtype=torch.float32, device=dev)
-        self.df_sync = torch.zeros(4, dtype=torch.int32, device=dev)        # [arrival counter, sticky error word, -, -]
-        self.df_nvalid = (C.c_int32 * 8)(*([c.audio_card] * 8))
-        d = _lib.DepthFrameDesc()
-        d.M, d.D, d.E, d.Hp, d.H, d.hd, d.Q, d.L = M, D, E, self.Hp, c.codecformer_heads, D // c.codecformer_heads, c.dep_q, c.codecformer_layers
-        d.card, d.tok_stride = c.audio_card, c.dep_q + 1
-        d.tout, d.x, d.qkv, d.att, d.dh = (t.data_ptr() for t in (self.tout, self.dx, self.dqkv, self.datt, self.dh))
-        d.logits, d.dkv, d.ss_part = self.df_logits.data_ptr(), self.dkv_all.data_ptr(), self.df_ss.data_ptr()
-        d.tokens, d.barrier = self.tokens.data_ptr(), self.df_sync.data_ptr()
-        pk = self.m._packed
-        for k in range(c.dep_q):
-            d.w_in[k] = P[self.m._DN["din"].format(k)].data_ptr()
-            tab = self.text_emb if k == 0 else self.dep_emb[k - 1]
-            d.emb[k], d.emb_rows[k] = tab.data_ptr(), tab.shape[0]
-            d.w_head[k] = P[self.m._DN["dhead"].format(k)].data_ptr()
-        for l in range(c.codecformer_layers):
-            p = self.m._DN["dlayer"].format(l)
-            d.w_qkv[l] = P[f"{p}.self_attn.in_proj_weight"].data_ptr()
-            d.w_out[l] = P[f"{p}.self_attn.out_proj.weight"].data_ptr()
-            d.a1[l], d.a2[l] = P[f"{p}.norm1.alpha"].data_ptr(), P[f"{p}.norm2.alpha"].data_ptr()
-            for k in range(c.dep_q):
-                d.w_gin[l * c.dep_q + k] = pk[f"gin.{l}.{k}"].data_ptr()
-                d.w_gout[l * c.dep_q + k] = pk[f"gout.{l}.{k}"].data_ptr()
-        h = C.c_void_p()
-        _lib.check(_lib.lib().rstnet_lm_depth_frame_create(C.byref(d), C.byref(h)), "depth_frame_create")
-        self.df = h
-
-    def _depth_frame(self, k0: int, k1: int, quirk: bool, sample: bool, top_k: int = 0, temp: float = 1.0, n_valid=None,
-                     step0_emb: Optional[torch.Tensor] = None):
-        if n_valid is not None:
-            for i, v in enumerate(n_valid):
-                self.df_nvalid[i] = int(v)
-        _lib.check(_lib.lib().rstnet_lm_depth_frame_run(self.df, k0, k1, int(quirk), int(sample), int(top_k), float(temp), self.seed,
-                                                        self.frame_counter.data_ptr(), self.df_nvalid,
-                                                        None if step0_emb is None else step0_emb.data_ptr(), ops._stream()),
-                   "depth_frame_run")
-
-    def __del__(self):
-        h = getattr(self, "df", None)
-        if h:
-            try:
-                _lib.lib().rstnet_lm_depth_frame_destroy(h)
-            except Exception:
-                pass
-            self.df = None
 
     def reset(self, streams=None):
         if streams is None:
@@ -783,7 +684,7 @@ class _LMState:
                        "rope_kv")
             _lib.check(L.rstnet_lm_ring_decode_attention_bf16(self.q.data_ptr(), self.kv[l].data_ptr(), self.offset.data_ptr(), ost,
                                                               self.att.data_ptr(), M, B, c.n_head, c.n_query_groups, c.head_size,
-                                                              self.cap, c.context, None if self.att_ws is None else self.att_ws.data_ptr(), st), "attention")
+                                                              self.cap, c.context, st), "attention")
             ly["proj"].run()   # + residual + norm_2 -> xn
             ly["fc"].run()     # + SiLU gating -> hmid
             ly["down"].run()   # + residual + next pre-norm -> xn (last layer: ln_f -> transformer_out)
@@ -904,11 +805,6 @@ class _LMState:
         if k != self.depth_step:
             raise RstnetError(f"depth steps must run in order: expected {self.depth_step}, got {k}")
         self.tout.copy_(transformer_out[:, 0])
-        if self.df is not None:
-            self.tokens[:, k].copy_(sequence[:, 0, 0])
-            self._replay(("depth", k), lambda: self._depth_frame(k, k + 1, True, False))
-            self.depth_step += 1
-            return self.df_logits[k].view(self.B, 1, 1, self.c.audio_card).clone()
         self._idbuf.copy_(sequence[:, 0, 0])
         self._replay(("depth", k), lambda: self._depth(k, self._idbuf, 1))
         self.depth_step += 1
@@ -919,13 +815,6 @@ class _LMState:
         (column k-1 feeds step k), tout [M, E]; writes out [M, dep_q, card]."""
         c = self.c
         self.tout.copy_(tout)
-        if self.df is not None:
-            # column k of `tokens` is the input token of step k: step 0 takes the features, step k >= 1 takes ids[:, k - 1]
-            self.tokens[:, 1:c.dep_q].copy_(ids[:, :c.dep_q - 1])
-            self.demb.copy_(start)
-            self._depth_frame(0, c.dep_q, False, False, step0_emb=self.demb)
-            out.copy_(self.df_logits.permute(1, 0, 2))
-            return
         self.tokens[:, :c.dep_q].copy_(ids)
         for k in range(c.dep_q):
             if k == 0:
@@ -954,12 +843,9 @@ class _LMState:
             self._temporal()
             self._sample(self.logits, c.padded_vocab_size, c.padded_vocab_size, tk_text, temp_text if sampling_text else 1.0, 0, 0)
             self.tout.copy_(self.out)
-            if self.df is not None:
-                self._depth_frame(0, c.dep_q, quirk, True, tk, temp if sampling else 1.0, [min(v, c.audio_card) for v in valid])
-            else:
-                for k in range(c.dep_q):
-                    self._depth(k, self.tokens[:, k], c.dep_q + 1, quirk=quirk)
-                    self._sample(self.dlogits, c.audio_card, min(valid[k], c.audio_card), tk, temp if sampling else 1.0, k + 1, k + 1)
+            for k in range(c.dep_q):
+                self._depth(k, self.tokens[:, k], c.dep_q + 1, quirk=quirk)
+                self._sample(self.dlogits, c.audio_card, min(valid[k], c.audio_card), tk, temp if sampling else 1.0, k + 1, k + 1)
             ops.counter_add(self.frame_counter, 1)
 
         self._replay(("frame", tk_text, float(temp_text), tk, float(temp), valid, bool(quirk)), frame)

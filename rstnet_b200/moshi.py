@@ -96,7 +96,7 @@ class _MoshiState(_LMState):
                                                             self.freqs.data_ptr(), st), "rope_pair_kv")
             _lib.check(L.rstnet_lm_ring_decode_attention_bf16(self.q.data_ptr(), self.kv[l].data_ptr(), self.offset.data_ptr(), 1,
                                                               self.att.data_ptr(), M, B, c.n_head, c.n_head, c.head_size, self.cap,
-                                                              c.context, None, st), "attention")
+                                                              c.context, st), "attention")
             ly["proj"].run()
             ly["fc"].run()
             ly["down"].run()
@@ -193,7 +193,6 @@ class LMModel(nn.Module):
         self._state: Optional[_MoshiState] = None
         self._packed = None
         self.use_cuda_graphs = True
-        self.use_depth_frame_kernel = False
 
     # ---- state_dict keys identical to the reference (`depformer.` lives under a private name: `depformer` is an API object)
     def state_dict(self, *a, **kw):

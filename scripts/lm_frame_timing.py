@@ -1,4 +1,4 @@
-"""Time one LM frame (7B shapes, B = 32, full 2048-key ring): temporal graph and whole-frame graph.  RSTNET_PDL=0/1."""
+"""Time one LM frame (7B shapes, B = 32, full 2048-key ring): temporal graph and whole-frame graph."""
 import json
 import os
 import sys
@@ -32,7 +32,7 @@ with m.streaming(B):
         kv.normal_()
     st.offset.fill_(2100); st.pos_host[:] = 2100
     seq = torch.randint(0, 2048, (B, 9, 1), device=dev)
-    r = {"pdl": os.environ.get("RSTNET_PDL", "1"), "B": B}
+    r = {"B": B}
     r["temporal_graph_ms"] = timeit(lambda: (st._replay(("temporal",), st._temporal)))
     st.offset.fill_(2100)
     r["frame_graph_ms"] = timeit(lambda: m.forward_step(seq))

@@ -27,7 +27,7 @@ __device__ __forceinline__ bf16 f2b(float v) { return __float2bfloat16(v); }
 // x[b] = ((e_0 + e_1) + ... + e_{nq-1}) + wte[text]; every add rounds to bf16 as the eager bf16 model does;
 // id -1 contributes an exact zero row (ScaledEmbedding, :505-517).
 // nn.Embedding raises on ids outside the table; here such an id (anything but the zero token -1 below 0, or >= rows)
-// yields a NaN row and sets error bit 1.
+// yields a NaN row and sets error bit 0 (1).
 __global__ void embed_sum_kernel(const long long* __restrict__ seq, int seq_stride, const bf16* __restrict__ wte,
                                  const bf16* const* __restrict__ tables, int n_q, int E, bf16* __restrict__ x,
                                  long long wte_rows, long long table_rows) {
@@ -98,7 +98,7 @@ __global__ void rms_norm_kernel(const bf16* __restrict__ x, const bf16* __restri
 // writes rotated q to q_out [row][n_head*hs] (head h = g*q_per_kv + j), rotated k and v into kv[2][B][n_kv][cap][hs] at
 // slot (pos % cap)  (lit_model.py:560-573, 620-634).  Only the first rope_n dims rotate (rotary_percentage < 1,
 // llama_streaming.py:979-982); the tables are [rope_rows][rope_n].  A position beyond the tables (the reference's
-// cos.index_select would raise) poisons q/k with NaN and sets error bit 2.
+// cos.index_select would raise) poisons q/k with NaN and sets error bit 1 (2).
 __global__ void rope_kv_append_bf16_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ cosb, const bf16* __restrict__ sinb,
                                            const long long* __restrict__ offset, bf16* __restrict__ q_out, bf16* __restrict__ kv,
                                            int ostride, int B, int n_kv, int q_per_kv, int hs, int cap, int rope_n,

@@ -213,7 +213,7 @@ __global__ void rvq_finish_kernel(const float* __restrict__ pval, const int* __r
 }
 
 // Sticky device-side error word (rstnet_device_error_flags): F.embedding raises on a code outside [0, bins); here the
-// code is clamped (no out-of-bounds read) and bit 1 is set.
+// code is clamped (no out-of-bounds read) and bit 0 (1) is set.
 __device__ unsigned int g_rvq_dev_err = 0;
 unsigned int rvq_read_errors(bool clear) {
   unsigned int v = 0;

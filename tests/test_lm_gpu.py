@@ -11,6 +11,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+import test_lm_kernels_gpu as KT
 from oracle import lm_oracle as L
 from rstnet_b200 import _lib, ops
 from rstnet_b200.lm import GPT, Config, SkinnyGemm
@@ -30,24 +31,34 @@ def _rel(a, b):
     return float((a - b).abs().max() / b.abs().max().clamp(min=1e-6))
 
 
-@pytest.mark.parametrize("M,K,N,res", [(64, 4096, 512, False), (64, 256, 768, False), (3, 256, 152064 // 64, True), (64, 11008, 256, True),
-                                       (17, 1024, 2050, False), (64, 2816, 1024, True), (128, 512, 640, False)])
-def test_skinny_gemm_vs_torch(M, K, N, res):
+@pytest.mark.parametrize("M,K,N,res,max_splits", [
+    (64, 4096, 512, False, 8), (64, 256, 768, False, 8), (3, 256, 152064 // 64, True, 8), (64, 11008, 256, True, 8),
+    (17, 1024, 2050, False, 8), (64, 2816, 1024, True, 8), (128, 512, 640, False, 8),
+    # M = 1, 16, 17, 33, 64, 65, 128: every wgmma N instantiation and its padding.  K = 64 * 67: no split count divides the
+    # 67 chunks and every count leaves >= 8 per slice, so max_splits forces 1, 2, 3, 4, 6 and 8 slices with ragged last ones.
+    # K = 64: one chunk.  N % 128 != 0 throughout; N % 4 != 0 cannot split.  R aliases out as in lm.py's residual stream.
+    (1, 4288, 1000, True, 8), (16, 4288, 1000, False, 6), (17, 4288, 1000, True, 3), (33, 4288, 1000, True, 4),
+    (64, 4288, 2600, False, 2), (65, 4288, 1000, True, 8), (128, 4288, 640, True, 6), (17, 4288, 1000, False, 1),
+    (65, 4288, 1000, False, 2), (16, 4288, 2600, True, 3), (33, 4288, 2047, False, 8), (1, 64, 130, True, 8),
+    (64, 64, 1000, True, 1), (128, 64, 1000, False, 8)])
+def test_skinny_gemm_vs_torch(M, K, N, res, max_splits):
+    """fin_mode 0 vs float64 under the per-element bound of test_lm_kernels_gpu.py.  The workspace is NaN before the run,
+    so the K slices that wrote partials show the split count that actually ran; it must be the one max_splits forces."""
     g = torch.Generator().manual_seed(M + K + N)
     x = torch.randn(M, K, generator=g).to(BF)
     w = (torch.randn(N, K, generator=g) / K ** 0.5).to(BF)
     r = torch.randn(M, N, generator=g).to(BF) if res else None
-    ref = x.float() @ w.float().t()
-    if res:
-        ref = ref + r.float()
+    ref, S = KT.gemm_ref(x, w, r)
     xd, wd = x.to(DEV), w.to(DEV)
-    out = r.to(DEV).clone() if res else torch.empty(M, N, dtype=BF, device=DEV)
-    ws = torch.empty(8 * M * N, dtype=torch.float32, device=DEV)
-    plan = SkinnyGemm(xd, wd, out, out if res else None, ws)
+    out = r.to(DEV).clone() if res else torch.full((M, N), float("nan"), dtype=BF, device=DEV)
+    ws = torch.full((max_splits * M * N,), float("nan"), dtype=torch.float32, device=DEV)
+    plan = SkinnyGemm(xd, wd, out, out if res else None, ws, max_splits=max_splits)
     plan.run()
     torch.cuda.synchronize()
-    err = (out.float().cpu() - ref).abs().max().item()
-    assert err <= 2e-2 * max(1.0, ref.abs().max().item()), err
+    n = KT.k_slices_written(ws, M, N, max_splits)
+    assert n != 1, "a single K slice writes out directly, not through the workspace"
+    assert max(n, 1) == KT.forced_splits(N, K, max_splits), n
+    KT.check_bound(f"skinny fin_mode 0 M {M} K {K} N {N} splits {max(n, 1)}", out, ref, KT.GEMM_C * S, 0.99)
 
 
 @pytest.mark.parametrize("M,K,I", [(64, 1024, 2816), (5, 256, 96), (128, 512, 704)])
@@ -529,36 +540,33 @@ def test_cfg3_shape_wrapped_ring_vs_reference_eager_on_gpu():
 
 @pytest.mark.parametrize("B", [4, 64, 37, 128])
 def test_attention_full_window_2047_keys_vs_sdpa(B):
-    """ring_decode_attention at head 128, capacity 2048, wrapped: vs SDPA over exactly the keys RingKVCache.complete
-    leaves attendable (MHA and a GQA grouping).  B > 8 puts streams at different fill levels (few keys, partially filled
-    ring, wrapped) in one launch; B = 128 is the most rows one launch takes (lm.MAX_ROWS)."""
+    """ring_decode_attention at capacity 2048, wrapped, vs a float64 softmax over exactly the keys RingKVCache.complete
+    leaves attendable, under the per-element bound of test_lm_kernels_gpu.py: MHA, GQA with an even and an odd q_per_kv
+    (12 / 4 runs one query head per CTA with n_kv < n_head), MQA, head size 64, and windows shorter than the ring
+    (context < cap).  B > 8 puts streams at different fill levels (few keys, partially filled ring, wrapped) in one launch;
+    B = 128 is the most rows one launch takes (lm.MAX_ROWS)."""
     lib, st_ = _lib.lib(), ops._stream()
-    hs, cap = 128, 2048
-    g = torch.Generator().manual_seed(9)
-    for nh, nkv in ((8, 8), (16, 4)):
-        kv = torch.randn(2, B, nkv, cap, hs, generator=g).to(BF).to(DEV)
-        q = torch.randn(B, nh, hs, generator=g).to(BF).to(DEV)
+    cap = 2048
+    g = torch.Generator(device=DEV).manual_seed(9)
+    for nh, nkv, hs, context in ((8, 8, 128, cap), (16, 4, 128, cap), (12, 4, 128, 1500), (8, 1, 128, cap), (8, 4, 64, 300)):
+        kv = torch.randn(2, B, nkv, cap, hs, generator=g, device=DEV).to(BF)
+        q = torch.randn(B, nh, hs, generator=g, device=DEV).to(BF)
         pos_b = torch.full((B,), cap + 100, dtype=torch.int64)  # the query's own key sits at slot pos % cap
         if B > 8:
             pos_b[1], pos_b[2], pos_b[3], pos_b[4] = 0, 5, 40, 1000
         offset = pos_b.to(DEV)
-        out = torch.zeros(B, nh * hs, dtype=BF, device=DEV)
+        out = torch.full((B, nh * hs), float("nan"), dtype=BF, device=DEV)
         _lib.check(lib.rstnet_lm_ring_decode_attention_bf16(q.data_ptr(), kv.data_ptr(), offset.data_ptr(), 1, out.data_ptr(), B, B,
-                                                            nh, nkv, hs, cap, cap, st_))
-        slots = torch.arange(cap, device=DEV)
-        k_, v_ = kv[0].float(), kv[1].float()
+                                                            nh, nkv, hs, cap, context, st_))
         rep = nh // nkv
-        k_, v_ = k_.repeat_interleave(rep, 1), v_.repeat_interleave(rep, 1)
-        mask = torch.zeros(B, 1, 1, cap, dtype=torch.bool, device=DEV)
+        ref = torch.empty(B, nh, hs, dtype=torch.float64, device=DEV)
+        slack = torch.empty(B, nh, 1, dtype=torch.float64, device=DEV)
         for b in range(B):
-            pos = int(pos_b[b])
-            if pos >= cap - 1:
-                mask[b, 0, 0] = slots != (pos + 1) % cap        # labelled end_offset -> masked (the ring quirk)
-            else:
-                mask[b, 0, 0] = slots <= pos
-        ref = F.scaled_dot_product_attention(q.float()[:, :, None], k_, v_, attn_mask=mask, scale=1.0 / hs ** 0.5)[:, :, 0]
-        err = (out.float().view(B, nh, hs) - ref).abs().max().item()
-        assert err <= 1.5e-2, (nh, nkv, err)
+            keys = KT.ring_keys(int(pos_b[b]), cap, context).to(DEV)
+            k_, v_ = kv[0, b][:, keys], kv[1, b][:, keys]                      # [n_kv, keys, hs]; head h = g * rep + j
+            ref[b] = KT.softmax_attention64(q[b].view(nkv, rep, hs), k_, v_, hs ** -0.5).reshape(nh, hs)
+            slack[b] = KT.ATTN_C * v_.double().abs().amax((1, 2)).repeat_interleave(rep)[:, None]
+        KT.check_bound(f"ring attention nh {nh} n_kv {nkv} hs {hs} context {context} B {B}", out.view(B, nh, hs), ref, slack, 0.98)
 
 
 def test_per_stream_reset_and_state_swap(small_lm):

@@ -227,7 +227,8 @@ int rstnet_rvq_decode_gather_f32(const int64_t* codes, const float* E, float* q,
  * in LoRAQKVLinear/LoRALinear after merge (llama_streaming.py:113-143, 368-406), LLaMAMLP
  * (lit_model.py:399-403), lm_head (:691), codecformer_in / multi_linear / gating / audio_linears
  * (llama_streaming.py:727-749, modules/transformer.py:155-179, modules/gating.py:12-21).
- * 1 <= M <= 128, K % 64 == 0.  The plan embeds the pointers. */
+ * 1 <= M <= 256, K % 64 == 0 (M > 256 is rejected); each weight tile is read once for all M rows (wgmma N = M
+ * rounded up to 16, 32, 64, 128 or 256).  The plan embeds the pointers. */
 typedef struct rstnet_skinny_plan rstnet_skinny_plan;
 int64_t rstnet_skinny_gemm_workspace(int32_t M, int32_t N, int32_t max_splits);
 int rstnet_skinny_gemm_create(const void* X, const void* W, const void* R, void* out, float* partial_ws,

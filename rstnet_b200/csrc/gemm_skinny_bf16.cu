@@ -1,11 +1,12 @@
 // Weight-streaming skinny GEMM for the LM decode step (wgmma, bf16 operands, fp32 accumulate in
-// registers):   out[m, n] = sum_k X[m, k] * W[n, k]  (+ R[m, n]),   M = concurrent streams (<= 128).
+// registers):   out[m, n] = sum_k X[m, k] * W[n, k]  (+ R[m, n]),   M = concurrent streams (<= 256).
 //
 // The step is HBM-bound (each bf16 weight is used for M MACs), so the design goal is to keep
 // every SM pulling weight tiles at full rate: the weight matrix is the MMA "A" operand (128 rows of
-// W per CTA = two m64 wgmmas), the activations are the "B" operand (wgmma N = M rounded up to 16, 32, 64 or 128), both
-// K-major exactly as nn.Linear stores them, 4-stage TMA ring of 128x64 bf16 weight tiles, two CTAs per SM, and
-// split-K across CTAs when N/128 alone cannot fill the machine (fp32 partials + finalize kernel).
+// W per CTA = two m64 wgmmas), the activations are the "B" operand (wgmma N = M rounded up to 16, 32, 64, 128 or 256),
+// both K-major exactly as nn.Linear stores them, 4-stage TMA ring of 128x64 bf16 weight tiles, and split-K across CTAs
+// when N/128 alone cannot fill the machine (fp32 partials + finalize kernel).  Every weight tile is read once for all M
+// streams: 256 streams cost one pass over the weights, not two.
 // Replaces F.linear in CausalSelfAttention / LLaMAMLP / lm_head (models/llama_streaming.py:935-998,
 // models/lit_model.py:399-403) and in the depth transformer (modules/transformer.py:155-179, gating.py:12-21).
 #include <cuda_bf16.h>
@@ -23,11 +24,15 @@ using namespace tc;
 constexpr int SK_BN = 128;      // weight rows per CTA (two m64 wgmmas)
 constexpr int SK_BK = 64;       // bf16 elements per 128-byte swizzle row
 constexpr int SK_W_BYTES = SK_BN * 128;
-constexpr int SK_THREADS = 160; // one consumer warpgroup + the TMA warp
 constexpr int SK_STAGES = 4;
 
-template <int NB>   // wgmma N: streams rounded up to 16, 32, 64 or 128
+template <int NB>   // wgmma N: streams rounded up to 16, 32, 64, 128 or 256
 struct SkCfg {
+  // consumer warpgroups: a 64 x 256 fp32 accumulator is 128 registers per thread, so at NB = 256 each of two warpgroups
+  // owns one 64-row half of the weight tile; below, one warpgroup holds both halves
+  static constexpr int WG = NB > 128 ? 2 : 1;
+  static constexpr int THREADS = 128 * WG + 32;   // + the TMA warp
+  static constexpr int MIN_BLOCKS = WG == 1 ? 2 : 1;
   static constexpr int STAGE_BYTES = SK_W_BYTES + ((NB * 128 + 1023) & ~1023);
   static constexpr int SMEM_BYTES = SK_STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
 };
@@ -43,12 +48,15 @@ struct SkParams {
   __nv_bfloat16* aux;        // [M][N/2] gated output (gate_interleaved)
 };
 
-// Thread roles (160 threads): warpgroup 0 = consumers (wgmma issue + epilogue), warp 4 = TMA producer.  A consumer
-// thread (warp wq, lane = 4 gq + tq) ends with the accumulators of weight rows n0 + 64 h + 16 wq + gq (+ 8), streams
-// 8 b + 2 tq (+ 1) for both 64-row halves h.
+// Thread roles (160 threads, NB <= 128): warpgroup 0 = consumers (wgmma issue + epilogue), warp 4 = TMA producer.  A
+// consumer thread (warp wq, lane = 4 gq + tq) ends with the accumulators of weight rows n0 + 64 h + 16 wq + gq (+ 8),
+// streams 8 b + 2 tq (+ 1) for both 64-row halves h.
+// NB = 256 (288 threads): warpgroups 0 and 1 are consumers, warpgroup h owning half h only (wq = warp % 4, same row and
+// stream mapping), and warp 8 is the TMA producer.  Both warpgroups read the stage's one X tile.
 template <int NB>
-__global__ void __launch_bounds__(SK_THREADS, 2)
+__global__ void __launch_bounds__(SkCfg<NB>::THREADS, SkCfg<NB>::MIN_BLOCKS)
 gemm_skinny_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX, const SkParams p) {
+  constexpr int WG = SkCfg<NB>::WG;
   constexpr int STAGES = SK_STAGES;
   constexpr int STAGE_BYTES = SkCfg<NB>::STAGE_BYTES;
   constexpr int NR = NB / 2;   // accumulator registers per thread of one 64 x NB wgmma
@@ -68,13 +76,13 @@ gemm_skinny_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 4);   // one arrival per consumer warp
+      mbar_init(&empty[s], 4 * WG);   // one arrival per consumer warp
     }
     fence_barrier_init();
   }
   __syncthreads();
 
-  if (warp == 4) {
+  if (warp == 4 * WG) {
     if (elect_one()) {
       tma_prefetch_desc(&tmW);
       tma_prefetch_desc(&tmX);
@@ -90,36 +98,39 @@ gemm_skinny_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
     return;
   }
 
-  float c0[NR], c1[NR];   // weight rows [0, 64) and [64, 128) of the tile
+  // weight rows [0, 64) and [64, 128) of the tile; with two warpgroups, c0 holds the warpgroup's own half and c1 is unused
+  float c0[NR], c1[NR];
 #pragma unroll
   for (int j = 0; j < NR; ++j) c0[j] = c1[j] = 0.f;
   const uint32_t smem0 = smem_u32(smem);
+  const uint32_t half0 = WG == 1 ? 0u : (uint32_t)(warp / 4) * (64 * 128);
   for (int kit = 0; kit < k_count; ++kit) {
     const int s = kit % STAGES;
     mbar_wait(&full[s], (kit / STAGES) & 1);
     const uint32_t st = smem0 + (uint32_t)(s * STAGE_BYTES);
-    const uint64_t dw0 = gmma_desc_sw128(st), dw1 = gmma_desc_sw128(st + 64 * 128), dx = gmma_desc_sw128(st + SK_W_BYTES);
+    const uint64_t dw0 = gmma_desc_sw128(st + half0), dw1 = gmma_desc_sw128(st + 64 * 128), dx = gmma_desc_sw128(st + SK_W_BYTES);
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < 4; ++k) {  // 4 x (K = 16 bf16 = 32 bytes)
       const uint32_t acc_in = (kit > 0 || k > 0) ? 1u : 0u;
       wgmma_bf16_ss<NB>(c0, dw0 + (uint64_t)(2 * k), dx + (uint64_t)(2 * k), acc_in);
-      wgmma_bf16_ss<NB>(c1, dw1 + (uint64_t)(2 * k), dx + (uint64_t)(2 * k), acc_in);
+      if constexpr (WG == 1) wgmma_bf16_ss<NB>(c1, dw1 + (uint64_t)(2 * k), dx + (uint64_t)(2 * k), acc_in);
     }
     wgmma_commit();
     wgmma_wait<0>();
     fence_acc(c0);
-    fence_acc(c1);
+    if constexpr (WG == 1) fence_acc(c1);
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[s]);
   }
 
   // epilogue: weight rows n, streams m
   const int gq = lane / 4, tq = lane % 4;
+  const int wq = WG == 1 ? warp : warp % 4;
   auto store = [&](const float (&c)[NR], int half) {
 #pragma unroll
     for (int e = 0; e < 2; ++e) {
-      const int n = n0 + 64 * half + 16 * warp + gq + 8 * e;
+      const int n = n0 + 64 * half + 16 * wq + gq + 8 * e;
       const bool nv = n < p.N;
 #pragma unroll
       for (int b = 0; b < NB / 8; ++b) {
@@ -149,8 +160,8 @@ gemm_skinny_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
       }
     }
   };
-  store(c0, 0);
-  store(c1, 1);
+  store(c0, WG == 1 ? 0 : warp / 4);
+  if constexpr (WG == 1) store(c1, 1);
 }
 
 // plain finalize: out = bf16(sum_s partial[s] + R), 4 elements per thread (N % 4 == 0)
@@ -279,7 +290,8 @@ static SkinnyKernel skinny_kernel(int nb) {
     case 16: return gemm_skinny_kernel<16>;
     case 32: return gemm_skinny_kernel<32>;
     case 64: return gemm_skinny_kernel<64>;
-    default: return gemm_skinny_kernel<128>;
+    case 128: return gemm_skinny_kernel<128>;
+    default: return gemm_skinny_kernel<256>;
   }
 }
 static int skinny_smem(int nb) {
@@ -287,13 +299,15 @@ static int skinny_smem(int nb) {
     case 16: return SkCfg<16>::SMEM_BYTES;
     case 32: return SkCfg<32>::SMEM_BYTES;
     case 64: return SkCfg<64>::SMEM_BYTES;
-    default: return SkCfg<128>::SMEM_BYTES;
+    case 128: return SkCfg<128>::SMEM_BYTES;
+    default: return SkCfg<256>::SMEM_BYTES;
   }
 }
+static int skinny_threads(int nb) { return nb > 128 ? SkCfg<256>::THREADS : SkCfg<128>::THREADS; }
 // one-time opt-in to the instantiation's dynamic shared memory (per device, like smem_optin)
 static void skinny_optin(int nb) {
-  static unsigned long long done[4] = {0, 0, 0, 0};
-  const int idx = nb == 16 ? 0 : nb == 32 ? 1 : nb == 64 ? 2 : 3;
+  static unsigned long long done[5] = {0, 0, 0, 0, 0};
+  const int idx = nb == 16 ? 0 : nb == 32 ? 1 : nb == 64 ? 2 : nb == 128 ? 3 : 4;
   smem_optin(skinny_kernel(nb), skinny_smem(nb), done[idx]);
 }
 }  // namespace rstnet
@@ -336,12 +350,12 @@ extern "C" int rstnet_skinny_gemm_create_fused(const void* X, const void* W, con
   RSTNET_REQUIRE(fin_mode != 1 || N % (4 * FIN_CL) == 0, "skinny_gemm_create: fused RMSNorm needs N %% 16 == 0 (N=%d)", N);
   RSTNET_REQUIRE(fin_mode == 0 || fin_mode == 3 || (partial_ws && aux_out && N % 4 == 0 && (fin_mode == 2 || norm_w)),
                  "skinny_gemm_create: fused finalize needs a workspace, an aux output and N %% 4 == 0");
-  RSTNET_REQUIRE(M >= 1 && M <= 128 && N >= 1 && K >= SK_BK && K % SK_BK == 0, "skinny_gemm_create: need 1<=M<=128, K %% 64 == 0 (M=%d N=%d K=%d)", M, N, K);
+  RSTNET_REQUIRE(M >= 1 && M <= 256 && N >= 1 && K >= SK_BK && K % SK_BK == 0, "skinny_gemm_create: need 1<=M<=256, K %% 64 == 0 (M=%d N=%d K=%d)", M, N, K);
   RSTNET_REQUIRE((uintptr_t)X % 16 == 0 && (uintptr_t)W % 16 == 0, "skinny_gemm_create: X and W must be 16-byte aligned");
   EncodeTiledFn2 enc = get_encode_fn2();
   RSTNET_REQUIRE(enc != nullptr, "skinny_gemm_create: cuTensorMapEncodeTiled unavailable");
   rstnet_skinny_plan* pl = new rstnet_skinny_plan();
-  const int NB = M <= 16 ? 16 : M <= 32 ? 32 : M <= 64 ? 64 : 128;
+  const int NB = M <= 16 ? 16 : M <= 32 ? 32 : M <= 64 ? 64 : M <= 128 ? 128 : 256;
   const int n_tiles = ceil_div(N, SK_BN);
   const int kchunks = K / SK_BK;
   int splits = 1;
@@ -353,6 +367,12 @@ extern "C" int rstnet_skinny_gemm_create_fused(const void* X, const void* W, con
     float best = 1e30f;
     for (int c : cand) {
       if (c > max_splits || (c > 1 && kchunks / c < 8)) continue;
+      // M > 128 runs one CTA per SM, and a split count whose CTAs need a second wave (n_tiles * c > SMs) waits for it:
+      // at the Llama-3.2-3B widths with M = 256 on an H100 the 1.5-per-SM choice took 1.8-1.9x the time of the best
+      // split count (QKV, N 5120 K 3072: 6 splits 0.117 ms, 3 splits 0.061 ms).  The largest one-wave count left (the
+      // closest to `want`) was the fastest measured for 7 of the 8 split-K shapes of that model and within 15 % for the
+      // other one (attention proj: 4 splits 0.058 ms, 3 splits 0.051 ms).
+      if (NB == 256 && c > 1 && c * n_tiles > sm_count()) continue;
       const float r = (float)c > want ? (float)c / want : want / (float)c;
       if (r < best) { best = r; splits = c; }
     }
@@ -388,7 +408,8 @@ extern "C" int rstnet_skinny_gemm_create_fused(const void* X, const void* W, con
   p.k_iters = ceil_div(kchunks, splits);
   pl->grid = dim3((unsigned)n_tiles, (unsigned)splits);
   // 4 stages (<= 98 KB with M <= 64): two CTAs fit per SM, so a GEMM whose tile count is not a multiple of the SM count
-  // still keeps every SM streaming (bandwidth-bound CTAs progress at equal rates) and prologues overlap main loops
+  // still keeps every SM streaming (bandwidth-bound CTAs progress at equal rates) and prologues overlap main loops.
+  // M = 65..128 (130 KB) and 129..256 (194 KB) run one CTA per SM.
   pl->smem = (size_t)skinny_smem(NB);
   *outp = pl;
   return 0;
@@ -398,7 +419,7 @@ extern "C" int rstnet_skinny_gemm_run(const rstnet_skinny_plan* pl, rstnet_strea
   RSTNET_REQUIRE(pl != nullptr, "skinny_gemm_run: null plan");
   skinny_optin(pl->nb);
   cudaStream_t st = (cudaStream_t)stream;
-  skinny_kernel(pl->nb)<<<pl->grid, dim3(SK_THREADS), pl->smem, st>>>(pl->tmW, pl->tmX, pl->p);
+  skinny_kernel(pl->nb)<<<pl->grid, dim3(skinny_threads(pl->nb)), pl->smem, st>>>(pl->tmW, pl->tmX, pl->p);
   count_launch();
   if (int e = check_launch("gemm_skinny")) return e;
   const long long MN = (long long)pl->p.M * pl->p.N;

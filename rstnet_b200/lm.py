@@ -33,7 +33,9 @@ from . import _lib, ops
 from ._lib import RstnetError
 from .codec import _register, on_own_device
 
-MAX_ROWS = 128   # rows (stream, position) pairs per GEMM launch: the N operand of the weight-streaming GEMM
+MAX_ROWS = 128   # rows (stream, position) pairs per launch of a prefill chunk or a forward_local slice
+MAX_STREAMS = 256   # streams of one decode scope (one position each): the widest weight-streaming GEMM reads each weight
+                    # tile once for up to 256 rows
 
 
 @dataclass
@@ -512,7 +514,9 @@ class _LMState:
         c, dev = m.config, m.device
         self.m, self.B, self.c, self.tn = m, B, c, tn
         M = self.M = B * tn
-        if M > MAX_ROWS:
+        if tn == 1 and B > MAX_STREAMS:
+            raise RstnetError(f"at most {MAX_STREAMS} streams per streaming scope (got {B})")
+        if tn > 1 and M > MAX_ROWS:
             raise RstnetError(f"at most {MAX_ROWS} rows per launch sequence (got {B} streams x {tn} positions)")
         bf = torch.bfloat16
         P = {k: v for k, v in m.named_parameters()}
@@ -768,7 +772,8 @@ class _LMState:
                 return self.out.view(B, 1, c.n_embd).clone(), self.logits.view(B, 1, c.padded_vocab_size).clone()
             self._replay(("temporal_nohead",), lambda: self._temporal(head=False))
             return None
-        # prefill: chunks of tn consecutive positions for all streams (tn * B <= MAX_ROWS rows per launch sequence).
+        # prefill: chunks of tn consecutive positions for all streams (tn * B <= MAX_ROWS rows per launch sequence; more
+        # than MAX_ROWS streams go one position per pass through the decode state).
         # A multi-position chunk appends all its keys before any of its queries run, so it must not overwrite a ring slot
         # one of those queries still needs: tn > 1 only while the ring does not wrap inside the chunk.
         outs, logits = [], []

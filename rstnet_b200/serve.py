@@ -22,6 +22,7 @@ from typing import Deque, Dict, Hashable, List, Optional, Tuple
 import torch
 
 from ._lib import RstnetError
+from .lm import MAX_STREAMS
 
 FRAME_SAMPLES = 1920       # 80 ms at 24 kHz = one 12.5 Hz frame (moshi/server.py:57: sample_rate / frame_rate)
 FRAME_SECONDS = 0.08
@@ -88,8 +89,9 @@ class DuplexEngine:
 
     def __init__(self, codec, gpt, capacity: int, *, use_sampling: bool = True, temp_text: float = 0.7, top_k_text: int = 25,
                  temp: float = 0.8, top_k: int = 30):
-        if capacity > 128:
-            raise RstnetError("the LM step takes at most 128 streams per scope (one weight-streaming GEMM pass)")
+        if capacity > MAX_STREAMS:
+            raise RstnetError(f"the LM step takes at most {MAX_STREAMS} streams per scope (one weight-streaming GEMM pass), "
+                              f"got {capacity}")
         self.codec, self.gpt, self.B = codec, gpt, capacity
         self.dev = gpt.device
         self.sampling = dict(use_sampling=use_sampling, temp_text=temp_text, top_k_text=top_k_text, temp=temp, top_k=top_k)

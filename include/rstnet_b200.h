@@ -216,6 +216,27 @@ int rstnet_rvq_decode_gather_f32(const int64_t* codes, const float* E, float* q,
                                  int32_t n_q, int32_t n_q_semantic, int32_t dim, int32_t bins,
                                  int32_t time_major, rstnet_stream_t stream);
 
+/* ---- polyphase sinc resampling, fp32: torchaudio.transforms.Resample(orig, new) with its defaults (sinc_interp_hann,
+ * lowpass_filter_width 6, rolloff 0.99), which the reference calls wherever it reads audio
+ * (MLLM_v2/tools/tokenizer/MimiCodec/mimi_tokenizer.py:40,67; MLLM_v2/egs/moshi_ft/data_scripts/offline_tokenization.py:51;
+ * AudioCodec/MimiCodec/inference.py:24-34).  With g = gcd(orig, new), o = orig/g input samples per block, n = new/g
+ * output phases per block:
+ *   out[r*out_row_stride + q] (q = j*n + p < out_len) = sum_{i<S} xv(r, j*o + x_shift + start[p] + i) * taps[p*S + i]
+ *   xv(r, t) = x[r*x_row_stride + t] if 0 <= t < x_len, else 0
+ * taps (device fp32 [n][S]) is the fp32 table trimmed to each phase's run of nonzero taps, zero-padded at the end;
+ * start (device int32 [n]) the run's first tap, every start[p] in [0, start_max] (a phase outside it is written as NaN).
+ * The sum starts at +0.0f and accumulates with fmaf in increasing i, whatever the tiling.
+ *   batch form:     x_shift = -w, x_len = L, out_len = ceil(n*L/o) (torchaudio's zero padding is the bounds check);
+ *   streaming form: x = a carry buffer, x_shift = 0, x_len = carry + chunk (the two forms are bit-identical).
+ * The trimmed table is capped at RSTNET_RESAMPLE_MAX_TABLE_BYTES (n*S*4).  Non-finite input: a NaN / Inf poisons only
+ * the outputs whose nonzero run covers it, where torchaudio's full-width conv1d also multiplies it by the zero taps
+ * around the run (and so poisons every output whose full window covers it); for finite input the two sums agree up to
+ * rounding, and up to the sign of zero. */
+#define RSTNET_RESAMPLE_MAX_TABLE_BYTES (48 * 1024)
+int rstnet_resample_f32(const float* x, int64_t x_row_stride, int64_t x_len, int64_t x_shift, const float* taps,
+                        const int32_t* start, int32_t n, int32_t o, int32_t S, int32_t start_max, float* out,
+                        int64_t out_row_stride, int64_t out_len, int32_t rows, rstnet_stream_t stream);
+
 /* ======================================================================================
  * Speech-text LM decode step (MLLM_v2/models/llama_streaming.py GPT under `with gpt.streaming(B)`),
  * bf16 activations / weights, fp32 accumulation.  One token per stream: rows are streams.

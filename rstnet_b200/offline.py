@@ -2,16 +2,19 @@
 
   * `tokenize_utterances` / `python -m rstnet_b200.offline tokenize`: the Mimi branch of
     MLLM_v2/egs/pretraining/local/offline_codec_tokenization.py (and tools/data_scripts/offline_tokenization.py): every
-    utterance -> int16 codes [8, T], collected in a dict `utt_id -> tensor` and written with `torch.save` -- the on-disk
-    format the reference's data loader reads (tools/tokenizer/MimiCodec/mimi_tokenizer.py:44,72).  Unlike the reference
+    utterance -> int16 codes [8, T] of its 24 kHz audio, collected in a dict `utt_id -> tensor` and written with
+    `torch.save` -- the on-disk format the reference's data loader reads (tools/tokenizer/MimiCodec/mimi_tokenizer.py:44,72).  Unlike the reference
     (one clip per call) clips of EQUAL length are encoded as one batch (>= 96 of them: on the tensor cores); clips are
     never padded to a common length, because the codec's convs zero-pad each LAYER's input at the end of a clip
     (modules/conv.py:245-254), so audio padding would change a clip's last frame.
   * `reconstruct_directory` / `python -m rstnet_b200.offline reconstruct`: AudioCodec/MimiCodec/inference.py:111-148 -- every
-    wav of a directory through encode -> decode, written under the same name.
+    wav of a directory through encode -> decode, written under the same name at 24 kHz.
 
-24 kHz mono PCM wav in / out through scipy.io.wavfile (this image has neither torchaudio nor soundfile); other sample rates
-are rejected rather than resampled (the reference resamples with torchaudio / julius).
+Audio at any integer sample rate is resampled to 24 kHz on the GPU the way the reference does it,
+torchaudio.transforms.Resample(sr, 24000) with its defaults (mimi_tokenizer.py:40,67; inference.py:24-34 `convert_audio`:
+mean over channels, then Resample), by rstnet_b200.audio.Resample: clips of one (rate, length) group in one launch.
+24 kHz clips go straight to the codec, as before.  Wav files are read and written through scipy.io.wavfile (mono mix of
+the channels; integer PCM scaled to [-1, 1]).
 """
 from __future__ import annotations
 
@@ -24,6 +27,7 @@ from typing import Dict, Iterable, Tuple
 import numpy as np
 import torch
 
+from .audio import Resample
 from .codec import MimiCodec
 
 
@@ -39,19 +43,28 @@ def _as_row(wav: torch.Tensor) -> torch.Tensor:
 
 
 @torch.no_grad()
-def tokenize_utterances(codec: MimiCodec, items: Iterable[Tuple[str, torch.Tensor]], batch_size: int = 256) -> Dict[str, torch.Tensor]:
-    """{utt_id: int16 [n_q, ceil(L / 1920)]} -- identical to MimiTokenizer.tokenize on every clip."""
+def tokenize_utterances(codec: MimiCodec, items: Iterable[Tuple], batch_size: int = 256) -> Dict[str, torch.Tensor]:
+    """{utt_id: int16 [n_q, ceil(L24 / 1920)]} -- identical to MimiTokenizer.tokenize on every clip.  An item is
+    (utt_id, wav) for 24 kHz audio or (utt_id, wav, sample_rate); other rates are resampled to 24 kHz first
+    (Resample(sample_rate, 24000), one launch per batch of equal rate and length)."""
     dev = codec.device
     by_len = defaultdict(list)
-    for utt, wav in items:
+    for item in items:
+        utt, wav = item[0], item[1]
+        sr = int(item[2]) if len(item) > 2 else codec.sample_rate
         w = _as_row(wav)
         if w.numel():
-            by_len[w.numel()].append((utt, w))
+            by_len[(sr, w.numel())].append((utt, w))
     out: Dict[str, torch.Tensor] = {}
-    for L, group in by_len.items():
+    resamplers: Dict[int, Resample] = {}
+    for (sr, L), group in by_len.items():
+        if sr != codec.sample_rate and sr not in resamplers:
+            resamplers[sr] = Resample(sr, codec.sample_rate)
         for i in range(0, len(group), batch_size):
             part = group[i:i + batch_size]
             x = torch.stack([w for _, w in part])[:, None].to(dev)            # [B, 1, L]
+            if sr != codec.sample_rate:
+                x = resamplers[sr](x)                                        # [B, 1, ceil(L * 24000 / sr)]
             codes = codec.encode(x).to(torch.int16).cpu()                    # [B, n_q, T]
             for (utt, _), c in zip(part, codes):
                 out[utt] = c.clone()
@@ -87,8 +100,9 @@ def reconstruct_directory(codec: MimiCodec, src: str, dst: str) -> int:
         if not name.lower().endswith(".wav"):
             continue
         wav, sr = read_wav(os.path.join(src, name))
+        wav = wav.to(codec.device)
         if sr != codec.sample_rate:
-            raise ValueError(f"{name}: {sr} Hz; resample to {codec.sample_rate} Hz first")
+            wav = Resample(sr, codec.sample_rate)(wav)                       # convert_audio (inference.py:24-34)
         codes = codec.encode(wav[None, None].to(codec.device))
         rec = codec.decode(codes)[0, 0, : wav.numel()]
         if float(rec.abs().max()) > 0.99:
@@ -127,9 +141,7 @@ def main(argv=None) -> int:
             for line in open(args.wav_scp):
                 utt, path = line.strip().split(None, 1)
                 wav, sr = read_wav(path)
-                if sr != codec.sample_rate:
-                    raise ValueError(f"{utt}: {sr} Hz; resample to {codec.sample_rate} Hz first")
-                yield utt, wav
+                yield utt, wav, sr
         toks = tokenize_utterances(codec, items(), args.batch_size)
         save_tokens(toks, args.output_file)
         print(f"tokenized {len(toks)} utterances -> {args.output_file}")

@@ -8,13 +8,16 @@ What the batch form needs beyond the reference's all-or-nothing streaming state,
     the position counters of held rows do not advance; codec.py / lm.py)
   * no re-capture of CUDA graphs when sessions come and go            -> all of the above are device-side flags/counters
 The websocket / Opus transport of server.py (:98-103, 141-153, 163) is out of scope (SURVEY.md §8: networking); sessions
-push raw 24 kHz PCM chunks and receive (tokens, PCM) per tick.
+push raw PCM chunks of 80 ms and receive (tokens, PCM) per tick.  The codec runs at 24 kHz; a `DuplexEngine` built with
+another client `sample_rate` resamples every row on the GPU on the way in and on the way out (rstnet_b200.audio), so its
+sessions push and receive PCM at their own rate.
 
 `FrameScheduler` is pure host logic over an engine object with `reset_rows(rows)` and `step(pcm_rows, active) ->
 {row: (tokens, pcm)}`; `DuplexEngine` is that engine for a MimiCodec + GPT pair on a GPU.
 """
 from __future__ import annotations
 
+import math
 import time
 from collections import deque
 from typing import Deque, Dict, Hashable, List, Optional, Tuple
@@ -22,10 +25,22 @@ from typing import Deque, Dict, Hashable, List, Optional, Tuple
 import torch
 
 from ._lib import RstnetError
+from .audio import StreamingResampler
 from .lm import MAX_STREAMS
 
 FRAME_SAMPLES = 1920       # 80 ms at 24 kHz = one 12.5 Hz frame (moshi/server.py:57: sample_rate / frame_rate)
 FRAME_SECONDS = 0.08
+CODEC_RATE = 24000
+
+
+def check_client_rate(sample_rate) -> int:
+    """A client rate r works iff gcd(r, 24000) is a multiple of 25: then 80 ms (2r/25 samples) is a whole number of
+    resampling blocks in both directions (r -> 24 kHz and 24 kHz -> r).  Covers 8, 11.025, 16, 22.05, 32, 44.1 and 48 kHz."""
+    if isinstance(sample_rate, bool) or not isinstance(sample_rate, (int, float)) or int(sample_rate) != sample_rate \
+            or int(sample_rate) <= 0 or math.gcd(int(sample_rate), CODEC_RATE) % 25 != 0:
+        raise RstnetError(f"unsupported client sample rate {sample_rate!r}: a rate r must be a positive integer with "
+                          f"gcd(r, {CODEC_RATE}) % 25 == 0 (so that 80 ms is a whole number of resampling blocks)")
+    return int(sample_rate)
 
 
 class FrameScheduler:
@@ -85,10 +100,16 @@ class DuplexEngine:
     """One streaming scope of a MimiCodec and a GPT for `capacity` sessions: per tick, for all rows at once,
     encode the sessions' 80 ms chunks -> one LM frame (temporal step + 8 depth steps + sampling) -> decode the generated
     codes (the three calls of server.py:128-136).  The LM input frame of a row is [its previous text token, the 8 codes of
-    its input audio]; the generated audio codes are restricted to ids < 2048 (decodable)."""
+    its input audio]; the generated audio codes are restricted to ids < 2048 (decodable).
+
+    `sample_rate` is the sessions' PCM rate (see `check_client_rate`): each pushes and receives sample_rate * 0.08 samples
+    per tick.  At any rate other than 24000 two StreamingResamplers run for all rows at once, r -> 24 kHz before the
+    encode and 24 kHz -> r after the decode; row resets and the held-row mask apply to both."""
 
     def __init__(self, codec, gpt, capacity: int, *, use_sampling: bool = True, temp_text: float = 0.7, top_k_text: int = 25,
-                 temp: float = 0.8, top_k: int = 30):
+                 temp: float = 0.8, top_k: int = 30, sample_rate: int = CODEC_RATE):
+        self.sample_rate = check_client_rate(sample_rate)
+        self.frame_samples = self.sample_rate * 2 // 25                       # 80 ms at the client rate
         if capacity > MAX_STREAMS:
             raise RstnetError(f"the LM step takes at most {MAX_STREAMS} streams per scope (one weight-streaming GEMM pass), "
                               f"got {capacity}")
@@ -97,11 +118,18 @@ class DuplexEngine:
         self.sampling = dict(use_sampling=use_sampling, temp_text=temp_text, top_k_text=top_k_text, temp=temp, top_k=top_k)
         codec.streaming_forever(capacity)
         gpt.streaming_forever(capacity)
-        self.pcm_in = torch.zeros(capacity, 1, FRAME_SAMPLES, dtype=torch.float32).pin_memory()
+        F = self.frame_samples
+        self.pcm_in = torch.zeros(capacity, 1, F, dtype=torch.float32).pin_memory()
         self.pcm_dev = torch.zeros(capacity, 1, FRAME_SAMPLES, dtype=torch.float32, device=self.dev)
+        self.up = self.down = None
+        if self.sample_rate != CODEC_RATE:
+            self.up = StreamingResampler(self.sample_rate, CODEC_RATE, capacity, self.dev)
+            self.down = StreamingResampler(CODEC_RATE, self.sample_rate, capacity, self.dev)
+            self.pcm_client_dev = torch.zeros(capacity, 1, F, dtype=torch.float32, device=self.dev)
+            self.pcm_out_dev = torch.zeros(capacity, F, dtype=torch.float32, device=self.dev)
         self.prev_text = torch.full((capacity, 1, 1), gpt.text_initial_token_id, dtype=torch.int64, device=self.dev)
         self.tok_host = torch.zeros(capacity, gpt.config.dep_q + 1, dtype=torch.int64).pin_memory()
-        self.pcm_host = torch.zeros(capacity, 1, FRAME_SAMPLES, dtype=torch.float32).pin_memory()
+        self.pcm_host = torch.zeros(capacity, 1, F, dtype=torch.float32).pin_memory()
         self.mask_host = torch.zeros(capacity, dtype=torch.int64).pin_memory()
         self.latencies_ms: List[float] = []
 
@@ -109,23 +137,34 @@ class DuplexEngine:
         self.codec.reset_streaming(streams=list(rows))
         self.gpt.reset_streaming(streams=list(rows))
         self.prev_text[list(rows)] = self.gpt.text_initial_token_id
+        if self.up is not None:
+            self.up.reset(rows)
+            self.down.reset(rows)
 
     @torch.no_grad()
     def step(self, pcm_rows: Dict[int, torch.Tensor], active: List[int]):
         t0 = time.perf_counter()
         self.mask_host.zero_()
         for r, chunk in pcm_rows.items():
-            self.pcm_in[r, 0].copy_(torch.as_tensor(chunk, dtype=torch.float32).reshape(FRAME_SAMPLES))
+            self.pcm_in[r, 0].copy_(torch.as_tensor(chunk, dtype=torch.float32).reshape(self.frame_samples))
             self.mask_host[r] = 1
         self.codec.set_active_streams(self.mask_host)
         self.gpt.set_active_streams(self.mask_host)
-        self.pcm_dev.copy_(self.pcm_in, non_blocking=True)
+        if self.up is None:
+            self.pcm_dev.copy_(self.pcm_in, non_blocking=True)
+        else:
+            self.up.set_active(self.mask_host)
+            self.down.set_active(self.mask_host)
+            self.pcm_client_dev.copy_(self.pcm_in, non_blocking=True)
+            self.up(self.pcm_client_dev[:, 0], out=self.pcm_dev[:, 0])                  # r -> 24 kHz, all rows
         codes = self.codec.encode(self.pcm_dev)                                   # [B, 8, 1]
         frame = torch.cat([self.prev_text, codes], dim=1)                        # [B, 9, 1]
         toks = self.gpt.forward_step(frame, audio_valid=2048, **self.sampling)    # [B, 9]
         held = (self.mask_host == 0).to(self.dev)
         self.prev_text.copy_(torch.where(held[:, None, None], self.prev_text, toks[:, :1, None]))
         pcm = self.codec.decode(toks[:, 1:, None].clamp(max=self.codec.codebook_size - 1))   # [B, 1, 1920]
+        if self.down is not None:
+            pcm = self.down(pcm[:, 0], out=self.pcm_out_dev)[:, None]                  # 24 kHz -> r, all rows
         self.tok_host.copy_(toks, non_blocking=True)
         self.pcm_host.copy_(pcm, non_blocking=True)
         torch.cuda.current_stream().synchronize()

@@ -324,6 +324,24 @@ int rstnet_lm_sample_bf16(const void* logits, int32_t rows, int32_t V, int32_t n
                           uint32_t seed, const int64_t* step_counter, int64_t* tokens, int32_t tok_stride,
                           rstnet_stream_t stream);
 
+/* ---- the acoustic-delay token cache of LMGen.step (models/model.py:490-562; moshi/models/lm.py LMGen.step), per stream:
+ * the eager cache writes, input copy, write-back and gather of that step, as two launches around the LM frame.
+ * cache [B][K][CT] int64 (K = n_q + 1 codebooks, CT = max_delay + 2); off [B] int64, the stream's step count; active [B]
+ * int64 (NULL = every stream active), a stream with 0 is HELD: nothing of its cache, off, valid or out is written;
+ * delays [K] int64 (device).  Column indices are taken modulo CT.  Token ids (incl. -1 zero / -2 ungenerated) are copied
+ * unchanged.
+ * cache_in, before the temporal step: for active streams, user[b][k - dep_q - 1] -> column off + delays[k] of every
+ * k > dep_q, then the initial token (text_init for k = 0, audio_init otherwise) -> column off of every k with
+ * off <= delays[k]; then seq[b][0..K) = column off for every stream (held streams: ids < -1 become -1).  */
+int rstnet_lm_delay_cache_in(int64_t* cache, const int64_t* off, const int64_t* active, const int64_t* delays,
+                             const int64_t* user, int32_t user_stride, int64_t* seq, int32_t seq_stride, int32_t B, int32_t K,
+                             int32_t dep_q, int32_t CT, int64_t text_init, int64_t audio_init, rstnet_stream_t stream);
+/* cache_out, after the last depth sample, active streams: tokens[b][0..dep_q] -> column off + 1; off += 1;
+ * out[b][k] = column off - max_delay + delays[k] of k = 0..dep_q; valid[b] = off > max_delay.  CT == max_delay + 2. */
+int rstnet_lm_delay_cache_out(int64_t* cache, int64_t* off, const int64_t* active, const int64_t* delays,
+                              const int64_t* tokens, int32_t tok_stride, int64_t* out, int32_t out_stride, int64_t* valid,
+                              int32_t B, int32_t K, int32_t dep_q, int32_t CT, int32_t max_delay, rstnet_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -835,6 +835,12 @@ class _LMState:
             raise RstnetError(f"forward_step takes sequence [{self.B}, {c.n_q + 1}, 1], got {tuple(sequence.shape)}")
         self._advance_host(1)
         self.seq.copy_(sequence[:, :, 0])
+        self._replay(*self._frame(use_sampling, temp_text, top_k_text, temp, top_k, audio_valid, quirk))
+        return self.tokens.clone()
+
+    def _frame(self, use_sampling, temp_text, top_k_text, temp, top_k, audio_valid, quirk):
+        """(graph key, launch sequence) of one generated frame from the ids in self.seq to the tokens in self.tokens."""
+        c = self.c
         # kernel convention: 0 = argmax, k > 0 = top-k, -1 = multinomial over the whole (valid) support
         sampling_text = use_sampling and temp_text > 0.0
         sampling = use_sampling and temp > 0.0
@@ -853,5 +859,4 @@ class _LMState:
                 self._sample(self.dlogits, c.audio_card, min(valid[k], c.audio_card), tk, temp if sampling else 1.0, k + 1, k + 1)
             ops.counter_add(self.frame_counter, 1)
 
-        self._replay(("frame", tk_text, float(temp_text), tk, float(temp), valid, bool(quirk)), frame)
-        return self.tokens.clone()
+        return ("frame", tk_text, float(temp_text), tk, float(temp), valid, bool(quirk)), frame

@@ -11,9 +11,14 @@ embedding, a text head, and the depth transformer with per-codebook-step weights
   * ``LMGen(lm, use_sampling, temp, temp_text, top_k, top_k_text).step(input_tokens[B, K_in, 1]) -> [B, dep_q+1, 1] | None``
     with the delay cache of :490-562 (acoustic delays, initial tokens, `max_delay` warm-up frames returning None).
 
+Extensions for serving a batch of sessions (rstnet_b200.serve.MoshiDuplexEngine): the delay cache keeps one step count per
+row, so `LMGen.reset_streaming(streams=...)` restarts single rows and `LMGen.set_active_streams(mask)` holds rows, each
+with its own warm-up (`LMGen.valid_rows()`).
+
 The kernels are the GPT path's (rstnet_b200/lm.py): weight-streaming wgmma GEMMs with fused Kyutai RMSNorm / SiLU gating
-finalizes, ring decode attention, the depth transformer, device-side sampling; plus the bf16 pair-RoPE kernel.  One
-`LMGen.step` is one CUDA-graph replay.
+finalizes, ring decode attention, the depth transformer, device-side sampling; plus the bf16 pair-RoPE kernel and the
+two delay-cache kernels (csrc/delay_cache.cu).  One `LMGen.step` is one input copy and one CUDA-graph replay: cache_in,
+the temporal step, text sampling, the dep_q depth steps with sampling, cache_out.
 """
 from __future__ import annotations
 
@@ -292,6 +297,12 @@ class LMModel(nn.Module):
             raise ValueError("Trying to reset streaming, but the model wasn't streaming.")
         self._state.reset(streams)
 
+    def set_active_streams(self, mask) -> None:
+        """Extension for batched serving: hold the rows whose flag is 0 during the following steps (as GPT does)."""
+        if self._state is None:
+            raise ValueError("the model is not streaming")
+        self._state.set_active(mask)
+
     def _st(self) -> _MoshiState:
         if self._state is None:
             raise RstnetError("only the streaming decode path is implemented: call inside `with lm.streaming(B):`")
@@ -321,8 +332,36 @@ class LMModel(nn.Module):
         raise NotImplementedError("training forward is out of scope; use LMGen.step / forward_text / forward_depformer")
 
 
+class _GenState:
+    """One `LMGen.streaming(B)` scope: the delay cache with one step count per row (device), the host mirror of those
+    counts, and the LMModel scope the generator drives.  The cache kernels read the LMModel scope's `active` flags."""
+
+    def __init__(self, gen: "LMGen", lm_state: _MoshiState, B: int):
+        lm = gen.lm_model
+        dev, K, i64 = lm.device, lm.num_codebooks, torch.int64
+        self.gen, self.lm, self.B = gen, lm_state, B
+        self.cache = torch.full((B, K, gen.max_delay + 2), lm.ungenerated_token_id, device=dev, dtype=i64)
+        self.off = torch.zeros(B, dtype=i64, device=dev)
+        self.valid = torch.zeros(B, dtype=i64, device=dev)
+        self.out = torch.zeros(B, lm.dep_q + 1, dtype=i64, device=dev)
+        self.user = torch.zeros(B, K - lm.dep_q - 1, dtype=i64, device=dev)
+        self.off_host = np.zeros(B, dtype=np.int64)
+        self.stepped = np.zeros(B, dtype=bool)      # rows that were active in the last step
+
+    @property
+    def offset(self) -> int:
+        """The reference's single step count; defined while every row is at the same step (see `off_host`)."""
+        if (self.off_host != self.off_host[0]).any():
+            raise RstnetError("the rows of this scope are at different steps: read off_host")
+        return int(self.off_host[0])
+
+
 class LMGen(nn.Module):
-    """``models.model.LMGen`` (:440-597): the streaming generator over an LMModel with the acoustic-delay token cache."""
+    """``models.model.LMGen`` (:440-597): the streaming generator over an LMModel with the acoustic-delay token cache.
+
+    The cache keeps one step count per row, so a batch row can be restarted (`reset_streaming(streams=...)`) or held
+    (`set_active_streams`) while the other rows go on; `valid_rows()` tells which rows produced output on the last step.
+    A scope whose rows all start together behaves exactly as the reference."""
 
     def __init__(self, lm_model: LMModel, use_sampling: bool = True, temp: float = 0.8, temp_text: float = 0.7, top_k: int = 250,
                  top_k_text: int = 25, check: bool = False):
@@ -332,7 +371,7 @@ class LMGen(nn.Module):
             use_sampling, temp, temp_text, top_k, top_k_text, check
         self.max_delay = max(lm_model.delays)
         self.delays_cuda = torch.tensor(lm_model.delays, device=lm_model.device, dtype=torch.long)
-        self._st = None
+        self._st: Optional[_GenState] = None
 
     @property
     def is_streaming(self) -> bool:
@@ -341,8 +380,7 @@ class LMGen(nn.Module):
     def streaming_forever(self, batch_size: int):
         lm = self.lm_model
         lm.streaming_forever(batch_size)
-        cache = torch.full((batch_size, lm.num_codebooks, self.max_delay + 2), lm.ungenerated_token_id, device=lm.device, dtype=torch.long)
-        self._st = SimpleNamespace(cache=cache, initial=lm._get_initial_token(), offset=0)
+        self._st = _GenState(self, lm._st(), batch_size)
 
     @contextmanager
     def streaming(self, batch_size: int):
@@ -353,14 +391,79 @@ class LMGen(nn.Module):
             self._st = None
             self.lm_model._state = None
 
-    def reset_streaming(self):
+    def _require(self) -> _GenState:
+        if self._st is None:
+            raise ValueError("the generator is not streaming")
+        return self._st
+
+    def reset_streaming(self, streams=None):
+        """Restart every row, or (extension) only the rows in `streams`: their cache back to ungenerated, their step count
+        and their LMModel rows to 0.  The other rows and the captured graph are untouched."""
         if self._st is None:
             raise ValueError("Trying to reset streaming, but the generator wasn't streaming.")
-        self._st.offset = 0
-        self.lm_model.reset_streaming()
+        st = self._st
+        self.lm_model.reset_streaming(streams)          # checks the row indices
+        rows_h = slice(None) if streams is None else np.asarray(streams, dtype=np.int64).reshape(-1)
+        rows = rows_h if streams is None else torch.from_numpy(rows_h).to(st.off.device)
+        st.cache[rows] = self.lm_model.ungenerated_token_id
+        st.off[rows] = 0
+        st.valid[rows] = 0
+        st.off_host[rows_h] = 0
+        st.stepped[rows_h] = False
+
+    def set_active_streams(self, mask) -> None:
+        """Extension for batched serving: the rows whose flag is 0 are held by the following steps -- their cache, step
+        count and LMModel rows keep their exact state.  None = every row steps."""
+        self._require()
+        self.lm_model.set_active_streams(mask)
+
+    def valid_rows(self) -> np.ndarray:
+        """Host bool [B]: the rows that produced output on the last step (stepped, and past their `max_delay` warm-up
+        steps).  The other rows of that step's result carry no tokens."""
+        st = self._require()
+        return st.stepped & (st.off_host > self.max_delay)
+
+    def get_streaming_state(self):
+        """modules/streaming.py:128-136: the generator and its LMModel are one streaming module here; the state object is
+        opaque and owned by the caller until it is set back."""
+        return {"": self._st}
+
+    def set_streaming_state(self, state):
+        """modules/streaming.py:138-151: installs a scope of this generator (and its LMModel scope)."""
+        state = dict(state)
+        if "" not in state:
+            raise RuntimeError("Expected to find a streaming state for .")
+        st = state.pop("")
+        if state:
+            raise RuntimeError(f"Some states were not consumed: {list(state.keys())}")
+        if st is not None and (not isinstance(st, _GenState) or st.gen is not self):
+            raise RuntimeError("the streaming state belongs to another generator")
+        self._st = st
+        self.lm_model._state = None if st is None else st.lm
+
+    def _frame(self, st: _GenState):
+        """(graph key, launch sequence): cache_in -> temporal step + text sampling + dep_q depth steps with sampling
+        (sample_token over the whole card: LMGen uses plain `sample_token`, models/model.py:528-533, 581-586) -> cache_out."""
+        lm, ms, L = self.lm_model, st.lm, _lib.lib()
+        key, frame = ms._frame(self.use_sampling, self.temp_text, self.top_k_text, self.temp, self.top_k, lm.card, True)
+        K, CT = lm.num_codebooks, st.cache.shape[2]
+
+        def step():
+            _lib.check(L.rstnet_lm_delay_cache_in(st.cache.data_ptr(), st.off.data_ptr(), ms.active.data_ptr(),
+                                                  self.delays_cuda.data_ptr(), st.user.data_ptr(), st.user.shape[1],
+                                                  ms.seq.data_ptr(), ms.seq.shape[1], st.B, K, lm.dep_q, CT,
+                                                  lm.text_initial_token_id, lm.initial_token_id, ops._stream()), "delay_cache_in")
+            frame()
+            _lib.check(L.rstnet_lm_delay_cache_out(st.cache.data_ptr(), st.off.data_ptr(), ms.active.data_ptr(),
+                                                   self.delays_cuda.data_ptr(), ms.tokens.data_ptr(), ms.tokens.shape[1],
+                                                   st.out.data_ptr(), st.out.shape[1], st.valid.data_ptr(), st.B, K, lm.dep_q,
+                                                   CT, self.max_delay, ops._stream()), "delay_cache_out")
+        return ("lmgen",) + key, step
 
     @torch.no_grad()
     def step(self, input_tokens: torch.Tensor) -> Optional[torch.Tensor]:
+        """One step of every active row: -> [B, dep_q + 1, 1] in the delayed layout, or None while every row is still in
+        its `max_delay` warm-up steps.  One input copy and one graph replay."""
         st = self._st
         if st is None:
             raise RuntimeError("You should wrap those calls with a `with lm_gen.streaming(): ...`.")
@@ -370,28 +473,18 @@ class LMGen(nn.Module):
         assert S == 1, "Only support being given steps one by one."
         needed = lm.num_codebooks - lm.dep_q - 1
         assert Ki == needed, f"We expect {needed} tokens from the user stream, got {Ki}."
-        CT = st.cache.shape[2]
-        for q_other in range(Ki):                                   # the user's stream goes into the cache at its delay
-            k = lm.dep_q + 1 + q_other
-            wp = (st.offset + lm.delays[k]) % CT
-            st.cache[:, k, wp:wp + 1] = input_tokens[:, q_other]
-        position = st.offset % CT
-        for k, delay in enumerate(lm.delays):                        # delayed codebooks start from the initial token
-            if st.offset <= delay:
-                st.cache[:, k, position] = st.initial[:, k, 0]
-        input_ = st.cache[:, :, position:position + 1]
+        if B != st.B:
+            raise RstnetError(f"streaming batch size is {st.B}, got {B}")
+        ms = st.lm
+        ms._advance_host(1)
+        st.user.copy_(input_tokens[:, :, 0])
+        ms._replay(*self._frame(st))
+        act = ms.active_host != 0
         if self.check:
-            assert not (input_ == lm.ungenerated_token_id).any(), (st.offset, input_)
-        # temporal step + text sampling + dep_q depth steps with sampling: one graph replay (sample_token over the whole
-        # card: LMGen uses plain `sample_token`, models/model.py:528-533, 581-586)
-        toks = lm._st().forward_step(input_, self.use_sampling, self.temp_text, self.top_k_text, self.temp, self.top_k,
-                                     lm.card, True)                  # [B, dep_q + 1]
-        st.offset += 1
-        position = st.offset % CT
-        st.cache[:, 0, position] = toks[:, 0]
-        st.cache[:, 1:lm.dep_q + 1, position] = toks[:, 1:]
-        if st.offset <= self.max_delay:
+            seq = ms.seq.cpu()[torch.from_numpy(act)]
+            assert not (seq == lm.ungenerated_token_id).any(), (st.off_host, seq)
+        st.off_host += act
+        st.stepped[:] = act
+        if not (st.off_host > self.max_delay).any():
             return None
-        gen_delays = self.delays_cuda[:lm.dep_q + 1]
-        index = ((st.offset - self.max_delay + gen_delays) % CT).view(1, -1, 1).expand(B, -1, 1)
-        return st.cache.gather(dim=2, index=index)
+        return st.out[:, :, None].clone()

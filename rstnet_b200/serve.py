@@ -13,7 +13,8 @@ another client `sample_rate` resamples every row on the GPU on the way in and on
 sessions push and receive PCM at their own rate.
 
 `FrameScheduler` is pure host logic over an engine object with `reset_rows(rows)` and `step(pcm_rows, active) ->
-{row: (tokens, pcm)}`; `DuplexEngine` is that engine for a MimiCodec + GPT pair on a GPU.
+{row: (tokens, pcm)}`; `DuplexEngine` is that engine for a MimiCodec + GPT pair on a GPU, `MoshiDuplexEngine` for the
+MimiCodec + `LMGen(LMModel)` pair server.py itself runs (rstnet_b200.moshi).
 """
 from __future__ import annotations
 
@@ -170,3 +171,86 @@ class DuplexEngine:
         torch.cuda.current_stream().synchronize()
         self.latencies_ms.append(1e3 * (time.perf_counter() - t0))
         return {r: (self.tok_host[r].clone(), self.pcm_host[r, 0].clone()) for r in active}
+
+
+class MoshiDuplexEngine:
+    """The serving loop of server.py:128-136 -- `mimi.encode -> lm_gen.step(codes) -> mimi.decode(tokens[:, 1:])` --
+    for `capacity` sessions in one streaming scope of a MimiCodec and an `LMGen` (rstnet_b200.moshi).
+
+    Every session has its own warm-up: `LMGen` returns no tokens for a row's first `max_delay` steps, and for those steps
+    the codec's decoder is held for that row (the reference does not call `mimi.decode` then) while its encoder advances.
+    `step` returns {row: (tokens, pcm)}, tokens = int64 [dep_q + 1] (text token, then the audio codes that were decoded),
+    pcm = float32 [sample_rate * 0.08]; a row in its warm-up gets (None, None), as the reference's `lm_gen.step` returns
+    None.  Text-piece decoding and the transport stay with the caller.  `sample_rate` as for `DuplexEngine`."""
+
+    def __init__(self, codec, lm_gen, capacity: int, *, sample_rate: int = CODEC_RATE):
+        self.sample_rate = check_client_rate(sample_rate)
+        self.frame_samples = self.sample_rate * 2 // 25                       # 80 ms at the client rate
+        if capacity > MAX_STREAMS:
+            raise RstnetError(f"the LM step takes at most {MAX_STREAMS} streams per scope (one weight-streaming GEMM pass), "
+                              f"got {capacity}")
+        lm = lm_gen.lm_model
+        n_user = lm.num_codebooks - lm.dep_q - 1
+        if codec.n_q != n_user:
+            raise RstnetError(f"the codec emits {codec.n_q} codes per frame, the LM takes {n_user} user codebooks")
+        self.codec, self.lm_gen, self.B = codec, lm_gen, capacity
+        self.dev = lm.device
+        codec.streaming_forever(capacity)
+        lm_gen.streaming_forever(capacity)
+        F = self.frame_samples
+        pin = self.dev.type == "cuda"                                           # False: host logic under a test's fakes
+        self.pcm_in = torch.zeros(capacity, 1, F, dtype=torch.float32, pin_memory=pin)
+        self.pcm_dev = torch.zeros(capacity, 1, FRAME_SAMPLES, dtype=torch.float32, device=self.dev)
+        self.up = self.down = None
+        if self.sample_rate != CODEC_RATE:
+            self.up = StreamingResampler(self.sample_rate, CODEC_RATE, capacity, self.dev)
+            self.down = StreamingResampler(CODEC_RATE, self.sample_rate, capacity, self.dev)
+            self.pcm_client_dev = torch.zeros(capacity, 1, F, dtype=torch.float32, device=self.dev)
+            self.pcm_out_dev = torch.zeros(capacity, F, dtype=torch.float32, device=self.dev)
+        self.tok_host = torch.zeros(capacity, lm.dep_q + 1, dtype=torch.int64, pin_memory=pin)
+        self.pcm_host = torch.zeros(capacity, 1, F, dtype=torch.float32, pin_memory=pin)
+        self.mask_host = torch.zeros(capacity, dtype=torch.int64, pin_memory=pin)
+        self.dec_mask_host = torch.zeros(capacity, dtype=torch.int64, pin_memory=pin)
+        self.dec_mask_dev = torch.zeros(capacity, dtype=torch.int64, device=self.dev)
+        self.latencies_ms: List[float] = []
+
+    def reset_rows(self, rows) -> None:
+        self.codec.reset_streaming(streams=list(rows))
+        self.lm_gen.reset_streaming(streams=list(rows))
+        if self.up is not None:
+            self.up.reset(rows)
+            self.down.reset(rows)
+
+    @torch.no_grad()
+    def step(self, pcm_rows: Dict[int, torch.Tensor], active: List[int]):
+        t0 = time.perf_counter()
+        self.mask_host.zero_()
+        for r, chunk in pcm_rows.items():
+            self.pcm_in[r, 0].copy_(torch.as_tensor(chunk, dtype=torch.float32).reshape(self.frame_samples))
+            self.mask_host[r] = 1
+        self.codec.set_active_streams(self.mask_host)
+        self.lm_gen.set_active_streams(self.mask_host)
+        if self.up is None:
+            self.pcm_dev.copy_(self.pcm_in, non_blocking=True)
+        else:
+            self.up.set_active(self.mask_host)
+            self.pcm_client_dev.copy_(self.pcm_in, non_blocking=True)
+            self.up(self.pcm_client_dev[:, 0], out=self.pcm_dev[:, 0])                  # r -> 24 kHz, all rows
+        codes = self.codec.encode(self.pcm_dev)                                   # [B, 8, 1]
+        toks = self.lm_gen.step(codes)                                           # [B, dep_q + 1, 1] or None
+        valid = self.lm_gen.valid_rows()                                         # host mirror: no device sync
+        if toks is not None:
+            # rows in their warm-up keep their decoder state: decode mask = active & valid, a device-to-device copy
+            self.dec_mask_host.copy_(torch.from_numpy(valid.astype("int64")))
+            self.dec_mask_dev.copy_(self.dec_mask_host, non_blocking=True)
+            self.codec.set_active_streams(self.dec_mask_dev)
+            pcm = self.codec.decode(toks[:, 1:].clamp(0, self.codec.codebook_size - 1))   # [B, 1, 1920]
+            if self.down is not None:
+                self.down.set_active(self.dec_mask_dev)
+                pcm = self.down(pcm[:, 0], out=self.pcm_out_dev)[:, None]                  # 24 kHz -> r, all rows
+            self.tok_host.copy_(toks[:, :, 0], non_blocking=True)
+            self.pcm_host.copy_(pcm, non_blocking=True)
+        if self.dev.type == "cuda":
+            torch.cuda.current_stream(self.dev).synchronize()
+        self.latencies_ms.append(1e3 * (time.perf_counter() - t0))
+        return {r: (self.tok_host[r].clone(), self.pcm_host[r, 0].clone()) if valid[r] else (None, None) for r in active}

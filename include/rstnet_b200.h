@@ -163,6 +163,8 @@ int rstnet_rows_copy_table_f32(const rstnet_row_copy* table_dev, int32_t n_entri
  * stream so that a single stream can be reset / admitted while the others keep running) */
 int rstnet_counter_add(int64_t* counter, int64_t delta, int32_t n, const int64_t* active /* optional, [n]: 0 = hold */,
                        rstnet_stream_t stream);
+/* counter[i] += delta[i] for i < n (delta [n] int64 on the device): positions of a ragged prefill chunk. */
+int rstnet_counter_add_rows(int64_t* counter, const int64_t* delta, int32_t n, rstnet_stream_t stream);
 
 /* ---- nn.LayerNorm over the last dim, eps inside sqrt (modules/transformer.py:113-114).
  * x row (b,t) at x + b*x_batch_stride + t*dim; y is contiguous [batch*rows_per_batch, dim]. */
@@ -292,6 +294,14 @@ int rstnet_lm_rope_kv_append_bf16(const void* qkv, const void* cos_tab, const vo
                                   const int64_t* offset, int32_t offset_stride /* 0 shared, 1 per stream */, void* q_out,
                                   void* kv, int32_t rows, int32_t B, int32_t n_head, int32_t n_kv, int32_t hs, int32_t cap,
                                   rstnet_stream_t stream);
+/* Row-mapped form (ragged prefill of some streams of a live scope, GPT.prefill_streams; serves the prompt pass of
+ * infer_no_streaming.py:232-240 for a batch of utterances with different prompt lengths): row r is stream row_stream[r] at
+ * position offset[row_stream[r]] + row_tl[r] (per-stream counters); row_stream[r] == -1 marks a padding row that reads
+ * and writes nothing.  Any order of (stream, position) pairs; the same compiled kernel as the uniform form. */
+int rstnet_lm_rope_kv_append_rows_bf16(const void* qkv, const void* cos_tab, const void* sin_tab, int64_t rope_rows,
+                                       int32_t rope_n, const int64_t* offset, const int32_t* row_stream, const int32_t* row_tl,
+                                       void* q_out, void* kv, int32_t rows, int32_t B, int32_t n_head, int32_t n_kv, int32_t hs,
+                                       int32_t cap, rstnet_stream_t stream);
 /* ---- Kyutai pair-RoPE for the Moshi-style LMModel's temporal transformer (models/model.py:364-389; modules/rope.py:11-68,
  * modules/transformer.py:391-399): qkv [rows][3][H][hd] ((p h d) layout); (even, odd) pairs of q / k rotate by
  * freqs[p] * (offset + tl) (freqs [hd/2] fp32 = exp(-ln(max_period) * 2 p / hd), from the host), fp32 inside, one rounding
@@ -307,6 +317,10 @@ int rstnet_lm_rope_pair_kv_append_bf16(const void* qkv, const int64_t* offset, i
 int rstnet_lm_ring_decode_attention_bf16(const void* q, const void* kv, const int64_t* offset, int32_t offset_stride,
                                          void* out, int32_t rows, int32_t B, int32_t n_head, int32_t n_kv, int32_t hs,
                                          int32_t cap, int32_t context, rstnet_stream_t stream);
+/* Row-mapped form: rows as rstnet_lm_rope_kv_append_rows_bf16 (padding rows write no output). */
+int rstnet_lm_ring_decode_attention_rows_bf16(const void* q, const void* kv, const int64_t* offset, const int32_t* row_stream,
+                                              const int32_t* row_tl, void* out, int32_t rows, int32_t B, int32_t n_head,
+                                              int32_t n_kv, int32_t hs, int32_t cap, int32_t context, rstnet_stream_t stream);
 /* out[m][c] = silu(ab[m][c]) * ab[m][I + c]   (LLaMAMLP / ActivationGating) */
 int rstnet_lm_silu_mul_bf16(const void* ab, void* out, int32_t M, int32_t I, rstnet_stream_t stream);
 /* ---- depth transformer attention at codebook step `step` (keys 0..step, capacity dep_q <= 8, no RoPE):
@@ -323,6 +337,14 @@ int rstnet_lm_depth_attention_bf16(const void* qkv, void* kvd, void* out, int32_
 int rstnet_lm_sample_bf16(const void* logits, int32_t rows, int32_t V, int32_t n_valid, int32_t top_k, float temp,
                           uint32_t seed, const int64_t* step_counter, int64_t* tokens, int32_t tok_stride,
                           rstnet_stream_t stream);
+/* Per-row form (InferenceImp over a batch of utterances, each with its own candidate sets infer_no_streaming.py:264-283
+ * and its own random stream): row r samples ids < n_valid_rows[r * n_valid_stride] (NULL: the scalar n_valid for every
+ * row; top_k is clamped per row) with the RNG keyed by (seed, step_rows[r], key_rows[r]) in place of
+ * (seed, *step_counter, r).  With key_rows[r] == r, step_rows[r] == *step_counter and one n_valid it draws exactly the
+ * tokens rstnet_lm_sample_bf16 draws: both run one compiled kernel. */
+int rstnet_lm_sample_rows_bf16(const void* logits, int32_t rows, int32_t V, int32_t n_valid, const int32_t* n_valid_rows,
+                               int32_t n_valid_stride, int32_t top_k, float temp, uint32_t seed, const int64_t* step_rows,
+                               const uint32_t* key_rows, int64_t* tokens, int32_t tok_stride, rstnet_stream_t stream);
 
 /* ---- the acoustic-delay token cache of LMGen.step (models/model.py:490-562; moshi/models/lm.py LMGen.step), per stream:
  * the eager cache writes, input copy, write-back and gather of that step, as two launches around the LM frame.

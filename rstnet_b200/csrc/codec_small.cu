@@ -175,6 +175,10 @@ __global__ void counter_add_kernel(long long* c, long long d, int n, const long 
     if (!active || active[i] != 0) c[i] += d;
 }
 
+__global__ void counter_add_rows_kernel(long long* c, const long long* __restrict__ d, int n) {
+  for (int i = threadIdx.x; i < n; i += blockDim.x) c[i] += d[i];
+}
+
 // ---------------------------------------------------------------- LayerNorm: one warp per row
 __global__ void layer_norm_kernel(const float* __restrict__ x, long long xbs, const float* __restrict__ w,
                                   const float* __restrict__ bias, float* __restrict__ y, long long rows, int rows_per_batch,
@@ -301,6 +305,13 @@ extern "C" int rstnet_counter_add(int64_t* counter, int64_t delta, int32_t n, co
   counter_add_kernel<<<1, n >= 256 ? 256 : 32, 0, (cudaStream_t)stream>>>((long long*)counter, delta, n, (const long long*)active);
   count_launch();
   return check_launch("counter_add");
+}
+
+extern "C" int rstnet_counter_add_rows(int64_t* counter, const int64_t* delta, int32_t n, rstnet_stream_t stream) {
+  RSTNET_REQUIRE(counter && delta && n >= 1, "counter_add_rows: bad argument");
+  counter_add_rows_kernel<<<1, n >= 256 ? 256 : 32, 0, (cudaStream_t)stream>>>((long long*)counter, (const long long*)delta, n);
+  count_launch();
+  return check_launch("counter_add_rows");
 }
 
 extern "C" int rstnet_layer_norm_f32(const float* x, int64_t x_batch_stride, const float* weight, const float* bias,

@@ -99,13 +99,24 @@ __global__ void rms_norm_kernel(const bf16* __restrict__ x, const bf16* __restri
 // slot (pos % cap)  (lit_model.py:560-573, 620-634).  Only the first rope_n dims rotate (rotary_percentage < 1,
 // llama_streaming.py:979-982); the tables are [rope_rows][rope_n].  A position beyond the tables (the reference's
 // cos.index_select would raise) poisons q/k with NaN and sets error bit 1 (2).
+// Row map (ragged prefill of some streams): with row_stream set, row r is stream row_stream[r] at position
+// offset[row_stream[r]] + row_tl[r] instead; row_stream[r] == -1 is a padding row that reads and writes nothing.  A runtime
+// branch, not a second instantiation, so the uniform and the mapped launch run one compiled body (DESIGN.md §6).
 __global__ void rope_kv_append_bf16_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ cosb, const bf16* __restrict__ sinb,
                                            const long long* __restrict__ offset, bf16* __restrict__ q_out, bf16* __restrict__ kv,
                                            int ostride, int B, int n_kv, int q_per_kv, int hs, int cap, int rope_n,
-                                           long long rope_rows) {
+                                           long long rope_rows, const int* __restrict__ row_stream, const int* __restrict__ row_tl) {
   const int row = blockIdx.x / n_kv, g = blockIdx.x % n_kv;
-  const int b = row % B;
-  const long long pos = offset[(long long)b * ostride] + row / B;   // per-stream counters (ostride 1) or one shared (0)
+  int b, tl;
+  if (row_stream) {
+    b = row_stream[row];
+    if (b < 0) return;
+    tl = row_tl[row];
+  } else {
+    b = row % B;
+    tl = row / B;
+  }
+  const long long pos = offset[(long long)b * ostride] + tl;   // per-stream counters (ostride 1) or one shared (0)
   const int slot = (int)(pos % cap);
   const bool bad = pos >= rope_rows;
   if (bad && threadIdx.x == 0) atomicOr(&g_lm_dev_err, 2u);
@@ -175,7 +186,8 @@ __global__ void rope_pair_kv_append_bf16_kernel(const bf16* __restrict__ qkv, co
 // one CTA per (G query heads sharing a kv head, row); 8 lanes share a key row (16 dims = 32 bytes each, so a warp load
 // covers 4 whole 256-byte rows = 1 KB contiguous); per-group online softmax, combined across groups / warps at the end.
 // Mask = RingKVCache.complete + (pos_k>=0)&(delta>=0)&(delta<context) (llama_streaming.py:983-992).
-// Row r = tl*B + b queries stream b at position *offset + tl; all positions of the launch are already in the ring
+// Row r = tl*B + b queries stream b at position *offset + tl, or, with row_stream set, the row map of
+// rope_kv_append_bf16_kernel (padding rows write nothing); all positions of the launch are already in the ring
 // (the caller guarantees no slot a query still needs has been overwritten: see GPT.forward_global's prefill path).
 // The K/V rows travel through a per-lane cp.async ring in shared memory, ATT_STAGES - 1 sweeps (of 32 keys per CTA) in
 // flight per warp -- every lane copies and reads back only its own 16-byte pieces, so cp.async.wait_group is the only
@@ -186,19 +198,28 @@ template <int HS, int G>
 __global__ void __launch_bounds__(ATT_WARPS * 32, (G == 1 ? 3 : 2)) ring_decode_attention_kernel(const bf16* __restrict__ q, const bf16* __restrict__ kv,
                                                                     const long long* __restrict__ offset, bf16* __restrict__ out,
                                                                     int ostride, int B, int nh, int n_kv, int cap, int context,
-                                                                    float scale) {
+                                                                    float scale, const int* __restrict__ row_stream,
+                                                                    const int* __restrict__ row_tl) {
   constexpr int ST = ATT_STAGES;
   constexpr int DPL = HS / 8;  // dims per lane
   __shared__ float sm_m[G][ATT_WARPS], sm_l[G][ATT_WARPS], sm_acc[G][ATT_WARPS][HS];
   const int nhg = nh / G;
   const int hg = blockIdx.x % nhg, row = blockIdx.x / nhg;
   const int h0 = hg * G;
-  const int b = row % B;
+  int b, tl;
+  if (row_stream) {
+    b = row_stream[row];
+    if (b < 0) return;   // the whole CTA serves this row
+    tl = row_tl[row];
+  } else {
+    b = row % B;
+    tl = row / B;
+  }
   const int g = h0 / (nh / n_kv);
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   const int grp = lane / 8, sub = lane % 8;
   constexpr int nwarps = ATT_WARPS;
-  const long long pos = offset[(long long)b * ostride] + row / B;  // position of the query; its key/value were appended just before
+  const long long pos = offset[(long long)b * ostride] + tl;  // position of the query; its key/value were appended just before
   long long lo = pos - context + 1;
   if (lo < 0) lo = 0;
   if (lo < pos + 2 - cap) lo = pos + 2 - cap;  // ring quirk: the oldest slot is labelled end_offset and masked
@@ -332,11 +353,13 @@ __global__ void __launch_bounds__(ATT_WARPS * 32, (G == 1 ? 3 : 2)) ring_decode_
 // one CTA per (row, head group); the dynamic shared memory is the cp.async ring: stages x warps x lanes x (K, V pieces) x 16 B
 template <int HS, int G>
 void launch_ring_decode_attention(cudaStream_t st, const bf16* q, const bf16* kv, const long long* offset, bf16* out, int ostride,
-                                  int rows, int B, int nh, int n_kv, int cap, int context, float scale) {
+                                  int rows, int B, int nh, int n_kv, int cap, int context, float scale, const int* row_stream,
+                                  const int* row_tl) {
   constexpr int smem = ATT_STAGES * ATT_WARPS * 32 * (HS / 64) * 2 * 16;
   static unsigned long long attr = 0;
   smem_optin(ring_decode_attention_kernel<HS, G>, smem, attr);
-  ring_decode_attention_kernel<HS, G><<<rows * (nh / G), ATT_WARPS * 32, smem, st>>>(q, kv, offset, out, ostride, B, nh, n_kv, cap, context, scale);
+  ring_decode_attention_kernel<HS, G><<<rows * (nh / G), ATT_WARPS * 32, smem, st>>>(q, kv, offset, out, ostride, B, nh, n_kv, cap, context, scale,
+                                                                                                    row_stream, row_tl);
 }
 
 // ---------------------------------------------------------------- SiLU gating: out = silu(a) * b  (bf16 roundings as eager)
@@ -603,11 +626,28 @@ __device__ __noinline__ void sample_row(const bf16* __restrict__ lr, int n_valid
   }
 }
 
+// Per-row parameters (batches of utterances at different points of their generation): with step_rows set, row r draws
+// its noise from (seed, step_rows[r], key_rows[r]) instead of (seed, *step_counter, r); with nvalid_rows set, its
+// candidates are the ids < nvalid_rows[r * nv_stride] (top_k clamped to them as the host does for one n_valid).
+// Runtime branches around one call of the same sample_row body, so both forms draw identical tokens from identical inputs.
 __global__ void sample_kernel(const bf16* __restrict__ logits, int V, int n_valid, int top_k, float temp, uint32_t seed,
-                              const long long* __restrict__ step_counter, long long* __restrict__ tokens, int tok_stride) {
+                              const long long* __restrict__ step_counter, long long* __restrict__ tokens, int tok_stride,
+                              const int* __restrict__ nvalid_rows, int nv_stride, const long long* __restrict__ step_rows,
+                              const uint32_t* __restrict__ key_rows) {
   const int row = blockIdx.x;
-  const uint32_t stepc = step_counter ? (uint32_t)(*step_counter) : 0u;
-  sample_row(logits + (long long)row * V, n_valid, top_k, temp, seed, stepc, row, tokens + (long long)row * tok_stride);
+  uint32_t stepc, key = (uint32_t)row;
+  if (step_rows) {
+    stepc = (uint32_t)step_rows[row];
+    key = key_rows[row];
+  } else {
+    stepc = step_counter ? (uint32_t)(*step_counter) : 0u;
+  }
+  if (nvalid_rows) {
+    n_valid = nvalid_rows[(long long)row * nv_stride];
+    if (n_valid <= 0 || n_valid > V) n_valid = V;
+    if (top_k > n_valid) top_k = n_valid;
+  }
+  sample_row(logits + (long long)row * V, n_valid, top_k, temp, seed, stepc, (int)key, tokens + (long long)row * tok_stride);
 }
 
 }  // namespace rstnet
@@ -650,9 +690,24 @@ extern "C" int rstnet_lm_rope_kv_append_bf16(const void* qkv, const void* cos_ta
   RSTNET_REQUIRE(rope_n >= 0 && rope_n <= hs && rope_n % 2 == 0 && rope_rows > 0, "lm_rope_kv_append: bad rope table (%d of %d dims)", rope_n, hs);
   rope_kv_append_bf16_kernel<<<dim3(rows * n_kv), dim3(64), 0, (cudaStream_t)stream>>>((const bf16*)qkv, (const bf16*)cos_tab,
              (const bf16*)sin_tab, (const long long*)offset, (bf16*)q_out, (bf16*)kv, offset_stride ? 1 : 0, B, n_kv, n_head / n_kv, hs,
-             cap, rope_n, (long long)rope_rows);
+             cap, rope_n, (long long)rope_rows, nullptr, nullptr);
   count_launch();
   return check_launch("lm_rope_kv_append");
+}
+
+extern "C" int rstnet_lm_rope_kv_append_rows_bf16(const void* qkv, const void* cos_tab, const void* sin_tab, int64_t rope_rows,
+                                                  int32_t rope_n, const int64_t* offset, const int32_t* row_stream,
+                                                  const int32_t* row_tl, void* q_out, void* kv, int32_t rows, int32_t B,
+                                                  int32_t n_head, int32_t n_kv, int32_t hs, int32_t cap, rstnet_stream_t stream) {
+  RSTNET_REQUIRE(qkv && cos_tab && sin_tab && offset && row_stream && row_tl && q_out && kv, "lm_rope_kv_append_rows: null pointer");
+  RSTNET_REQUIRE(rows > 0 && B > 0, "lm_rope_kv_append_rows: bad shape (rows %d, B %d)", rows, B);
+  RSTNET_REQUIRE(n_kv > 0 && n_head % n_kv == 0, "lm_rope_kv_append_rows: n_head (%d) must be a multiple of n_kv (%d)", n_head, n_kv);
+  RSTNET_REQUIRE(rope_n >= 0 && rope_n <= hs && rope_n % 2 == 0 && rope_rows > 0, "lm_rope_kv_append_rows: bad rope table (%d of %d dims)", rope_n, hs);
+  rope_kv_append_bf16_kernel<<<dim3(rows * n_kv), dim3(64), 0, (cudaStream_t)stream>>>((const bf16*)qkv, (const bf16*)cos_tab,
+             (const bf16*)sin_tab, (const long long*)offset, (bf16*)q_out, (bf16*)kv, 1, B, n_kv, n_head / n_kv, hs, cap, rope_n,
+             (long long)rope_rows, (const int*)row_stream, (const int*)row_tl);
+  count_launch();
+  return check_launch("lm_rope_kv_append_rows");
 }
 
 extern "C" int rstnet_lm_rope_pair_kv_append_bf16(const void* qkv, const int64_t* offset, int32_t offset_stride, void* q_out, void* kv,
@@ -679,9 +734,27 @@ extern "C" int rstnet_lm_ring_decode_attention_bf16(const void* q, const void* k
   const auto launch = hs == 128 ? (G == 2 ? launch_ring_decode_attention<128, 2> : launch_ring_decode_attention<128, 1>)
                                 : (G == 2 ? launch_ring_decode_attention<64, 2> : launch_ring_decode_attention<64, 1>);
   launch((cudaStream_t)stream, (const bf16*)q, (const bf16*)kv, (const long long*)offset, (bf16*)out, offset_stride ? 1 : 0, rows, B,
-         n_head, n_kv, cap, context, scale);
+         n_head, n_kv, cap, context, scale, nullptr, nullptr);
   count_launch();
   return check_launch("lm_ring_decode_attention");
+}
+
+extern "C" int rstnet_lm_ring_decode_attention_rows_bf16(const void* q, const void* kv, const int64_t* offset, const int32_t* row_stream,
+                                                         const int32_t* row_tl, void* out, int32_t rows, int32_t B, int32_t n_head,
+                                                         int32_t n_kv, int32_t hs, int32_t cap, int32_t context, rstnet_stream_t stream) {
+  RSTNET_REQUIRE(q && kv && offset && row_stream && row_tl && out, "lm_ring_decode_attention_rows: null pointer");
+  RSTNET_REQUIRE(hs == 128 || hs == 64, "lm_ring_decode_attention_rows: head_size must be 64 or 128 (got %d)", hs);
+  RSTNET_REQUIRE(rows > 0 && B > 0, "lm_ring_decode_attention_rows: bad shape (rows %d, B %d)", rows, B);
+  RSTNET_REQUIRE(n_kv > 0 && n_head % n_kv == 0, "lm_ring_decode_attention_rows: n_head (%d) must be a multiple of n_kv (%d)", n_head, n_kv);
+  const float scale = 1.0f / sqrtf((float)hs);
+  const int q_per_kv = n_head / n_kv;
+  const int G = q_per_kv % 2 == 0 ? 2 : 1;
+  const auto launch = hs == 128 ? (G == 2 ? launch_ring_decode_attention<128, 2> : launch_ring_decode_attention<128, 1>)
+                                : (G == 2 ? launch_ring_decode_attention<64, 2> : launch_ring_decode_attention<64, 1>);
+  launch((cudaStream_t)stream, (const bf16*)q, (const bf16*)kv, (const long long*)offset, (bf16*)out, 1, rows, B, n_head, n_kv, cap,
+         context, scale, (const int*)row_stream, (const int*)row_tl);
+  count_launch();
+  return check_launch("lm_ring_decode_attention_rows");
 }
 
 extern "C" int rstnet_lm_silu_mul_bf16(const void* ab, void* out, int32_t M, int32_t I, rstnet_stream_t stream) {
@@ -712,7 +785,21 @@ extern "C" int rstnet_lm_sample_bf16(const void* logits, int32_t rows, int32_t V
   if (n_valid <= 0 || n_valid > V) n_valid = V;
   if (top_k > n_valid) top_k = n_valid;   // torch.topk would raise; the whole support is the natural reading
   sample_kernel<<<dim3(rows), dim3(1024), 0, (cudaStream_t)stream>>>((const bf16*)logits, V, n_valid, top_k, temp, (uint32_t)seed,
-             (const long long*)step_counter, (long long*)tokens, tok_stride);
+             (const long long*)step_counter, (long long*)tokens, tok_stride, nullptr, 0, nullptr, nullptr);
   count_launch();
   return check_launch("lm_sample");
+}
+
+extern "C" int rstnet_lm_sample_rows_bf16(const void* logits, int32_t rows, int32_t V, int32_t n_valid, const int32_t* n_valid_rows,
+                                          int32_t n_valid_stride, int32_t top_k, float temp, uint32_t seed, const int64_t* step_rows,
+                                          const uint32_t* key_rows, int64_t* tokens, int32_t tok_stride, rstnet_stream_t stream) {
+  RSTNET_REQUIRE(logits && tokens && step_rows && key_rows && rows > 0 && V > 0, "lm_sample_rows: bad argument");
+  RSTNET_REQUIRE(top_k <= SAMPLE_CAND && (top_k == 0 || temp > 0.f), "lm_sample_rows: top_k <= %d and temp > 0 required (top_k=%d)", SAMPLE_CAND, top_k);
+  if (n_valid <= 0 || n_valid > V) n_valid = V;
+  if (!n_valid_rows && top_k > n_valid) top_k = n_valid;   // with per-row candidate counts the kernel clamps per row
+  sample_kernel<<<dim3(rows), dim3(1024), 0, (cudaStream_t)stream>>>((const bf16*)logits, V, n_valid, top_k, temp, (uint32_t)seed,
+             nullptr, (long long*)tokens, tok_stride, (const int*)n_valid_rows, n_valid_stride, (const long long*)step_rows,
+             key_rows);
+  count_launch();
+  return check_launch("lm_sample_rows");
 }

@@ -36,6 +36,8 @@ from .codec import _register, on_own_device
 MAX_ROWS = 128   # rows (stream, position) pairs per launch of a prefill chunk or a forward_local slice
 MAX_STREAMS = 256   # streams of one decode scope (one position each): the widest weight-streaming GEMM reads each weight
                     # tile once for up to 256 rows
+ROW_BUCKETS = (16, 32, 64, 128)   # launch widths of a ragged prefill chunk (padding rows fill the rest): one chunk state and
+                                  # one set of GEMM plans per width
 
 
 @dataclass
@@ -481,15 +483,24 @@ class GPT(nn.Module):
     @torch.no_grad()
     @on_own_device
     def forward_step(self, sequence: torch.Tensor, *, use_sampling: bool = True, temp_text: float = 0.7, top_k_text: int = 25,
-                     temp: float = 0.8, top_k: int = 30, audio_valid=2049, depth_ring_quirk: bool = True) -> torch.Tensor:
+                     temp: float = 0.8, top_k: int = 30, audio_valid=2049, depth_ring_quirk: bool = True, sample_key=None,
+                     sample_step=None) -> torch.Tensor:
         """One generated frame: temporal step on sequence[B,9,1], text token, then the 8 depth steps, each sampled
         on the device (sample_token / sample_token_audio[_2048], utils/sampling.py:85-154: use_sampling False ->
         argmax over the whole card; True -> temperature + top-k (top_k == 0: plain multinomial) over ids <
         audio_valid).  Returns tokens [B, 9] (text, audio_0..7).  With use_cuda_graphs the whole frame is a single
-        graph replay.  depth_ring_quirk False evaluates the depth steps as forward_local does (see there)."""
+        graph replay.  depth_ring_quirk False evaluates the depth steps as forward_local does (see there).
+
+        Per-row sampling (every row an utterance at its own point of generation): audio_valid as an int tensor
+        [B, dep_q] gives each row its own candidate counts, and each row draws its noise from its own key and step
+        counter instead of (row, scope frame counter).  sample_key [B] (uint32 values) and sample_step [B] (int64), when
+        given, set the scope's per-row keys and step counters before the frame; otherwise they keep their values.  The
+        step counters start at 0 (scope entry, reset_streaming of the row) and advance by one per frame for active rows.
+        All three live in fixed device buffers, so one captured graph serves every frame."""
         if self._state is None:
             raise RstnetError("forward_step is a streaming call: use it inside `with gpt.streaming(B):`")
-        return self._state.forward_step(sequence, use_sampling, temp_text, top_k_text, temp, top_k, audio_valid, depth_ring_quirk)
+        return self._state.forward_step(sequence, use_sampling, temp_text, top_k_text, temp, top_k, audio_valid, depth_ring_quirk,
+                                        sample_key, sample_step)
 
     @torch.no_grad()
     @on_own_device
@@ -499,6 +510,17 @@ class GPT(nn.Module):
         if self._state is None:
             raise RstnetError("prefill is a streaming call: use it inside `with gpt.streaming(B):`")
         self._state.forward_global(sequence, want_outputs=False)
+
+    @torch.no_grad()
+    @on_own_device
+    def prefill_streams(self, prompts) -> None:
+        """Feed each listed stream its own prompt: prompts {stream: int64 [9, T_s]}.  Stream s takes T_s positions from its
+        current one on (KV ring + position counter, as prefill does for all streams); every other stream -- ring, position
+        counter, active flag -- is left untouched, so utterances can join a scope while others are mid-generation.  The
+        rows of all listed streams are packed into launches of at most MAX_ROWS rows."""
+        if self._state is None:
+            raise RstnetError("prefill_streams is a streaming call: use it inside `with gpt.streaming(B):`")
+        self._state.prefill_streams(prompts)
 
     def forward(self, *a, **kw):
         raise NotImplementedError("training / teacher-forcing forward is out of scope; use forward_global / forward_local")
@@ -510,10 +532,15 @@ class _LMState:
     has tn > 1 rows per stream and shares the parent's KV rings and position counters; a `parts == ("depth",)` state
     only holds the depth transformer (forward_local)."""
 
-    def __init__(self, m: GPT, B: int, tn: int = 1, parent: Optional["_LMState"] = None, parts=("temporal", "depth")):
+    def __init__(self, m: GPT, B: int, tn: int = 1, parent: Optional["_LMState"] = None, parts=("temporal", "depth"),
+                 rows: Optional[int] = None):
+        """rows: a ragged prefill chunk of that many rows (with `parent`): row r is stream row_stream[r] at position
+        offset + row_tl[r] (-1: padding), and the counters advance by `delta` per stream."""
         c, dev = m.config, m.device
         self.m, self.B, self.c, self.tn = m, B, c, tn
-        M = self.M = B * tn
+        M = self.M = B * tn if rows is None else rows
+        if rows is not None and (parent is None or rows > MAX_ROWS):
+            raise RstnetError(f"a ragged prefill chunk has a parent scope and at most {MAX_ROWS} rows (got {rows})")
         if tn == 1 and B > MAX_STREAMS:
             raise RstnetError(f"at most {MAX_STREAMS} streams per streaming scope (got {B})")
         if tn > 1 and M > MAX_ROWS:
@@ -552,7 +579,12 @@ class _LMState:
         self.seed = 1234
         self.depth_step: Optional[int] = None
         self.children: Dict[int, "_LMState"] = {}
+        self.row_children: Dict[int, "_LMState"] = {}
         self.has_temporal = "temporal" in parts
+        self.row_mapped = rows is not None
+        if self.row_mapped:
+            self.row_stream, self.row_tl = z(M, dtype=torch.int32), z(M, dtype=torch.int32)
+            self.delta = z(B, dtype=torch.int64)
 
         if self.has_temporal:
             self._build_temporal(P, G, z, parent)
@@ -564,6 +596,10 @@ class _LMState:
             self.tokens = z(M, c.dep_q + 1, dtype=torch.int64)
             self._idbuf = z(M, dtype=torch.int64)
             self.frame_counter = z(1, dtype=torch.int64)
+            # per-row sampling (forward_step with an audio_valid table): candidate counts, RNG keys, step counters
+            self.row_valid = z(M, c.dep_q, dtype=torch.int32)
+            self.row_key = z(M, dtype=torch.int32)
+            self.row_step = z(M, dtype=torch.int64)
             hd = D // c.codecformer_heads
             self.dkv_all = z(c.codecformer_layers, 2, M, c.codecformer_heads, c.dep_q, hd)
             self.dkv = [self.dkv_all[l] for l in range(c.codecformer_layers)]
@@ -668,6 +704,10 @@ class _LMState:
             self.pos_host[idx.numpy()] = 0
         if hasattr(self, "frame_counter"):
             self.frame_counter.zero_()
+            if streams is None:
+                self.row_step.zero_()
+            else:
+                self.row_step[idx.to(self.row_step.device)] = 0
         self.depth_step = None
 
     # ---- launch sequences -------------------------------------------------------------------
@@ -682,6 +722,20 @@ class _LMState:
         _lib.check(L.rstnet_lm_rms_norm_bf16(self.x.data_ptr(), self.n1_first.data_ptr(), self.xn.data_ptr(), M, E, c.norm_eps, 0, st), "rms")
         for l, ly in enumerate(self.layers):
             ly["qkv"].run()
+            if self.row_mapped:
+                _lib.check(L.rstnet_lm_rope_kv_append_rows_bf16(self.qkv.data_ptr(), self.cos.data_ptr(), self.sin.data_ptr(),
+                                                                self.cos.shape[0], c.rope_n_elem, self.offset.data_ptr(),
+                                                                self.row_stream.data_ptr(), self.row_tl.data_ptr(), self.q.data_ptr(),
+                                                                self.kv[l].data_ptr(), M, B, c.n_head, c.n_query_groups,
+                                                                c.head_size, self.cap, st), "rope_kv_rows")
+                _lib.check(L.rstnet_lm_ring_decode_attention_rows_bf16(self.q.data_ptr(), self.kv[l].data_ptr(), self.offset.data_ptr(),
+                                                                       self.row_stream.data_ptr(), self.row_tl.data_ptr(),
+                                                                       self.att.data_ptr(), M, B, c.n_head, c.n_query_groups,
+                                                                       c.head_size, self.cap, c.context, st), "attention_rows")
+                ly["proj"].run()
+                ly["fc"].run()
+                ly["down"].run()
+                continue
             _lib.check(L.rstnet_lm_rope_kv_append_bf16(self.qkv.data_ptr(), self.cos.data_ptr(), self.sin.data_ptr(), self.cos.shape[0],
                                                        c.rope_n_elem, self.offset.data_ptr(), ost, self.q.data_ptr(),
                                                        self.kv[l].data_ptr(), M, B, c.n_head, c.n_query_groups, c.head_size, self.cap, st),
@@ -694,7 +748,10 @@ class _LMState:
             ly["down"].run()   # + residual + next pre-norm -> xn (last layer: ln_f -> transformer_out)
         if head:
             self.head.run()
-        ops.counter_add(self.offset, self.tn, self.active)
+        if self.row_mapped:
+            _lib.check(L.rstnet_counter_add_rows(self.offset.data_ptr(), self.delta.data_ptr(), B, st), "counter_add_rows")
+        else:
+            ops.counter_add(self.offset, self.tn, self.active)
 
     def _depth(self, k: int, ids: Optional[torch.Tensor], id_stride: int, quirk: bool = True):
         """ids None: the step's input embedding is already in self.demb (forward_local passes features for step 0)."""
@@ -721,6 +778,14 @@ class _LMState:
         _lib.check(_lib.lib().rstnet_lm_sample_bf16(logits.data_ptr(), self.M, V, n_valid, top_k, float(temp), self.seed + salt,
                                                     self.frame_counter.data_ptr(), self.tokens.data_ptr() + 8 * col,
                                                     self.c.dep_q + 1, ops._stream()), "sample")
+
+    def _sample_rows(self, logits: torch.Tensor, V: int, per_row_valid: Optional[int], top_k: int, temp: float, col: int, salt: int):
+        """per_row_valid: column of row_valid holding the rows' candidate counts (None: all V ids)"""
+        nv = None if per_row_valid is None else self.row_valid.data_ptr() + 4 * per_row_valid
+        _lib.check(_lib.lib().rstnet_lm_sample_rows_bf16(logits.data_ptr(), self.M, V, V, nv, self.c.dep_q, top_k, float(temp),
+                                                         self.seed + salt, self.row_step.data_ptr(), self.row_key.data_ptr(),
+                                                         self.tokens.data_ptr() + 8 * col, self.c.dep_q + 1, ops._stream()),
+                   "sample_rows")
 
     def _replay(self, key, fn):
         if not self.m.use_cuda_graphs:
@@ -804,6 +869,55 @@ class _LMState:
             return None
         return torch.cat(outs, 1), torch.cat(logits, 1)
 
+    def prefill_streams(self, prompts):
+        c, dev = self.c, self.m.device
+        K = c.n_q + 1
+        todo = []   # [stream, prompt [T, K] on the device, positions fed]
+        for s, p in prompts.items():
+            s = int(s)
+            if not 0 <= s < self.B:
+                raise RstnetError(f"stream index {s} outside [0, {self.B})")
+            if p.dim() != 2 or p.shape[0] != K:
+                raise RstnetError(f"the prompt of stream {s} must be [{K}, T], got {tuple(p.shape)}")
+            if p.shape[1] > self.m.max_seq_length:
+                raise ValueError(f"Cannot forward sequence of length {p.shape[1]}, max seq length is only {self.m.max_seq_length}.")
+            if int(self.pos_host[s]) + p.shape[1] > self.cos.shape[0]:
+                raise IndexError(f"position {int(self.pos_host[s]) + p.shape[1] - 1} of stream {s} is beyond block_size = "
+                                 f"{self.cos.shape[0]} (RoPE table exhausted; reset the stream or raise Config.block_size)")
+            if p.shape[1] > 0:
+                todo.append([s, p.to(device=dev, dtype=torch.int64).t(), 0])
+        while todo:
+            rs, rt, parts = [], [], []
+            delta = np.zeros(self.B, dtype=np.int64)
+            for it in todo:
+                s, p, done = it
+                budget = MAX_ROWS - len(rs)
+                if budget == 0:
+                    break
+                # a chunk appends all its keys before any of its queries run: several positions of a stream only while its
+                # ring does not wrap inside the chunk (as forward_global's prefill), one per chunk after that
+                tn = min(p.shape[0] - done, budget, max(1, self.cap - int(self.pos_host[s])))
+                rs += [s] * tn
+                rt += range(tn)
+                parts.append(p[done:done + tn])
+                delta[s] = tn
+                it[2] += tn
+            n = len(rs)
+            M = next(b for b in ROW_BUCKETS if b >= n)
+            ch = self.row_children.get(M)
+            if ch is None:
+                ch = self.row_children[M] = _LMState(self.m, self.B, parent=self, parts=("temporal",), rows=M)
+            pad = M - n
+            ch.row_stream.copy_(torch.tensor(rs + [-1] * pad, dtype=torch.int32))
+            ch.row_tl.copy_(torch.tensor(rt + [0] * pad, dtype=torch.int32))
+            ch.delta.copy_(torch.from_numpy(delta))
+            if pad:
+                parts.append(torch.full((pad, K), self.m.zero_token_id, dtype=torch.int64, device=dev))   # an all-zero-token row
+            ch.seq.copy_(torch.cat(parts))
+            ch._temporal(head=False)
+            self.pos_host += delta
+            todo = [it for it in todo if it[2] < it[1].shape[0]]
+
     def forward_codecformer(self, k: int, sequence: torch.Tensor, transformer_out: torch.Tensor):
         if self.depth_step is None:
             raise RstnetError("call inside `with gpt.codecformer.streaming(B):`")
@@ -829,14 +943,50 @@ class _LMState:
                 self._depth(k, self.tokens[:, k - 1], c.dep_q + 1, quirk=False)
             out[:, k].copy_(self.dlogits)
 
-    def forward_step(self, sequence, use_sampling, temp_text, top_k_text, temp, top_k, audio_valid, quirk=True):
+    def forward_step(self, sequence, use_sampling, temp_text, top_k_text, temp, top_k, audio_valid, quirk=True, sample_key=None,
+                     sample_step=None):
         c = self.c
         if sequence.shape[0] != self.B or sequence.shape[2] != 1:
             raise RstnetError(f"forward_step takes sequence [{self.B}, {c.n_q + 1}, 1], got {tuple(sequence.shape)}")
+        per_row = torch.is_tensor(audio_valid)
+        if per_row:
+            if tuple(audio_valid.shape) != (self.B, c.dep_q):
+                raise RstnetError(f"a per-row audio_valid is [{self.B}, {c.dep_q}], got {tuple(audio_valid.shape)}")
+            if sample_key is not None:
+                k = torch.as_tensor(sample_key, dtype=torch.int64).reshape(self.B) & 0xFFFFFFFF
+                self.row_key.copy_(torch.where(k >= 2 ** 31, k - 2 ** 32, k).to(torch.int32))   # the uint32 bits
+            if sample_step is not None:
+                self.row_step.copy_(torch.as_tensor(sample_step, dtype=torch.int64).reshape(self.B))
+        elif sample_key is not None or sample_step is not None:
+            raise RstnetError("sample_key / sample_step select per-row sampling: pass audio_valid as a [B, dep_q] tensor")
         self._advance_host(1)
         self.seq.copy_(sequence[:, :, 0])
-        self._replay(*self._frame(use_sampling, temp_text, top_k_text, temp, top_k, audio_valid, quirk))
+        if per_row:
+            self.row_valid.copy_(audio_valid)
+            self._replay(*self._frame_rows(use_sampling, temp_text, top_k_text, temp, top_k, quirk))
+        else:
+            self._replay(*self._frame(use_sampling, temp_text, top_k_text, temp, top_k, audio_valid, quirk))
         return self.tokens.clone()
+
+    def _frame_rows(self, use_sampling, temp_text, top_k_text, temp, top_k, quirk):
+        """_frame with per-row candidate counts (row_valid), RNG keys (row_key) and step counters (row_step)."""
+        c = self.c
+        sampling_text = use_sampling and temp_text > 0.0
+        sampling = use_sampling and temp > 0.0
+        tk_text = (top_k_text if top_k_text > 0 else -1) if sampling_text else 0
+        tk = (top_k if top_k > 0 else -1) if sampling else 0
+
+        def frame():
+            self._temporal()
+            self._sample_rows(self.logits, c.padded_vocab_size, None, tk_text, temp_text if sampling_text else 1.0, 0, 0)
+            self.tout.copy_(self.out)
+            for k in range(c.dep_q):
+                self._depth(k, self.tokens[:, k], c.dep_q + 1, quirk=quirk)
+                # the 2048 / 2049 candidate sets exist on the sampling path only (sampling.py:107-154)
+                self._sample_rows(self.dlogits, c.audio_card, k if sampling else None, tk, temp if sampling else 1.0, k + 1, k + 1)
+            ops.counter_add(self.row_step, 1, self.active)
+
+        return ("frame_rows", tk_text, float(temp_text), tk, float(temp), bool(quirk)), frame
 
     def _frame(self, use_sampling, temp_text, top_k_text, temp, top_k, audio_valid, quirk):
         """(graph key, launch sequence) of one generated frame from the ids in self.seq to the tokens in self.tokens."""

@@ -9,6 +9,10 @@
     (modules/conv.py:245-254), so audio padding would change a clip's last frame.
   * `reconstruct_directory` / `python -m rstnet_b200.offline reconstruct`: AudioCodec/MimiCodec/inference.py:111-148 -- every
     wav of a directory through encode -> decode, written under the same name at 24 kHz.
+  * `synthesize` / `python -m rstnet_b200.offline synthesize`: the TTS loop of infer_no_streaming.py main() (:119-143) over a
+    whole corpus (`torch.save`d dict utt_id -> int64 [9, L]) with InferenceImp.generate_many: utterances of any prompt and
+    generation length decode together, a finished row taking the next utterance.  Writes utt_id -> int16 codes [8, T] and,
+    with a codec, one 24 kHz 16-bit wav per utterance (Mimi decode of equal-length groups, as main()'s detokenize).
 
 Audio at any integer sample rate is resampled to 24 kHz on the GPU the way the reference does it,
 torchaudio.transforms.Resample(sr, 24000) with its defaults (mimi_tokenizer.py:40,67; inference.py:24-34 `convert_audio`:
@@ -112,6 +116,58 @@ def reconstruct_directory(codec: MimiCodec, src: str, dst: str) -> int:
     return n
 
 
+@torch.no_grad()
+def synthesize(imp, corpus: Dict[str, torch.Tensor], capacity: int = 32, seeds=None) -> Dict[str, torch.Tensor]:
+    """{utt_id: int16 [8, T]} for every utterance of `corpus` ({utt_id: int64 [9, L]}), through imp.generate_many."""
+    items = ((utt, torch.as_tensor(seq, dtype=torch.int64)) for utt, seq in corpus.items())
+    return {utt: codes.to(torch.int16).cpu() for utt, codes in imp.generate_many(items, capacity, seeds=seeds)}
+
+
+@torch.no_grad()
+def write_codes_wav(codec: MimiCodec, codes: Dict[str, torch.Tensor], dst: str, batch_size: int = 64) -> int:
+    """One `<utt_id>_sample.wav` per utterance (main()'s file name), 24 kHz 16-bit: codes of equal length decode as one batch."""
+    os.makedirs(dst, exist_ok=True)
+    by_len = defaultdict(list)
+    for utt, c in codes.items():
+        if c.shape[-1] > 0:
+            by_len[c.shape[-1]].append(utt)
+    for T, utts in by_len.items():
+        for i in range(0, len(utts), batch_size):
+            part = utts[i:i + batch_size]
+            wav = codec.decode(torch.stack([codes[u] for u in part]).to(torch.int64))
+            for u, w in zip(part, wav):
+                write_wav(os.path.join(dst, f"{u}_sample.wav"), w[0], codec.sample_rate)
+    return sum(len(u) for u in by_len.values())
+
+
+def _load_gpt(config_path: str, checkpoint: str, device: str):
+    """GPT(Config from json) with the checkpoint's ['model'] weights, `module.` prefixes stripped
+    (utils/train_utils.py:resume_for_inference), in bf16 on `device`."""
+    import json
+    from .lm import GPT, Config
+    m = GPT(Config(**json.load(open(config_path))))
+    sd = torch.load(checkpoint, map_location="cpu")["model"]
+    m.load_state_dict({k.split("module.")[-1] if k.startswith("module.") else k: v for k, v in sd.items()})
+    return m.to(device, torch.bfloat16).eval()
+
+
+def _synthesize_cli(args) -> int:
+    from .infer import InferenceImp
+    model = _load_gpt(args.config, args.checkpoint, args.device)
+    imp = InferenceImp(None, model, "sampling", args.temp_text, args.top_k_text, args.temp, args.top_k, "TTS")
+    imp.use_sampling = args.use_sampling
+    corpus = torch.load(args.input, map_location="cpu")
+    codes = synthesize(imp, corpus, args.capacity)
+    save_tokens(codes, args.output_file)
+    print(f"synthesized {len(codes)} utterances -> {args.output_file}")
+    if args.wav_dir:
+        if not args.codec_weights:
+            raise SystemExit("--wav-dir needs --codec-weights")
+        codec = _load_codec(argparse.Namespace(weights=args.codec_weights, config=args.codec_config, device=args.device))
+        print(f"wrote {write_codes_wav(codec, codes, args.wav_dir)} wavs -> {args.wav_dir}")
+    return 0
+
+
 def _load_codec(args) -> MimiCodec:
     import json
     cfg = json.load(open(args.config)) if args.config else dict(encoder_rates=[8, 6, 5, 4], codebook_size=2048, codebook_dim=256, rvq_layers=8)
@@ -134,7 +190,25 @@ def main(argv=None) -> int:
     sub.choices["tokenize"].add_argument("--batch-size", type=int, default=256)
     sub.choices["reconstruct"].add_argument("--input", required=True)
     sub.choices["reconstruct"].add_argument("--output", required=True)
+    p = sub.add_parser("synthesize", help="TTS codes for a corpus of utterances (infer_no_streaming.py main())")
+    p.add_argument("--input", required=True, help="torch.save'd dict utt_id -> int64 [9, L]")
+    p.add_argument("--config", required=True, help="json with the GPT Config fields")
+    p.add_argument("--checkpoint", required=True, help="training checkpoint ({'model': state_dict})")
+    p.add_argument("--output-file", required=True, help="torch.save'd dict utt_id -> int16 [8, T]")
+    p.add_argument("--capacity", type=int, default=32, help="utterances decoded together (<= 256)")
+    p.add_argument("--use-sampling", action=argparse.BooleanOptionalAction, default=True,
+                   help="sample (the reference hard-codes this); --no-use-sampling decodes by argmax")
+    p.add_argument("--temp", type=float, default=0.8)
+    p.add_argument("--top-k", type=int, default=30)
+    p.add_argument("--temp-text", type=float, default=0.7)
+    p.add_argument("--top-k-text", type=int, default=25)
+    p.add_argument("--wav-dir", default=None, help="also write <utt_id>_sample.wav here (needs --codec-weights)")
+    p.add_argument("--codec-weights", default=None)
+    p.add_argument("--codec-config", default=None, help="json with the MimiCodec constructor arguments")
+    p.add_argument("--device", default="cuda")
     args = ap.parse_args(argv)
+    if args.cmd == "synthesize":
+        return _synthesize_cli(args)
     codec = _load_codec(args)
     if args.cmd == "tokenize":
         def items():

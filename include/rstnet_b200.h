@@ -111,7 +111,14 @@ int rstnet_tc_gemm_run(const rstnet_tc_plan* plan, rstnet_stream_t stream);
 void rstnet_tc_gemm_destroy(rstnet_tc_plan* plan);
 /* the plan's tile grid: M tiles (I tiles x O_out), N tiles, tile width */
 int rstnet_tc_gemm_grid(const rstnet_tc_plan* plan, int32_t* grid_x, int32_t* grid_y, int32_t* tile_n);
-/* hi[i] = tf32_rna(x[i]); lo[i] = tf32_rna(x[i] - hi[i])  (one-time weight preparation for precision 0) */
+/* hi[i] = tf32_rna(x[i]); lo[i] = tf32_rna(x[i] - hi[i])  (one-time weight preparation for precision 0)
+ * tf32_rna rounds to nearest with ties away from zero.  Non-finite x: NaN -> hi a quiet NaN (a NaN in the top 19 bits, the
+ * ones the tensor core reads), lo = 0; +-Inf -> hi = +-Inf, lo = 0.  Finite x with |x| >= 0x7F7FF000 (about 3.4e38)
+ * rounds to hi = +-Inf and lo = -+Inf: keep weights and activations below that.
+ * Non-finite activations: a NaN or +-Inf in A (after pre_act) gives the non-finite outputs the float64 contraction gives,
+ * with the same class, at both precisions.  An infinite WEIGHT at precision 0 gives a non-finite output where the float64
+ * result is +-Inf, but it may be NaN: the split product adds a_lo * w_hi = a_lo * Inf, which is NaN where a_lo == 0 and
+ * opposes a_hi * Inf where a_lo has the other sign. */
 int rstnet_tf32_split_f32(const float* x, float* hi, float* lo, int64_t n, rstnet_stream_t stream);
 
 /* ---- first SEANet encoder conv, Cin == 1 (modules/seanet.py:177-187): sample (b, t) at

@@ -62,7 +62,18 @@ struct TcCfg {
 // the magnitude bits and clear the low 13 bits (cvt.rna.tf32.f32 gives the same value but runs at
 // the slow conversion rate).  |x - hi| <= 2^-12 |x|, so with lo = rna(x - hi) the split
 // x ~ hi + lo is good to 2^-24 |x|: fp32-equivalent products.
-__device__ __forceinline__ float tf32_rna(float x) { return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u); }
+// A NaN is quieted instead: the add would carry its payload into the exponent or the sign (0x7FFFFFFF, the NaN CUDA
+// arithmetic returns, would become -0 and 0x7F800001 +Inf), and the tensor core reads only the top 19 bits.  Finite x
+// with |x| >= 0x7F7FF000 (about 3.4e38) rounds to Inf, as rna does.
+__device__ __forceinline__ float tf32_rna(float x) {
+  const uint32_t u = __float_as_uint(x);
+  return __uint_as_float((x != x ? u | 0x00400000u : u + 0x1000u) & 0xFFFFE000u);
+}
+// lo = rna(x - hi).  x - hi is NaN only for x = +-Inf or NaN, where hi alone carries the value: lo = 0.
+__device__ __forceinline__ float tf32_rna_lo(float x, float hi) {
+  const float d = x - hi;
+  return d != d ? 0.f : __uint_as_float((__float_as_uint(d) + 0x1000u) & 0xFFFFE000u);
+}
 
 // fused activation of the tensor-core path (ELU through ex2.approx, common.cuh)
 __device__ __forceinline__ float act_tc(float x, int act) {
@@ -165,9 +176,19 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
               const float e = __expf(v) - 1.f;
               v = v > 0.f ? v : e;
             }
-            const float h = tf32_rna(v);
-            ah[k][e] = __float_as_uint(h);
-            al[k][e] = __float_as_uint(tf32_rna(v - h));
+            if (Cfg::SPLIT) {
+              // A non-finite x enters as (hi, lo) = (0, x - 0): the subtraction returns +-Inf or the canonical quiet NaN
+              // 0x7FFFFFFF, which the mask keeps (no rounding add for it).  (hi, lo) = (Inf, 0) would make a_hi * b_lo
+              // add Inf * w_lo, which is NaN for w_lo == 0 and for w_lo of the other sign, where x * w is +-Inf.
+              // Finite x: the rna split above, bit for bit.
+              const bool nonfinite = !(fabsf(v) < INFINITY);
+              const float h = nonfinite ? 0.f : __uint_as_float((__float_as_uint(v) + 0x1000u) & 0xFFFFE000u);
+              const float d = v - h;
+              ah[k][e] = __float_as_uint(h);
+              al[k][e] = (__float_as_uint(d) + (nonfinite ? 0u : 0x1000u)) & 0xFFFFE000u;
+            } else {
+              ah[k][e] = __float_as_uint(tf32_rna(v));
+            }
           }
         }
         const uint64_t db = gmma_desc_sw128(st + TC_A_BYTES);
@@ -367,7 +388,7 @@ __global__ void tf32_split_kernel(const float* __restrict__ x, float* __restrict
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const float v = x[i], h = tf32_rna(v);
     hi[i] = h;
-    lo[i] = tf32_rna(v - h);
+    lo[i] = tf32_rna_lo(v, h);
   }
 }
 }  // namespace rstnet

@@ -111,6 +111,36 @@ int rstnet_tc_gemm_run(const rstnet_tc_plan* plan, rstnet_stream_t stream);
 void rstnet_tc_gemm_destroy(rstnet_tc_plan* plan);
 /* the plan's tile grid: M tiles (I tiles x O_out), N tiles, tile width */
 int rstnet_tc_gemm_grid(const rstnet_tc_plan* plan, int32_t* grid_x, int32_t* grid_y, int32_t* tile_n);
+/* ---- one SEANet residual block (modules/seanet.py SEANetResnetBlock, kernel 3, compress 2) of C = 64 or 128 channels
+ * on the tensor cores, as one plan and one launch:
+ *   h[i, t] = ELU(b1 + sum_{tap<3} W1[:, tap*C:(tap+1)*C] ELU(y[i, t - 2 + tap]))        (C -> C/2)
+ *   out[i, t] = ELU(y[i, t] + b2 + W2 h[i, t])                                              (C/2 -> C, + skip)
+ * the block plus the ELU that follows it in the encoder and decoder.  Element c of stream i at row `row` of the raw
+ * input is Y[row*y_o_stride + i*y_i_stride + c]; rows 0 and 1 are the causal context of output step 0, so output step t
+ * reads rows t, t + 1, t + 2 and y_rows >= O_out + 2.  Output element (i, t, c) goes to
+ * out + t*out_o_stride + i*out_i_stride + c.  Precision 0 only (3xTF32): W1 / W1_lo are the TF32 split of
+ * the k3 weights [C/2][3C] (K = tap-major, channel-minor), W2 / W2_lo of the 1x1 weights [C][C/2] (rstnet_tf32_split_f32).
+ * The result is bit-identical to the two rstnet_tc_gemm launches (k3 with pre_act = post_act = ELU into a hidden
+ * buffer, then 1x1 with R = y and post_act = ELU); the hidden tensor stays in shared memory and y is read once. */
+typedef struct rstnet_tc_resblock_plan rstnet_tc_resblock_plan;
+typedef struct {
+  const float* Y;
+  int64_t y_i_stride, y_o_stride;
+  int32_t channels;
+  int32_t I_out, O_out, y_rows;
+  const float* W1;
+  const float* W1_lo;
+  const float* b1;
+  const float* W2;
+  const float* W2_lo;
+  const float* b2;
+  float* out;
+  int64_t out_i_stride, out_o_stride;
+} rstnet_tc_resblock_desc;
+int rstnet_tc_resblock_create(const rstnet_tc_resblock_desc* desc, rstnet_tc_resblock_plan** out);
+int rstnet_tc_resblock_run(const rstnet_tc_resblock_plan* plan, rstnet_stream_t stream);
+void rstnet_tc_resblock_destroy(rstnet_tc_resblock_plan* plan);
+
 /* hi[i] = tf32_rna(x[i]); lo[i] = tf32_rna(x[i] - hi[i])  (one-time weight preparation for precision 0)
  * tf32_rna rounds to nearest with ties away from zero.  Non-finite x: NaN -> hi a quiet NaN (a NaN in the top 19 bits, the
  * ones the tensor core reads), lo = 0; +-Inf -> hi = +-Inf, lo = 0.  Finite x with |x| >= 0x7F7FF000 (about 3.4e38)

@@ -16,7 +16,8 @@ ACT_NONE, ACT_ELU, ACT_GELU = 0, 1, 2
 # every symbol include/rstnet_b200.h declares (tests assert the .so exports all of them)
 SYMBOLS = [
     "rstnet_version", "rstnet_last_error", "rstnet_launch_count", "rstnet_device_error_flags",
-    "rstnet_gemm_rows_f32", "rstnet_tc_gemm_create", "rstnet_tc_gemm_run", "rstnet_tc_gemm_destroy", "rstnet_tc_gemm_grid", "rstnet_tf32_split_f32", "rstnet_conv1d_cin1_f32", "rstnet_conv1d_cout1_f32",
+    "rstnet_gemm_rows_f32", "rstnet_tc_gemm_create", "rstnet_tc_gemm_run", "rstnet_tc_gemm_destroy", "rstnet_tc_gemm_grid",
+    "rstnet_tc_resblock_create", "rstnet_tc_resblock_run", "rstnet_tc_resblock_destroy", "rstnet_tf32_split_f32", "rstnet_conv1d_cin1_f32", "rstnet_conv1d_cout1_f32",
     "rstnet_convtr1d_depthwise_f32", "rstnet_rows_fill_f32", "rstnet_rows_copy_table_f32",
     "rstnet_counter_add", "rstnet_layer_norm_f32", "rstnet_rope_kv_append_f32",
     "rstnet_ring_attention_f32", "rstnet_rope_ring_attention_f32", "rstnet_rvq_encode_workspace", "rstnet_rvq_encode_f32",
@@ -55,6 +56,16 @@ class TcGemmDesc(C.Structure):
         ("bias", C.c_void_p), ("scale", C.c_void_p),
         ("n_split", C.c_int32), ("pre_act", C.c_int32), ("post_act", C.c_int32), ("precision", C.c_int32),
         ("C2", C.c_void_p), ("act2", C.c_int32),
+    ]
+
+
+class TcResblockDesc(C.Structure):
+    _fields_ = [
+        ("Y", C.c_void_p), ("y_i_stride", C.c_int64), ("y_o_stride", C.c_int64),
+        ("channels", C.c_int32), ("I_out", C.c_int32), ("O_out", C.c_int32), ("y_rows", C.c_int32),
+        ("W1", C.c_void_p), ("W1_lo", C.c_void_p), ("b1", C.c_void_p),
+        ("W2", C.c_void_p), ("W2_lo", C.c_void_p), ("b2", C.c_void_p),
+        ("out", C.c_void_p), ("out_i_stride", C.c_int64), ("out_o_stride", C.c_int64),
     ]
 
 
@@ -98,6 +109,10 @@ def lib() -> C.CDLL:
     L.rstnet_tc_gemm_destroy.argtypes = [vp]
     L.rstnet_tc_gemm_destroy.restype = None
     L.rstnet_tc_gemm_grid.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)]
+    L.rstnet_tc_resblock_create.argtypes = [C.POINTER(TcResblockDesc), C.POINTER(C.c_void_p)]
+    L.rstnet_tc_resblock_run.argtypes = [vp, vp]
+    L.rstnet_tc_resblock_destroy.argtypes = [vp]
+    L.rstnet_tc_resblock_destroy.restype = None
     L.rstnet_tf32_split_f32.argtypes = [vp, vp, vp, i64, vp]
     L.rstnet_conv1d_cin1_f32.argtypes = [vp, i64, i64, vp, vp, vp, vp, i64, i64, i32, i32, i32, i32, i32, i32, vp]
     L.rstnet_conv1d_cout1_f32.argtypes = [vp, i64, i64, vp, vp, vp, i64, i32, i32, i32, i32, vp]

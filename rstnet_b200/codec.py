@@ -180,6 +180,9 @@ class MimiCodec(nn.Module):
         # clips run the tensor-core path (a 128-row tile = 128 clips at one time step), smaller ones the fp32 CUDA-core path
         self.batch_tensor_cores_min = 96
         self.fused_rope_attention = True     # streaming steps: RoPE + KV append inside the attention launch
+        # tensor-core plans at precision 0: each 64- and 128-channel resblock is one launch (rstnet_tc_resblock) that reads
+        # the raw input once and keeps the hidden tensor on chip, instead of an ELU'd copy + k3 conv + 1x1 conv
+        self.fused_resblock = True
         # resblocks up to this width read the raw tensor and apply ELU in the operand transform (_Plan.elu_in_transform).
         # 0 = never (default): the ELU'd copy was the faster form where both were timed (scripts/codec_ab.py)
         self.elu_in_transform_max_channels = 0
@@ -560,6 +563,33 @@ class _Plan:
         MimiCodec.elu_in_transform_max_channels defaults to 0; time it with scripts/codec_ab.py before changing that."""
         return self.tc and C <= self.eng.m.elu_in_transform_max_channels and self.precision == 0 and self.eng.m.resblock_tensor_cores
 
+    def fused_resblock(self, C: int) -> bool:
+        """Tensor-core plans: is the C-channel resblock one rstnet_tc_resblock launch?  It reads the raw tensor (the buffer
+        layout of elu_in_transform: the raw tensor owns the carry rows, no ELU'd copy) and keeps the hidden tensor in
+        shared memory.  Same values as the two-launch form, bit for bit."""
+        return (self.tc and C in (64, 128) and self.precision == 0 and self.eng.m.resblock_tensor_cores
+                and self.eng.m.fused_resblock)
+
+    def raw_resblock_input(self, C: int) -> bool:
+        """Does the resblock input buffer itself carry the causal context (no separate ELU'd copy)?"""
+        return not self.tc or self.elu_in_transform(C) or self.fused_resblock(C)
+
+    def resblock(self, y: _Buf, ya: _Buf, h: Optional[_Buf], w1, w2, out: _Buf, T: int):
+        """SEANetResnetBlock (ELU, k3 C -> C/2, ELU, 1x1 C/2 -> C, + skip) followed by ELU: out rows [out.ctx, +T) from y
+        rows [y.ctx, +T).  ya: the buffer the k3 conv reads, with the 2 causal context rows: y itself, or the ELU'd copy
+        its producer wrote.  h: the hidden tensor (None when the block is fused)."""
+        if self.fused_resblock(y.C):
+            assert ya is y and y.ctx == 2 and self.tc
+            B = self.B
+            w1_hi, w1_lo = self.tc_weights(w1)
+            w2_hi, w2_lo = self.tc_weights(w2)
+            plan = ops.TcResblock(y.t, 0, y.C, B * y.C, y.rows, B, T, w1_hi, w1_lo, w1["bias"], w2_hi, w2_lo, w2["bias"],
+                                  out.t, out.off(out.ctx), out.C, B * out.C)
+            self.add(plan.run)
+            return
+        self.conv(ya, 0, 1, w1, h, 0, T, pre=ACT_ELU if ya is y else ACT_NONE, post=ACT_ELU, ffma=self.tc)
+        self.conv(h, 0, 1, w2, out, out.ctx, T, post=ACT_ELU, R=y, r_row0=y.ctx, ffma=self.tc)
+
     @staticmethod
     def tc_weights(pack):
         """TF32 (hi, lo) split of a weight pack, computed once and cached on the pack."""
@@ -734,10 +764,10 @@ class _EncPlan(_Plan):
         y, ya, h, r_ = [], [], [], []  # ya: ELU'd copies feeding the resblocks' first conv (tensor-core plans)
         C = nf
         for i, ratio in enumerate(eng.enc_ratios):
-            own_copy = self.tc and not self.elu_in_transform(C)
+            own_copy = not self.raw_resblock_input(C)
             y.append(self.buf(0 if own_copy else m.residual_kernel_size - 1, T[i], 0, C))
             ya.append(self.buf(m.residual_kernel_size - 1, T[i], 0, C) if own_copy else y[-1])
-            h.append(self.buf(0, T[i], 0, C // m.compress))
+            h.append(None if self.fused_resblock(C) else self.buf(0, T[i], 0, C // m.compress))
             r_.append(self.buf(ratio, T[i], T[i + 1] * ratio - T[i], C))
             C *= 2
         y4 = self.buf(m.last_kernel_size - 1, F, 0, C)
@@ -759,8 +789,7 @@ class _EncPlan(_Plan):
         for i, ratio in enumerate(eng.enc_ratios):
             w1, w2 = eng.e_res[i]
             # SEANetResnetBlock: ELU -> k3 -> ELU -> k1, + skip; the ELU that follows is fused as post_act
-            self.conv(ya[i], 0, 1, w1, h[i], 0, T[i], pre=ACT_ELU if ya[i] is y[i] else ACT_NONE, post=ACT_ELU, ffma=self.tc)
-            self.conv(h[i], 0, 1, w2, r_[i], r_[i].ctx, T[i], post=ACT_ELU, R=y[i], r_row0=y[i].ctx, ffma=self.tc)
+            self.resblock(y[i], ya[i], h[i], w1, w2, r_[i], T[i])
             if i + 1 < len(y):
                 nxt = y[i + 1]
                 self.conv(r_[i], 0, ratio, eng.e_down[i], nxt, nxt.ctx, T[i + 1],
@@ -827,10 +856,10 @@ class _DecPlan(_Plan):
         Tin = F
         for i, r in enumerate(eng.ratios):
             Tout = Tin * r
-            own_copy = self.tc and not self.elu_in_transform(C // 2)
+            own_copy = not self.raw_resblock_input(C // 2)
             yd.append(self.buf(0 if own_copy else m.residual_kernel_size - 1, Tout, 0, C // 2))
             yda.append(self.buf(m.residual_kernel_size - 1, Tout, 0, C // 2) if own_copy else yd[-1])
-            hd_.append(self.buf(0, Tout, 0, C // 2 // m.compress))
+            hd_.append(None if self.fused_resblock(C // 2) else self.buf(0, Tout, 0, C // 2 // m.compress))
             last = i == len(eng.ratios) - 1
             a.append(self.buf((m.last_kernel_size - 1) if last else 1, Tout, 0, C // 2))
             C //= 2
@@ -851,14 +880,14 @@ class _DecPlan(_Plan):
                       out2_row0=yda[i].ctx)
             Tout = Tin * r
             w1, w2 = eng.d_res[i]
-            self.conv(yda[i], 0, 1, w1, hd_[i], 0, Tout, pre=ACT_ELU if yda[i] is yd[i] else ACT_NONE, post=ACT_ELU, ffma=self.tc)
-            self.conv(hd_[i], 0, 1, w2, a[i + 1], a[i + 1].ctx, Tout, post=ACT_ELU, R=yd[i], r_row0=yd[i].ctx, ffma=self.tc)
+            self.resblock(yd[i], yda[i], hd_[i], w1, w2, a[i + 1], Tout)
             Tin = Tout
         last = a[-1]
         self.add(lambda: ops.conv1d_cout1(last.t, last.bs, last.ts, eng.d_final_w, eng.d_final_b, wav, Lout, B, Lout, last.C,
                                           m.last_kernel_size))
         self.finish_streaming([qup, X] + a + yda, F)
-        self.debug_bufs = {"qup": [qup], "X": [X], "a": a, "yd": yd, "yda": yda, "hd": hd_}   # scripts/diag_rows.py
+        # scripts/diag_rows.py (fused resblocks have no hidden buffer)
+        self.debug_bufs = {"qup": [qup], "X": [X], "a": a, "yd": yd, "yda": yda, "hd": [b for b in hd_ if b is not None]}
 
     def run(self, codes: torch.Tensor, graphs: Optional[bool]) -> torch.Tensor:
         self.codes_in.copy_(codes)

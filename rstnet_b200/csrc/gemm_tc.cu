@@ -82,9 +82,58 @@ __device__ __forceinline__ float act_tc(float x, int act) {
   return x;
 }
 
+// The register-A fragments of one 32-wide K stage: thread (gq, tq) of its warp reads rows r0 and r0 + 8, columns tq and
+// tq + 4 of every 8-wide K step out of a swizzled [128][32] fp32 tile at shared address `st` (a_row, a_sw: see the
+// consumer below), applies the pre-activation and splits (SPLIT) or rounds each value.
 // PRE_ELU: the fused pre-activation (ELU or none) is a template parameter and evaluated branch-free, so the consumer
 // path from one wgmma group to the next has no data-dependent divergence (ptxas would otherwise serialise the wgmmas
 // behind compiler-inserted warpgroup arrives).
+template <bool SPLIT, bool PRE_ELU>
+__device__ __forceinline__ void tc_build_a(uint32_t st, uint32_t a_row, uint32_t a_sw, uint32_t (&ah)[4][4], uint32_t (&al)[4][4]) {
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {   // a[e]: row r0 + 8 (e & 1), column 8 k + tq + 4 (e >> 1)
+      const uint32_t chunk = (uint32_t)(2 * k + (e >> 1));
+      float v;
+      asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(st + a_row + (e & 1) * 1024u + ((chunk ^ a_sw) << 4)));
+      if (PRE_ELU) {   // elu_fast, as a select: x > 0 ? x : exp(x) - 1
+        const float e = __expf(v) - 1.f;
+        v = v > 0.f ? v : e;
+      }
+      if (SPLIT) {
+        // A non-finite x enters as (hi, lo) = (0, x - 0): the subtraction returns +-Inf or the canonical quiet NaN
+        // 0x7FFFFFFF, which the mask keeps (no rounding add for it).  (hi, lo) = (Inf, 0) would make a_hi * b_lo
+        // add Inf * w_lo, which is NaN for w_lo == 0 and for w_lo of the other sign, where x * w is +-Inf.
+        // Finite x: the rna split above, bit for bit.
+        const bool nonfinite = !(fabsf(v) < INFINITY);
+        const float h = nonfinite ? 0.f : __uint_as_float((__float_as_uint(v) + 0x1000u) & 0xFFFFE000u);
+        const float d = v - h;
+        ah[k][e] = __float_as_uint(h);
+        al[k][e] = (__float_as_uint(d) + (nonfinite ? 0u : 0x1000u)) & 0xFFFFE000u;
+      } else {
+        ah[k][e] = __float_as_uint(tf32_rna(v));
+      }
+    }
+  }
+}
+
+// The wgmmas of one K stage: a_hi * b_hi into d0; a_lo * b_hi + a_hi * b_lo into d1 (SPLIT).  first: the stage starts
+// fresh accumulators.
+template <int BN, bool SPLIT>
+__device__ __forceinline__ void tc_mma_stage(float (&d0)[BN / 2], float (&d1)[BN / 2], const uint32_t (&ah)[4][4],
+                                             const uint32_t (&al)[4][4], uint64_t db, uint64_t dbl, bool first) {
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {   // 4 x (K = 8 tf32 = 32 bytes) per 128-byte row
+    const uint32_t acc_in = (first && k == 0) ? 0u : 1u;
+    wgmma_tf32_rs<BN>(d0, ah[k], db + (uint64_t)(2 * k), acc_in);                 // a_hi * b_hi
+    if (SPLIT) {
+      wgmma_tf32_rs<BN>(d1, al[k], db + (uint64_t)(2 * k), acc_in);               // a_lo * b_hi
+      wgmma_tf32_rs<BN>(d1, ah[k], dbl + (uint64_t)(2 * k), 1u);                  // a_hi * b_lo
+    }
+  }
+}
+
 template <int BN, int PREC, bool PRE_ELU>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
@@ -165,44 +214,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         mbar_wait(&full[s], (g / S) & 1);
         const uint32_t st = smem0 + (uint32_t)(s * Cfg::STAGE_BYTES);
         uint32_t ah[4][4], al[4][4];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {   // a[e]: row r0 + 8 (e & 1), column 8 k + tq + 4 (e >> 1)
-            const uint32_t chunk = (uint32_t)(2 * k + (e >> 1));
-            float v;
-            asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(st + a_row + (e & 1) * 1024u + ((chunk ^ a_sw) << 4)));
-            if (PRE_ELU) {   // elu_fast, as a select: x > 0 ? x : exp(x) - 1
-              const float e = __expf(v) - 1.f;
-              v = v > 0.f ? v : e;
-            }
-            if (Cfg::SPLIT) {
-              // A non-finite x enters as (hi, lo) = (0, x - 0): the subtraction returns +-Inf or the canonical quiet NaN
-              // 0x7FFFFFFF, which the mask keeps (no rounding add for it).  (hi, lo) = (Inf, 0) would make a_hi * b_lo
-              // add Inf * w_lo, which is NaN for w_lo == 0 and for w_lo of the other sign, where x * w is +-Inf.
-              // Finite x: the rna split above, bit for bit.
-              const bool nonfinite = !(fabsf(v) < INFINITY);
-              const float h = nonfinite ? 0.f : __uint_as_float((__float_as_uint(v) + 0x1000u) & 0xFFFFE000u);
-              const float d = v - h;
-              ah[k][e] = __float_as_uint(h);
-              al[k][e] = (__float_as_uint(d) + (nonfinite ? 0u : 0x1000u)) & 0xFFFFE000u;
-            } else {
-              ah[k][e] = __float_as_uint(tf32_rna(v));
-            }
-          }
-        }
+        tc_build_a<Cfg::SPLIT, PRE_ELU>(st, a_row, a_sw, ah, al);
         const uint64_t db = gmma_desc_sw128(st + TC_A_BYTES);
         const uint64_t dbl = gmma_desc_sw128(st + TC_A_BYTES + Cfg::B_BYTES);
         wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {   // 4 x (K = 8 tf32 = 32 bytes) per 128-byte row
-          const uint32_t acc_in = (u == 0 && k == 0) ? 0u : 1u;   // a chunk starts fresh accumulators
-          wgmma_tf32_rs<BN>(d0, ah[k], db + (uint64_t)(2 * k), acc_in);                 // a_hi * b_hi
-          if (Cfg::SPLIT) {
-            wgmma_tf32_rs<BN>(d1, al[k], db + (uint64_t)(2 * k), acc_in);               // a_lo * b_hi
-            wgmma_tf32_rs<BN>(d1, ah[k], dbl + (uint64_t)(2 * k), 1u);                  // a_hi * b_lo
-          }
-        }
+        tc_mma_stage<BN, Cfg::SPLIT>(d0, d1, ah, al, db, dbl, u == 0);   // a chunk starts fresh accumulators
         wgmma_commit();
         // the group's A operand is registers the next stage's fragments would overwrite: it must retire first
         wgmma_wait<0>();
@@ -249,6 +265,223 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             *reinterpret_cast<float2*>(crow2 + coff) = make_float2(act_tc(v.x, p.act2), act_tc(v.y, p.act2));
           *reinterpret_cast<float2*>(crow + coff) = make_float2(act_tc(v.x, p.post_act), act_tc(v.y, p.post_act));
         }
+      }
+    }
+  }
+}
+
+// ---------------------------------------------------------------- fused SEANet residual block (C = 64 or 128)
+//   h = ELU(b1 + conv_k3(ELU(y)))   (C -> C/2, causal: output step t reads y rows t-2, t-1, t)
+//   r = ELU(y + b2 + W2 h)          (1x1, C/2 -> C)
+// in one persistent launch at precision 0, with the same operations in the same order as the two gemm_tc launches it
+// replaces.  A tile is 128 streams at one time step.  Phase 1 is gemm_tc's K loop over 3 taps x C/32 stages of raw y
+// (ELU in the fragment build) against W1 (N = C/2); its epilogue writes h into shared memory as [128][32] swizzled
+// blocks, the layout the fragment builder reads.  Phase 2 takes A = h from there and B = W2 from the ring, one stage per
+// 64-column N slice (both K stages of the slice in it).  The residual y[t] is the A tile of phase 1's tap-2 stages: the
+// consumers keep those ring slots until the slice's epilogue has read them, so y is read from HBM once and the hidden
+// tensor never leaves the SM.
+constexpr int RB_B_BYTES = 64 * 128;                         // one W stage of up to 64 rows x 32 fp32
+constexpr int RB_STAGE_BYTES = TC_A_BYTES + 2 * RB_B_BYTES;  // 32 KB: [y 128 x 32 | W hi | W lo]
+constexpr int RB_STAGES = 6;
+
+struct RbParams {
+  float* out;
+  long long o_i_stride, o_o_stride;
+  const float* b1;
+  const float* b2;
+  int I_out, i_tiles, m_tiles;
+};
+
+template <int C>
+struct RbCfg {
+  static constexpr int N1 = C / 2;         // hidden width
+  static constexpr int KCH = C / 32;       // phase-1 stages per tap
+  static constexpr int P1 = 3 * KCH;       // phase-1 stages
+  static constexpr int NS = C / 64;        // phase-2 N slices (one ring stage each)
+  static constexpr int K2 = N1 / 32;       // phase-2 K stages per slice
+  static constexpr int H_BYTES = K2 * TC_A_BYTES;
+  static constexpr int SMEM_BYTES = RB_STAGES * RB_STAGE_BYTES + H_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  // phase 2's stages must not land on the slots still held for the residual (else the producer would wait on the
+  // consumers, which wait on it)
+  static constexpr bool ring_ok() {
+    for (int j = 0; j < NS; ++j)
+      for (int kc = 0; kc < KCH; ++kc)
+        if ((P1 + j) % RB_STAGES == (2 * KCH + kc) % RB_STAGES) return false;
+    return RB_STAGES >= KCH + NS;
+  }
+  static_assert(ring_ok(), "ring too small for the held residual stages");
+  static_assert(K2 * 2 * RB_B_BYTES <= RB_STAGE_BYTES, "a phase-2 slice must fit one stage");
+};
+
+template <int C>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+resblock_tc_kernel(const __grid_constant__ CUtensorMap tmY, const __grid_constant__ CUtensorMap tmW1,
+                   const __grid_constant__ CUtensorMap tmW1lo, const __grid_constant__ CUtensorMap tmW2,
+                   const __grid_constant__ CUtensorMap tmW2lo, const RbParams p) {
+  using Cfg = RbCfg<C>;
+  constexpr int S = RB_STAGES;
+  constexpr int CH = TC_CHUNK_STAGES;
+  constexpr int N1 = Cfg::N1, NR1 = N1 / 2, KCH = Cfg::KCH, P1 = Cfg::P1;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* hs = smem + S * RB_STAGE_BYTES;                     // h: K2 blocks of [128][32] fp32, 128-byte swizzle
+  uint64_t* full = reinterpret_cast<uint64_t*>(hs + Cfg::H_BYTES);
+  uint64_t* empty = full + S;
+  const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < S; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], TC_CONSUMER_WARPS);
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (warp == TC_CONSUMER_WARPS) {
+    // ================= TMA producer
+    if (elect_one()) {
+      tma_prefetch_desc(&tmY);
+      tma_prefetch_desc(&tmW1);
+      tma_prefetch_desc(&tmW1lo);
+      tma_prefetch_desc(&tmW2);
+      tma_prefetch_desc(&tmW2lo);
+      int g = 0;
+      for (int t = blockIdx.x; t < p.m_tiles; t += gridDim.x) {
+        const int i0 = (t % p.i_tiles) * TC_BM, ot = t / p.i_tiles;
+        for (int kit = 0; kit < P1; ++kit, ++g) {
+          const int s = g % S;
+          mbar_wait(&empty[s], ((g / S) & 1) ^ 1);
+          const int tap = kit / KCH, kc = kit % KCH;
+          uint8_t* st = smem + s * RB_STAGE_BYTES;
+          mbar_arrive_expect_tx(&full[s], TC_A_BYTES + 2 * N1 * 128);
+          tma_load_3d(st, &tmY, &full[s], kc * TC_BKE, i0, ot + tap);
+          tma_load_2d(st + TC_A_BYTES, &tmW1, &full[s], kit * TC_BKE, 0);
+          tma_load_2d(st + TC_A_BYTES + RB_B_BYTES, &tmW1lo, &full[s], kit * TC_BKE, 0);
+        }
+        for (int ns = 0; ns < Cfg::NS; ++ns, ++g) {
+          const int s = g % S;
+          mbar_wait(&empty[s], ((g / S) & 1) ^ 1);
+          uint8_t* st = smem + s * RB_STAGE_BYTES;
+          mbar_arrive_expect_tx(&full[s], Cfg::K2 * 2 * RB_B_BYTES);
+#pragma unroll
+          for (int kc = 0; kc < Cfg::K2; ++kc) {   // [W2 hi k0 | W2 lo k0 | W2 hi k1 | W2 lo k1]
+            tma_load_2d(st + kc * 2 * RB_B_BYTES, &tmW2, &full[s], kc * TC_BKE, ns * 64);
+            tma_load_2d(st + kc * 2 * RB_B_BYTES + RB_B_BYTES, &tmW2lo, &full[s], kc * TC_BKE, ns * 64);
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  // ================= consumers (fragment ownership as in gemm_tc_kernel)
+  const int wg = warp / 4, wq = warp % 4, gq = lane / 4, tq = lane % 4;
+  const int r0 = wg * 64 + wq * 16 + gq;
+  const uint32_t a_row = (uint32_t)r0 * 128u + (uint32_t)tq * 4u, a_sw = (uint32_t)(r0 & 7);
+  const uint32_t smem0 = smem_u32(smem), hs0 = smem_u32(hs);
+  int g = 0;
+  for (int t = blockIdx.x; t < p.m_tiles; t += gridDim.x) {
+    const int i0 = (t % p.i_tiles) * TC_BM, ot = t / p.i_tiles;
+    const int g_res = g + 2 * KCH;   // ring index of the first tap-2 stage: y[t], channels 0..31
+    {
+      // ---- phase 1: k3 conv C -> C/2 over ELU(y), promoted every CH stages
+      float acc[NR1], d0[NR1], d1[NR1];
+#pragma unroll
+      for (int j = 0; j < NR1; ++j) acc[j] = d0[j] = d1[j] = 0.f;
+      for (int k0 = 0; k0 < P1; k0 += CH) {
+        const int nst = P1 - k0 < CH ? P1 - k0 : CH;
+        for (int u = 0; u < nst; ++u, ++g) {
+          const int s = g % S;
+          mbar_wait(&full[s], (g / S) & 1);
+          const uint32_t st = smem0 + (uint32_t)(s * RB_STAGE_BYTES);
+          uint32_t ah[4][4], al[4][4];
+          tc_build_a<true, true>(st, a_row, a_sw, ah, al);
+          wgmma_fence();
+          tc_mma_stage<N1, true>(d0, d1, ah, al, gmma_desc_sw128(st + TC_A_BYTES), gmma_desc_sw128(st + TC_A_BYTES + RB_B_BYTES),
+                                 u == 0);
+          wgmma_commit();
+          wgmma_wait<0>();
+          __syncwarp();
+          if (lane == 0 && k0 + u < 2 * KCH) mbar_arrive(&empty[s]);   // tap-2 stages stay until the residual is read
+        }
+        fence_acc(d0);
+        fence_acc(d1);
+#pragma unroll
+        for (int j = 0; j < NR1; ++j) acc[j] += d0[j] + d1[j];
+      }
+      // ---- h = ELU(acc + b1) -> shared memory.  Each warpgroup writes and reads only its own 64 rows: the barrier
+      // before the write waits for the warpgroup's phase-2 reads of the previous tile, the one after publishes h.
+      named_bar_sync(1 + wg, 128);
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int r = r0 + 8 * hh;
+#pragma unroll
+        for (int b = 0; b < N1 / 8; ++b) {
+          const int n = 8 * b + 2 * tq;
+          const float2 bb = *reinterpret_cast<const float2*>(p.b1 + n);
+          float2 v = make_float2(acc[4 * b + 2 * hh], acc[4 * b + 2 * hh + 1]);
+          v.x += bb.x; v.y += bb.y;
+          const uint32_t cc = (uint32_t)(n % 32);
+          const uint32_t addr = hs0 + (uint32_t)(n / 32) * TC_A_BYTES + (uint32_t)r * 128u + (((cc >> 2) ^ (uint32_t)(r & 7)) << 4) +
+                                (cc & 3u) * 4u;
+          asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(act_tc(v.x, ACT_ELU)), "f"(act_tc(v.y, ACT_ELU))
+                       : "memory");
+        }
+      }
+      named_bar_sync(1 + wg, 128);
+    }
+    // ---- phase 2: 1x1 conv C/2 -> C, one 64-column slice at a time; epilogue + residual + ELU -> global
+    for (int ns = 0; ns < Cfg::NS; ++ns, ++g) {
+      const int s = g % S;
+      mbar_wait(&full[s], (g / S) & 1);
+      const uint32_t st = smem0 + (uint32_t)(s * RB_STAGE_BYTES);
+      float acc[32], d0[32], d1[32];
+#pragma unroll
+      for (int j = 0; j < 32; ++j) d0[j] = d1[j] = 0.f;
+#pragma unroll
+      for (int kc = 0; kc < Cfg::K2; ++kc) {
+        uint32_t ah[4][4], al[4][4];
+        tc_build_a<true, false>(hs0 + (uint32_t)(kc * TC_A_BYTES), a_row, a_sw, ah, al);
+        const uint32_t wst = st + (uint32_t)(kc * 2 * RB_B_BYTES);
+        wgmma_fence();
+        tc_mma_stage<64, true>(d0, d1, ah, al, gmma_desc_sw128(wst), gmma_desc_sw128(wst + RB_B_BYTES), kc == 0);
+        wgmma_commit();
+        wgmma_wait<0>();
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[s]);
+      fence_acc(d0);
+      fence_acc(d1);
+#pragma unroll
+      for (int j = 0; j < 32; ++j) {
+        acc[j] = 0.f;
+        acc[j] += d0[j] + d1[j];
+      }
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int r = r0 + 8 * hh;
+        const int i = i0 + r;
+        if (i >= p.I_out) continue;
+        float* orow = p.out + (long long)ot * p.o_o_stride + (long long)i * p.o_i_stride;
+#pragma unroll
+        for (int b = 0; b < 8; ++b) {
+          const int n = ns * 64 + 8 * b + 2 * tq;
+          const float2 bb = *reinterpret_cast<const float2*>(p.b2 + n);
+          float2 v = make_float2(acc[4 * b + 2 * hh], acc[4 * b + 2 * hh + 1]);
+          v.x += bb.x; v.y += bb.y;
+          const uint32_t cc = (uint32_t)(n % 32);
+          const int rs = (g_res + n / 32) % S;   // the tap-2 stage holding y[t], channels n / 32 * 32 ...
+          const float2 rr = *reinterpret_cast<const float2*>(smem + rs * RB_STAGE_BYTES + r * 128 +
+                                                             (((cc >> 2) ^ (uint32_t)(r & 7)) << 4) + (cc & 3u) * 4u);
+          v.x += rr.x; v.y += rr.y;
+          *reinterpret_cast<float2*>(orow + n) = make_float2(act_tc(v.x, ACT_ELU), act_tc(v.y, ACT_ELU));
+        }
+      }
+      __syncwarp();
+      if (lane == 0) {   // this slice's residual stages are read
+        mbar_arrive(&empty[(g_res + 2 * ns) % S]);
+        mbar_arrive(&empty[(g_res + 2 * ns + 1) % S]);
       }
     }
   }
@@ -377,6 +610,84 @@ extern "C" int rstnet_tc_gemm_run(const rstnet_tc_plan* pl, rstnet_stream_t stre
 }
 
 extern "C" void rstnet_tc_gemm_destroy(rstnet_tc_plan* pl) { delete pl; }
+
+struct rstnet_tc_resblock_plan {
+  CUtensorMap tmY, tmW1, tmW1lo, tmW2, tmW2lo;
+  RbParams p;
+  dim3 grid;
+  int channels;
+};
+
+static int encode_2d(CUtensorMap* m, const float* base, int cols, int rows, int box_rows) {
+  cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  cuuint64_t gstr[1] = {(cuuint64_t)cols * 4};
+  cuuint32_t box[2] = {TC_BKE, (cuuint32_t)box_rows};
+  cuuint32_t estr[2] = {1, 1};
+  return (int)get_encode_fn()(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)base, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                              CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+}
+
+extern "C" int rstnet_tc_resblock_create(const rstnet_tc_resblock_desc* d, rstnet_tc_resblock_plan** out) {
+  RSTNET_REQUIRE(d && out, "tc_resblock_create: null argument");
+  RSTNET_REQUIRE(d->Y && d->W1 && d->W1_lo && d->b1 && d->W2 && d->W2_lo && d->b2 && d->out, "tc_resblock_create: null pointer");
+  const int Cc = d->channels;
+  RSTNET_REQUIRE(Cc == 64 || Cc == 128, "tc_resblock_create: channels must be 64 or 128 (got %d)", Cc);
+  RSTNET_REQUIRE(d->I_out > 0 && d->O_out > 0 && d->y_rows >= d->O_out + 2, "tc_resblock_create: bad shape");
+  RSTNET_REQUIRE((uintptr_t)d->Y % 16 == 0 && (uintptr_t)d->W1 % 16 == 0 && (uintptr_t)d->W1_lo % 16 == 0 && (uintptr_t)d->W2 % 16 == 0 &&
+                     (uintptr_t)d->W2_lo % 16 == 0 && (uintptr_t)d->out % 16 == 0 && (uintptr_t)d->b1 % 8 == 0 &&
+                     (uintptr_t)d->b2 % 8 == 0 && d->y_i_stride % 4 == 0 && d->y_o_stride % 4 == 0 && d->out_i_stride % 4 == 0 &&
+                     d->out_o_stride % 4 == 0,
+                 "tc_resblock_create: 16-byte alignment required");
+  RSTNET_REQUIRE(get_encode_fn() != nullptr, "tc_resblock_create: cuTensorMapEncodeTiled unavailable (no CUDA driver?)");
+  rstnet_tc_resblock_plan* pl = new rstnet_tc_resblock_plan();
+  pl->channels = Cc;
+  int r;
+  {
+    cuuint64_t gdim[3] = {(cuuint64_t)Cc, (cuuint64_t)d->I_out, (cuuint64_t)d->y_rows};
+    cuuint64_t gstr[2] = {(cuuint64_t)d->y_i_stride * 4, (cuuint64_t)d->y_o_stride * 4};
+    cuuint32_t box[3] = {TC_BKE, TC_BM, 1};
+    cuuint32_t estr[3] = {1, 1, 1};
+    r = (int)get_encode_fn()(&pl->tmY, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, (void*)d->Y, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  }
+  if (r == CUDA_SUCCESS) r = encode_2d(&pl->tmW1, d->W1, 3 * Cc, Cc / 2, Cc / 2);
+  if (r == CUDA_SUCCESS) r = encode_2d(&pl->tmW1lo, d->W1_lo, 3 * Cc, Cc / 2, Cc / 2);
+  if (r == CUDA_SUCCESS) r = encode_2d(&pl->tmW2, d->W2, Cc / 2, Cc, 64);
+  if (r == CUDA_SUCCESS) r = encode_2d(&pl->tmW2lo, d->W2_lo, Cc / 2, Cc, 64);
+  if (r != CUDA_SUCCESS) {
+    delete pl;
+    set_error("tc_resblock_create: cuTensorMapEncodeTiled failed with %d", r);
+    return 3;
+  }
+  RbParams& p = pl->p;
+  p.out = d->out; p.o_i_stride = d->out_i_stride; p.o_o_stride = d->out_o_stride;
+  p.b1 = d->b1; p.b2 = d->b2;
+  p.I_out = d->I_out;
+  p.i_tiles = ceil_div(d->I_out, TC_BM);
+  p.m_tiles = p.i_tiles * d->O_out;
+  const int sms = sm_count();
+  pl->grid = dim3((unsigned)(p.m_tiles < sms ? p.m_tiles : sms));
+  *out = pl;
+  return 0;
+}
+
+template <int Cc>
+static int rb_launch(const rstnet_tc_resblock_plan* pl, cudaStream_t st) {
+  constexpr int smem = RbCfg<Cc>::SMEM_BYTES;
+  static unsigned long long attr = 0;
+  smem_optin(resblock_tc_kernel<Cc>, smem, attr);
+  resblock_tc_kernel<Cc><<<pl->grid, TC_THREADS, smem, st>>>(pl->tmY, pl->tmW1, pl->tmW1lo, pl->tmW2, pl->tmW2lo, pl->p);
+  count_launch();
+  return check_launch("tc_resblock");
+}
+
+extern "C" int rstnet_tc_resblock_run(const rstnet_tc_resblock_plan* pl, rstnet_stream_t stream) {
+  RSTNET_REQUIRE(pl != nullptr, "tc_resblock_run: null plan");
+  cudaStream_t st = (cudaStream_t)stream;
+  return pl->channels == 64 ? rb_launch<64>(pl, st) : rb_launch<128>(pl, st);
+}
+
+extern "C" void rstnet_tc_resblock_destroy(rstnet_tc_resblock_plan* pl) { delete pl; }
 extern "C" int rstnet_tc_gemm_grid(const rstnet_tc_plan* pl, int32_t* gx, int32_t* gy, int32_t* bn) {
   if (!pl) return 1;
   *gx = pl->p.m_tiles; *gy = pl->p.n_tiles; *bn = pl->bn;

@@ -113,6 +113,49 @@ class TcGemm:
             self._h = None
 
 
+class TcResblock:
+    """One SEANet residual block of C = 64 or 128 channels as one tensor-core launch (rstnet_tc_resblock_create / run /
+    destroy): out = ELU(y + b2 + W2 ELU(b1 + conv_k3(ELU(y)))), bit-identical to the two TcGemm launches it replaces.
+
+    Y: raw block input, element c of stream i at row `row` = Y[y_off + row*y_o_stride + i*y_i_stride + c], rows 0 and 1
+    the causal context of output step 0.  W1 / W1_lo: [C/2, 3C] TF32 split, W2 / W2_lo: [C, C/2]; offsets / strides in
+    elements; see include/rstnet_b200.h."""
+
+    def __init__(self, Y, y_off, y_i_stride, y_o_stride, y_rows, I_out, O_out, W1, W1_lo, b1, W2, W2_lo, b2, out, out_off,
+                 out_i_stride, out_o_stride):
+        _cuda(Y, W1, W1_lo, b1, W2, W2_lo, b2, out)
+        Cc = W2.shape[0]
+        assert tuple(W1.shape) == (Cc // 2, 3 * Cc) and tuple(W2.shape) == (Cc, Cc // 2), (W1.shape, W2.shape)
+        d = _lib.TcResblockDesc()
+        d.Y = Y.data_ptr() + 4 * y_off
+        d.y_i_stride, d.y_o_stride = y_i_stride, y_o_stride
+        d.channels, d.I_out, d.O_out, d.y_rows = Cc, I_out, O_out, y_rows
+        d.W1, d.W1_lo, d.b1 = W1.data_ptr(), W1_lo.data_ptr(), b1.data_ptr()
+        d.W2, d.W2_lo, d.b2 = W2.data_ptr(), W2_lo.data_ptr(), b2.data_ptr()
+        d.out = out.data_ptr() + 4 * out_off
+        d.out_i_stride, d.out_o_stride = out_i_stride, out_o_stride
+        self._keep = (Y, W1, W1_lo, b1, W2, W2_lo, b2, out)  # the plan embeds raw pointers
+        self.shape = dict(C=Cc, I=I_out, O=O_out)
+        n = I_out * O_out
+        self.flops = 2.0 * n * (W1.numel() + W2.numel())  # both convs, one fp32-equivalent product per MAC
+        # algorithmic HBM bytes: y once (with its 2 context rows), the weights once (hi and lo) and the biases, out once
+        self.bytes = 4.0 * (Cc * I_out * (O_out + 2) + 2 * (W1.numel() + W2.numel()) + b1.numel() + b2.numel() + n * Cc)
+        self._h = C.c_void_p()
+        _lib.check(_lib.lib().rstnet_tc_resblock_create(C.byref(d), C.byref(self._h)), "tc_resblock_create")
+
+    def run(self):
+        _lib.check(_lib.lib().rstnet_tc_resblock_run(self._h, _stream()), "tc_resblock_run")
+
+    def __del__(self):
+        h = getattr(self, "_h", None)
+        if h:
+            try:
+                _lib.lib().rstnet_tc_resblock_destroy(h)
+            except Exception:
+                pass
+            self._h = None
+
+
 def conv1d_cin1(x, x_bs, x_ts, w, bias, out, out_off, out_bs, out_ts, batch, T, Cout, k, post_act=ACT_NONE, out2=None,
                 out2_off=0, act2=ACT_NONE):
     _cuda(x, w, out, out2)

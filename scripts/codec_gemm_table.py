@@ -1,4 +1,5 @@
-"""Per-shape table of the codec's tensor-core GEMM launches over one streaming frame (256 streams): time, FLOP/s, bytes/s."""
+"""Per-shape table of the codec's tensor-core GEMM launches (TcGemm, and the fused resblocks, TcResblock) over one streaming
+frame (256 streams): time, FLOP/s, bytes/s."""
 import sys, json
 import torch
 sys.path.insert(0, ".")
@@ -11,6 +12,7 @@ from specs import mimi_spec as S
 m = bench._mimi(dev, S)
 rec = []
 orig_init, orig_run = ops.TcGemm.__init__, ops.TcGemm.run
+orig_rb_run = ops.TcResblock.run
 
 
 def init(self, A, a_off, a_i_stride, a_o_stride, a_c_extent, a_i_extent, a_o_extent, W, Kc, C_, c_off, c_i_stride, c_o_stride, I_out, O_out, **kw):
@@ -26,8 +28,15 @@ def run(self):
     rec.append((e0, e1, self))
 
 
+def rb_run(self):   # the fused resblock launch (its shape: channels, streams, time steps)
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record(); orig_rb_run(self); e1.record()
+    rec.append((e0, e1, self))
+
+
 ops.TcGemm.__init__ = init
 ops.TcGemm.run = run
+ops.TcResblock.run = rb_run
 m.use_cuda_graphs = False
 m.streaming_forever(B)
 x = torch.randn(B, 1, 1920 * 4, device=dev)
@@ -46,7 +55,7 @@ for e0, e1, p in rec:
     d = rows.setdefault(key, [0, 0.0, p])
     d[0] += 1; d[1] += e0.elapsed_time(e1)
 tot = sum(v[1] for v in rows.values()) / n
-print(f"total GEMM time per frame {tot*1e3:.0f} us over {len(rec)//n} launches")
+print(f"total GEMM + resblock time per frame {tot*1e3:.0f} us over {len(rec)//n} launches")
 print(f"{'us/launch':>9} {'n':>3} {'%':>5} {'TF/s':>6} {'TB/s':>5}  shape")
 for key, (cnt, ms, p) in sorted(rows.items(), key=lambda kv: -kv[1][1]):
     us = ms * 1e3 / cnt

@@ -383,6 +383,24 @@ int rstnet_lm_sample_rows_bf16(const void* logits, int32_t rows, int32_t V, int3
                                int32_t n_valid_stride, int32_t top_k, float temp, uint32_t seed, const int64_t* step_rows,
                                const uint32_t* key_rows, int64_t* tokens, int32_t tok_stride, rstnet_stream_t stream);
 
+/* ---- teacher-forced scoring: F.cross_entropy(ignore_index, reduction='none'), argmax and the mask sums of
+ * CrossEntropyAndAccuracy (models/model.py:31-65) over bf16 logit rows.  Row i (V logits at logits + i * row_stride;
+ * any stride >= V, rows need not be 16-byte aligned) belongs to group g = i % groups (the codebook) and to accumulator
+ * slot row_slot[i] (NULL: slot 0, n_slots == 1; a negative slot is a padding row: it is not read and adds nothing).
+ * Per row (fp32): nll[i] = logsumexp(x) - x[labels[i]], 0 when labels[i] == ignore_ids[g] (ignore_ids may be NULL),
+ * NaN when a logit is NaN; pred[i] = torch.argmax (first maximum; a NaN is the maximum).  A label outside [0, V) that is
+ * not the ignore id is where F.cross_entropy raises: that row's nll is NaN and error bit 0 is set
+ * (rstnet_device_error_flags).
+ * Then, in fp64, acc[(slot * groups + g) * 5 + k] += over the slot's rows of group g:
+ *   k = 0: sum weights[i] * nll[i]; 1: #(weights != 0); 2: #(weights == 1); 3: #(pred == label and weights != 0);
+ *   4: #(pred == label and weights == 1).
+ * The sums run in a fixed order (a second launch, no atomics): identical calls give identical bytes.  Two launches,
+ * graph-capturable. */
+int rstnet_lm_cross_entropy_bf16(const void* logits, int64_t row_stride, int32_t rows, int32_t V, int32_t groups,
+                                 const int64_t* labels, const int64_t* ignore_ids, const float* weights,
+                                 const int32_t* row_slot, int32_t n_slots, float* nll, int32_t* pred, double* acc,
+                                 rstnet_stream_t stream);
+
 /* ---- the acoustic-delay token cache of LMGen.step (models/model.py:490-562; moshi/models/lm.py LMGen.step), per stream:
  * the eager cache writes, input copy, write-back and gather of that step, as two launches around the LM frame.
  * cache [B][K][CT] int64 (K = n_q + 1 codebooks, CT = max_delay + 2); off [B] int64, the stream's step count; active [B]

@@ -28,7 +28,7 @@ SYMBOLS = [
     "rstnet_lm_ring_decode_attention_bf16", "rstnet_lm_silu_mul_bf16", "rstnet_lm_depth_attention_bf16", "rstnet_lm_sample_bf16",
     "rstnet_resample_f32", "rstnet_lm_delay_cache_in", "rstnet_lm_delay_cache_out",
     "rstnet_lm_rope_kv_append_rows_bf16", "rstnet_lm_ring_decode_attention_rows_bf16", "rstnet_lm_sample_rows_bf16",
-    "rstnet_counter_add_rows",
+    "rstnet_counter_add_rows", "rstnet_lm_cross_entropy_bf16",
 ]
 
 RESAMPLE_MAX_TABLE_BYTES = 48 * 1024   # RSTNET_RESAMPLE_MAX_TABLE_BYTES
@@ -153,6 +153,7 @@ def lib() -> C.CDLL:
     L.rstnet_lm_ring_decode_attention_rows_bf16.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp]
     L.rstnet_lm_sample_rows_bf16.argtypes = [vp, i32, i32, i32, vp, i32, i32, f32, C.c_uint32, vp, vp, vp, i32, vp]
     L.rstnet_counter_add_rows.argtypes = [vp, vp, i32, vp]
+    L.rstnet_lm_cross_entropy_bf16.argtypes = [vp, i64, i32, i32, i32, vp, vp, vp, vp, i32, vp, vp, vp, vp]
     for name in SYMBOLS:
         fn = getattr(L, name)
         if fn.restype is C.c_int and name not in ("rstnet_version",):

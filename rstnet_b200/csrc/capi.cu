@@ -34,6 +34,7 @@ int check_launch(const char* what) {
 namespace rstnet {
 unsigned int lm_read_errors(bool clear);
 unsigned int rvq_read_errors(bool clear);
+unsigned int ce_read_errors(bool clear);
 }
 
 extern "C" int rstnet_version(void) { return 205; }
@@ -41,7 +42,7 @@ extern "C" int rstnet_version(void) { return 205; }
 // 2 = RoPE position beyond the cos/sin tables.  Kernels cannot raise; they poison their output (NaN) and set a bit.
 extern "C" uint32_t rstnet_device_error_flags(int clear) {
   cudaDeviceSynchronize();
-  return rstnet::lm_read_errors(clear != 0) | rstnet::rvq_read_errors(clear != 0);
+  return rstnet::lm_read_errors(clear != 0) | rstnet::rvq_read_errors(clear != 0) | rstnet::ce_read_errors(clear != 0);
 }
 extern "C" const char* rstnet_last_error(void) { return rstnet::g_err; }
 extern "C" int64_t rstnet_launch_count(void) { return rstnet::g_launches.load(); }

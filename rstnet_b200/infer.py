@@ -15,6 +15,12 @@ Only the 'TTS' task is runnable upstream (the other branches reference undefined
 continuously batched scope: a row that finishes is refilled with the next utterance (ragged prefill of that row alone,
 ``GPT.prefill_streams``), and every row samples with its own candidate sets and random stream, so an utterance's codes do
 not depend on its row, on its admission time or on the other utterances.
+
+Mode 'teacher-force' (infer_no_streaming.py:172-182) scores a sequence instead of generating: ``InferenceImp.score_many``
+packs the frames of several utterances into shared ragged chunks (the row map of ``GPT.prefill_streams``) run with the
+lm_head on, and feeds each chunk's text logits, and the depth transformer's audio logits on the same rows, to the
+cross-entropy kernel, which adds into one accumulator slot per utterance; ``__call__`` in that mode is score_many on one
+utterance.
 """
 from __future__ import annotations
 
@@ -59,8 +65,13 @@ class InferenceImp(object):
         self.temp_text, self.top_k_text, self.temp, self.top_k = temp_text, top_k_text, temp, top_k
 
     @torch.no_grad()
-    def __call__(self, seq: torch.Tensor, mask: torch.Tensor) -> torch.Tensor:
-        """seq [9, L] (one utterance, as upstream) -> codes [8, T'] after reverse_delay."""
+    def __call__(self, seq: torch.Tensor, mask: torch.Tensor):
+        """seq [9, L] (one utterance, as upstream) -> codes [8, T'] after reverse_delay.  In mode 'teacher-force'
+        (infer_no_streaming.py:172-182, before any padding removal or task check) -> (loss_audio / 8, loss_text) as 0-dim
+        fp64 tensors: score_many on this one utterance."""
+        if self.mode == "teacher-force":
+            _, met = next(self.score_many([(None, seq, mask)], capacity=1))
+            return (torch.tensor(met["loss_audio"], dtype=torch.float64), torch.tensor(met["loss_text"], dtype=torch.float64))
         return self.generate(seq.unsqueeze(0).expand(self.n_samples, -1, -1))[0]
 
     @torch.no_grad()
@@ -101,7 +112,121 @@ class InferenceImp(object):
         if self.task_name != "TTS":
             raise NotImplementedError("only task 'TTS' is runnable in the reference loop (infer_no_streaming.py:184-226)")
         if self.mode == "teacher-force":
-            raise NotImplementedError("teacher-force mode is the training forward (out of scope)")
+            raise NotImplementedError("teacher-force mode scores sequences (__call__ / score_many), it does not generate")
+
+    def _score_item(self, seq, mask) -> Tuple[torch.Tensor, torch.Tensor, int]:
+        """Host-side checks of one scoring item -> (seq int64 [9, L], mask fp32 [9, L], frames to score).  Trailing frames
+        whose mask is zero in every codebook are dropped: the model is causal, so they change no earlier logit, and their
+        rows add nothing to any sum."""
+        m = self.model
+        K = m.config.n_q + 1
+        seq, mask = torch.as_tensor(seq), torch.as_tensor(mask)
+        if seq.dim() != 2 or seq.shape[0] != K:
+            raise RstnetError(f"a scored sequence is [{K}, L], got {tuple(seq.shape)}")
+        if tuple(mask.shape) != tuple(seq.shape):
+            raise RstnetError(f"the mask must have the sequence's shape {tuple(seq.shape)}, got {tuple(mask.shape)}")
+        seq, mask = seq.to("cpu", torch.int64), mask.to("cpu", torch.float32)
+        used = torch.nonzero((mask != 0).any(0))
+        L = int(used[-1]) + 1 if used.numel() else 0
+        if L > m.config.context:
+            raise RstnetError(f"{L} frames to score (after dropping all-zero-mask frames) > context = {m.config.context}: "
+                              "the non-streaming temporal transformer holds at most `context` positions")
+        return seq[:, :L], mask[:, :L], L
+
+    def _score_metrics(self, sums_audio: torch.Tensor, sums_text: torch.Tensor, frames: int) -> dict:
+        from .lm import combine_sums
+        dep_q = sums_audio.shape[0]
+        a, t = combine_sums(sums_audio, [1] * dep_q), combine_sums(sums_text, [1])
+        return {"frames": frames, "loss_audio": float(a["loss"]) / dep_q, "loss_text": float(t["loss"]),
+                "acc_all_audio": float(a["acc_all"]), "acc_target_audio": float(a["acc_target"]),
+                "acc_all_text": float(t["acc_all"]), "acc_target_text": float(t["acc_target"]),
+                "sums_audio": sums_audio.tolist(), "sums_text": sums_text.tolist()}
+
+    @torch.no_grad()
+    def score_many(self, items: Iterable[Tuple[object, torch.Tensor, torch.Tensor]], capacity: int = 8) -> Iterator[Tuple]:
+        """Teacher-forced scoring (infer_no_streaming.py --inference_mode teacher-force) of (utt_id, seq [9, L], mask [9, L])
+        items: yields (utt_id, metrics) in completion order.  metrics: loss_audio (the reference's loss_audio / 8: the mean
+        over the codebooks of sum(mask * nll) / #(mask != 0), ignore id 2049), loss_text (ignore id 128003), acc_all /
+        acc_target of audio and text, frames scored and the per-codebook sums sums_audio [8][5], sums_text [1][5] (fields
+        lm.CE_FIELDS).  A group whose mask is zero throughout gives NaN, as upstream.
+
+        Up to `capacity` utterances are live, one stream each; their frames are packed into ragged chunks of at most
+        MAX_ROWS rows (GPT.prefill_streams' row map) run with the lm_head on; each chunk's rows go to the text
+        cross-entropy, through the depth transformer on the same rows, and to the audio cross-entropy, whose sums land in
+        the utterance's own accumulator slot.  No [L, V] logits are kept."""
+        from .lm import cross_entropy_sums
+        if not 1 <= capacity <= MAX_STREAMS:
+            raise RstnetError(f"capacity must be in [1, {MAX_STREAMS}] (got {capacity})")
+        m = self.model
+        dev, c = m.device, m.config
+        K, Q = m.num_codebooks, c.dep_q
+        f32, i64 = torch.float32, torch.int64
+        ign_text = torch.tensor([self.text_pad_token], dtype=i64, device=dev)
+        ign_audio = torch.full((Q,), self.acoustic_pad_token, dtype=i64, device=dev)
+        acc_text = torch.zeros(capacity, 1, 5, dtype=torch.float64, device=dev)
+        acc_audio = torch.zeros(capacity, Q, 5, dtype=torch.float64, device=dev)
+        source = iter(items)
+        free, live, todo = list(range(capacity)), {}, []
+        exhausted = False
+        with m.streaming(capacity):
+            st = m._state
+            init = m._get_initial_token()[0]                                   # [9, 1]
+            while True:
+                admitted = []
+                while free and not exhausted:
+                    try:
+                        utt, seq, mask = next(source)
+                    except StopIteration:
+                        exhausted = True
+                        break
+                    seq, mask, L = self._score_item(seq, mask)
+                    if L == 0:
+                        yield utt, self._score_metrics(torch.zeros(Q, 5, dtype=torch.float64), torch.zeros(1, 5, dtype=torch.float64), 0)
+                        continue
+                    s = free.pop(0)
+                    feed = torch.cat([init, seq[:, :L - 1].to(dev)], dim=1)        # [initial token, seq[:, :-1]]
+                    todo.append([s, feed.t().contiguous(), 0])
+                    live[s] = dict(utt=utt, seq=seq.t().numpy(), mask=mask.t().numpy(), L=L)
+                    admitted.append(s)
+                if admitted:
+                    m.reset_streaming(streams=admitted)
+                    acc_text[admitted] = 0
+                    acc_audio[admitted] = 0
+                if not todo:
+                    break
+                ch, segs = st.row_chunk(todo, head=True)
+                M = ch.M
+                # labels / weights / accumulator slots of the chunk's rows; padding rows: ignore ids, weight 0, slot -1
+                lab = np.empty((M, K), dtype=np.int64)
+                lab[:, 0], lab[:, 1:] = self.text_pad_token, self.acoustic_pad_token
+                w = np.zeros((M, K), dtype=np.float32)
+                slot = np.full(M, -1, dtype=np.int32)
+                for s, r0, t0, tn in segs:
+                    u = live[s]
+                    lab[r0:r0 + tn] = u["seq"][t0:t0 + tn]
+                    w[r0:r0 + tn] = u["mask"][t0:t0 + tn]
+                    slot[r0:r0 + tn] = s
+                lab_d = torch.from_numpy(lab).to(dev)
+                w_d = torch.from_numpy(w).to(dev)
+                slot_d = torch.from_numpy(slot).to(dev)
+                cross_entropy_sums(ch.logits, lab_d[:, 0].contiguous(), w_d[:, 0].contiguous(), 1, ign_text, slot_d, acc_text)
+                dst = m._depth_state(M)
+                if not hasattr(dst, "score_logits"):
+                    dst.score_logits = torch.empty(M, Q, c.audio_card, dtype=torch.bfloat16, device=dev)
+                dst.depth_teacher(ch.out, lab_d, dst.score_logits)
+                cross_entropy_sums(dst.score_logits.view(M * Q, c.audio_card), lab_d[:, 1:].reshape(-1).contiguous(),
+                                   w_d[:, 1:].reshape(-1).contiguous(), Q, ign_audio,
+                                   slot_d.repeat_interleave(Q).contiguous(), acc_audio)
+                done = [it for it in todo if it[2] == it[1].shape[0]]
+                todo = [it for it in todo if it[2] < it[1].shape[0]]
+                if done:
+                    m.check_device_errors()
+                    sa, stx = acc_audio.cpu(), acc_text.cpu()
+                    for s, _, _ in done:
+                        u = live.pop(s)
+                        free.append(s)
+                        yield u["utt"], self._score_metrics(sa[s], stx[s], u["L"])
+            m.check_device_errors()
 
     def _layout(self, seq: torch.Tensor) -> Tuple[int, int]:
         """seq [9, L] -> (prompt length P, frames to generate G) after stripping the pad frames

@@ -472,13 +472,17 @@ class GPT(nn.Module):
         out = torch.empty(rows, c.dep_q, c.audio_card, dtype=torch.bfloat16, device=self.device)
         for r0 in range(0, rows, MAX_ROWS):
             n = min(MAX_ROWS, rows - r0)
-            st = self._local_states.get(n)
-            if st is None:
-                if len(self._local_states) >= 4:
-                    self._local_states.clear()
-                st = self._local_states[n] = _LMState(self, n, parts=("depth",))
-            st.depth_local(start[r0:r0 + n], ids[r0:r0 + n], tout[r0:r0 + n], out[r0:r0 + n])
+            self._depth_state(n).depth_local(start[r0:r0 + n], ids[r0:r0 + n], tout[r0:r0 + n], out[r0:r0 + n])
         return out.view(B, S, c.dep_q, c.audio_card)
+
+    def _depth_state(self, n: int) -> "_LMState":
+        """the depth-transformer-only state of n rows (forward_local, teacher-forced scoring)"""
+        st = self._local_states.get(n)
+        if st is None:
+            if len(self._local_states) >= 4:
+                self._local_states.clear()
+            st = self._local_states[n] = _LMState(self, n, parts=("depth",))
+        return st
 
     @torch.no_grad()
     @on_own_device
@@ -522,8 +526,103 @@ class GPT(nn.Module):
             raise RstnetError("prefill_streams is a streaming call: use it inside `with gpt.streaming(B):`")
         self._state.prefill_streams(prompts)
 
-    def forward(self, *a, **kw):
-        raise NotImplementedError("training / teacher-forcing forward is out of scope; use forward_global / forward_local")
+    @torch.no_grad()
+    @on_own_device
+    def forward(self, sequence: torch.Tensor, input_pos: Optional[torch.Tensor] = None, lm_head_chunk_size: int = 0):
+        """llama_streaming.py:651-663, the teacher-forced forward: the temporal transformer (non-streaming forward_global)
+        over [initial token, sequence[:, :, :-1]], then the depth transformer (forward_local) started from the text
+        embedding of each frame's own text token and fed sequence[:, 1:dep_q+1].  sequence [B, 9, S] ->
+        (audio_logits [B, S, dep_q, card], text_logits [B, S, V]), bf16 (text_logits.squeeze(1) as upstream: [B, V] at S == 1).
+        At most config.context frames (the existing limit of the non-streaming forward_global).  Evaluation only: no
+        gradients.  lm_head_chunk_size is accepted and ignored, as upstream."""
+        if self._state is not None:
+            raise RstnetError("GPT.forward is the non-streaming teacher-forced form: call it outside `with gpt.streaming(B):`")
+        if input_pos is not None:
+            raise RstnetError("GPT.forward with input_pos (the KV-cache form) is not implemented; use gpt.streaming(B)")
+        B, K, S = sequence.shape
+        sequence = sequence.to(device=self.device, dtype=torch.int64)
+        start = self._get_initial_token().repeat(B, 1, 1)
+        transformer_out, text_logits = self.forward_global(torch.cat([start, sequence[:, :, :-1]], dim=2))
+        text_logits = text_logits.squeeze(1)
+        local_start = self.codecformer_text_emb(sequence[:, 0, :])
+        audio_logits = self.forward_local(local_start, sequence[:, 1:self.config.dep_q + 1, :], transformer_out)
+        return audio_logits, text_logits
+
+
+# ------------------------------------------------------------------------------------------- teacher-forced scoring
+CE_FIELDS = ("loss_sum", "count", "count_target", "correct", "correct_target")   # the 5 sums of one (slot, group)
+
+
+def cross_entropy_sums(logits: torch.Tensor, labels: torch.Tensor, weights: torch.Tensor, groups: int,
+                       ignore_ids: Optional[torch.Tensor] = None, row_slot: Optional[torch.Tensor] = None,
+                       acc: Optional[torch.Tensor] = None, nll: Optional[torch.Tensor] = None,
+                       pred: Optional[torch.Tensor] = None):
+    """rstnet_lm_cross_entropy_bf16 on bf16 rows logits [rows, V] (last dim contiguous, any row stride): row i is group
+    i % groups and slot row_slot[i] (None: slot 0).  labels int64 [rows], weights fp32 [rows], ignore_ids int64 [groups],
+    all on the logits' device.  Adds into acc fp64 [slots, groups, 5] (see CE_FIELDS; allocated zero when None) and
+    returns (acc, nll fp32 [rows], pred int32 [rows])."""
+    if logits.device.type != "cuda" or logits.dtype != torch.bfloat16:
+        raise RstnetError(f"the cross-entropy kernel reads bf16 logits on CUDA (got {logits.dtype} on {logits.device})")
+    if logits.dim() != 2 or logits.stride(1) != 1:
+        raise RstnetError("logits must be [rows, V] with contiguous rows")
+    rows, V = logits.shape
+    dev = logits.device
+    n_slots = 1 if row_slot is None else (acc.shape[0] if acc is not None else int(row_slot.max()) + 1)
+    for t, dt, n in ((labels, torch.int64, rows), (weights, torch.float32, rows)) + (
+            ((row_slot, torch.int32, rows),) if row_slot is not None else ()) + (
+            ((ignore_ids, torch.int64, groups),) if ignore_ids is not None else ()):
+        if t.dtype != dt or t.device != dev or t.numel() != n or not t.is_contiguous():
+            raise RstnetError(f"cross_entropy_sums: expected a contiguous {dt} tensor of {n} elements on {dev}")
+    if acc is None:
+        acc = torch.zeros(n_slots, groups, 5, dtype=torch.float64, device=dev)
+    nll = torch.empty(rows, dtype=torch.float32, device=dev) if nll is None else nll
+    pred = torch.empty(rows, dtype=torch.int32, device=dev) if pred is None else pred
+    p = lambda t: None if t is None else t.data_ptr()
+    _lib.check(_lib.lib().rstnet_lm_cross_entropy_bf16(logits.data_ptr(), logits.stride(0), rows, V, groups, labels.data_ptr(),
+                                                       p(ignore_ids), weights.data_ptr(), p(row_slot), n_slots, nll.data_ptr(),
+                                                       pred.data_ptr(), acc.data_ptr(), ops._stream()), "lm_cross_entropy")
+    return acc, nll, pred
+
+
+def combine_sums(sums, loss_weights) -> Dict[str, torch.Tensor]:
+    """The host half of CrossEntropyAndAccuracy: sums [G, 5] (CE_FIELDS) -> loss = sum_g w_g * loss_sum_g / count_g (a group
+    without a non-zero mask gives 0/0 = NaN, kept), acc_all / acc_target pooled over the groups.  fp64 scalars."""
+    s = torch.as_tensor(sums, dtype=torch.float64).cpu().reshape(-1, 5)
+    w = torch.as_tensor([float(x) for x in loss_weights], dtype=torch.float64)
+    loss = (s[:, 0] / s[:, 1] * w).sum()
+    return {"acc_all": s[:, 3].sum() / s[:, 1].sum(), "acc_target": s[:, 4].sum() / s[:, 2].sum(), "loss": loss}
+
+
+def CrossEntropyAndAccuracy(logits, y, masks, loss_weights, ignore_ids=None):
+    """models/model.py:31-65 on bf16 logits [B, T, G, V] (CUDA): labels y [B, G, T], masks [B, G, T] (float weights: loss
+    rows are multiplied by them, `!= 0` and `== 1` select the counted tokens), one loss weight and ignore id per group.
+    -> (loss, {'acc_all', 'acc_target', 'loss'}) as 0-dim fp64 tensors.  The per-row losses are fp32 and the sums fp64
+    (upstream: bf16 rows).  A label outside [0, V) that is not its group's ignore id raises IndexError, as F.cross_entropy."""
+    if logits.dim() != 4:
+        raise RstnetError(f"logits must be [B, T, G, V], got {tuple(logits.shape)}")
+    B, T, G, V = logits.shape
+    dev = logits.device
+    y, masks = torch.as_tensor(y).to(dev), torch.as_tensor(masks).to(dev)
+    if tuple(y.shape) != (B, G, T) or tuple(masks.shape) != (B, G, T):
+        raise RstnetError(f"labels and masks must be [B, G, T] = {(B, G, T)}, got {tuple(y.shape)} and {tuple(masks.shape)}")
+    if len(loss_weights) != G:
+        raise RstnetError(f"{len(loss_weights)} loss weights for {G} groups")
+    if ignore_ids is not None and len(ignore_ids) != G:
+        raise RstnetError(f"{len(ignore_ids)} ignore ids for {G} groups")
+    try:
+        rows = logits.view(B * T * G, V)
+    except RuntimeError:
+        rows = logits.contiguous().view(B * T * G, V)
+    labels = y.permute(0, 2, 1).reshape(-1).to(torch.int64).contiguous()
+    weights = masks.permute(0, 2, 1).reshape(-1).to(torch.float32).contiguous()
+    ign = None if ignore_ids is None else torch.as_tensor([int(i) for i in ignore_ids], dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        acc, _, _ = cross_entropy_sums(rows, labels, weights, G, ign)
+        flags = int(_lib.lib().rstnet_device_error_flags(1))
+    if flags & 1:
+        raise IndexError("a label was outside [0, V) and not its group's ignore id (Target out of bounds)")
+    m = combine_sums(acc[0], loss_weights)
+    return m["loss"], m
 
 
 class _LMState:
@@ -887,36 +986,49 @@ class _LMState:
             if p.shape[1] > 0:
                 todo.append([s, p.to(device=dev, dtype=torch.int64).t(), 0])
         while todo:
-            rs, rt, parts = [], [], []
-            delta = np.zeros(self.B, dtype=np.int64)
-            for it in todo:
-                s, p, done = it
-                budget = MAX_ROWS - len(rs)
-                if budget == 0:
-                    break
-                # a chunk appends all its keys before any of its queries run: several positions of a stream only while its
-                # ring does not wrap inside the chunk (as forward_global's prefill), one per chunk after that
-                tn = min(p.shape[0] - done, budget, max(1, self.cap - int(self.pos_host[s])))
-                rs += [s] * tn
-                rt += range(tn)
-                parts.append(p[done:done + tn])
-                delta[s] = tn
-                it[2] += tn
-            n = len(rs)
-            M = next(b for b in ROW_BUCKETS if b >= n)
-            ch = self.row_children.get(M)
-            if ch is None:
-                ch = self.row_children[M] = _LMState(self.m, self.B, parent=self, parts=("temporal",), rows=M)
-            pad = M - n
-            ch.row_stream.copy_(torch.tensor(rs + [-1] * pad, dtype=torch.int32))
-            ch.row_tl.copy_(torch.tensor(rt + [0] * pad, dtype=torch.int32))
-            ch.delta.copy_(torch.from_numpy(delta))
-            if pad:
-                parts.append(torch.full((pad, K), self.m.zero_token_id, dtype=torch.int64, device=dev))   # an all-zero-token row
-            ch.seq.copy_(torch.cat(parts))
-            ch._temporal(head=False)
-            self.pos_host += delta
+            self.row_chunk(todo)
             todo = [it for it in todo if it[2] < it[1].shape[0]]
+
+    def row_chunk(self, todo, head: bool = False):
+        """One launch sequence of a ragged prefill: rows of the [stream, feed [T, K] on the device, positions fed] entries
+        of `todo`, in order, up to MAX_ROWS; advances each entry's count and its stream's position.  head: also run the
+        lm_head.  -> (chunk state, [(stream, first row, first position fed, positions)] per stream in the chunk); the
+        chunk's out / logits rows are valid until the next chunk of the same width."""
+        c, dev = self.c, self.m.device
+        K = c.n_q + 1
+        rs, rt, parts, segs = [], [], [], []
+        delta = np.zeros(self.B, dtype=np.int64)
+        for it in todo:
+            s, p, done = it
+            budget = MAX_ROWS - len(rs)
+            if budget == 0:
+                break
+            if done >= p.shape[0]:
+                continue
+            # a chunk appends all its keys before any of its queries run: several positions of a stream only while its
+            # ring does not wrap inside the chunk (as forward_global's prefill), one per chunk after that
+            tn = min(p.shape[0] - done, budget, max(1, self.cap - int(self.pos_host[s])))
+            segs.append((s, len(rs), done, tn))
+            rs += [s] * tn
+            rt += range(tn)
+            parts.append(p[done:done + tn])
+            delta[s] = tn
+            it[2] += tn
+        n = len(rs)
+        M = next(b for b in ROW_BUCKETS if b >= n)
+        ch = self.row_children.get(M)
+        if ch is None:
+            ch = self.row_children[M] = _LMState(self.m, self.B, parent=self, parts=("temporal",), rows=M)
+        pad = M - n
+        ch.row_stream.copy_(torch.tensor(rs + [-1] * pad, dtype=torch.int32))
+        ch.row_tl.copy_(torch.tensor(rt + [0] * pad, dtype=torch.int32))
+        ch.delta.copy_(torch.from_numpy(delta))
+        if pad:
+            parts.append(torch.full((pad, K), self.m.zero_token_id, dtype=torch.int64, device=dev))   # an all-zero-token row
+        ch.seq.copy_(torch.cat(parts))
+        ch._temporal(head=head)
+        self.pos_host += delta
+        return ch, segs
 
     def forward_codecformer(self, k: int, sequence: torch.Tensor, transformer_out: torch.Tensor):
         if self.depth_step is None:
@@ -941,6 +1053,17 @@ class _LMState:
                 self._depth(0, None, 0, quirk=False)
             else:
                 self._depth(k, self.tokens[:, k - 1], c.dep_q + 1, quirk=False)
+            out[:, k].copy_(self.dlogits)
+
+    def depth_teacher(self, tout: torch.Tensor, frames: torch.Tensor, out: torch.Tensor):
+        """forward_local on self.M rows whose step-0 feature is the embedding of the row's own text token (GPT.forward):
+        frames int64 [M, dep_q + 1] = (text, audio_0 .. audio_{dep_q-1}) of each row, tout [M, E]; writes out
+        [M, dep_q, card].  The text embedding is the bounds-checked gather of the decode step, not a host-side lookup."""
+        c = self.c
+        self.tout.copy_(tout)
+        self.tokens.copy_(frames)
+        for k in range(c.dep_q):
+            self._depth(k, self.tokens[:, k], c.dep_q + 1, quirk=False)
             out[:, k].copy_(self.dlogits)
 
     def forward_step(self, sequence, use_sampling, temp_text, top_k_text, temp, top_k, audio_valid, quirk=True, sample_key=None,

@@ -9,6 +9,10 @@
     (modules/conv.py:245-254), so audio padding would change a clip's last frame.
   * `reconstruct_directory` / `python -m rstnet_b200.offline reconstruct`: AudioCodec/MimiCodec/inference.py:111-148 -- every
     wav of a directory through encode -> decode, written under the same name at 24 kHz.
+  * `score` / `python -m rstnet_b200.offline score`: infer_no_streaming.py main() with --inference_mode teacher-force
+    (:174-182) over a corpus (`torch.save`d dict utt_id -> {"seq": int64 [9, L], "mask": float [9, L]}) with
+    InferenceImp.score_many: per-utterance losses / accuracies to a json file, and one json line with the mean
+    loss_audio / 8, perplexity_audio = exp(that mean) and the mean text loss.
   * `synthesize` / `python -m rstnet_b200.offline synthesize`: the TTS loop of infer_no_streaming.py main() (:119-143) over a
     whole corpus (`torch.save`d dict utt_id -> int64 [9, L]) with InferenceImp.generate_many: utterances of any prompt and
     generation length decode together, a finished row taking the next utterance.  Writes utt_id -> int16 codes [8, T] and,
@@ -168,6 +172,36 @@ def _synthesize_cli(args) -> int:
     return 0
 
 
+@torch.no_grad()
+def score(imp, corpus: Dict[str, dict], capacity: int = 8) -> Dict[str, dict]:
+    """{utt_id: metrics} of InferenceImp.score_many over `corpus` ({utt_id: {"seq": int64 [9, L], "mask": float [9, L]}})."""
+    items = ((utt, torch.as_tensor(d["seq"]), torch.as_tensor(d["mask"])) for utt, d in corpus.items())
+    return dict(imp.score_many(items, capacity))
+
+
+def score_summary(metrics: Dict[str, dict]) -> dict:
+    """main()'s teacher-force report (infer_no_streaming.py:174-182): perplexity_audio = exp(mean over utterances of
+    loss_audio / 8); the mean text loss beside it."""
+    import math
+    n = len(metrics)
+    la = sum(m["loss_audio"] for m in metrics.values()) / n if n else float("nan")
+    lt = sum(m["loss_text"] for m in metrics.values()) / n if n else float("nan")
+    return {"utterances": n, "loss_audio": la, "perplexity_audio": math.exp(la) if la == la else float("nan"), "loss_text": lt}
+
+
+def _score_cli(args) -> int:
+    import json
+    from .infer import InferenceImp
+    model = _load_gpt(args.config, args.checkpoint, args.device)
+    imp = InferenceImp(None, model, "teacher-force", 0.7, 25, 0.8, 30, "TTS")
+    corpus = torch.load(args.input, map_location="cpu")
+    metrics = score(imp, corpus, args.capacity)
+    with open(args.output_file, "w") as f:
+        json.dump(metrics, f)
+    print(json.dumps(score_summary(metrics)))
+    return 0
+
+
 def _load_codec(args) -> MimiCodec:
     import json
     cfg = json.load(open(args.config)) if args.config else dict(encoder_rates=[8, 6, 5, 4], codebook_size=2048, codebook_dim=256, rvq_layers=8)
@@ -178,6 +212,27 @@ def _load_codec(args) -> MimiCodec:
 
 
 def main(argv=None) -> int:
+    args = build_parser().parse_args(argv)
+    if args.cmd == "synthesize":
+        return _synthesize_cli(args)
+    if args.cmd == "score":
+        return _score_cli(args)
+    codec = _load_codec(args)
+    if args.cmd == "tokenize":
+        def items():
+            for line in open(args.wav_scp):
+                utt, path = line.strip().split(None, 1)
+                wav, sr = read_wav(path)
+                yield utt, wav, sr
+        toks = tokenize_utterances(codec, items(), args.batch_size)
+        save_tokens(toks, args.output_file)
+        print(f"tokenized {len(toks)} utterances -> {args.output_file}")
+    else:
+        print(f"reconstructed {reconstruct_directory(codec, args.input, args.output)} files -> {args.output}")
+    return 0
+
+
+def build_parser() -> argparse.ArgumentParser:
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     sub = ap.add_subparsers(dest="cmd", required=True)
     for name in ("tokenize", "reconstruct"):
@@ -206,22 +261,14 @@ def main(argv=None) -> int:
     p.add_argument("--codec-weights", default=None)
     p.add_argument("--codec-config", default=None, help="json with the MimiCodec constructor arguments")
     p.add_argument("--device", default="cuda")
-    args = ap.parse_args(argv)
-    if args.cmd == "synthesize":
-        return _synthesize_cli(args)
-    codec = _load_codec(args)
-    if args.cmd == "tokenize":
-        def items():
-            for line in open(args.wav_scp):
-                utt, path = line.strip().split(None, 1)
-                wav, sr = read_wav(path)
-                yield utt, wav, sr
-        toks = tokenize_utterances(codec, items(), args.batch_size)
-        save_tokens(toks, args.output_file)
-        print(f"tokenized {len(toks)} utterances -> {args.output_file}")
-    else:
-        print(f"reconstructed {reconstruct_directory(codec, args.input, args.output)} files -> {args.output}")
-    return 0
+    p = sub.add_parser("score", help="teacher-forced losses / audio perplexity of a corpus (infer_no_streaming.py teacher-force)")
+    p.add_argument("--input", required=True, help="torch.save'd dict utt_id -> {'seq': int64 [9, L], 'mask': float [9, L]}")
+    p.add_argument("--config", required=True, help="json with the GPT Config fields")
+    p.add_argument("--checkpoint", required=True, help="training checkpoint ({'model': state_dict})")
+    p.add_argument("--output-file", required=True, help="json file of per-utterance metrics")
+    p.add_argument("--capacity", type=int, default=8, help="utterances packed into the same chunks (<= 256)")
+    p.add_argument("--device", default="cuda")
+    return ap
 
 
 if __name__ == "__main__":

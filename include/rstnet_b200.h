@@ -185,6 +185,15 @@ int rstnet_rows_fill_f32(float* buf, int64_t batch_stride, int32_t batch, int32_
                          int32_t only_if_zero_stride /* 0: one shared counter; 1: one per stream, stream of column c of
                          batch b = b*(C/channels_per_stream) + c/channels_per_stream */,
                          int32_t channels_per_stream, rstnet_stream_t stream);
+/* fill_tail: the right padding a non-streaming StreamingConv1d applies at the end of a clip (modules/conv.py:245-254: zeros
+ * for the SEANet convs, replicate for ConvDownsample1d), applied inside a streaming chunk whose clip ends there.  Stream s
+ * (numbered as in rows_fill) keeps rows [row0, row0 + n_s) with n_s = min(nrows, ceil(valid[s] / valid_div)); rows
+ * [row0 + n_s, row0 + nrows) := 0 (mode 0) or := row row0 + n_s - 1 (mode 1, needs row0 >= 1).  valid: device int64
+ * [streams] (samples of the clip in this chunk; valid_div = the layer's total stride, so n_s is the layer's ceil-chain
+ * length), read at run time: one captured launch serves every step, and a stream with n_s == nrows is left alone. */
+int rstnet_rows_fill_tail_f32(float* buf, int64_t batch_stride, int32_t batch, int32_t C, int32_t row0, int32_t nrows,
+                              int32_t mode, const int64_t* valid, int64_t valid_div, int32_t channels_per_stream,
+                              rstnet_stream_t stream);
 typedef struct {
   float* buf;
   int64_t batch_stride; /* elements */

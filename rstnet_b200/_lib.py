@@ -28,7 +28,7 @@ SYMBOLS = [
     "rstnet_lm_ring_decode_attention_bf16", "rstnet_lm_silu_mul_bf16", "rstnet_lm_depth_attention_bf16", "rstnet_lm_sample_bf16",
     "rstnet_resample_f32", "rstnet_lm_delay_cache_in", "rstnet_lm_delay_cache_out",
     "rstnet_lm_rope_kv_append_rows_bf16", "rstnet_lm_ring_decode_attention_rows_bf16", "rstnet_lm_sample_rows_bf16",
-    "rstnet_counter_add_rows", "rstnet_lm_cross_entropy_bf16",
+    "rstnet_counter_add_rows", "rstnet_lm_cross_entropy_bf16", "rstnet_rows_fill_tail_f32",
 ]
 
 RESAMPLE_MAX_TABLE_BYTES = 48 * 1024   # RSTNET_RESAMPLE_MAX_TABLE_BYTES
@@ -118,6 +118,7 @@ def lib() -> C.CDLL:
     L.rstnet_conv1d_cout1_f32.argtypes = [vp, i64, i64, vp, vp, vp, i64, i32, i32, i32, i32, vp]
     L.rstnet_convtr1d_depthwise_f32.argtypes = [vp, i64, i64, vp, vp, i64, i64, i32, i32, i32, i32, vp]
     L.rstnet_rows_fill_f32.argtypes = [vp, i64, i32, i32, i32, i32, i32, i32, vp, i32, i32, vp]
+    L.rstnet_rows_fill_tail_f32.argtypes = [vp, i64, i32, i32, i32, i32, i32, vp, i64, i32, vp]
     L.rstnet_rows_copy_table_f32.argtypes = [vp, i32, i32, vp, vp]
     L.rstnet_counter_add.argtypes = [vp, i64, i32, vp, vp]
     L.rstnet_layer_norm_f32.argtypes = [vp, i64, vp, vp, vp, i32, i32, i32, f32, vp]

@@ -149,6 +149,26 @@ __global__ void rows_fill_kernel(float* __restrict__ buf, long long bs, int C, i
   }
 }
 
+// The end of a clip inside a chunk (ragged corpus batches): stream s keeps its first n_s rows, n_s = min(nrows, ceil(valid[s]
+// / valid_div)), and rows [row0 + n_s, row0 + nrows) become 0 (mode 0) or copies of row row0 + n_s - 1 (mode 1).  One block
+// row per stream (blockIdx.y = b * (C / cps) + column block, the stream numbering of rows_fill_kernel); a stream with
+// n_s == nrows -- every stream not in its final chunk -- leaves at once, so the launch costs nothing on most steps.
+__global__ void rows_fill_tail_kernel(float* __restrict__ buf, long long bs, int C, int cps, int row0, int nrows, int mode,
+                                      const long long* __restrict__ valid, long long valid_div) {
+  const int s = blockIdx.y;
+  const long long v = valid[s];
+  const long long n = v <= 0 ? 0 : min((long long)nrows, (v + valid_div - 1) / valid_div);
+  if (n >= nrows) return;
+  const int spb = C / cps;
+  float* base = buf + (long long)(s / spb) * bs + (long long)(s % spb) * cps;
+  const float* src = base + (row0 + n - 1) * (long long)C;   // mode 1 only (row0 >= 1 then, checked on the host)
+  const long long total = (nrows - n) * cps;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % cps);
+    base[(row0 + n + i / cps) * C + c] = mode == 1 ? src[c] : 0.f;
+  }
+}
+
 // Each thread owns one channel column and moves its rows in ascending order, so a carry that is
 // longer than the chunk (src and dst row ranges overlap, src_row >= dst_row) still shifts correctly.
 // active (optional): one flag per stream; a stream whose flag is 0 keeps its carry rows (a frame scheduler "holds" the
@@ -286,6 +306,27 @@ extern "C" int rstnet_rows_fill_f32(float* buf, int64_t bs, int32_t batch, int32
                                                                      channels_per_stream);
   count_launch();
   return check_launch("rows_fill");
+}
+
+extern "C" int rstnet_rows_fill_tail_f32(float* buf, int64_t bs, int32_t batch, int32_t C, int32_t row0, int32_t nrows,
+                                         int32_t mode, const int64_t* valid, int64_t valid_div, int32_t channels_per_stream,
+                                         rstnet_stream_t stream) {
+  RSTNET_REQUIRE(buf && valid, "rows_fill_tail: null pointer");
+  if (channels_per_stream <= 0) channels_per_stream = C;
+  RSTNET_REQUIRE(C > 0 && C % channels_per_stream == 0, "rows_fill_tail: C (%d) must be a multiple of channels_per_stream (%d)", C,
+                 channels_per_stream);
+  RSTNET_REQUIRE(valid_div >= 1 && row0 >= 0 && (mode == 0 || (mode == 1 && row0 >= 1)),
+                 "rows_fill_tail: bad argument (valid_div=%lld row0=%d mode=%d; mode 1 needs a row before row0)",
+                 (long long)valid_div, row0, mode);
+  if (nrows <= 0 || batch <= 0) return 0;
+  const long long streams = (long long)batch * (C / channels_per_stream);
+  RSTNET_REQUIRE(streams <= 65535, "rows_fill_tail: too many streams (%lld)", streams);
+  int gx = ceil_div((long long)nrows * channels_per_stream, 256);
+  if (gx > 32) gx = 32;
+  rows_fill_tail_kernel<<<dim3(gx, (unsigned)streams), 256, 0, (cudaStream_t)stream>>>(buf, bs, C, channels_per_stream, row0, nrows,
+                                                                                      mode, (const long long*)valid, valid_div);
+  count_launch();
+  return check_launch("rows_fill_tail");
 }
 
 extern "C" int rstnet_rows_copy_table_f32(const rstnet_row_copy* table_dev, int32_t n_entries, int32_t batch,

@@ -7,8 +7,13 @@
     (one clip per call) clips of EQUAL length are encoded as one batch (>= 96 of them: on the tensor cores); clips are
     never padded to a common length, because the codec's convs zero-pad each LAYER's input at the end of a clip
     (modules/conv.py:245-254), so audio padding would change a clip's last frame.
+  * `tokenize_corpus` / `tokenize --capacity N`: the same output through MimiCodec.encode_many -- clips of every length
+    in one continuous batch of N rows on the streaming tensor-core path, equal to the per-clip result wherever the RVQ
+    decision margin exceeds fp32 rounding (bit for bit on the fp32 CUDA-core path); without --capacity, tokenize stays
+    pinned bit for bit to MimiTokenizer.tokenize.
   * `reconstruct_directory` / `python -m rstnet_b200.offline reconstruct`: AudioCodec/MimiCodec/inference.py:111-148 -- every
-    wav of a directory through encode -> decode, written under the same name at 24 kHz.
+    wav of a directory through encode -> decode, written under the same name at 24 kHz.  `reconstruct_corpus` /
+    `reconstruct --capacity N`: the same through encode_many -> decode_many.
   * `score` / `python -m rstnet_b200.offline score`: infer_no_streaming.py main() with --inference_mode teacher-force
     (:174-182) over a corpus (`torch.save`d dict utt_id -> {"seq": int64 [9, L], "mask": float [9, L]}) with
     InferenceImp.score_many: per-utterance losses / accuracies to a json file, and one json line with the mean
@@ -79,6 +84,29 @@ def tokenize_utterances(codec: MimiCodec, items: Iterable[Tuple], batch_size: in
     return out
 
 
+def _clips_24k(codec: MimiCodec, items: Iterable[Tuple], resamplers: Dict[int, Resample]):
+    """(utt_id, 24 kHz wav [L] on the host) of every non-empty item; other rates through Resample(sr, 24000), one clip at a time."""
+    for item in items:
+        utt, wav = item[0], item[1]
+        sr = int(item[2]) if len(item) > 2 else codec.sample_rate
+        w = _as_row(wav)
+        if not w.numel():
+            continue
+        if sr != codec.sample_rate:
+            if sr not in resamplers:
+                resamplers[sr] = Resample(sr, codec.sample_rate)
+            w = resamplers[sr](w.to(codec.device)).cpu()
+        yield utt, w
+
+
+@torch.no_grad()
+def tokenize_corpus(codec: MimiCodec, items: Iterable[Tuple], capacity: int = 128) -> Dict[str, torch.Tensor]:
+    """`tokenize_utterances`' items and output ({utt_id: int16 [n_q, ceil(L24 / 1920)]}, empty clips skipped) through
+    MimiCodec.encode_many: up to `capacity` clips of any lengths encode together, a finished clip's row taking the next."""
+    clips = _clips_24k(codec, items, {})
+    return {utt: codes.to(torch.int16) for utt, codes in codec.encode_many(clips, capacity)}
+
+
 def save_tokens(tokens: Dict[str, torch.Tensor], path: str) -> None:
     torch.save(tokens, path)
 
@@ -115,6 +143,34 @@ def reconstruct_directory(codec: MimiCodec, src: str, dst: str) -> int:
         rec = codec.decode(codes)[0, 0, : wav.numel()]
         if float(rec.abs().max()) > 0.99:
             print(f"Clipping!! {name}: max scale {float(rec.abs().max()):.3f}", file=sys.stderr)   # inference.py:check_clipping2
+        write_wav(os.path.join(dst, name), rec, codec.sample_rate)
+        n += 1
+    return n
+
+
+@torch.no_grad()
+def reconstruct_corpus(codec: MimiCodec, src: str, dst: str, capacity: int = 128) -> int:
+    """reconstruct_directory through encode_many -> decode_many: up to `capacity` files of any lengths in flight."""
+    os.makedirs(dst, exist_ok=True)
+    names = sorted(n for n in os.listdir(src) if n.lower().endswith(".wav"))
+    lengths: Dict[str, int] = {}
+    resamplers: Dict[int, Resample] = {}
+
+    def clips():
+        for name in names:
+            wav, sr = read_wav(os.path.join(src, name))
+            if sr != codec.sample_rate and wav.numel():
+                if sr not in resamplers:
+                    resamplers[sr] = Resample(sr, codec.sample_rate)
+                wav = resamplers[sr](wav.to(codec.device)).cpu()
+            lengths[name] = wav.numel()
+            yield name, wav
+
+    n = 0
+    for name, rec in codec.decode_many(codec.encode_many(clips(), capacity), capacity):
+        rec = rec[: lengths.pop(name)]
+        if rec.numel() and float(rec.abs().max()) > 0.99:
+            print(f"Clipping!! {name}: max scale {float(rec.abs().max()):.3f}", file=sys.stderr)
         write_wav(os.path.join(dst, name), rec, codec.sample_rate)
         n += 1
     return n
@@ -224,11 +280,18 @@ def main(argv=None) -> int:
                 utt, path = line.strip().split(None, 1)
                 wav, sr = read_wav(path)
                 yield utt, wav, sr
-        toks = tokenize_utterances(codec, items(), args.batch_size)
+        if args.capacity is None:
+            toks = tokenize_utterances(codec, items(), args.batch_size)
+        else:
+            toks = tokenize_corpus(codec, items(), args.capacity)
         save_tokens(toks, args.output_file)
         print(f"tokenized {len(toks)} utterances -> {args.output_file}")
     else:
-        print(f"reconstructed {reconstruct_directory(codec, args.input, args.output)} files -> {args.output}")
+        if args.capacity is None:
+            n = reconstruct_directory(codec, args.input, args.output)
+        else:
+            n = reconstruct_corpus(codec, args.input, args.output, args.capacity)
+        print(f"reconstructed {n} files -> {args.output}")
     return 0
 
 
@@ -240,6 +303,9 @@ def build_parser() -> argparse.ArgumentParser:
         p.add_argument("--weights", required=True, help="checkpoint (state_dict, or {'codec_model': state_dict})")
         p.add_argument("--config", default=None, help="json with the MimiCodec constructor arguments")
         p.add_argument("--device", default="cuda")
+        p.add_argument("--capacity", type=int, default=None,
+                       help="clips in flight at once: encode (and decode) every length in one continuous batch on the "
+                            "streaming tensor-core path; without it, equal-length groups as MimiTokenizer does clip by clip")
     sub.choices["tokenize"].add_argument("--wav-scp", required=True, help="kaldi wav.scp: <utt_id> <path>")
     sub.choices["tokenize"].add_argument("--output-file", required=True)
     sub.choices["tokenize"].add_argument("--batch-size", type=int, default=256)

@@ -184,6 +184,14 @@ def rows_fill(buf, bs, batch, Cch, row0, nrows, mode=0, src_row=0, only_if_zero=
                                                _p(only_if_zero), oz_stride, channels_per_stream, _stream()), "rows_fill")
 
 
+def rows_fill_tail(buf, bs, batch, Cch, row0, nrows, mode, valid, valid_div=1, channels_per_stream=0):
+    """Per stream s: rows [row0 + n_s, row0 + nrows) := 0 (mode 0) or := row row0 + n_s - 1 (mode 1), with
+    n_s = min(nrows, ceil(valid[s] / valid_div)); valid: device int64 [streams] (see the header)."""
+    _cuda(buf, valid)
+    _lib.check(_lib.lib().rstnet_rows_fill_tail_f32(buf.data_ptr(), bs, batch, Cch, row0, nrows, mode, valid.data_ptr(), valid_div,
+                                                    channels_per_stream, _stream()), "rows_fill_tail")
+
+
 def rows_copy_table(table_dev: torch.Tensor, n_entries: int, batch: int, active: Optional[torch.Tensor] = None):
     _lib.check(_lib.lib().rstnet_rows_copy_table_f32(table_dev.data_ptr(), n_entries, batch, _p(active), _stream()), "rows_copy_table")
 

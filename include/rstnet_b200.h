@@ -391,6 +391,27 @@ int rstnet_lm_sample_bf16(const void* logits, int32_t rows, int32_t V, int32_t n
 int rstnet_lm_sample_rows_bf16(const void* logits, int32_t rows, int32_t V, int32_t n_valid, const int32_t* n_valid_rows,
                                int32_t n_valid_stride, int32_t top_k, float temp, uint32_t seed, const int64_t* step_rows,
                                const uint32_t* key_rows, int64_t* tokens, int32_t tok_stride, rstnet_stream_t stream);
+/* General form with nucleus (top-p) sampling and per-row settings.  Modes as rstnet_lm_sample_bf16, plus: top_k != 0
+ * and 0 < top_p < 1 -> nucleus (sample_top_p, utils/sampling.py:66-82; it takes precedence over top_k): with
+ * w_i = exp((l_i - max) / temp) over the ids < n_valid, id t is kept iff the mass of the ids before it in the order
+ * (logit desc, index asc) is <= top_p * sum(w); equal logits at the cut are kept lowest index first.  The draw is the
+ * first maximum of the top_k < 0 score over the kept ids, so it equals the top_k < 0 draw whenever that draw is kept.
+ * Masses are summed in fixed point (2^-40): identical calls and graph replays give identical tokens.  top_p >= 1 is the
+ * top_k < 0 multinomial; top_p == 0 leaves the mode to top_k.  Unlike the reference's masked audio samplers (NaN with
+ * top_p > 0) the distribution is renormalised over the ids < n_valid.
+ * Settings: top_k_rows / temp_rows / top_p_rows (all three or none; int32 / fp32 / fp32) give row r the entry at
+ * r * param_stride in place of the scalars, so one [rows, 2] table serves the text head (column 0) and the audio heads
+ * (column 1).  The tables are read on the device: the caller validates them (top_k <= 1024, temp > 0 where top_k != 0,
+ * top_p finite and >= 0).  The scalars are validated here when no table is given.
+ * RNG: keyed by (seed, step_rows[r], key_rows[r]) when step_rows / key_rows are given (both or neither), else by
+ * (seed, *step_counter, r) (step_counter NULL: step 0).  Candidates: n_valid_rows as rstnet_lm_sample_rows_bf16.
+ * With top_p == 0 everywhere it draws exactly the tokens of rstnet_lm_sample_bf16 / rstnet_lm_sample_rows_bf16 on the
+ * same inputs: all three run one compiled kernel. */
+int rstnet_lm_sample_params_bf16(const void* logits, int32_t rows, int32_t V, int32_t n_valid, const int32_t* n_valid_rows,
+                                 int32_t n_valid_stride, int32_t top_k, float temp, float top_p, const int32_t* top_k_rows,
+                                 const float* temp_rows, const float* top_p_rows, int32_t param_stride, uint32_t seed,
+                                 const int64_t* step_counter, const int64_t* step_rows, const uint32_t* key_rows,
+                                 int64_t* tokens, int32_t tok_stride, rstnet_stream_t stream);
 
 /* ---- teacher-forced scoring: F.cross_entropy(ignore_index, reduction='none'), argmax and the mask sums of
  * CrossEntropyAndAccuracy (models/model.py:31-65) over bf16 logit rows.  Row i (V logits at logits + i * row_stride;

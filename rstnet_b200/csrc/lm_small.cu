@@ -470,12 +470,43 @@ __device__ __forceinline__ float gumbel_of(uint32_t seed, uint32_t stepc, uint32
   return -logf(-logf(uni));   // argmax_i (l_i/temp + G_i)  ==  argmax_i softmax(l/temp)_i / Exp(1)_i
 }
 
+// the multinomial score of id i: one expression shared by the multinomial, top_k > 64 and nucleus draws, so a token
+// kept by two of them has the same score in both
+__device__ __forceinline__ float multinomial_score(float l, float inv_t, uint32_t seed, uint32_t stepc, uint32_t row, uint32_t i) {
+  return l * inv_t + gumbel_of(seed, stepc, row, i);
+}
+
+// Nucleus: the order key with -0 folded onto +0 (equal logits take the same key, so ties go lowest index first), and
+// the weight exp((l - max) / temp) in 2^-40 fixed point (<= 2^40 per id, < 2^58 for 152 064 ids).  Integer sums give
+// the same mass whatever the order of the atomics.  NaN logits and weights below 2^-40 weigh 0.
+constexpr int SAMPLE_MHISTS = 4;
+__device__ __forceinline__ uint32_t nucleus_key(bf16 v) {
+  const unsigned short u = __bfloat16_as_ushort(v);
+  return bf16_order_key(__ushort_as_bfloat16(u == 0x8000u ? (unsigned short)0 : u));
+}
+__device__ __forceinline__ unsigned long long nucleus_weight(float l, float mx, float inv_t) {
+  const float w = expf((l - mx) * inv_t);
+  return w > 0.f ? (unsigned long long)(w * 1099511627776.0f) : 0ull;
+}
+__device__ __forceinline__ float key_value(uint32_t k) {   // inverse of bf16_order_key
+  const unsigned short u = (k & 0x8000u) ? (unsigned short)(k & 0x7FFFu) : (unsigned short)(~k & 0xFFFFu);
+  return b2f(__ushort_as_bfloat16(u));
+}
+
 // top_k == 0: argmax.  1..64: ordered selection of the top-k (below), noise keyed by rank.  65..SAMPLE_CAND: threshold
 // select (the k largest by (value desc, index asc), found with the histogram + candidate list), noise keyed by token id.
 // top_k < 0: multinomial over all n_valid ids (sample_token with top_k == 0, utils/sampling.py:97-101).
+// top_k != 0 and 0 < top_p < 1: nucleus (sample_top_p, utils/sampling.py:66-82; it takes precedence over top_k as in
+// sample_token).  With w_i = exp((l_i - max) / temp) and Z = sum of w over the ids < n_valid, id t is kept iff the mass of
+// the ids before it in the order (logit desc, index asc) is <= top_p * Z, so the kept set is a prefix holding the top
+// token.  Equal logits have equal weights; at the cut they are taken lowest index first.  The draw is the first maximum
+// of the multinomial score over the kept ids, so it equals the top_k < 0 draw whenever that draw is kept (in particular
+// whenever every id is kept).  The cut: two 256-bin passes over the order key with counts and fixed-point masses.
+// Deviation: the reference's masked audio samplers (sample_token_audio[_2048] with top_p > 0) give NaN, because they mask
+// with -inf before the cumulative sum; here the distribution is restricted to the ids < n_valid and renormalised.
 // All threads of the block call it (any block size that is a multiple of 32, <= 1024); writes *token_out.
-__device__ __noinline__ void sample_row(const bf16* __restrict__ lr, int n_valid, int top_k, float temp, uint32_t seed, uint32_t stepc,
-                                        int row, long long* __restrict__ token_out) {
+__device__ __noinline__ void sample_row(const bf16* __restrict__ lr, int n_valid, int top_k, float temp, float top_p, uint32_t seed,
+                                        uint32_t stepc, int row, long long* __restrict__ token_out) {
   __shared__ float s_val[32];
   __shared__ int s_idx[32];
   __shared__ float top_v[64];
@@ -484,14 +515,156 @@ __device__ __noinline__ void sample_row(const bf16* __restrict__ lr, int n_valid
   __shared__ float cand_v[SAMPLE_CAND];
   __shared__ int cand_i[SAMPLE_CAND];
   __shared__ int s_sel[5];   // [0] high-byte bin, [1] count above the threshold key, [2] threshold key, [3] candidate count, [4] ties taken
+  __shared__ unsigned long long mhist[SAMPLE_MHISTS][256];
+  __shared__ unsigned long long s_mass[2];   // nucleus: [0] mass above the cut bin / key, [1] floor(top_p * Z)
   const int tid = threadIdx.x, nthr = blockDim.x;
+
+  if (top_k != 0 && top_p > 0.f && top_p < 1.f) {
+    const float inv_t = 1.0f / temp;
+    float mx = -INFINITY;
+    int mi = 0;
+    for (int i = tid; i < n_valid; i += nthr) mx = fmaxf(mx, b2f(lr[i]));
+    block_argmax(mx, mi, s_val, s_idx);
+    if (mx > -INFINITY) {   // (all -inf: the multinomial path below)
+      int* myh = hist[(tid / 32) % SAMPLE_HISTS];
+      unsigned long long* mym = mhist[(tid / 32) % SAMPLE_MHISTS];
+      for (int pass = 0; pass < 2; ++pass) {
+        for (int i = tid; i < SAMPLE_HISTS * 256; i += nthr) (&hist[0][0])[i] = 0;
+        for (int i = tid; i < SAMPLE_MHISTS * 256; i += nthr) (&mhist[0][0])[i] = 0ull;
+        __syncthreads();
+        const uint32_t b1 = pass ? (uint32_t)s_sel[0] : 0u;
+        // Warp-aggregated: the lanes of a warp that fall into one bin add their count and mass with one atomic each. An LM
+        // head occupies a handful of high-byte bins, so one atomic per id would serialise on them.  The masses (< 2^41
+        // per id) are summed across the lanes in two 20-bit halves, which cannot overflow 32 bits.
+        for (int base = 0; base < n_valid; base += nthr) {
+          const int i = base + tid;
+          uint32_t bin = 0xFFFFFFFFu;   // no bin: past the row, or outside the bin of pass 1
+          unsigned long long w = 0;
+          if (i < n_valid) {
+            const bf16 v = lr[i];
+            const uint32_t k = nucleus_key(v);
+            if (pass == 0 || (k >> 8) == b1) {
+              bin = pass ? (k & 255u) : (k >> 8);
+              w = nucleus_weight(b2f(v), mx, inv_t);
+            }
+          }
+          const unsigned peers = __match_any_sync(0xffffffffu, bin);
+          const unsigned lo = __reduce_add_sync(peers, (unsigned)(w & 0xFFFFFull));
+          const unsigned hi = __reduce_add_sync(peers, (unsigned)(w >> 20));
+          if (bin != 0xFFFFFFFFu && (int)(tid % 32) == __ffs(peers) - 1) {
+            atomicAdd(&myh[bin], __popc(peers));
+            const unsigned long long m = ((unsigned long long)hi << 20) + lo;
+            if (m) atomicAdd(&mym[bin], m);
+          }
+        }
+        __syncthreads();
+        if (tid < 256) {
+          int c = 0;
+          unsigned long long m = 0;
+#pragma unroll
+          for (int h = 0; h < SAMPLE_HISTS; ++h) c += hist[h][tid];
+#pragma unroll
+          for (int h = 0; h < SAMPLE_MHISTS; ++h) m += mhist[h][tid];
+          hist[0][tid] = c;
+          mhist[0][tid] = m;
+        }
+        __syncthreads();
+        if (tid == 0) {
+          unsigned long long above = 0;
+          if (pass == 0) {
+            for (int b = 0; b < 256; ++b) above += mhist[0][b];   // Z
+            s_mass[1] = (unsigned long long)((double)top_p * (double)above);
+            above = 0;
+          } else {
+            above = s_mass[0];
+          }
+          const unsigned long long cut_mass = s_mass[1];
+          int cut = 0;
+          unsigned long long cut_above = 0;
+          // the lowest non-empty bin whose mass above is <= top_p * Z: every id above it is kept, none below it
+          for (int b = 255; b >= 0; --b) {
+            if (!hist[0][b]) continue;
+            if (above > cut_mass) break;
+            cut = b;
+            cut_above = above;
+            above += mhist[0][b];
+          }
+          s_mass[0] = cut_above;
+          if (pass == 0) {
+            s_sel[0] = cut;
+          } else {
+            const uint32_t key = ((uint32_t)s_sel[0] << 8) | (uint32_t)cut;
+            const int cnt = hist[0][cut];
+            const unsigned long long w = nucleus_weight(key_value(key), mx, inv_t);
+            const unsigned long long fit = w ? (cut_mass - cut_above) / w + 1ull : (unsigned long long)cnt;
+            s_sel[1] = fit < (unsigned long long)cnt ? (int)fit : cnt;   // ties at the cut key to keep, lowest ids first
+            s_sel[2] = (int)key;
+            s_sel[3] = cnt;
+            s_sel[4] = 0x7fffffff;   // the largest kept id at the cut key
+          }
+        }
+        __syncthreads();
+      }
+      const uint32_t thr = (uint32_t)s_sel[2];
+      const int need = s_sel[1], cnt = s_sel[3];
+      if (need < cnt) {
+        if (cnt <= SAMPLE_CAND) {
+          if (tid == 0) s_sel[0] = 0;
+          __syncthreads();
+          for (int i = tid; i < n_valid; i += nthr)
+            if (nucleus_key(lr[i]) == thr) cand_i[atomicAdd(&s_sel[0], 1)] = i;
+          __syncthreads();
+          for (int t = tid; t < cnt; t += nthr) {
+            const int id = cand_i[t];
+            int rank = 0;
+            for (int j = 0; j < cnt; ++j) rank += cand_i[j] < id ? 1 : 0;
+            if (rank == need - 1) s_sel[4] = id;
+          }
+        } else {
+          // more than SAMPLE_CAND logits share the cut value: walk the row in index order, counting ties
+          if (tid == 0) s_sel[0] = 0;
+          for (int base = 0; base < n_valid; base += nthr) {
+            const int i = base + tid;
+            const bool tie = i < n_valid && nucleus_key(lr[i]) == thr;
+            const unsigned bal = __ballot_sync(0xffffffffu, tie);
+            const int wpre = __popc(bal & ((1u << (tid % 32)) - 1u));
+            __syncthreads();
+            if (tid % 32 == 0) s_idx[tid / 32] = __popc(bal);
+            __syncthreads();
+            int before = s_sel[0];
+            for (int w = 0; w < tid / 32; ++w) before += s_idx[w];
+            if (tie && before + wpre == need - 1) s_sel[4] = i;
+            __syncthreads();
+            if (tid == 0) { int t = 0; for (int w = 0; w < nthr / 32; ++w) t += s_idx[w]; s_sel[0] += t; }
+            __syncthreads();
+            if (s_sel[0] >= need) break;
+          }
+        }
+        __syncthreads();
+      }
+      const int last = s_sel[4];
+      float bv = -INFINITY;
+      int bi = 0x7fffffff;
+      for (int i = tid; i < n_valid; i += nthr) {
+        const bf16 v = lr[i];
+        const uint32_t k = nucleus_key(v);
+        if (k > thr || (k == thr && i <= last)) {
+          const float sc = multinomial_score(b2f(v), inv_t, seed, stepc, (uint32_t)row, (uint32_t)i);
+          if (sc > bv) { bv = sc; bi = i; }
+        }
+      }
+      block_argmax(bv, bi, s_val, s_idx);
+      if (tid == 0) *token_out = bi;
+      return;
+    }
+  }
 
   if (top_k < 0) {   // full multinomial
     float bv = -INFINITY;
     int bi = 0x7fffffff;
     const float inv_t = 1.0f / temp;
     for (int i = tid; i < n_valid; i += nthr) {
-      const float sc = b2f(lr[i]) * inv_t + gumbel_of(seed, stepc, (uint32_t)row, (uint32_t)i);
+      const float sc = multinomial_score(b2f(lr[i]), inv_t, seed, stepc, (uint32_t)row, (uint32_t)i);
       if (sc > bv) { bv = sc; bi = i; }
     }
     block_argmax(bv, bi, s_val, s_idx);
@@ -560,7 +733,7 @@ __device__ __noinline__ void sample_row(const bf16* __restrict__ lr, int n_valid
           in = rank < need;
         }
         if (in) {
-          const float sc = v * inv_t + gumbel_of(seed, stepc, (uint32_t)row, (uint32_t)id);
+          const float sc = multinomial_score(v, inv_t, seed, stepc, (uint32_t)row, (uint32_t)id);
           if (sc > bv || (sc == bv && id < bi)) { bv = sc; bi = id; }
         }
       }
@@ -579,7 +752,7 @@ __device__ __noinline__ void sample_row(const bf16* __restrict__ lr, int n_valid
         for (int w = 0; w < tid / 32; ++w) before += s_idx[w];
         const bool in = i < n_valid && (k > thr || (tie && before + wpre < need));
         if (in) {
-          const float sc = b2f(lr[i]) * inv_t + gumbel_of(seed, stepc, (uint32_t)row, (uint32_t)i);
+          const float sc = multinomial_score(b2f(lr[i]), inv_t, seed, stepc, (uint32_t)row, (uint32_t)i);
           if (sc > bv || (sc == bv && i < bi)) { bv = sc; bi = i; }
         }
         __syncthreads();
@@ -629,11 +802,16 @@ __device__ __noinline__ void sample_row(const bf16* __restrict__ lr, int n_valid
 // Per-row parameters (batches of utterances at different points of their generation): with step_rows set, row r draws
 // its noise from (seed, step_rows[r], key_rows[r]) instead of (seed, *step_counter, r); with nvalid_rows set, its
 // candidates are the ids < nvalid_rows[r * nv_stride] (top_k clamped to them as the host does for one n_valid).
-// Runtime branches around one call of the same sample_row body, so both forms draw identical tokens from identical inputs.
-__global__ void sample_kernel(const bf16* __restrict__ logits, int V, int n_valid, int top_k, float temp, uint32_t seed,
+// With topk_rows set (temp_rows and topp_rows with it), row r samples with top_k / temp / top_p from entry r * prm_stride
+// of the three tables instead of the scalars; the host validates the tables, and the kernel clamps what would leave
+// SAMPLE_CAND or the candidates (top_k), and reads temp <= 0 (or NaN) as argmax and a top_p that is not >= 0 as 0.
+// Runtime branches around one call of the same sample_row body, so all forms draw identical tokens from identical inputs.
+// Two 1 024-thread blocks per SM (32 registers, as before the nucleus mode; ptxas reports no spills).
+__global__ void __launch_bounds__(1024, 2) sample_kernel(const bf16* __restrict__ logits, int V, int n_valid, int top_k, float temp, float top_p, uint32_t seed,
                               const long long* __restrict__ step_counter, long long* __restrict__ tokens, int tok_stride,
                               const int* __restrict__ nvalid_rows, int nv_stride, const long long* __restrict__ step_rows,
-                              const uint32_t* __restrict__ key_rows) {
+                              const uint32_t* __restrict__ key_rows, const int* __restrict__ topk_rows,
+                              const float* __restrict__ temp_rows, const float* __restrict__ topp_rows, int prm_stride) {
   const int row = blockIdx.x;
   uint32_t stepc, key = (uint32_t)row;
   if (step_rows) {
@@ -647,7 +825,17 @@ __global__ void sample_kernel(const bf16* __restrict__ logits, int V, int n_vali
     if (n_valid <= 0 || n_valid > V) n_valid = V;
     if (top_k > n_valid) top_k = n_valid;
   }
-  sample_row(logits + (long long)row * V, n_valid, top_k, temp, seed, stepc, (int)key, tokens + (long long)row * tok_stride);
+  if (topk_rows) {
+    const long long o = (long long)row * prm_stride;
+    top_k = topk_rows[o];
+    temp = temp_rows[o];
+    top_p = topp_rows[o];
+    if (top_k > SAMPLE_CAND) top_k = SAMPLE_CAND;
+    if (top_k > n_valid) top_k = n_valid;
+    if (!(temp > 0.f)) { top_k = 0; temp = 1.f; }
+    if (!(top_p >= 0.f)) top_p = 0.f;
+  }
+  sample_row(logits + (long long)row * V, n_valid, top_k, temp, top_p, seed, stepc, (int)key, tokens + (long long)row * tok_stride);
 }
 
 }  // namespace rstnet
@@ -784,8 +972,8 @@ extern "C" int rstnet_lm_sample_bf16(const void* logits, int32_t rows, int32_t V
   RSTNET_REQUIRE(top_k <= SAMPLE_CAND && (top_k == 0 || temp > 0.f), "lm_sample: top_k <= %d and temp > 0 required (top_k=%d)", SAMPLE_CAND, top_k);
   if (n_valid <= 0 || n_valid > V) n_valid = V;
   if (top_k > n_valid) top_k = n_valid;   // torch.topk would raise; the whole support is the natural reading
-  sample_kernel<<<dim3(rows), dim3(1024), 0, (cudaStream_t)stream>>>((const bf16*)logits, V, n_valid, top_k, temp, (uint32_t)seed,
-             (const long long*)step_counter, (long long*)tokens, tok_stride, nullptr, 0, nullptr, nullptr);
+  sample_kernel<<<dim3(rows), dim3(1024), 0, (cudaStream_t)stream>>>((const bf16*)logits, V, n_valid, top_k, temp, 0.f, (uint32_t)seed,
+             (const long long*)step_counter, (long long*)tokens, tok_stride, nullptr, 0, nullptr, nullptr, nullptr, nullptr, nullptr, 0);
   count_launch();
   return check_launch("lm_sample");
 }
@@ -797,9 +985,34 @@ extern "C" int rstnet_lm_sample_rows_bf16(const void* logits, int32_t rows, int3
   RSTNET_REQUIRE(top_k <= SAMPLE_CAND && (top_k == 0 || temp > 0.f), "lm_sample_rows: top_k <= %d and temp > 0 required (top_k=%d)", SAMPLE_CAND, top_k);
   if (n_valid <= 0 || n_valid > V) n_valid = V;
   if (!n_valid_rows && top_k > n_valid) top_k = n_valid;   // with per-row candidate counts the kernel clamps per row
-  sample_kernel<<<dim3(rows), dim3(1024), 0, (cudaStream_t)stream>>>((const bf16*)logits, V, n_valid, top_k, temp, (uint32_t)seed,
+  sample_kernel<<<dim3(rows), dim3(1024), 0, (cudaStream_t)stream>>>((const bf16*)logits, V, n_valid, top_k, temp, 0.f, (uint32_t)seed,
              nullptr, (long long*)tokens, tok_stride, (const int*)n_valid_rows, n_valid_stride, (const long long*)step_rows,
-             key_rows);
+             key_rows, nullptr, nullptr, nullptr, 0);
   count_launch();
   return check_launch("lm_sample_rows");
+}
+
+extern "C" int rstnet_lm_sample_params_bf16(const void* logits, int32_t rows, int32_t V, int32_t n_valid, const int32_t* n_valid_rows,
+                                            int32_t n_valid_stride, int32_t top_k, float temp, float top_p, const int32_t* top_k_rows,
+                                            const float* temp_rows, const float* top_p_rows, int32_t param_stride, uint32_t seed,
+                                            const int64_t* step_counter, const int64_t* step_rows, const uint32_t* key_rows,
+                                            int64_t* tokens, int32_t tok_stride, rstnet_stream_t stream) {
+  RSTNET_REQUIRE(logits && tokens && rows > 0 && V > 0, "lm_sample_params: bad argument");
+  const bool tables = top_k_rows || temp_rows || top_p_rows;
+  RSTNET_REQUIRE(!tables || (top_k_rows && temp_rows && top_p_rows && param_stride > 0),
+                 "lm_sample_params: the top_k / temp / top_p tables go together, with a stride > 0");
+  RSTNET_REQUIRE(!step_rows == !key_rows, "lm_sample_params: step_rows and key_rows go together");
+  RSTNET_REQUIRE(!n_valid_rows || n_valid_stride > 0, "lm_sample_params: n_valid_rows needs a stride > 0");
+  if (!tables) {
+    RSTNET_REQUIRE(top_k <= SAMPLE_CAND && (top_k == 0 || temp > 0.f), "lm_sample_params: top_k <= %d and temp > 0 required (top_k=%d)",
+                   SAMPLE_CAND, top_k);
+    RSTNET_REQUIRE(isfinite(top_p) && top_p >= 0.f, "lm_sample_params: top_p must be finite and >= 0 (got %g)", (double)top_p);
+  }
+  if (n_valid <= 0 || n_valid > V) n_valid = V;
+  if (!n_valid_rows && top_k > n_valid) top_k = n_valid;   // with per-row candidate counts the kernel clamps per row
+  sample_kernel<<<dim3(rows), dim3(1024), 0, (cudaStream_t)stream>>>((const bf16*)logits, V, n_valid, top_k, temp, top_p, (uint32_t)seed,
+             (const long long*)step_counter, (long long*)tokens, tok_stride, (const int*)n_valid_rows, n_valid_stride,
+             (const long long*)step_rows, key_rows, (const int*)top_k_rows, temp_rows, top_p_rows, param_stride);
+  count_launch();
+  return check_launch("lm_sample_params");
 }

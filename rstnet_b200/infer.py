@@ -30,7 +30,7 @@ import numpy as np
 import torch
 
 from ._lib import RstnetError
-from .lm import GPT, MAX_STREAMS
+from .lm import GPT, MAX_STREAMS, Sampling
 
 
 def candidate_counts(pre_gen_len: int, minlen: int, g_idx: int, dep_q: int = 8) -> List[int]:
@@ -63,6 +63,11 @@ class InferenceImp(object):
         self.mode = mode
         self.use_sampling = True          # upstream hard-codes True (:162); set the attribute to False for argmax decoding
         self.temp_text, self.top_k_text, self.temp, self.top_k = temp_text, top_k_text, temp, top_k
+        self.top_p_text, self.top_p = 0.0, 0.0   # nucleus sampling of the text / audio heads (0: off, as upstream's callers)
+
+    def sampling(self) -> Sampling:
+        """the instance's settings as one Sampling (validated)"""
+        return Sampling(bool(self.use_sampling), self.temp_text, self.top_k_text, self.top_p_text, self.temp, self.top_k, self.top_p)
 
     @torch.no_grad()
     def __call__(self, seq: torch.Tensor, mask: torch.Tensor):
@@ -100,7 +105,8 @@ class InferenceImp(object):
                 # and for codebooks > 0 once g_len > minlen, otherwise 2048
                 valid = tuple(candidate_counts(pre_gen_len, minlen, g_idx))
                 toks = m.forward_step(cur, use_sampling=self.use_sampling, temp_text=self.temp_text, top_k_text=self.top_k_text,
-                                      temp=self.temp, top_k=self.top_k, audio_valid=valid, depth_ring_quirk=False)
+                                      temp=self.temp, top_k=self.top_k, audio_valid=valid, depth_ring_quirk=False,
+                                      top_p_text=self.top_p_text, top_p=self.top_p)
                 frames.append(toks)
                 cur = toks[:, :, None]
             m.check_device_errors()
@@ -242,17 +248,26 @@ class InferenceImp(object):
 
     @torch.no_grad()
     def generate_many(self, items: Iterable[Tuple[object, torch.Tensor]], capacity: int,
-                      seeds: Optional[Dict[object, int]] = None, return_frames: bool = False) -> Iterator[Tuple]:
+                      seeds: Optional[Dict[object, int]] = None, return_frames: bool = False,
+                      sampling: Optional[Dict[object, Sampling]] = None) -> Iterator[Tuple]:
         """Continuous batching over (utt_id, seq [9, L]) items, each in its own TTS layout: yields (utt_id, codes [8, G-1])
         in completion order.  Up to `capacity` utterances decode together, one graph replay per frame; a finished row is
         held until the next utterance is admitted into it (its prompt fed through GPT.prefill_streams while the other
         rows keep their state).  Each utterance samples with its own candidate sets (candidate_counts) and its own random
         stream, keyed by seeds[utt_id] (default 0) and its own frame count from 0: with the defaults its codes are those
-        of generate() on that utterance alone.  return_frames: yield (utt_id, codes, raw frames [G, 9]) as generate does."""
+        of generate() on that utterance alone.  return_frames: yield (utt_id, codes, raw frames [G, 9]) as generate does.
+        sampling: {utt_id: Sampling} gives those utterances their own settings (the others take the instance's); each
+        utterance's codes are then those of generate() on it alone with its settings, whatever the others' settings.
+        The settings are rows of device tables: changing them captures no new graph."""
         self._check_task()
         if not 1 <= capacity <= MAX_STREAMS:
             raise RstnetError(f"capacity must be in [1, {MAX_STREAMS}] (got {capacity})")
         m, seeds = self.model, seeds or {}
+        if sampling is not None:
+            default = self.sampling()
+            for utt, sp in sampling.items():
+                if not isinstance(sp, Sampling):
+                    raise RstnetError(f"sampling[{utt!r}] must be a Sampling (got {type(sp).__name__})")
         dev, B = m.device, capacity
         n_cb = m.num_codebooks
         dep_q = n_cb - 1                 # text + dep_q audio codebooks per frame
@@ -300,9 +315,13 @@ class InferenceImp(object):
                 for r in occupied:
                     st = rows[r]
                     table[r] = torch.tensor(candidate_counts(st["P"], st["G"], st["g"], dep_q), dtype=torch.int32)
+                per_row = None
+                if sampling is not None:
+                    per_row = [sampling.get(rows[r]["utt"], default) if rows[r] is not None else default for r in range(B)]
                 toks = m.forward_step(cur, use_sampling=self.use_sampling, temp_text=self.temp_text, top_k_text=self.top_k_text,
                                       temp=self.temp, top_k=self.top_k, audio_valid=table,
-                                      sample_key=keys if admitted else None, depth_ring_quirk=False)
+                                      sample_key=keys if admitted else None, depth_ring_quirk=False,
+                                      top_p_text=self.top_p_text, top_p=self.top_p, sampling=per_row)
                 history[frame] = toks
                 frame += 1
                 cur = toks[:, :, None].clone()

@@ -38,6 +38,51 @@ MAX_STREAMS = 256   # streams of one decode scope (one position each): the wides
                     # tile once for up to 256 rows
 ROW_BUCKETS = (16, 32, 64, 128)   # launch widths of a ragged prefill chunk (padding rows fill the rest): one chunk state and
                                   # one set of GEMM plans per width
+SAMPLE_CAND = 1024   # the sampler's largest top_k
+
+
+@dataclass(frozen=True)
+class Sampling:
+    """The sampling settings of one generated stream (sample_token, utils/sampling.py:85-105), for the text head
+    (temp_text / top_k_text / top_p_text) and the audio heads (temp / top_k / top_p).  use_sampling False, or a temperature
+    <= 0, is argmax; otherwise top_p > 0 is nucleus sampling (it takes precedence over top_k, as in the reference),
+    top_k > 0 top-k, and top_p 0 with top_k <= 0 the plain multinomial (as forward_step reads top_k <= 0).  Defaults: GPT.forward_step's.  Validated once, here."""
+    use_sampling: bool = True
+    temp_text: float = 0.7
+    top_k_text: int = 25
+    top_p_text: float = 0.0
+    temp: float = 0.8
+    top_k: int = 30
+    top_p: float = 0.0
+
+    def __post_init__(self):
+        for name in ("temp_text", "temp", "top_p_text", "top_p"):
+            v = getattr(self, name)
+            if isinstance(v, bool) or not isinstance(v, (int, float)) or not np.isfinite(v):
+                raise RstnetError(f"Sampling.{name} must be a finite number (got {v!r})")
+            if name.startswith("top_p") and v < 0:
+                raise RstnetError(f"Sampling.{name} must be >= 0 (got {v!r})")
+        for name in ("top_k_text", "top_k"):
+            v = getattr(self, name)
+            if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or v > SAMPLE_CAND:
+                raise RstnetError(f"Sampling.{name} must be an int <= {SAMPLE_CAND} (got {v!r})")
+
+    def heads(self):
+        """((top_k, temp, top_p) of the text head, (...) of the audio heads) in the sampler's convention: top_k 0 argmax,
+        > 0 top-k, -1 the multinomial over every candidate; 0 < top_p < 1 nucleus.  top_p >= 1 keeps every candidate,
+        which is the multinomial."""
+        return (_head_mode(self.use_sampling, self.temp_text, self.top_k_text, self.top_p_text),
+                _head_mode(self.use_sampling, self.temp, self.top_k, self.top_p))
+
+
+def _head_mode(use_sampling, temp, top_k, top_p):
+    if not (use_sampling and temp > 0.0):
+        return 0, 1.0, 0.0
+    if top_p >= 1.0:
+        return -1, float(temp), 0.0
+    if top_p > 0.0:
+        return -1, float(temp), float(top_p)
+    return (int(top_k) if top_k > 0 else -1), float(temp), 0.0
 
 
 @dataclass
@@ -488,7 +533,7 @@ class GPT(nn.Module):
     @on_own_device
     def forward_step(self, sequence: torch.Tensor, *, use_sampling: bool = True, temp_text: float = 0.7, top_k_text: int = 25,
                      temp: float = 0.8, top_k: int = 30, audio_valid=2049, depth_ring_quirk: bool = True, sample_key=None,
-                     sample_step=None) -> torch.Tensor:
+                     sample_step=None, top_p_text: float = 0.0, top_p: float = 0.0, sampling=None) -> torch.Tensor:
         """One generated frame: temporal step on sequence[B,9,1], text token, then the 8 depth steps, each sampled
         on the device (sample_token / sample_token_audio[_2048], utils/sampling.py:85-154: use_sampling False ->
         argmax over the whole card; True -> temperature + top-k (top_k == 0: plain multinomial) over ids <
@@ -500,11 +545,20 @@ class GPT(nn.Module):
         counter instead of (row, scope frame counter).  sample_key [B] (uint32 values) and sample_step [B] (int64), when
         given, set the scope's per-row keys and step counters before the frame; otherwise they keep their values.  The
         step counters start at 0 (scope entry, reset_streaming of the row) and advance by one per frame for active rows.
-        All three live in fixed device buffers, so one captured graph serves every frame."""
+        All three live in fixed device buffers, so one captured graph serves every frame.
+
+        top_p_text / top_p > 0: nucleus sampling of the text / audio heads (sample_top_p, utils/sampling.py:66-82; it
+        takes precedence over top_k).  With both 0 the frame launches exactly what it launched without them.
+
+        Per-row settings: sampling, a list of B `Sampling` (with a per-row audio_valid table), replaces the scalar settings
+        (use_sampling .. top_k, top_p_text, top_p) by each row's own.  They live in device tables of the scope, written
+        only when they change, so changing a row's settings replays the same graph."""
         if self._state is None:
             raise RstnetError("forward_step is a streaming call: use it inside `with gpt.streaming(B):`")
+        if sampling is None and (top_p_text or top_p):
+            Sampling(use_sampling, temp_text, top_k_text, top_p_text, temp, top_k, top_p)   # validates a nucleus frame's settings
         return self._state.forward_step(sequence, use_sampling, temp_text, top_k_text, temp, top_k, audio_valid, depth_ring_quirk,
-                                        sample_key, sample_step)
+                                        sample_key, sample_step, top_p_text, top_p, sampling)
 
     @torch.no_grad()
     @on_own_device
@@ -699,6 +753,11 @@ class _LMState:
             self.row_valid = z(M, c.dep_q, dtype=torch.int32)
             self.row_key = z(M, dtype=torch.int32)
             self.row_step = z(M, dtype=torch.int64)
+            # per-row settings (forward_step(sampling=...)): column 0 the text head, column 1 the audio heads
+            self.row_topk = z(M, 2, dtype=torch.int32)
+            self.row_temp = z(M, 2, dtype=torch.float32)
+            self.row_topp = z(M, 2, dtype=torch.float32)
+            self._row_params = None   # (the Sampling list last uploaded to the three tables, its argmax rows)
             hd = D // c.codecformer_heads
             self.dkv_all = z(c.codecformer_layers, 2, M, c.codecformer_heads, c.dep_q, hd)
             self.dkv = [self.dkv_all[l] for l in range(c.codecformer_layers)]
@@ -886,6 +945,42 @@ class _LMState:
                                                          self.tokens.data_ptr() + 8 * col, self.c.dep_q + 1, ops._stream()),
                    "sample_rows")
 
+    def _sample_params(self, logits: torch.Tensor, V: int, n_valid: int, per_row_valid: Optional[int], mode, head: Optional[int],
+                       col: int, salt: int, per_row_rng: bool):
+        """The general sampler: mode = (top_k, temp, top_p) for every row, or head = the column of the row_topk / row_temp /
+        row_topp tables; per_row_valid as _sample_rows (None: n_valid); per_row_rng: row_key / row_step in place of
+        (row, frame_counter)."""
+        nv = None if per_row_valid is None else self.row_valid.data_ptr() + 4 * per_row_valid
+        tk, temp, tp = mode if mode is not None else (0, 1.0, 0.0)
+        tabs = [None, None, None] if head is None else [t.data_ptr() + 4 * head for t in (self.row_topk, self.row_temp, self.row_topp)]
+        _lib.check(_lib.lib().rstnet_lm_sample_params_bf16(
+            logits.data_ptr(), self.M, V, n_valid, nv, self.c.dep_q, tk, float(temp), float(tp), *tabs, 2, self.seed + salt,
+            None if per_row_rng else self.frame_counter.data_ptr(), self.row_step.data_ptr() if per_row_rng else None,
+            self.row_key.data_ptr() if per_row_rng else None, self.tokens.data_ptr() + 8 * col, self.c.dep_q + 1, ops._stream()),
+            "sample_params")
+
+    def set_row_sampling(self, sampling):
+        """sampling: B `Sampling` -> the scope's per-row tables, uploaded from pinned memory without a synchronise, and
+        only when the settings differ from the last call's (an unchanged list costs one comparison of B tuples).
+        Returns a device bool [B, 1] of the rows whose audio heads take the argmax, or None when every row samples."""
+        last = self._row_params
+        if last is not None and list(sampling) == last[0]:
+            return last[1]
+        if len(sampling) != self.B or not all(isinstance(s, Sampling) for s in sampling):
+            raise RstnetError(f"sampling must be a list of {self.B} Sampling")
+        heads = [s.heads() for s in sampling]
+        tk = np.array([[h[0][0], h[1][0]] for h in heads], dtype=np.int32)
+        te = np.array([[h[0][1], h[1][1]] for h in heads], dtype=np.float32)
+        tp = np.array([[h[0][2], h[1][2]] for h in heads], dtype=np.float32)
+        for dst, src in zip((self.row_topk, self.row_temp, self.row_topp), (tk, te, tp)):
+            dst[:self.B].copy_(torch.from_numpy(src).pin_memory(), non_blocking=True)
+        argmax = tk[:, 1] == 0
+        argmax_dev = None
+        if argmax.any():
+            argmax_dev = torch.from_numpy(argmax[:, None].copy()).pin_memory().to(self.row_valid.device, non_blocking=True)
+        self._row_params = (list(sampling), argmax_dev)
+        return argmax_dev
+
     def _replay(self, key, fn):
         if not self.m.use_cuda_graphs:
             fn()
@@ -1067,11 +1162,13 @@ class _LMState:
             out[:, k].copy_(self.dlogits)
 
     def forward_step(self, sequence, use_sampling, temp_text, top_k_text, temp, top_k, audio_valid, quirk=True, sample_key=None,
-                     sample_step=None):
+                     sample_step=None, top_p_text=0.0, top_p=0.0, sampling=None):
         c = self.c
         if sequence.shape[0] != self.B or sequence.shape[2] != 1:
             raise RstnetError(f"forward_step takes sequence [{self.B}, {c.n_q + 1}, 1], got {tuple(sequence.shape)}")
         per_row = torch.is_tensor(audio_valid)
+        if sampling is not None and not per_row:
+            raise RstnetError("per-row sampling settings go with per-row candidate counts: pass audio_valid as a [B, dep_q] tensor")
         if per_row:
             if tuple(audio_valid.shape) != (self.B, c.dep_q):
                 raise RstnetError(f"a per-row audio_valid is [{self.B}, {c.dep_q}], got {tuple(audio_valid.shape)}")
@@ -1082,14 +1179,69 @@ class _LMState:
                 self.row_step.copy_(torch.as_tensor(sample_step, dtype=torch.int64).reshape(self.B))
         elif sample_key is not None or sample_step is not None:
             raise RstnetError("sample_key / sample_step select per-row sampling: pass audio_valid as a [B, dep_q] tensor")
+        if sampling is not None:
+            argmax = self.set_row_sampling(sampling)
+            if argmax is not None:
+                # the 2048 / 2049 candidate sets exist on the sampling path only: argmax rows take the whole card
+                audio_valid = torch.where(argmax, c.audio_card, audio_valid.to(argmax.device))
         self._advance_host(1)
         self.seq.copy_(sequence[:, :, 0])
-        if per_row:
+        if sampling is not None:
             self.row_valid.copy_(audio_valid)
-            self._replay(*self._frame_rows(use_sampling, temp_text, top_k_text, temp, top_k, quirk))
+            self._replay(*self._frame_params(quirk))
+        elif per_row:
+            self.row_valid.copy_(audio_valid)
+            if top_p_text or top_p:
+                self._replay(*self._frame_nucleus(use_sampling, temp_text, top_k_text, top_p_text, temp, top_k, top_p, None, quirk))
+            else:
+                self._replay(*self._frame_rows(use_sampling, temp_text, top_k_text, temp, top_k, quirk))
+        elif top_p_text or top_p:
+            self._replay(*self._frame_nucleus(use_sampling, temp_text, top_k_text, top_p_text, temp, top_k, top_p, audio_valid, quirk))
         else:
             self._replay(*self._frame(use_sampling, temp_text, top_k_text, temp, top_k, audio_valid, quirk))
         return self.tokens.clone()
+
+    def _frame_nucleus(self, use_sampling, temp_text, top_k_text, top_p_text, temp, top_k, top_p, audio_valid, quirk):
+        """_frame (audio_valid given) or _frame_rows (None: row_valid, row_key, row_step) with top_p: every head through the
+        general sampler, one setting for all rows."""
+        c = self.c
+        rows = audio_valid is None
+        mt, ma = Sampling(use_sampling, temp_text, top_k_text, top_p_text, temp, top_k, top_p).heads()
+        sampling = ma[0] != 0
+        valid = (c.audio_card,) * c.dep_q
+        if sampling and not rows:
+            valid = tuple(audio_valid) if isinstance(audio_valid, (tuple, list)) else (audio_valid,) * c.dep_q
+
+        def frame():
+            self._temporal()
+            self._sample_params(self.logits, c.padded_vocab_size, c.padded_vocab_size, None, mt, None, 0, 0, rows)
+            self.tout.copy_(self.out)
+            for k in range(c.dep_q):
+                self._depth(k, self.tokens[:, k], c.dep_q + 1, quirk=quirk)
+                self._sample_params(self.dlogits, c.audio_card, min(valid[k], c.audio_card), k if (rows and sampling) else None,
+                                    ma, None, k + 1, k + 1, rows)
+            if rows:
+                ops.counter_add(self.row_step, 1, self.active)
+            else:
+                ops.counter_add(self.frame_counter, 1)
+
+        return ("frame_nucleus", mt, ma, None if rows else valid, bool(quirk)), frame
+
+    def _frame_params(self, quirk):
+        """_frame_rows with every row's settings read from the row_topk / row_temp / row_topp tables: one graph whatever
+        the settings.  row_valid already holds the whole card for the rows whose audio heads take the argmax."""
+        c = self.c
+
+        def frame():
+            self._temporal()
+            self._sample_params(self.logits, c.padded_vocab_size, c.padded_vocab_size, None, None, 0, 0, 0, True)
+            self.tout.copy_(self.out)
+            for k in range(c.dep_q):
+                self._depth(k, self.tokens[:, k], c.dep_q + 1, quirk=quirk)
+                self._sample_params(self.dlogits, c.audio_card, c.audio_card, k, None, 1, k + 1, k + 1, True)
+            ops.counter_add(self.row_step, 1, self.active)
+
+        return ("frame_params", bool(quirk)), frame
 
     def _frame_rows(self, use_sampling, temp_text, top_k_text, temp, top_k, quirk):
         """_frame with per-row candidate counts (row_valid), RNG keys (row_key) and step counters (row_step)."""

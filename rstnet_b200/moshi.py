@@ -34,7 +34,7 @@ from torch import nn
 from . import _lib, ops
 from ._lib import RstnetError
 from .codec import _register, on_own_device
-from .lm import GPT, SkinnyGemm, _DepthScope, _LMState  # noqa: F401
+from .lm import GPT, Sampling, SkinnyGemm, _DepthScope, _LMState  # noqa: F401
 
 
 class _MoshiState(_LMState):
@@ -364,11 +364,15 @@ class LMGen(nn.Module):
     A scope whose rows all start together behaves exactly as the reference."""
 
     def __init__(self, lm_model: LMModel, use_sampling: bool = True, temp: float = 0.8, temp_text: float = 0.7, top_k: int = 250,
-                 top_k_text: int = 25, check: bool = False):
+                 top_k_text: int = 25, check: bool = False, top_p: float = 0.0, top_p_text: float = 0.0):
         super().__init__()
         self.lm_model = lm_model
         self.use_sampling, self.temp, self.temp_text, self.top_k, self.top_k_text, self.check = \
             use_sampling, temp, temp_text, top_k, top_k_text, check
+        self.top_p, self.top_p_text = top_p, top_p_text
+        if top_p or top_p_text:
+            self.default_sampling()   # validates
+        self._row_sampling: Optional[list] = None   # per-row Sampling once a row was given its own settings
         self.max_delay = max(lm_model.delays)
         self.delays_cuda = torch.tensor(lm_model.delays, device=lm_model.device, dtype=torch.long)
         self._st: Optional[_GenState] = None
@@ -381,6 +385,7 @@ class LMGen(nn.Module):
         lm = self.lm_model
         lm.streaming_forever(batch_size)
         self._st = _GenState(self, lm._st(), batch_size)
+        self._row_sampling = None
 
     @contextmanager
     def streaming(self, batch_size: int):
@@ -410,6 +415,29 @@ class LMGen(nn.Module):
         st.valid[rows] = 0
         st.off_host[rows_h] = 0
         st.stepped[rows_h] = False
+
+    def default_sampling(self) -> Sampling:
+        return Sampling(bool(self.use_sampling), self.temp_text, self.top_k_text, self.top_p_text, self.temp, self.top_k, self.top_p)
+
+    def set_stream_sampling(self, streams, sampling: Optional[Sampling] = None, seed: Optional[int] = None) -> None:
+        """Extension for batched serving: give the rows in `streams` their own settings (None: the generator's) and their
+        own random stream keyed by `seed` (None: 0) and the row's step count (0 at reset_streaming of the row).  From the
+        first call on, every row samples through the per-row tables and keys, so a row's tokens no longer depend on which
+        row it is or when it started; until then the scope draws exactly as before.  Rows reset without a seed share key 0:
+        two of them with the same settings and input draw the same tokens, so pass distinct seeds to decorrelate them."""
+        st = self._require()
+        if sampling is not None and not isinstance(sampling, Sampling):
+            raise RstnetError(f"sampling must be a Sampling (got {type(sampling).__name__})")
+        rows = [int(r) for r in np.asarray(streams, dtype=np.int64).reshape(-1)]
+        if any(not 0 <= r < st.B for r in rows):
+            raise RstnetError(f"stream index outside [0, {st.B})")
+        if self._row_sampling is None or len(self._row_sampling) != st.B:
+            self._row_sampling = [self.default_sampling()] * st.B
+            st.lm.row_key.zero_()
+        key = int(seed or 0) & 0xFFFFFFFF
+        for r in rows:
+            self._row_sampling[r] = sampling if sampling is not None else self.default_sampling()
+        st.lm.row_key[rows] = key - 2 ** 32 if key >= 2 ** 31 else key   # the uint32 bits
 
     def set_active_streams(self, mask) -> None:
         """Extension for batched serving: the rows whose flag is 0 are held by the following steps -- their cache, step
@@ -445,7 +473,14 @@ class LMGen(nn.Module):
         """(graph key, launch sequence): cache_in -> temporal step + text sampling + dep_q depth steps with sampling
         (sample_token over the whole card: LMGen uses plain `sample_token`, models/model.py:528-533, 581-586) -> cache_out."""
         lm, ms, L = self.lm_model, st.lm, _lib.lib()
-        key, frame = ms._frame(self.use_sampling, self.temp_text, self.top_k_text, self.temp, self.top_k, lm.card, True)
+        if self._row_sampling is not None:
+            ms.set_row_sampling(self._row_sampling)     # row_valid stays 0: every row samples over the whole card
+            key, frame = ms._frame_params(True)
+        elif self.top_p or self.top_p_text:
+            key, frame = ms._frame_nucleus(self.use_sampling, self.temp_text, self.top_k_text, self.top_p_text, self.temp,
+                                           self.top_k, self.top_p, lm.card, True)
+        else:
+            key, frame = ms._frame(self.use_sampling, self.temp_text, self.top_k_text, self.temp, self.top_k, lm.card, True)
         K, CT = lm.num_codebooks, st.cache.shape[2]
 
         def step():

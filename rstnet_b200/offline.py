@@ -216,6 +216,9 @@ def _synthesize_cli(args) -> int:
     model = _load_gpt(args.config, args.checkpoint, args.device)
     imp = InferenceImp(None, model, "sampling", args.temp_text, args.top_k_text, args.temp, args.top_k, "TTS")
     imp.use_sampling = args.use_sampling
+    imp.top_p, imp.top_p_text = args.top_p, args.top_p_text
+    if args.top_p or args.top_p_text:
+        imp.sampling()   # validates a nucleus run's settings before the model runs
     corpus = torch.load(args.input, map_location="cpu")
     codes = synthesize(imp, corpus, args.capacity)
     save_tokens(codes, args.output_file)
@@ -323,6 +326,8 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--top-k", type=int, default=30)
     p.add_argument("--temp-text", type=float, default=0.7)
     p.add_argument("--top-k-text", type=int, default=25)
+    p.add_argument("--top-p", type=float, default=0.0, help="nucleus sampling of the audio heads (0: off; takes precedence over --top-k)")
+    p.add_argument("--top-p-text", type=float, default=0.0, help="nucleus sampling of the text head (0: off)")
     p.add_argument("--wav-dir", default=None, help="also write <utt_id>_sample.wav here (needs --codec-weights)")
     p.add_argument("--codec-weights", default=None)
     p.add_argument("--codec-config", default=None, help="json with the MimiCodec constructor arguments")

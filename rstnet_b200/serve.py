@@ -23,11 +23,12 @@ import time
 from collections import deque
 from typing import Deque, Dict, Hashable, List, Optional, Tuple
 
+import numpy as np
 import torch
 
 from ._lib import RstnetError
 from .audio import StreamingResampler
-from .lm import MAX_STREAMS
+from .lm import MAX_STREAMS, Sampling
 
 FRAME_SAMPLES = 1920       # 80 ms at 24 kHz = one 12.5 Hz frame (moshi/server.py:57: sample_rate / frame_rate)
 FRAME_SECONDS = 0.08
@@ -56,9 +57,12 @@ class FrameScheduler:
         self.ticks = 0
 
     # ---- session lifecycle
-    def admit(self, session: Hashable) -> int:
+    def admit(self, session: Hashable, sampling=None, seed: Optional[int] = None) -> int:
         """Lease the lowest free row to `session` and restart that row's streaming state (server.py:156-158 does
-        `mimi.reset_streaming(); lm_gen.reset_streaming()` for its single session)."""
+        `mimi.reset_streaming(); lm_gen.reset_streaming()` for its single session).  sampling (an lm.Sampling) / seed:
+        the session's own settings and random stream, passed to the engine's reset_rows; None: the engine's defaults.
+        Once any session brought settings, a session's random stream is its seed alone (None: 0): pass distinct seeds to
+        keep sessions with the same settings and input apart."""
         if session in self._row_of:
             raise RuntimeError(f"session {session!r} is already admitted")
         if not self._free:
@@ -67,7 +71,10 @@ class FrameScheduler:
         row = self._free.pop(0)
         self._row_of[session] = row
         self._queue[session] = deque()
-        self.engine.reset_rows([row])
+        if sampling is None and seed is None:
+            self.engine.reset_rows([row])
+        else:
+            self.engine.reset_rows([row], sampling=sampling, seed=seed)
         return row
 
     def release(self, session: Hashable) -> None:
@@ -108,7 +115,7 @@ class DuplexEngine:
     encode and 24 kHz -> r after the decode; row resets and the held-row mask apply to both."""
 
     def __init__(self, codec, gpt, capacity: int, *, use_sampling: bool = True, temp_text: float = 0.7, top_k_text: int = 25,
-                 temp: float = 0.8, top_k: int = 30, sample_rate: int = CODEC_RATE):
+                 temp: float = 0.8, top_k: int = 30, sample_rate: int = CODEC_RATE, top_p_text: float = 0.0, top_p: float = 0.0):
         self.sample_rate = check_client_rate(sample_rate)
         self.frame_samples = self.sample_rate * 2 // 25                       # 80 ms at the client rate
         if capacity > MAX_STREAMS:
@@ -117,6 +124,13 @@ class DuplexEngine:
         self.codec, self.gpt, self.B = codec, gpt, capacity
         self.dev = gpt.device
         self.sampling = dict(use_sampling=use_sampling, temp_text=temp_text, top_k_text=top_k_text, temp=temp, top_k=top_k)
+        if top_p_text or top_p:
+            self.sampling.update(top_p_text=top_p_text, top_p=top_p)
+        self._defaults = (use_sampling, temp_text, top_k_text, top_p_text, temp, top_k, top_p)
+        self.row_sampling: Optional[List[Sampling]] = None   # per-row settings once a session brought its own
+        self.row_keys = np.zeros(capacity, dtype=np.int64)
+        self._keys_dirty = False
+        self._valid_table = None
         codec.streaming_forever(capacity)
         gpt.streaming_forever(capacity)
         F = self.frame_samples
@@ -134,7 +148,22 @@ class DuplexEngine:
         self.mask_host = torch.zeros(capacity, dtype=torch.int64).pin_memory()
         self.latencies_ms: List[float] = []
 
-    def reset_rows(self, rows) -> None:
+    def reset_rows(self, rows, sampling=None, seed: Optional[int] = None) -> None:
+        """Restart `rows`.  sampling / seed give them their own settings and random stream (keyed by the seed and the
+        row's own frame count); from the first such call on, every row samples through per-row tables and keys, so a
+        session's tokens do not depend on its row or its admission tick.  Until then the engine draws exactly as before.
+        A session's random stream is its seed alone (None: 0): two sessions with the same settings, seed and input draw the
+        same tokens, so callers that want them decorrelated pass distinct seeds."""
+        if sampling is not None and not isinstance(sampling, Sampling):
+            raise RstnetError(f"sampling must be a Sampling (got {type(sampling).__name__})")
+        if sampling is not None or seed is not None or self.row_sampling is not None:
+            default = Sampling(*self._defaults)
+            if self.row_sampling is None:
+                self.row_sampling = [default] * self.B
+            for r in rows:
+                self.row_sampling[r] = sampling if sampling is not None else default
+                self.row_keys[r] = int(seed or 0) & 0xFFFFFFFF
+            self._keys_dirty = True
         self.codec.reset_streaming(streams=list(rows))
         self.gpt.reset_streaming(streams=list(rows))
         self.prev_text[list(rows)] = self.gpt.text_initial_token_id
@@ -160,7 +189,14 @@ class DuplexEngine:
             self.up(self.pcm_client_dev[:, 0], out=self.pcm_dev[:, 0])                  # r -> 24 kHz, all rows
         codes = self.codec.encode(self.pcm_dev)                                   # [B, 8, 1]
         frame = torch.cat([self.prev_text, codes], dim=1)                        # [B, 9, 1]
-        toks = self.gpt.forward_step(frame, audio_valid=2048, **self.sampling)    # [B, 9]
+        if self.row_sampling is None:
+            toks = self.gpt.forward_step(frame, audio_valid=2048, **self.sampling)    # [B, 9]
+        else:
+            if self._valid_table is None:
+                self._valid_table = torch.full((self.B, self.gpt.config.dep_q), 2048, dtype=torch.int32, device=self.dev)
+            toks = self.gpt.forward_step(frame, audio_valid=self._valid_table, sampling=self.row_sampling,
+                                         sample_key=self.row_keys if self._keys_dirty else None)
+            self._keys_dirty = False
         held = (self.mask_host == 0).to(self.dev)
         self.prev_text.copy_(torch.where(held[:, None, None], self.prev_text, toks[:, :1, None]))
         pcm = self.codec.decode(toks[:, 1:, None].clamp(max=self.codec.codebook_size - 1))   # [B, 1, 1920]
@@ -214,9 +250,12 @@ class MoshiDuplexEngine:
         self.dec_mask_dev = torch.zeros(capacity, dtype=torch.int64, device=self.dev)
         self.latencies_ms: List[float] = []
 
-    def reset_rows(self, rows) -> None:
+    def reset_rows(self, rows, sampling=None, seed: Optional[int] = None) -> None:
+        """Restart `rows`; sampling / seed as DuplexEngine.reset_rows (LMGen.set_stream_sampling)."""
         self.codec.reset_streaming(streams=list(rows))
         self.lm_gen.reset_streaming(streams=list(rows))
+        if sampling is not None or seed is not None or getattr(self.lm_gen, "_row_sampling", None) is not None:
+            self.lm_gen.set_stream_sampling(list(rows), sampling, seed)
         if self.up is not None:
             self.up.reset(rows)
             self.down.reset(rows)

@@ -335,19 +335,16 @@ int rstnet_lm_rms_norm_bf16(const void* x, const void* w, void* y, int32_t rows,
  * has Tn == 1; a prefill chunk several consecutive positions per stream).  qkv [rows][n_kv][n_head/n_kv + 2][hs] (litgpt
  * per-group interleave, llama_streaming.py:952-963; n_kv == n_head is MHA); q_out [rows][n_head*hs];
  * kv [2][B][n_kv][cap][hs] -- K/V are stored once per KV GROUP (the reference expands them to n_head copies before its
- * cache, :965-967; the attention result is the same).  A position >= rope_rows -> NaN q/k + error bit 1. */
+ * cache, :965-967; the attention result is the same).  A position >= rope_rows -> NaN q/k + error bit 1.
+ * Row map (ragged prefill of some streams of a live scope, GPT.prefill_streams; serves the prompt pass of
+ * infer_no_streaming.py:232-240 for a batch of utterances with different prompt lengths): with row_stream / row_tl given
+ * (both or neither; offset_stride must be 1), row r is stream row_stream[r] at position offset[row_stream[r]] + row_tl[r]
+ * instead, in any order of (stream, position) pairs, and rows need not be a multiple of B; row_stream[r] == -1 marks a
+ * padding row that reads and writes nothing.  Both forms run one compiled kernel. */
 int rstnet_lm_rope_kv_append_bf16(const void* qkv, const void* cos_tab, const void* sin_tab, int64_t rope_rows, int32_t rope_n,
-                                  const int64_t* offset, int32_t offset_stride /* 0 shared, 1 per stream */, void* q_out,
-                                  void* kv, int32_t rows, int32_t B, int32_t n_head, int32_t n_kv, int32_t hs, int32_t cap,
-                                  rstnet_stream_t stream);
-/* Row-mapped form (ragged prefill of some streams of a live scope, GPT.prefill_streams; serves the prompt pass of
- * infer_no_streaming.py:232-240 for a batch of utterances with different prompt lengths): row r is stream row_stream[r] at
- * position offset[row_stream[r]] + row_tl[r] (per-stream counters); row_stream[r] == -1 marks a padding row that reads
- * and writes nothing.  Any order of (stream, position) pairs; the same compiled kernel as the uniform form. */
-int rstnet_lm_rope_kv_append_rows_bf16(const void* qkv, const void* cos_tab, const void* sin_tab, int64_t rope_rows,
-                                       int32_t rope_n, const int64_t* offset, const int32_t* row_stream, const int32_t* row_tl,
-                                       void* q_out, void* kv, int32_t rows, int32_t B, int32_t n_head, int32_t n_kv, int32_t hs,
-                                       int32_t cap, rstnet_stream_t stream);
+                                  const int64_t* offset, int32_t offset_stride /* 0 shared, 1 per stream */,
+                                  const int32_t* row_stream, const int32_t* row_tl, void* q_out, void* kv, int32_t rows,
+                                  int32_t B, int32_t n_head, int32_t n_kv, int32_t hs, int32_t cap, rstnet_stream_t stream);
 /* ---- Kyutai pair-RoPE for the Moshi-style LMModel's temporal transformer (models/model.py:364-389; modules/rope.py:11-68,
  * modules/transformer.py:391-399): qkv [rows][3][H][hd] ((p h d) layout); (even, odd) pairs of q / k rotate by
  * freqs[p] * (offset + tl) (freqs [hd/2] fp32 = exp(-ln(max_period) * 2 p / hd), from the host), fp32 inside, one rounding
@@ -357,16 +354,13 @@ int rstnet_lm_rope_pair_kv_append_bf16(const void* qkv, const int64_t* offset, i
                                        int32_t rows, int32_t B, int32_t H, int32_t hd, int32_t cap, const float* freqs,
                                        rstnet_stream_t stream);
 /* ---- one query position per row over the ring with RingKVCache.complete's position labels and the
- * (pos_k>=0)&(delta>=0)&(delta<context) mask (llama_streaming.py:983-992), fp32 softmax. HBM-bound.  Rows as above;
- * every position of the launch must already be in the ring and no slot a query needs may have been overwritten
- * (callers keep *offset + Tn <= cap for Tn > 1). */
+ * (pos_k>=0)&(delta>=0)&(delta<context) mask (llama_streaming.py:983-992), fp32 softmax. HBM-bound.  Rows and row map as
+ * rstnet_lm_rope_kv_append_bf16 (padding rows write no output); every position of the launch must already be in the ring
+ * and no slot a query needs may have been overwritten (callers keep *offset + Tn <= cap for Tn > 1). */
 int rstnet_lm_ring_decode_attention_bf16(const void* q, const void* kv, const int64_t* offset, int32_t offset_stride,
-                                         void* out, int32_t rows, int32_t B, int32_t n_head, int32_t n_kv, int32_t hs,
-                                         int32_t cap, int32_t context, rstnet_stream_t stream);
-/* Row-mapped form: rows as rstnet_lm_rope_kv_append_rows_bf16 (padding rows write no output). */
-int rstnet_lm_ring_decode_attention_rows_bf16(const void* q, const void* kv, const int64_t* offset, const int32_t* row_stream,
-                                              const int32_t* row_tl, void* out, int32_t rows, int32_t B, int32_t n_head,
-                                              int32_t n_kv, int32_t hs, int32_t cap, int32_t context, rstnet_stream_t stream);
+                                         const int32_t* row_stream, const int32_t* row_tl, void* out, int32_t rows, int32_t B,
+                                         int32_t n_head, int32_t n_kv, int32_t hs, int32_t cap, int32_t context,
+                                         rstnet_stream_t stream);
 /* out[m][c] = silu(ab[m][c]) * ab[m][I + c]   (LLaMAMLP / ActivationGating) */
 int rstnet_lm_silu_mul_bf16(const void* ab, void* out, int32_t M, int32_t I, rstnet_stream_t stream);
 /* ---- depth transformer attention at codebook step `step` (keys 0..step, capacity dep_q <= 8, no RoPE):
@@ -375,38 +369,30 @@ int rstnet_lm_silu_mul_bf16(const void* ab, void* out, int32_t M, int32_t I, rst
  * on the last step; 0: non-streaming form (forward_local, :694-725; KVCacheResult.from_kv keeps every key). */
 int rstnet_lm_depth_attention_bf16(const void* qkv, void* kvd, void* out, int32_t B, int32_t H, int32_t hd, int32_t cap,
                                    int32_t step, int32_t ring_quirk, rstnet_stream_t stream);
-/* ---- sample_token / sample_token_audio[_2048] (utils/sampling.py:85-154): ids restricted to [0, n_valid);
- * top_k == 0 -> argmax (first maximum; use_sampling False); 1 <= top_k <= 1024 -> top-k + temperature +
- * exponential-noise multinomial (sample_top_k, :49-60); top_k < 0 -> temperature multinomial over all n_valid ids
- * (sample_token with top_k == 0, :97-101).  Counter-based RNG keyed by (seed, *step_counter, row).
- * tokens[row*tok_stride] = id. */
-int rstnet_lm_sample_bf16(const void* logits, int32_t rows, int32_t V, int32_t n_valid, int32_t top_k, float temp,
-                          uint32_t seed, const int64_t* step_counter, int64_t* tokens, int32_t tok_stride,
-                          rstnet_stream_t stream);
-/* Per-row form (InferenceImp over a batch of utterances, each with its own candidate sets infer_no_streaming.py:264-283
- * and its own random stream): row r samples ids < n_valid_rows[r * n_valid_stride] (NULL: the scalar n_valid for every
- * row; top_k is clamped per row) with the RNG keyed by (seed, step_rows[r], key_rows[r]) in place of
- * (seed, *step_counter, r).  With key_rows[r] == r, step_rows[r] == *step_counter and one n_valid it draws exactly the
- * tokens rstnet_lm_sample_bf16 draws: both run one compiled kernel. */
-int rstnet_lm_sample_rows_bf16(const void* logits, int32_t rows, int32_t V, int32_t n_valid, const int32_t* n_valid_rows,
-                               int32_t n_valid_stride, int32_t top_k, float temp, uint32_t seed, const int64_t* step_rows,
-                               const uint32_t* key_rows, int64_t* tokens, int32_t tok_stride, rstnet_stream_t stream);
-/* General form with nucleus (top-p) sampling and per-row settings.  Modes as rstnet_lm_sample_bf16, plus: top_k != 0
- * and 0 < top_p < 1 -> nucleus (sample_top_p, utils/sampling.py:66-82; it takes precedence over top_k): with
- * w_i = exp((l_i - max) / temp) over the ids < n_valid, id t is kept iff the mass of the ids before it in the order
- * (logit desc, index asc) is <= top_p * sum(w); equal logits at the cut are kept lowest index first.  The draw is the
- * first maximum of the top_k < 0 score over the kept ids, so it equals the top_k < 0 draw whenever that draw is kept.
- * Masses are summed in fixed point (2^-40): identical calls and graph replays give identical tokens.  top_p >= 1 is the
- * top_k < 0 multinomial; top_p == 0 leaves the mode to top_k.  Unlike the reference's masked audio samplers (NaN with
- * top_p > 0) the distribution is renormalised over the ids < n_valid.
- * Settings: top_k_rows / temp_rows / top_p_rows (all three or none; int32 / fp32 / fp32) give row r the entry at
+/* ---- sample_token / sample_token_audio[_2048] (utils/sampling.py:85-154): row r of logits [rows][V] draws one id
+ * among its candidates, the ids < n_valid (<= 0 or > V: all V), into tokens[r * tok_stride].  Modes:
+ *   top_k == 0 -> argmax (first maximum; use_sampling False);
+ *   1 <= top_k <= 1024 -> top-k + temperature + exponential-noise multinomial (sample_top_k, :49-60; top_k is clamped to
+ *     the candidates: torch.topk would raise, the whole support is the natural reading);
+ *   top_k < 0 -> temperature multinomial over all candidates (sample_token with top_k == 0, :97-101);
+ *   top_k != 0 and 0 < top_p < 1 -> nucleus (sample_top_p, :66-82; it takes precedence over top_k): with
+ *     w_i = exp((l_i - max) / temp) over the candidates, id t is kept iff the mass of the ids before it in the order
+ *     (logit desc, index asc) is <= top_p * sum(w); equal logits at the cut are kept lowest index first.  The draw is the
+ *     first maximum of the top_k < 0 score over the kept ids, so it equals the top_k < 0 draw whenever that draw is kept.
+ *     Masses are summed in fixed point (2^-40): identical calls and graph replays give identical tokens.  top_p >= 1 is
+ *     the top_k < 0 multinomial; top_p == 0 leaves the mode to top_k.  Unlike the reference's masked audio samplers (NaN
+ *     with top_p > 0) the distribution is renormalised over the candidates.
+ * Candidates per row (InferenceImp over a batch of utterances, each with its own candidate sets
+ * infer_no_streaming.py:264-283): n_valid_rows given, row r samples ids < n_valid_rows[r * n_valid_stride] (<= 0 or > V:
+ * all V) in place of the scalar n_valid, with top_k clamped per row.
+ * Settings per row: top_k_rows / temp_rows / top_p_rows (all three or none; int32 / fp32 / fp32) give row r the entry at
  * r * param_stride in place of the scalars, so one [rows, 2] table serves the text head (column 0) and the audio heads
  * (column 1).  The tables are read on the device: the caller validates them (top_k <= 1024, temp > 0 where top_k != 0,
  * top_p finite and >= 0).  The scalars are validated here when no table is given.
- * RNG: keyed by (seed, step_rows[r], key_rows[r]) when step_rows / key_rows are given (both or neither), else by
- * (seed, *step_counter, r) (step_counter NULL: step 0).  Candidates: n_valid_rows as rstnet_lm_sample_rows_bf16.
- * With top_p == 0 everywhere it draws exactly the tokens of rstnet_lm_sample_bf16 / rstnet_lm_sample_rows_bf16 on the
- * same inputs: all three run one compiled kernel. */
+ * RNG: counter-based, keyed by (seed, *step_counter, r) (step_counter NULL: step 0), or, with step_rows / key_rows given
+ * (both or neither; each utterance its own random stream), by (seed, step_rows[r], key_rows[r]).  With key_rows[r] == r,
+ * step_rows[r] == *step_counter, one n_valid and the scalars in every row of the tables, the per-row forms draw exactly
+ * the tokens of the scalar form: all forms run one compiled kernel. */
 int rstnet_lm_sample_params_bf16(const void* logits, int32_t rows, int32_t V, int32_t n_valid, const int32_t* n_valid_rows,
                                  int32_t n_valid_stride, int32_t top_k, float temp, float top_p, const int32_t* top_k_rows,
                                  const float* temp_rows, const float* top_p_rows, int32_t param_stride, uint32_t seed,

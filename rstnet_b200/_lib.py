@@ -25,10 +25,9 @@ SYMBOLS = [
     "rstnet_skinny_gemm_workspace", "rstnet_skinny_gemm_create", "rstnet_skinny_gemm_create_fused", "rstnet_skinny_gemm_run", "rstnet_skinny_gemm_destroy",
     "rstnet_lm_embed_sum_bf16", "rstnet_lm_embed_rows_bf16", "rstnet_lm_rms_norm_bf16", "rstnet_lm_rope_kv_append_bf16",
     "rstnet_lm_rope_pair_kv_append_bf16",
-    "rstnet_lm_ring_decode_attention_bf16", "rstnet_lm_silu_mul_bf16", "rstnet_lm_depth_attention_bf16", "rstnet_lm_sample_bf16",
-    "rstnet_resample_f32", "rstnet_lm_delay_cache_in", "rstnet_lm_delay_cache_out",
-    "rstnet_lm_rope_kv_append_rows_bf16", "rstnet_lm_ring_decode_attention_rows_bf16", "rstnet_lm_sample_rows_bf16",
-    "rstnet_counter_add_rows", "rstnet_lm_cross_entropy_bf16", "rstnet_rows_fill_tail_f32", "rstnet_lm_sample_params_bf16",
+    "rstnet_lm_ring_decode_attention_bf16", "rstnet_lm_silu_mul_bf16", "rstnet_lm_depth_attention_bf16",
+    "rstnet_resample_f32", "rstnet_lm_delay_cache_in", "rstnet_lm_delay_cache_out", "rstnet_counter_add_rows",
+    "rstnet_lm_cross_entropy_bf16", "rstnet_rows_fill_tail_f32", "rstnet_lm_sample_params_bf16",
 ]
 
 RESAMPLE_MAX_TABLE_BYTES = 48 * 1024   # RSTNET_RESAMPLE_MAX_TABLE_BYTES
@@ -141,18 +140,14 @@ def lib() -> C.CDLL:
     L.rstnet_device_error_flags.argtypes = [i32]
     L.rstnet_device_error_flags.restype = C.c_uint32
     L.rstnet_lm_rms_norm_bf16.argtypes = [vp, vp, vp, i32, i32, f32, i32, vp]
-    L.rstnet_lm_rope_kv_append_bf16.argtypes = [vp, vp, vp, i64, i32, vp, i32, vp, vp, i32, i32, i32, i32, i32, i32, vp]
+    L.rstnet_lm_rope_kv_append_bf16.argtypes = [vp, vp, vp, i64, i32, vp, i32, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]
     L.rstnet_lm_rope_pair_kv_append_bf16.argtypes = [vp, vp, i32, vp, vp, i32, i32, i32, i32, i32, vp, vp]
-    L.rstnet_lm_ring_decode_attention_bf16.argtypes = [vp, vp, vp, i32, vp, i32, i32, i32, i32, i32, i32, i32, vp]
+    L.rstnet_lm_ring_decode_attention_bf16.argtypes = [vp, vp, vp, i32, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp]
     L.rstnet_lm_silu_mul_bf16.argtypes = [vp, vp, i32, i32, vp]
     L.rstnet_lm_depth_attention_bf16.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]
-    L.rstnet_lm_sample_bf16.argtypes = [vp, i32, i32, i32, i32, f32, C.c_uint32, vp, vp, i32, vp]
     L.rstnet_resample_f32.argtypes = [vp, i64, i64, i64, vp, vp, i32, i32, i32, i32, vp, i64, i64, i32, vp]
     L.rstnet_lm_delay_cache_in.argtypes = [vp, vp, vp, vp, vp, i32, vp, i32, i32, i32, i32, i32, i64, i64, vp]
     L.rstnet_lm_delay_cache_out.argtypes = [vp, vp, vp, vp, vp, i32, vp, i32, vp, i32, i32, i32, i32, i32, vp]
-    L.rstnet_lm_rope_kv_append_rows_bf16.argtypes = [vp, vp, vp, i64, i32, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]
-    L.rstnet_lm_ring_decode_attention_rows_bf16.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp]
-    L.rstnet_lm_sample_rows_bf16.argtypes = [vp, i32, i32, i32, vp, i32, i32, f32, C.c_uint32, vp, vp, vp, i32, vp]
     L.rstnet_counter_add_rows.argtypes = [vp, vp, i32, vp]
     L.rstnet_lm_cross_entropy_bf16.argtypes = [vp, i64, i32, i32, i32, vp, vp, vp, vp, i32, vp, vp, vp, vp]
     L.rstnet_lm_sample_params_bf16.argtypes = [vp, i32, i32, i32, vp, i32, i32, f32, f32, vp, vp, vp, i32, C.c_uint32, vp, vp, vp,

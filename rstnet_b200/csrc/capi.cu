@@ -37,7 +37,7 @@ unsigned int rvq_read_errors(bool clear);
 unsigned int ce_read_errors(bool clear);
 }
 
-extern "C" int rstnet_version(void) { return 205; }
+extern "C" int rstnet_version(void) { return 206; }
 // Sticky device-side error bits of the CURRENT device (synchronises it): 1 = token / code id outside its table,
 // 2 = RoPE position beyond the cos/sin tables.  Kernels cannot raise; they poison their output (NaN) and set a bit.
 extern "C" uint32_t rstnet_device_error_flags(int clear) {

@@ -869,33 +869,21 @@ extern "C" int rstnet_lm_rms_norm_bf16(const void* x, const void* w, void* y, in
 }
 
 extern "C" int rstnet_lm_rope_kv_append_bf16(const void* qkv, const void* cos_tab, const void* sin_tab, int64_t rope_rows,
-                                             int32_t rope_n, const int64_t* offset, int32_t offset_stride, void* q_out, void* kv,
-                                             int32_t rows, int32_t B, int32_t n_head, int32_t n_kv, int32_t hs, int32_t cap,
-                                             rstnet_stream_t stream) {
+                                             int32_t rope_n, const int64_t* offset, int32_t offset_stride, const int32_t* row_stream,
+                                             const int32_t* row_tl, void* q_out, void* kv, int32_t rows, int32_t B, int32_t n_head,
+                                             int32_t n_kv, int32_t hs, int32_t cap, rstnet_stream_t stream) {
   RSTNET_REQUIRE(qkv && cos_tab && sin_tab && offset && q_out && kv, "lm_rope_kv_append: null pointer");
-  RSTNET_REQUIRE(rows > 0 && B > 0 && rows % B == 0, "lm_rope_kv_append: rows (%d) must be a multiple of the stream count (%d)", rows, B);
+  RSTNET_REQUIRE(!row_stream == !row_tl, "lm_rope_kv_append: row_stream and row_tl go together");
+  RSTNET_REQUIRE(!row_stream || offset_stride, "lm_rope_kv_append: a row map needs per-stream offsets (offset_stride 1)");
+  RSTNET_REQUIRE(rows > 0 && B > 0 && (row_stream || rows % B == 0),
+                 "lm_rope_kv_append: rows (%d) must be a multiple of the stream count (%d) without a row map", rows, B);
   RSTNET_REQUIRE(n_kv > 0 && n_head % n_kv == 0, "lm_rope_kv_append: n_head (%d) must be a multiple of n_kv (%d)", n_head, n_kv);
   RSTNET_REQUIRE(rope_n >= 0 && rope_n <= hs && rope_n % 2 == 0 && rope_rows > 0, "lm_rope_kv_append: bad rope table (%d of %d dims)", rope_n, hs);
   rope_kv_append_bf16_kernel<<<dim3(rows * n_kv), dim3(64), 0, (cudaStream_t)stream>>>((const bf16*)qkv, (const bf16*)cos_tab,
              (const bf16*)sin_tab, (const long long*)offset, (bf16*)q_out, (bf16*)kv, offset_stride ? 1 : 0, B, n_kv, n_head / n_kv, hs,
-             cap, rope_n, (long long)rope_rows, nullptr, nullptr);
+             cap, rope_n, (long long)rope_rows, (const int*)row_stream, (const int*)row_tl);
   count_launch();
   return check_launch("lm_rope_kv_append");
-}
-
-extern "C" int rstnet_lm_rope_kv_append_rows_bf16(const void* qkv, const void* cos_tab, const void* sin_tab, int64_t rope_rows,
-                                                  int32_t rope_n, const int64_t* offset, const int32_t* row_stream,
-                                                  const int32_t* row_tl, void* q_out, void* kv, int32_t rows, int32_t B,
-                                                  int32_t n_head, int32_t n_kv, int32_t hs, int32_t cap, rstnet_stream_t stream) {
-  RSTNET_REQUIRE(qkv && cos_tab && sin_tab && offset && row_stream && row_tl && q_out && kv, "lm_rope_kv_append_rows: null pointer");
-  RSTNET_REQUIRE(rows > 0 && B > 0, "lm_rope_kv_append_rows: bad shape (rows %d, B %d)", rows, B);
-  RSTNET_REQUIRE(n_kv > 0 && n_head % n_kv == 0, "lm_rope_kv_append_rows: n_head (%d) must be a multiple of n_kv (%d)", n_head, n_kv);
-  RSTNET_REQUIRE(rope_n >= 0 && rope_n <= hs && rope_n % 2 == 0 && rope_rows > 0, "lm_rope_kv_append_rows: bad rope table (%d of %d dims)", rope_n, hs);
-  rope_kv_append_bf16_kernel<<<dim3(rows * n_kv), dim3(64), 0, (cudaStream_t)stream>>>((const bf16*)qkv, (const bf16*)cos_tab,
-             (const bf16*)sin_tab, (const long long*)offset, (bf16*)q_out, (bf16*)kv, 1, B, n_kv, n_head / n_kv, hs, cap, rope_n,
-             (long long)rope_rows, (const int*)row_stream, (const int*)row_tl);
-  count_launch();
-  return check_launch("lm_rope_kv_append_rows");
 }
 
 extern "C" int rstnet_lm_rope_pair_kv_append_bf16(const void* qkv, const int64_t* offset, int32_t offset_stride, void* q_out, void* kv,
@@ -910,11 +898,15 @@ extern "C" int rstnet_lm_rope_pair_kv_append_bf16(const void* qkv, const int64_t
 }
 
 extern "C" int rstnet_lm_ring_decode_attention_bf16(const void* q, const void* kv, const int64_t* offset, int32_t offset_stride,
-                                                    void* out, int32_t rows, int32_t B, int32_t n_head, int32_t n_kv, int32_t hs,
-                                                    int32_t cap, int32_t context, rstnet_stream_t stream) {
+                                                    const int32_t* row_stream, const int32_t* row_tl, void* out, int32_t rows,
+                                                    int32_t B, int32_t n_head, int32_t n_kv, int32_t hs, int32_t cap, int32_t context,
+                                                    rstnet_stream_t stream) {
   RSTNET_REQUIRE(q && kv && offset && out, "lm_ring_decode_attention: null pointer");
+  RSTNET_REQUIRE(!row_stream == !row_tl, "lm_ring_decode_attention: row_stream and row_tl go together");
+  RSTNET_REQUIRE(!row_stream || offset_stride, "lm_ring_decode_attention: a row map needs per-stream offsets (offset_stride 1)");
   RSTNET_REQUIRE(hs == 128 || hs == 64, "lm_ring_decode_attention: head_size must be 64 or 128 (got %d)", hs);
-  RSTNET_REQUIRE(rows > 0 && B > 0 && rows % B == 0, "lm_ring_decode_attention: rows (%d) must be a multiple of the stream count (%d)", rows, B);
+  RSTNET_REQUIRE(rows > 0 && B > 0 && (row_stream || rows % B == 0),
+                 "lm_ring_decode_attention: rows (%d) must be a multiple of the stream count (%d) without a row map", rows, B);
   RSTNET_REQUIRE(n_kv > 0 && n_head % n_kv == 0, "lm_ring_decode_attention: n_head (%d) must be a multiple of n_kv (%d)", n_head, n_kv);
   const float scale = 1.0f / sqrtf((float)hs);
   const int q_per_kv = n_head / n_kv;
@@ -922,27 +914,9 @@ extern "C" int rstnet_lm_ring_decode_attention_bf16(const void* q, const void* k
   const auto launch = hs == 128 ? (G == 2 ? launch_ring_decode_attention<128, 2> : launch_ring_decode_attention<128, 1>)
                                 : (G == 2 ? launch_ring_decode_attention<64, 2> : launch_ring_decode_attention<64, 1>);
   launch((cudaStream_t)stream, (const bf16*)q, (const bf16*)kv, (const long long*)offset, (bf16*)out, offset_stride ? 1 : 0, rows, B,
-         n_head, n_kv, cap, context, scale, nullptr, nullptr);
+         n_head, n_kv, cap, context, scale, (const int*)row_stream, (const int*)row_tl);
   count_launch();
   return check_launch("lm_ring_decode_attention");
-}
-
-extern "C" int rstnet_lm_ring_decode_attention_rows_bf16(const void* q, const void* kv, const int64_t* offset, const int32_t* row_stream,
-                                                         const int32_t* row_tl, void* out, int32_t rows, int32_t B, int32_t n_head,
-                                                         int32_t n_kv, int32_t hs, int32_t cap, int32_t context, rstnet_stream_t stream) {
-  RSTNET_REQUIRE(q && kv && offset && row_stream && row_tl && out, "lm_ring_decode_attention_rows: null pointer");
-  RSTNET_REQUIRE(hs == 128 || hs == 64, "lm_ring_decode_attention_rows: head_size must be 64 or 128 (got %d)", hs);
-  RSTNET_REQUIRE(rows > 0 && B > 0, "lm_ring_decode_attention_rows: bad shape (rows %d, B %d)", rows, B);
-  RSTNET_REQUIRE(n_kv > 0 && n_head % n_kv == 0, "lm_ring_decode_attention_rows: n_head (%d) must be a multiple of n_kv (%d)", n_head, n_kv);
-  const float scale = 1.0f / sqrtf((float)hs);
-  const int q_per_kv = n_head / n_kv;
-  const int G = q_per_kv % 2 == 0 ? 2 : 1;
-  const auto launch = hs == 128 ? (G == 2 ? launch_ring_decode_attention<128, 2> : launch_ring_decode_attention<128, 1>)
-                                : (G == 2 ? launch_ring_decode_attention<64, 2> : launch_ring_decode_attention<64, 1>);
-  launch((cudaStream_t)stream, (const bf16*)q, (const bf16*)kv, (const long long*)offset, (bf16*)out, 1, rows, B, n_head, n_kv, cap,
-         context, scale, (const int*)row_stream, (const int*)row_tl);
-  count_launch();
-  return check_launch("lm_ring_decode_attention_rows");
 }
 
 extern "C" int rstnet_lm_silu_mul_bf16(const void* ab, void* out, int32_t M, int32_t I, rstnet_stream_t stream) {
@@ -963,33 +937,6 @@ extern "C" int rstnet_lm_depth_attention_bf16(const void* qkv, void* kvd, void* 
              step, ring_quirk);
   count_launch();
   return check_launch("lm_depth_attention");
-}
-
-extern "C" int rstnet_lm_sample_bf16(const void* logits, int32_t rows, int32_t V, int32_t n_valid, int32_t top_k, float temp,
-                                     uint32_t seed, const int64_t* step_counter, int64_t* tokens, int32_t tok_stride,
-                                     rstnet_stream_t stream) {
-  RSTNET_REQUIRE(logits && tokens && rows > 0 && V > 0, "lm_sample: bad argument");
-  RSTNET_REQUIRE(top_k <= SAMPLE_CAND && (top_k == 0 || temp > 0.f), "lm_sample: top_k <= %d and temp > 0 required (top_k=%d)", SAMPLE_CAND, top_k);
-  if (n_valid <= 0 || n_valid > V) n_valid = V;
-  if (top_k > n_valid) top_k = n_valid;   // torch.topk would raise; the whole support is the natural reading
-  sample_kernel<<<dim3(rows), dim3(1024), 0, (cudaStream_t)stream>>>((const bf16*)logits, V, n_valid, top_k, temp, 0.f, (uint32_t)seed,
-             (const long long*)step_counter, (long long*)tokens, tok_stride, nullptr, 0, nullptr, nullptr, nullptr, nullptr, nullptr, 0);
-  count_launch();
-  return check_launch("lm_sample");
-}
-
-extern "C" int rstnet_lm_sample_rows_bf16(const void* logits, int32_t rows, int32_t V, int32_t n_valid, const int32_t* n_valid_rows,
-                                          int32_t n_valid_stride, int32_t top_k, float temp, uint32_t seed, const int64_t* step_rows,
-                                          const uint32_t* key_rows, int64_t* tokens, int32_t tok_stride, rstnet_stream_t stream) {
-  RSTNET_REQUIRE(logits && tokens && step_rows && key_rows && rows > 0 && V > 0, "lm_sample_rows: bad argument");
-  RSTNET_REQUIRE(top_k <= SAMPLE_CAND && (top_k == 0 || temp > 0.f), "lm_sample_rows: top_k <= %d and temp > 0 required (top_k=%d)", SAMPLE_CAND, top_k);
-  if (n_valid <= 0 || n_valid > V) n_valid = V;
-  if (!n_valid_rows && top_k > n_valid) top_k = n_valid;   // with per-row candidate counts the kernel clamps per row
-  sample_kernel<<<dim3(rows), dim3(1024), 0, (cudaStream_t)stream>>>((const bf16*)logits, V, n_valid, top_k, temp, 0.f, (uint32_t)seed,
-             nullptr, (long long*)tokens, tok_stride, (const int*)n_valid_rows, n_valid_stride, (const long long*)step_rows,
-             key_rows, nullptr, nullptr, nullptr, 0);
-  count_launch();
-  return check_launch("lm_sample_rows");
 }
 
 extern "C" int rstnet_lm_sample_params_bf16(const void* logits, int32_t rows, int32_t V, int32_t n_valid, const int32_t* n_valid_rows,

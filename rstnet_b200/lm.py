@@ -873,34 +873,22 @@ class _LMState:
         c, B, M, L = self.c, self.B, self.M, _lib.lib()
         st = ops._stream()
         E = c.n_embd
-        ost = 1 if self.offset.numel() > 1 else 0
+        # a row map always indexes the position counters per stream (offset_stride 1), even with B == 1
+        rs, rt = (self.row_stream.data_ptr(), self.row_tl.data_ptr()) if self.row_mapped else (None, None)
+        ost = 1 if self.row_mapped or self.offset.numel() > 1 else 0
         _lib.check(L.rstnet_lm_embed_sum_bf16(self.seq.data_ptr(), c.n_q + 1, self.wte.data_ptr(), self.wte.shape[0],
                                               self.table_ptrs.data_ptr(), self.tables[0].shape[0], c.n_q, E, self.x.data_ptr(), M, st),
                    "lm_embed_sum")
         _lib.check(L.rstnet_lm_rms_norm_bf16(self.x.data_ptr(), self.n1_first.data_ptr(), self.xn.data_ptr(), M, E, c.norm_eps, 0, st), "rms")
         for l, ly in enumerate(self.layers):
             ly["qkv"].run()
-            if self.row_mapped:
-                _lib.check(L.rstnet_lm_rope_kv_append_rows_bf16(self.qkv.data_ptr(), self.cos.data_ptr(), self.sin.data_ptr(),
-                                                                self.cos.shape[0], c.rope_n_elem, self.offset.data_ptr(),
-                                                                self.row_stream.data_ptr(), self.row_tl.data_ptr(), self.q.data_ptr(),
-                                                                self.kv[l].data_ptr(), M, B, c.n_head, c.n_query_groups,
-                                                                c.head_size, self.cap, st), "rope_kv_rows")
-                _lib.check(L.rstnet_lm_ring_decode_attention_rows_bf16(self.q.data_ptr(), self.kv[l].data_ptr(), self.offset.data_ptr(),
-                                                                       self.row_stream.data_ptr(), self.row_tl.data_ptr(),
-                                                                       self.att.data_ptr(), M, B, c.n_head, c.n_query_groups,
-                                                                       c.head_size, self.cap, c.context, st), "attention_rows")
-                ly["proj"].run()
-                ly["fc"].run()
-                ly["down"].run()
-                continue
             _lib.check(L.rstnet_lm_rope_kv_append_bf16(self.qkv.data_ptr(), self.cos.data_ptr(), self.sin.data_ptr(), self.cos.shape[0],
-                                                       c.rope_n_elem, self.offset.data_ptr(), ost, self.q.data_ptr(),
+                                                       c.rope_n_elem, self.offset.data_ptr(), ost, rs, rt, self.q.data_ptr(),
                                                        self.kv[l].data_ptr(), M, B, c.n_head, c.n_query_groups, c.head_size, self.cap, st),
                        "rope_kv")
             _lib.check(L.rstnet_lm_ring_decode_attention_bf16(self.q.data_ptr(), self.kv[l].data_ptr(), self.offset.data_ptr(), ost,
-                                                              self.att.data_ptr(), M, B, c.n_head, c.n_query_groups, c.head_size,
-                                                              self.cap, c.context, st), "attention")
+                                                              rs, rt, self.att.data_ptr(), M, B, c.n_head, c.n_query_groups,
+                                                              c.head_size, self.cap, c.context, st), "attention")
             ly["proj"].run()   # + residual + norm_2 -> xn
             ly["fc"].run()     # + SiLU gating -> hmid
             ly["down"].run()   # + residual + next pre-norm -> xn (last layer: ln_f -> transformer_out)
@@ -932,32 +920,20 @@ class _LMState:
             ly["gout"].run()   # dx += out(dh) ; dn = norm1 of the next layer
         ds["head"].run()
 
-    def _sample(self, logits: torch.Tensor, V: int, n_valid: int, top_k: int, temp: float, col: int, salt: int):
-        _lib.check(_lib.lib().rstnet_lm_sample_bf16(logits.data_ptr(), self.M, V, n_valid, top_k, float(temp), self.seed + salt,
-                                                    self.frame_counter.data_ptr(), self.tokens.data_ptr() + 8 * col,
-                                                    self.c.dep_q + 1, ops._stream()), "sample")
-
-    def _sample_rows(self, logits: torch.Tensor, V: int, per_row_valid: Optional[int], top_k: int, temp: float, col: int, salt: int):
-        """per_row_valid: column of row_valid holding the rows' candidate counts (None: all V ids)"""
-        nv = None if per_row_valid is None else self.row_valid.data_ptr() + 4 * per_row_valid
-        _lib.check(_lib.lib().rstnet_lm_sample_rows_bf16(logits.data_ptr(), self.M, V, V, nv, self.c.dep_q, top_k, float(temp),
-                                                         self.seed + salt, self.row_step.data_ptr(), self.row_key.data_ptr(),
-                                                         self.tokens.data_ptr() + 8 * col, self.c.dep_q + 1, ops._stream()),
-                   "sample_rows")
-
-    def _sample_params(self, logits: torch.Tensor, V: int, n_valid: int, per_row_valid: Optional[int], mode, head: Optional[int],
-                       col: int, salt: int, per_row_rng: bool):
-        """The general sampler: mode = (top_k, temp, top_p) for every row, or head = the column of the row_topk / row_temp /
-        row_topp tables; per_row_valid as _sample_rows (None: n_valid); per_row_rng: row_key / row_step in place of
-        (row, frame_counter)."""
-        nv = None if per_row_valid is None else self.row_valid.data_ptr() + 4 * per_row_valid
+    def _sample(self, col: int, mode, n_valid: Optional[int], per_row_rng: bool):
+        """Draw column col of self.tokens: 0 the text head from self.logits, k + 1 audio head k from self.dlogits; the RNG
+        seed is salted by col.  mode: (top_k, temp, top_p) for every row, or None: the head's column of the row_topk /
+        row_temp / row_topp tables (0 text, 1 audio).  n_valid: the candidate count of every row, or None: column k of
+        row_valid.  per_row_rng: the RNG keyed by (row_step, row_key) in place of (frame_counter, row)."""
+        c = self.c
+        logits, V = (self.logits, c.padded_vocab_size) if col == 0 else (self.dlogits, c.audio_card)
+        nv = None if n_valid is not None else self.row_valid.data_ptr() + 4 * (col - 1)
         tk, temp, tp = mode if mode is not None else (0, 1.0, 0.0)
-        tabs = [None, None, None] if head is None else [t.data_ptr() + 4 * head for t in (self.row_topk, self.row_temp, self.row_topp)]
+        tabs = [None] * 3 if mode is not None else [t.data_ptr() + 4 * min(col, 1) for t in (self.row_topk, self.row_temp, self.row_topp)]
+        rng = (None, self.row_step.data_ptr(), self.row_key.data_ptr()) if per_row_rng else (self.frame_counter.data_ptr(), None, None)
         _lib.check(_lib.lib().rstnet_lm_sample_params_bf16(
-            logits.data_ptr(), self.M, V, n_valid, nv, self.c.dep_q, tk, float(temp), float(tp), *tabs, 2, self.seed + salt,
-            None if per_row_rng else self.frame_counter.data_ptr(), self.row_step.data_ptr() if per_row_rng else None,
-            self.row_key.data_ptr() if per_row_rng else None, self.tokens.data_ptr() + 8 * col, self.c.dep_q + 1, ops._stream()),
-            "sample_params")
+            logits.data_ptr(), self.M, V, V if n_valid is None else n_valid, nv, c.dep_q, tk, float(temp), float(tp), *tabs, 2,
+            self.seed + col, *rng, self.tokens.data_ptr() + 8 * col, c.dep_q + 1, ops._stream()), "sample")
 
     def set_row_sampling(self, sampling):
         """sampling: B `Sampling` -> the scope's per-row tables, uploaded from pinned memory without a synchronise, and
@@ -1186,102 +1162,37 @@ class _LMState:
                 audio_valid = torch.where(argmax, c.audio_card, audio_valid.to(argmax.device))
         self._advance_host(1)
         self.seq.copy_(sequence[:, :, 0])
-        if sampling is not None:
+        if per_row:
             self.row_valid.copy_(audio_valid)
-            self._replay(*self._frame_params(quirk))
-        elif per_row:
-            self.row_valid.copy_(audio_valid)
-            if top_p_text or top_p:
-                self._replay(*self._frame_nucleus(use_sampling, temp_text, top_k_text, top_p_text, temp, top_k, top_p, None, quirk))
-            else:
-                self._replay(*self._frame_rows(use_sampling, temp_text, top_k_text, temp, top_k, quirk))
-        elif top_p_text or top_p:
-            self._replay(*self._frame_nucleus(use_sampling, temp_text, top_k_text, top_p_text, temp, top_k, top_p, audio_valid, quirk))
+            valid = None
         else:
-            self._replay(*self._frame(use_sampling, temp_text, top_k_text, temp, top_k, audio_valid, quirk))
+            valid = tuple(audio_valid) if isinstance(audio_valid, (tuple, list)) else (audio_valid,) * c.dep_q
+        modes = None if sampling is not None else (_head_mode(use_sampling, temp_text, top_k_text, top_p_text),
+                                                   _head_mode(use_sampling, temp, top_k, top_p))
+        self._replay(*self._frame(modes, valid, per_row, quirk))
         return self.tokens.clone()
 
-    def _frame_nucleus(self, use_sampling, temp_text, top_k_text, top_p_text, temp, top_k, top_p, audio_valid, quirk):
-        """_frame (audio_valid given) or _frame_rows (None: row_valid, row_key, row_step) with top_p: every head through the
-        general sampler, one setting for all rows."""
+    def _frame(self, modes, valid, per_row_rng: bool, quirk):
+        """(graph key, launch sequence) of one generated frame from the ids in self.seq to the tokens in self.tokens.
+        modes: ((top_k, temp, top_p) of the text head, (...) of the audio heads) for every row, as _head_mode gives them, or
+        None: each row's own from the row_topk / row_temp / row_topp tables.  valid: the dep_q audio heads' candidate
+        counts for every row, or None: each row's own from row_valid.  per_row_rng: the RNG keyed by (row_step, row_key)
+        in place of (frame_counter, row); the frame advances the counter it keys by."""
         c = self.c
-        rows = audio_valid is None
-        mt, ma = Sampling(use_sampling, temp_text, top_k_text, top_p_text, temp, top_k, top_p).heads()
-        sampling = ma[0] != 0
-        valid = (c.audio_card,) * c.dep_q
-        if sampling and not rows:
-            valid = tuple(audio_valid) if isinstance(audio_valid, (tuple, list)) else (audio_valid,) * c.dep_q
+        if modes is not None and modes[1][0] == 0:
+            valid = (c.audio_card,) * c.dep_q   # the 2048 / 2049 masks exist on the sampling path only (sampling.py:107-154)
+        text, audio = modes if modes is not None else (None, None)
 
         def frame():
             self._temporal()
-            self._sample_params(self.logits, c.padded_vocab_size, c.padded_vocab_size, None, mt, None, 0, 0, rows)
+            self._sample(0, text, c.padded_vocab_size, per_row_rng)
             self.tout.copy_(self.out)
             for k in range(c.dep_q):
                 self._depth(k, self.tokens[:, k], c.dep_q + 1, quirk=quirk)
-                self._sample_params(self.dlogits, c.audio_card, min(valid[k], c.audio_card), k if (rows and sampling) else None,
-                                    ma, None, k + 1, k + 1, rows)
-            if rows:
+                self._sample(k + 1, audio, None if valid is None else min(valid[k], c.audio_card), per_row_rng)
+            if per_row_rng:
                 ops.counter_add(self.row_step, 1, self.active)
             else:
                 ops.counter_add(self.frame_counter, 1)
 
-        return ("frame_nucleus", mt, ma, None if rows else valid, bool(quirk)), frame
-
-    def _frame_params(self, quirk):
-        """_frame_rows with every row's settings read from the row_topk / row_temp / row_topp tables: one graph whatever
-        the settings.  row_valid already holds the whole card for the rows whose audio heads take the argmax."""
-        c = self.c
-
-        def frame():
-            self._temporal()
-            self._sample_params(self.logits, c.padded_vocab_size, c.padded_vocab_size, None, None, 0, 0, 0, True)
-            self.tout.copy_(self.out)
-            for k in range(c.dep_q):
-                self._depth(k, self.tokens[:, k], c.dep_q + 1, quirk=quirk)
-                self._sample_params(self.dlogits, c.audio_card, c.audio_card, k, None, 1, k + 1, k + 1, True)
-            ops.counter_add(self.row_step, 1, self.active)
-
-        return ("frame_params", bool(quirk)), frame
-
-    def _frame_rows(self, use_sampling, temp_text, top_k_text, temp, top_k, quirk):
-        """_frame with per-row candidate counts (row_valid), RNG keys (row_key) and step counters (row_step)."""
-        c = self.c
-        sampling_text = use_sampling and temp_text > 0.0
-        sampling = use_sampling and temp > 0.0
-        tk_text = (top_k_text if top_k_text > 0 else -1) if sampling_text else 0
-        tk = (top_k if top_k > 0 else -1) if sampling else 0
-
-        def frame():
-            self._temporal()
-            self._sample_rows(self.logits, c.padded_vocab_size, None, tk_text, temp_text if sampling_text else 1.0, 0, 0)
-            self.tout.copy_(self.out)
-            for k in range(c.dep_q):
-                self._depth(k, self.tokens[:, k], c.dep_q + 1, quirk=quirk)
-                # the 2048 / 2049 candidate sets exist on the sampling path only (sampling.py:107-154)
-                self._sample_rows(self.dlogits, c.audio_card, k if sampling else None, tk, temp if sampling else 1.0, k + 1, k + 1)
-            ops.counter_add(self.row_step, 1, self.active)
-
-        return ("frame_rows", tk_text, float(temp_text), tk, float(temp), bool(quirk)), frame
-
-    def _frame(self, use_sampling, temp_text, top_k_text, temp, top_k, audio_valid, quirk):
-        """(graph key, launch sequence) of one generated frame from the ids in self.seq to the tokens in self.tokens."""
-        c = self.c
-        # kernel convention: 0 = argmax, k > 0 = top-k, -1 = multinomial over the whole (valid) support
-        sampling_text = use_sampling and temp_text > 0.0
-        sampling = use_sampling and temp > 0.0
-        tk_text = (top_k_text if top_k_text > 0 else -1) if sampling_text else 0
-        tk = (top_k if top_k > 0 else -1) if sampling else 0
-        valid = tuple(audio_valid) if isinstance(audio_valid, (tuple, list)) else (audio_valid,) * c.dep_q
-        if not sampling:
-            valid = (c.audio_card,) * c.dep_q   # the 2048 / 2049 masks exist on the sampling path only (sampling.py:107-154)
-
-        def frame():
-            self._temporal()
-            self._sample(self.logits, c.padded_vocab_size, c.padded_vocab_size, tk_text, temp_text if sampling_text else 1.0, 0, 0)
-            self.tout.copy_(self.out)
-            for k in range(c.dep_q):
-                self._depth(k, self.tokens[:, k], c.dep_q + 1, quirk=quirk)
-                self._sample(self.dlogits, c.audio_card, min(valid[k], c.audio_card), tk, temp if sampling else 1.0, k + 1, k + 1)
-            ops.counter_add(self.frame_counter, 1)
-
-        return ("frame", tk_text, float(temp_text), tk, float(temp), valid, bool(quirk)), frame
+        return ("frame", "tables" if modes is None else modes, "rows" if valid is None else valid, per_row_rng, bool(quirk)), frame

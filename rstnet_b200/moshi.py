@@ -34,7 +34,7 @@ from torch import nn
 from . import _lib, ops
 from ._lib import RstnetError
 from .codec import _register, on_own_device
-from .lm import GPT, Sampling, SkinnyGemm, _DepthScope, _LMState  # noqa: F401
+from .lm import GPT, Sampling, SkinnyGemm, _DepthScope, _LMState, _head_mode  # noqa: F401
 
 
 class _MoshiState(_LMState):
@@ -100,8 +100,8 @@ class _MoshiState(_LMState):
                                                             self.kv[l].data_ptr(), M, B, c.n_head, c.head_size, self.cap,
                                                             self.freqs.data_ptr(), st), "rope_pair_kv")
             _lib.check(L.rstnet_lm_ring_decode_attention_bf16(self.q.data_ptr(), self.kv[l].data_ptr(), self.offset.data_ptr(), 1,
-                                                              self.att.data_ptr(), M, B, c.n_head, c.n_head, c.head_size, self.cap,
-                                                              c.context, st), "attention")
+                                                              None, None, self.att.data_ptr(), M, B, c.n_head, c.n_head, c.head_size,
+                                                              self.cap, c.context, st), "attention")
             ly["proj"].run()
             ly["fc"].run()
             ly["down"].run()
@@ -475,12 +475,11 @@ class LMGen(nn.Module):
         lm, ms, L = self.lm_model, st.lm, _lib.lib()
         if self._row_sampling is not None:
             ms.set_row_sampling(self._row_sampling)     # row_valid stays 0: every row samples over the whole card
-            key, frame = ms._frame_params(True)
-        elif self.top_p or self.top_p_text:
-            key, frame = ms._frame_nucleus(self.use_sampling, self.temp_text, self.top_k_text, self.top_p_text, self.temp,
-                                           self.top_k, self.top_p, lm.card, True)
+            key, frame = ms._frame(None, None, True, True)
         else:
-            key, frame = ms._frame(self.use_sampling, self.temp_text, self.top_k_text, self.temp, self.top_k, lm.card, True)
+            modes = (_head_mode(self.use_sampling, self.temp_text, self.top_k_text, self.top_p_text),
+                     _head_mode(self.use_sampling, self.temp, self.top_k, self.top_p))
+            key, frame = ms._frame(modes, (lm.card,) * ms.c.dep_q, False, True)
         K, CT = lm.num_codebooks, st.cache.shape[2]
 
         def step():

@@ -31,6 +31,12 @@ def _rel(a, b):
     return float((a - b).abs().max() / b.abs().max().clamp(min=1e-6))
 
 
+def _sample(logits, rows, V, n_valid, top_k, temp, seed, tokens_ptr, tok_stride):
+    """rstnet_lm_sample_params_bf16 in its scalar form (no tables, top_p 0), the RNG keyed by (seed, step 0, row)"""
+    _lib.check(_lib.lib().rstnet_lm_sample_params_bf16(logits.data_ptr(), rows, V, n_valid, None, 0, top_k, float(temp), 0.0, None,
+                                                       None, None, 0, seed, None, None, None, tokens_ptr, tok_stride, ops._stream()))
+
+
 @pytest.mark.parametrize("M,K,N,res,max_splits", [
     (64, 4096, 512, False, 8), (64, 256, 768, False, 8), (3, 256, 152064 // 64, True, 8), (64, 11008, 256, True, 8),
     (17, 1024, 2050, False, 8), (64, 2816, 1024, True, 8), (128, 512, 640, False, 8),
@@ -112,9 +118,10 @@ def test_rope_append_and_ring_decode_attention(hs, cap, context, steps):
         st = ops._stream()
         qkv_d = qkv.to(DEV).contiguous()
         _lib.check(lib.rstnet_lm_rope_kv_append_bf16(qkv_d.data_ptr(), cos_d.data_ptr(), sin_d.data_ptr(), cos_d.shape[0], hs,
-                                                     offset.data_ptr(), 0, qd.data_ptr(), kv.data_ptr(), B, B, nh, nh, hs, cap, st))
-        _lib.check(lib.rstnet_lm_ring_decode_attention_bf16(qd.data_ptr(), kv.data_ptr(), offset.data_ptr(), 0, out.data_ptr(), B, B,
-                                                            nh, nh, hs, cap, context, st))
+                                                     offset.data_ptr(), 0, None, None, qd.data_ptr(), kv.data_ptr(), B, B, nh, nh, hs, cap,
+                                                     st))
+        _lib.check(lib.rstnet_lm_ring_decode_attention_bf16(qd.data_ptr(), kv.data_ptr(), offset.data_ptr(), 0, None, None, out.data_ptr(),
+                                                            B, B, nh, nh, hs, cap, context, st))
         ops.counter_add(offset, 1)
         torch.cuda.synchronize()
         assert torch.equal(qd.cpu().view(B, nh, hs), qr[:, :, 0]), "rotated q must match bit for bit"
@@ -145,34 +152,32 @@ def test_norms_silu_embed_vs_oracle():
 
 
 def test_sampling_greedy_and_distribution():
-    lib, st = _lib.lib(), ops._stream()
     g = torch.Generator().manual_seed(5)
     logits = torch.randn(6, 5000, generator=g).to(BF)
     logits[2, 100] = logits[2, 4000] = 9.0  # tie -> first maximum
     toks = torch.zeros(6, 3, dtype=torch.int64, device=DEV)
     logits_d = logits.to(DEV).contiguous()
-    _lib.check(lib.rstnet_lm_sample_bf16(logits_d.data_ptr(), 6, 5000, 5000, 0, 1.0, 1, None, toks.data_ptr() + 8, 3, st))
+    _sample(logits_d, 6, 5000, 5000, 0, 1.0, 1, toks.data_ptr() + 8, 3)
     assert torch.equal(toks[:, 1].cpu(), torch.argmax(logits.float(), -1)) and int(toks[2, 1]) == 100
     # n_valid masks the tail (sample_token_audio_2048: ids >= 2048 never sampled)
-    _lib.check(lib.rstnet_lm_sample_bf16(logits_d.data_ptr(), 6, 5000, 90, 0, 1.0, 1, None, toks.data_ptr(), 3, st))
+    _sample(logits_d, 6, 5000, 90, 0, 1.0, 1, toks.data_ptr(), 3)
     assert int(toks[:, 0].max()) < 90
     # distribution of the exponential-noise multinomial over the top-k (utils/sampling.py:157-175 self-test)
     ps = torch.tensor([5.0, 2.0, 12.0, 6.0, 8.0, 1.0, 0.5, 4.0])
     lg = torch.log(ps).to(BF).repeat(4000, 1).contiguous().to(DEV)
     out = torch.zeros(4000, dtype=torch.int64, device=DEV)
-    _lib.check(lib.rstnet_lm_sample_bf16(lg.data_ptr(), 4000, 8, 8, 8, 1.0, 77, None, out.data_ptr(), 1, st))
+    _sample(lg, 4000, 8, 8, 8, 1.0, 77, out.data_ptr(), 1)
     cnt = torch.bincount(out.cpu(), minlength=8).float()
     target = torch.exp(torch.log(ps).to(BF).float())
     assert (cnt / cnt.sum() - target / target.sum()).abs().max().item() < 2.5e-2
     # top-k restricts the support
-    _lib.check(lib.rstnet_lm_sample_bf16(lg.data_ptr(), 4000, 8, 8, 3, 1.0, 78, None, out.data_ptr(), 1, st))
+    _sample(lg, 4000, 8, 8, 3, 1.0, 78, out.data_ptr(), 1)
     assert set(out.cpu().tolist()) <= {2, 4, 3}
 
 
 def test_sampling_large_vocab_candidate_list_matches_full_scan():
     """The 152k-entry text head goes through the histogram-select candidate list; it must pick exactly what the plain
     top_k-pass scan picks (same seed, same (value desc, index asc) order), ties at the threshold included."""
-    lib, st = _lib.lib(), ops._stream()
     g = torch.Generator().manual_seed(11)
     rows, V, small = 32, 151936, 4000
     logits = (torch.randn(rows, V, generator=g) * 2.0).to(BF)
@@ -184,8 +189,8 @@ def test_sampling_large_vocab_candidate_list_matches_full_scan():
     a = torch.zeros(rows, dtype=torch.int64, device=DEV)
     b = torch.zeros(rows, dtype=torch.int64, device=DEV)
     for top_k, seed in ((25, 5), (64, 6), (2, 7)):
-        _lib.check(lib.rstnet_lm_sample_bf16(ld.data_ptr(), rows, V, small, top_k, 0.8, seed, None, a.data_ptr(), 1, st))
-        _lib.check(lib.rstnet_lm_sample_bf16(ld.data_ptr(), rows, V, V, top_k, 0.8, seed, None, b.data_ptr(), 1, st))
+        _sample(ld, rows, V, small, top_k, 0.8, seed, a.data_ptr(), 1)
+        _sample(ld, rows, V, V, top_k, 0.8, seed, b.data_ptr(), 1)
         torch.cuda.synchronize()
         keep = torch.ones(rows, dtype=torch.bool); keep[4] = False   # row 4's top-k is not inside ids < small
         assert torch.equal(a.cpu()[keep], b.cpu()[keep]), top_k
@@ -193,7 +198,7 @@ def test_sampling_large_vocab_candidate_list_matches_full_scan():
         picked = logits.float().gather(1, b.cpu()[:, None])
         assert (picked >= topk).all()
         assert int(b[4]) < top_k     # all-equal row: the top-k are ids 0..top_k-1
-    _lib.check(lib.rstnet_lm_sample_bf16(ld.data_ptr(), rows, V, V, 0, 1.0, 1, None, b.data_ptr(), 1, st))
+    _sample(ld, rows, V, V, 0, 1.0, 1, b.data_ptr(), 1)
     assert torch.equal(b.cpu(), torch.argmax(logits.float(), -1))
 
 
@@ -556,8 +561,8 @@ def test_attention_full_window_2047_keys_vs_sdpa(B):
             pos_b[1], pos_b[2], pos_b[3], pos_b[4] = 0, 5, 40, 1000
         offset = pos_b.to(DEV)
         out = torch.full((B, nh * hs), float("nan"), dtype=BF, device=DEV)
-        _lib.check(lib.rstnet_lm_ring_decode_attention_bf16(q.data_ptr(), kv.data_ptr(), offset.data_ptr(), 1, out.data_ptr(), B, B,
-                                                            nh, nkv, hs, cap, context, st_))
+        _lib.check(lib.rstnet_lm_ring_decode_attention_bf16(q.data_ptr(), kv.data_ptr(), offset.data_ptr(), 1, None, None, out.data_ptr(),
+                                                            B, B, nh, nkv, hs, cap, context, st_))
         rep = nh // nkv
         ref = torch.empty(B, nh, hs, dtype=torch.float64, device=DEV)
         slack = torch.empty(B, nh, 1, dtype=torch.float64, device=DEV)
@@ -623,7 +628,6 @@ def test_block_size_and_bad_ids_fail_loudly(small_lm):
 
 def test_sampling_big_k_and_full_multinomial():
     """top_k > 64 (moshi's default is 250) and top_k == 0 with sampling (plain multinomial, utils/sampling.py:97-101)."""
-    lib, st_ = _lib.lib(), ops._stream()
     g = torch.Generator().manual_seed(2)
     rows, V = 64, 2050
     logits = (torch.randn(rows, V, generator=g) * 2).to(BF)
@@ -633,7 +637,7 @@ def test_sampling_big_k_and_full_multinomial():
     for k in (100, 250, 1000):
         seen = torch.zeros(rows, V, dtype=torch.bool)
         for seed in range(40):
-            _lib.check(lib.rstnet_lm_sample_bf16(ld.data_ptr(), rows, V, 2048, k, 1.0, seed, None, out.data_ptr(), 1, st_))
+            _sample(ld, rows, V, 2048, k, 1.0, seed, out.data_ptr(), 1)
             seen[torch.arange(rows), out.cpu()] = True
         lf = logits.float().clone(); lf[:, 2048:] = -float("inf")
         kth = lf.topk(k, dim=-1).values[:, -1:]
@@ -645,14 +649,14 @@ def test_sampling_big_k_and_full_multinomial():
     lg = torch.log(ps).to(BF).repeat(8000, 1).contiguous().to(DEV)
     o2 = torch.zeros(8000, dtype=torch.int64, device=DEV)
     for temp in (1.0, 0.5):
-        _lib.check(lib.rstnet_lm_sample_bf16(lg.data_ptr(), 8000, 8, 8, -1, temp, 3, None, o2.data_ptr(), 1, st_))
+        _sample(lg, 8000, 8, 8, -1, temp, 3, o2.data_ptr(), 1)
         cnt = torch.bincount(o2.cpu(), minlength=8).float()
         target = torch.softmax(torch.log(ps).to(BF).float() / temp, -1)
         assert (cnt / cnt.sum() - target).abs().max().item() < 2e-2, temp
     # a big-k pick over a 152k vocabulary with n_valid < V (candidate list path)
     big = (torch.randn(8, 151936, generator=g)).to(BF).to(DEV).contiguous()
     o3 = torch.zeros(8, dtype=torch.int64, device=DEV)
-    _lib.check(lib.rstnet_lm_sample_bf16(big.data_ptr(), 8, 151936, 151936, 250, 0.7, 1, None, o3.data_ptr(), 1, st_))
+    _sample(big, 8, 151936, 151936, 250, 0.7, 1, o3.data_ptr(), 1)
     kth = big.float().topk(250, dim=-1).values[:, -1]
     assert (big.float().gather(1, o3[:, None])[:, 0] >= kth).all()
 

@@ -342,8 +342,8 @@ def _rope_append(nh, nkv, hs, rope_n, offsets, Tn, cap, rope_rows, seed):
     kv = kv0.to(DEV)
     qkv_d, cos_d, sin_d, off_d = qkv.to(DEV), cos.to(DEV), sin.to(DEV), off.to(DEV)
     _lib.check(_lib.lib().rstnet_lm_rope_kv_append_bf16(qkv_d.data_ptr(), cos_d.data_ptr(), sin_d.data_ptr(), rope_rows, rope_n,
-                                                        off_d.data_ptr(), 1, q_out.data_ptr(), kv.data_ptr(), Tn * B, B, nh, nkv,
-                                                        hs, cap, ops._stream()))
+                                                        off_d.data_ptr(), 1, None, None, q_out.data_ptr(), kv.data_ptr(), Tn * B, B,
+                                                        nh, nkv, hs, cap, ops._stream()))
     torch.cuda.synchronize()
     # row tl * B + b is stream b at position offsets[b] + tl
     q, k, v = L.split_qkv(qkv.view(Tn, B, -1).transpose(0, 1).contiguous(), cfg)     # [B, heads, Tn, hs]

@@ -82,9 +82,14 @@ def test_sampling_heads():
 
 
 def test_params_entry_point_declared_and_bound():
+    """rstnet_lm_sample_params_bf16 is the sampler's only entry point"""
     src = open(os.path.join(ROOT, "include", "rstnet_b200.h")).read()
     assert "int rstnet_lm_sample_params_bf16(" in src
     assert "rstnet_lm_sample_params_bf16" in _lib.SYMBOLS
+    lib = _lib.lib()
+    for name in ("rstnet_lm_sample_bf16", "rstnet_lm_sample_rows_bf16"):
+        assert name not in src and name not in _lib.SYMBOLS and not hasattr(lib, name), name
+    assert lib.rstnet_version() == 206
 
 
 def test_synthesize_top_p_flags_parse():

@@ -1,6 +1,6 @@
 """Nucleus (top-p) sampling and per-row sampling settings on the GPU (-m gpu): rstnet_lm_sample_params_bf16 against the
 reference's kept sets (tests/golden/sampling_top_p.npz) and the float64 restatement (oracle/sampling_oracle.py), its exact
-relations to the multinomial and to the existing entry points, and the per-row settings through GPT.forward_step,
+relations to the multinomial and between its per-row and scalar forms, and the per-row settings through GPT.forward_step,
 InferenceImp.generate_many and LMGen."""
 import os
 
@@ -42,26 +42,6 @@ def params(logits, top_k=0, temp=1.0, top_p=0.0, *, n_valid=0, nv_rows=None, tab
     _lib.check(_lib.lib().rstnet_lm_sample_params_bf16(logits.data_ptr(), R, V, n_valid, p(nv), 1, top_k, float(temp), float(top_p),
                                                        p(tk), p(te), p(tp), 1, seed, p(sc), p(sr), p(kr), out.data_ptr(), 1,
                                                        ops._stream()), "sample_params")
-    return out.cpu()
-
-
-def legacy(logits, top_k, temp, *, n_valid=0, seed=1, step=None):
-    R, V = logits.shape
-    out = torch.zeros(R, dtype=torch.int64, device=DEV)
-    sc = None if step is None else torch.tensor([step], dtype=torch.int64, device=DEV)
-    _lib.check(_lib.lib().rstnet_lm_sample_bf16(logits.data_ptr(), R, V, n_valid, top_k, float(temp), seed,
-                                                None if sc is None else sc.data_ptr(), out.data_ptr(), 1, ops._stream()))
-    return out.cpu()
-
-
-def legacy_rows(logits, top_k, temp, nv_rows, step_rows, key_rows, seed=1):
-    R, V = logits.shape
-    out = torch.zeros(R, dtype=torch.int64, device=DEV)
-    nv = torch.as_tensor(nv_rows, dtype=torch.int32).to(DEV)
-    sr = torch.as_tensor(step_rows, dtype=torch.int64).to(DEV)
-    kr = _i32(key_rows)
-    _lib.check(_lib.lib().rstnet_lm_sample_rows_bf16(logits.data_ptr(), R, V, V, nv.data_ptr(), 1, top_k, float(temp), seed,
-                                                     sr.data_ptr(), kr.data_ptr(), out.data_ptr(), 1, ops._stream()))
     return out.cpu()
 
 
@@ -138,19 +118,26 @@ def test_empirical_distribution_matches_nucleus():
 
 # ------------------------------------------------------------------------------------------------ 4./5. per-row tables
 @pytest.mark.parametrize("top_k,temp", [(0, 1.0), (1, 0.8), (25, 0.7), (64, 1.1), (65, 0.8), (250, 0.8), (1024, 1.0), (-1, 0.8)])
-def test_uniform_table_equals_existing_entry_points(top_k, temp):
+def test_uniform_table_equals_scalar_form(top_k, temp):
+    """a settings table holding one setting draws what the scalar settings draw, with per-row candidate counts and RNG;
+    and the per-row RNG keyed (step s, row r) and the one-setting table draw what the scope counter at s draws"""
     R, V = 12, 2050
     g = torch.Generator().manual_seed(top_k + 2)
     lg = torch.randn(R, V, generator=g).mul(2).to(BF).to(DEV)
     nv = [2048, 2049, 2050, 2048] * 3
     kr, sr = [3 * r + 1 for r in range(R)], [r % 5 for r in range(R)]
-    want = legacy_rows(lg, top_k, temp, nv, sr, kr)
-    got = params(lg, 0, 1.0, 0.0, nv_rows=nv, tables=([top_k] * R, [temp] * R, [0.0] * R), step_rows=sr, key_rows=kr)
+    table = lambda n: ([top_k] * n, [temp] * n, [0.0] * n)   # noqa: E731
+    want = params(lg, top_k, temp, 0.0, nv_rows=nv, step_rows=sr, key_rows=kr)
+    got = params(lg, 0, 1.0, 0.0, nv_rows=nv, tables=table(R), step_rows=sr, key_rows=kr)
     assert torch.equal(got, want)
-    # the scalar form with the scope counter: rstnet_lm_sample_bf16
-    assert torch.equal(params(lg, top_k, temp, 0.0, n_valid=2049, step=6), legacy(lg, top_k, temp, n_valid=2049, step=6))
+    # the scalar form with the scope counter
+    want = params(lg, top_k, temp, 0.0, n_valid=2049, step=6)
+    assert torch.equal(params(lg, top_k, temp, 0.0, n_valid=2049, step_rows=[6] * R, key_rows=list(range(R))), want)
+    assert torch.equal(params(lg, n_valid=2049, tables=table(R), step=6), want)
     text = torch.randn(4, 152064, generator=g).to(BF).to(DEV)
-    assert torch.equal(params(text, top_k, temp, 0.0, step=2), legacy(text, top_k, temp, step=2))
+    want = params(text, top_k, temp, 0.0, step=2)
+    assert torch.equal(params(text, top_k, temp, 0.0, step_rows=[2] * 4, key_rows=list(range(4))), want)
+    assert torch.equal(params(text, tables=table(4), step=2), want)
 
 
 def test_mixed_modes_per_row():

@@ -2,9 +2,11 @@
 reuse, completion order, the per-row candidate table, and the C ABI of the ragged prefill / per-row sampling."""
 import os
 import random
+import re
 from contextlib import contextmanager
 
 import numpy as np
+import pytest
 import torch
 
 from rstnet_b200 import _lib
@@ -159,9 +161,42 @@ def test_capacity_is_bounded():
 
 def test_new_abi_symbols_declared_and_bound():
     header = open(os.path.join(ROOT, "include", "rstnet_b200.h")).read()
-    for name in ("rstnet_lm_rope_kv_append_rows_bf16", "rstnet_lm_ring_decode_attention_rows_bf16",
-                 "rstnet_lm_sample_rows_bf16", "rstnet_counter_add_rows"):
-        assert f"int {name}(" in header, name
-        assert name in _lib.SYMBOLS, name
+    assert "int rstnet_counter_add_rows(" in header and "rstnet_counter_add_rows" in _lib.SYMBOLS
+    # the row map is two arguments of the uniform entry points, straight after offset_stride
+    for name in ("rstnet_lm_rope_kv_append_bf16", "rstnet_lm_ring_decode_attention_bf16"):
+        decl = header[header.index(f"int {name}("):]
+        decl = " ".join(re.sub(r"\s*/\*.*?\*/", "", decl[:decl.index(");")]).split())
+        assert "int32_t offset_stride, const int32_t* row_stream, const int32_t* row_tl," in decl, (name, decl)
+        assert name in _lib.SYMBOLS
+    lib = _lib.lib()
+    for name in ("rstnet_lm_rope_kv_append_rows_bf16", "rstnet_lm_ring_decode_attention_rows_bf16", "rstnet_lm_sample_rows_bf16",
+                 "rstnet_lm_sample_bf16"):
+        assert name not in header and name not in _lib.SYMBOLS, name
+        assert not hasattr(lib, name), name
+    assert lib.rstnet_version() == 206
     capi = open(os.path.join(ROOT, "rstnet_b200", "csrc", "capi.cu")).read()
-    assert "rstnet_version(void) { return 205; }" in capi
+    assert "rstnet_version(void) { return 206; }" in capi
+
+
+@pytest.mark.parametrize("name", ["rstnet_lm_rope_kv_append_bf16", "rstnet_lm_ring_decode_attention_bf16"])
+def test_row_map_arguments_are_checked(name):
+    """Half a row map, or a row map with a shared offset (offset_stride 0), is an error return before any launch.  Every call
+    also carries n_kv 0, which the entry points reject later, so none of them can reach a launch."""
+    lib = _lib.lib()
+    fake = 1 << 20      # non-NULL pointers that are never dereferenced
+    fn = getattr(lib, name)
+
+    def call(offset_stride, row_stream, row_tl):
+        if name == "rstnet_lm_rope_kv_append_bf16":
+            return fn(fake, fake, fake, 64, 64, fake, offset_stride, row_stream, row_tl, fake, fake, 5, 2, 4, 0, 64, 16, None)
+        return fn(fake, fake, fake, offset_stride, row_stream, row_tl, fake, 5, 2, 4, 0, 64, 16, 16, None)
+
+    for args, msg in (((1, fake, None), "row_stream and row_tl go together"), ((1, None, fake), "row_stream and row_tl go together"),
+                      ((0, fake, fake), "a row map needs per-stream offsets")):
+        assert call(*args) != 0, args
+        assert msg in lib.rstnet_last_error().decode(), args
+    # the map's own checks pass with both pointers and offset_stride 1 (and rows 5 need not be a multiple of B 2): n_kv 0 fails
+    assert call(1, fake, fake) != 0
+    assert "multiple of n_kv" in lib.rstnet_last_error().decode()
+    assert call(1, None, None) != 0
+    assert "multiple of the stream count" in lib.rstnet_last_error().decode()

@@ -50,9 +50,9 @@ def test_row_mapped_rope_append_and_attention_equal_uniform(nh, nkv, hs, rope_n)
     # uniform launch over every (tl, stream) pair
     kv_u, q_u, att_u = kv0.clone(), torch.zeros(tn * B, nh * hs, dtype=BF, device=DEV), torch.zeros(tn * B, nh * hs, dtype=BF, device=DEV)
     _lib.check(lib.rstnet_lm_rope_kv_append_bf16(qkv_u.data_ptr(), cos.data_ptr(), sin.data_ptr(), rope_rows, rope_n, offset.data_ptr(), 1,
-                                                 q_u.data_ptr(), kv_u.data_ptr(), tn * B, B, nh, nkv, hs, cap, st))
-    _lib.check(lib.rstnet_lm_ring_decode_attention_bf16(q_u.data_ptr(), kv_u.data_ptr(), offset.data_ptr(), 1, att_u.data_ptr(), tn * B, B,
-                                                        nh, nkv, hs, cap, context, st))
+                                                 None, None, q_u.data_ptr(), kv_u.data_ptr(), tn * B, B, nh, nkv, hs, cap, st))
+    _lib.check(lib.rstnet_lm_ring_decode_attention_bf16(q_u.data_ptr(), kv_u.data_ptr(), offset.data_ptr(), 1, None, None, att_u.data_ptr(),
+                                                        tn * B, B, nh, nkv, hs, cap, context, st))
     # mapped launch: streams {0, 2, 3} in a shuffled order with padding rows in between; streams 1 and 4 are absent
     pairs = [(b, tl) for b in (0, 2, 3) for tl in range(tn)]
     random.Random(hs).shuffle(pairs)
@@ -66,10 +66,10 @@ def test_row_mapped_rope_append_and_attention_equal_uniform(nh, nkv, hs, rope_n)
     kv_m = kv0.clone()
     q_m = torch.full((M, nh * hs), nanb, dtype=BF, device=DEV)
     att_m = torch.full((M, nh * hs), nanb, dtype=BF, device=DEV)
-    _lib.check(lib.rstnet_lm_rope_kv_append_rows_bf16(qkv_m.data_ptr(), cos.data_ptr(), sin.data_ptr(), rope_rows, rope_n, offset.data_ptr(),
-                                                      rs.data_ptr(), rt.data_ptr(), q_m.data_ptr(), kv_m.data_ptr(), M, B, nh, nkv, hs, cap, st))
-    _lib.check(lib.rstnet_lm_ring_decode_attention_rows_bf16(q_m.data_ptr(), kv_m.data_ptr(), offset.data_ptr(), rs.data_ptr(), rt.data_ptr(),
-                                                             att_m.data_ptr(), M, B, nh, nkv, hs, cap, context, st))
+    _lib.check(lib.rstnet_lm_rope_kv_append_bf16(qkv_m.data_ptr(), cos.data_ptr(), sin.data_ptr(), rope_rows, rope_n, offset.data_ptr(), 1,
+                                                 rs.data_ptr(), rt.data_ptr(), q_m.data_ptr(), kv_m.data_ptr(), M, B, nh, nkv, hs, cap, st))
+    _lib.check(lib.rstnet_lm_ring_decode_attention_bf16(q_m.data_ptr(), kv_m.data_ptr(), offset.data_ptr(), 1, rs.data_ptr(), rt.data_ptr(),
+                                                        att_m.data_ptr(), M, B, nh, nkv, hs, cap, context, st))
     torch.cuda.synchronize()
     bits = lambda t: t.view(torch.int16)
     for r, (b, t) in enumerate(rows):
@@ -94,9 +94,18 @@ def test_counter_add_rows():
 
 
 # ------------------------------------------------------------------------------------------------ 3. per-row sampler
+def _sample(logits, rows, V, n_valid, top_k, temp, seed, out, counter=None, nv_table=None, nv_stride=0, steps=None, keys=None):
+    """rstnet_lm_sample_params_bf16 without settings tables or top_p: the RNG keyed by (seed, *counter, row), or by
+    (seed, steps[row], keys[row]) when those are given; candidates n_valid, or nv_table[row * nv_stride] when given"""
+    p = lambda t: None if t is None else t.data_ptr()
+    _lib.check(_lib.lib().rstnet_lm_sample_params_bf16(logits.data_ptr(), rows, V, n_valid, p(nv_table), nv_stride, top_k, temp, 0.0,
+                                                       None, None, None, 0, seed, p(counter), p(steps), p(keys), out.data_ptr(), 1,
+                                                       ops._stream()))
+
+
 @pytest.mark.parametrize("V", [2050, 20000])
 def test_row_sampler_equals_uniform_sampler(V):
-    lib, st = _lib.lib(), ops._stream()
+    """the sampler's per-row RNG and per-row candidate-count forms equal its scalar form"""
     rows, seed, step = 37, 77, 9
     g = torch.Generator(device="cpu").manual_seed(V)
     logits = (torch.randn(rows, V, generator=g) * 2).to(DEV, BF)
@@ -107,13 +116,12 @@ def test_row_sampler_equals_uniform_sampler(V):
 
     def uniform(n_valid, top_k, temp):
         out = torch.full((rows,), -1, dtype=torch.int64, device=DEV)
-        _lib.check(lib.rstnet_lm_sample_bf16(logits.data_ptr(), rows, V, n_valid, top_k, temp, seed, counter.data_ptr(), out.data_ptr(), 1, st))
+        _sample(logits, rows, V, n_valid, top_k, temp, seed, out, counter=counter)
         return out
 
     def per_row(nv_table, n_valid, top_k, temp):
         out = torch.full((rows,), -1, dtype=torch.int64, device=DEV)
-        _lib.check(lib.rstnet_lm_sample_rows_bf16(logits.data_ptr(), rows, V, n_valid, None if nv_table is None else nv_table.data_ptr(),
-                                                  2, top_k, temp, seed, steps.data_ptr(), keys.data_ptr(), out.data_ptr(), 1, st))
+        _sample(logits, rows, V, n_valid, top_k, temp, seed, out, nv_table=nv_table, nv_stride=2, steps=steps, keys=keys)
         return out
 
     for top_k, temp in ((0, 1.0), (1, 0.8), (30, 0.8), (64, 1.3), (100, 0.8), (1024, 0.7), (-1, 0.9)):
@@ -137,8 +145,7 @@ def test_row_sampler_equals_uniform_sampler(V):
     keys2 = perm.to(torch.int32).to(DEV)
     lg2 = logits[perm.to(DEV)].contiguous()
     out = torch.full((rows,), -1, dtype=torch.int64, device=DEV)
-    _lib.check(lib.rstnet_lm_sample_rows_bf16(lg2.data_ptr(), rows, V, V, None, 0, 30, 0.8, seed, steps.data_ptr(), keys2.data_ptr(),
-                                              out.data_ptr(), 1, st))
+    _sample(lg2, rows, V, V, 30, 0.8, seed, out, steps=steps, keys=keys2)
     assert torch.equal(out, uniform(V, 30, 0.8)[perm.to(DEV)])
 
 

@@ -340,11 +340,26 @@ int rstnet_lm_rms_norm_bf16(const void* x, const void* w, void* y, int32_t rows,
  * infer_no_streaming.py:232-240 for a batch of utterances with different prompt lengths): with row_stream / row_tl given
  * (both or neither; offset_stride must be 1), row r is stream row_stream[r] at position offset[row_stream[r]] + row_tl[r]
  * instead, in any order of (stream, position) pairs, and rows need not be a multiple of B; row_stream[r] == -1 marks a
- * padding row that reads and writes nothing.  Both forms run one compiled kernel. */
+ * padding row that reads and writes nothing.  Both forms run one compiled kernel.  This is the unpaged case of
+ * rstnet_lm_rope_kv_append_paged_bf16 (a contiguous ring per stream); both run the same kernel. */
 int rstnet_lm_rope_kv_append_bf16(const void* qkv, const void* cos_tab, const void* sin_tab, int64_t rope_rows, int32_t rope_n,
                                   const int64_t* offset, int32_t offset_stride /* 0 shared, 1 per stream */,
                                   const int32_t* row_stream, const int32_t* row_tl, void* q_out, void* kv, int32_t rows,
                                   int32_t B, int32_t n_head, int32_t n_kv, int32_t hs, int32_t cap, rstnet_stream_t stream);
+/* ---- paged KV: the same logical ring (position p in slot p % cap, same mask), stored in pages of P = 2^log2_page
+ * positions.  Slot s of stream b lives in page page_table[b * pages_stride + s / P], row s % P, of the pool
+ * kv[n_pages][2][n_kv][P][hs] (one pool per layer; a page index names the same positions in every layer, so one table
+ * serves them all).  page_table int32 [B][pages_stride] with pages_stride * P >= cap; an entry of -1 is unmapped and never
+ * dereferenced: a row whose own position falls on an unmapped page writes nothing (like a padding row).  Every byte
+ * stored and every sum is the contiguous form's; only addresses change.  Errors before any launch: a null table, a
+ * log2_page outside [RSTNET_KV_LOG2_PAGE_MIN, RSTNET_KV_LOG2_PAGE_MAX], pages_stride * P < cap. */
+#define RSTNET_KV_LOG2_PAGE_MIN 4
+#define RSTNET_KV_LOG2_PAGE_MAX 12
+int rstnet_lm_rope_kv_append_paged_bf16(const void* qkv, const void* cos_tab, const void* sin_tab, int64_t rope_rows,
+                                        int32_t rope_n, const int64_t* offset, int32_t offset_stride, const int32_t* row_stream,
+                                        const int32_t* row_tl, void* q_out, void* kv, int32_t rows, int32_t B, int32_t n_head,
+                                        int32_t n_kv, int32_t hs, int32_t cap, const int32_t* page_table, int32_t pages_stride,
+                                        int32_t log2_page, rstnet_stream_t stream);
 /* ---- Kyutai pair-RoPE for the Moshi-style LMModel's temporal transformer (models/model.py:364-389; modules/rope.py:11-68,
  * modules/transformer.py:391-399): qkv [rows][3][H][hd] ((p h d) layout); (even, odd) pairs of q / k rotate by
  * freqs[p] * (offset + tl) (freqs [hd/2] fp32 = exp(-ln(max_period) * 2 p / hd), from the host), fp32 inside, one rounding
@@ -356,11 +371,21 @@ int rstnet_lm_rope_pair_kv_append_bf16(const void* qkv, const int64_t* offset, i
 /* ---- one query position per row over the ring with RingKVCache.complete's position labels and the
  * (pos_k>=0)&(delta>=0)&(delta<context) mask (llama_streaming.py:983-992), fp32 softmax. HBM-bound.  Rows and row map as
  * rstnet_lm_rope_kv_append_bf16 (padding rows write no output); every position of the launch must already be in the ring
- * and no slot a query needs may have been overwritten (callers keep *offset + Tn <= cap for Tn > 1). */
+ * and no slot a query needs may have been overwritten (callers keep *offset + Tn <= cap for Tn > 1).  This is the unpaged
+ * case of rstnet_lm_paged_decode_attention_bf16; both run the same kernel. */
 int rstnet_lm_ring_decode_attention_bf16(const void* q, const void* kv, const int64_t* offset, int32_t offset_stride,
                                          const int32_t* row_stream, const int32_t* row_tl, void* out, int32_t rows, int32_t B,
                                          int32_t n_head, int32_t n_kv, int32_t hs, int32_t cap, int32_t context,
                                          rstnet_stream_t stream);
+/* ---- ring decode attention over a paged pool (page table as rstnet_lm_rope_kv_append_paged_bf16): the same keys in the
+ * same order and the same sums, so the output equals the contiguous form's bit for bit.  A row whose own position is
+ * on an unmapped page writes an all-zero output; a key slot on an unmapped page is not read (callers keep every key of a
+ * query's window mapped).  Same argument checks as the paged append. */
+int rstnet_lm_paged_decode_attention_bf16(const void* q, const void* kv, const int64_t* offset, int32_t offset_stride,
+                                          const int32_t* row_stream, const int32_t* row_tl, void* out, int32_t rows, int32_t B,
+                                          int32_t n_head, int32_t n_kv, int32_t hs, int32_t cap, int32_t context,
+                                          const int32_t* page_table, int32_t pages_stride, int32_t log2_page,
+                                          rstnet_stream_t stream);
 /* out[m][c] = silu(ab[m][c]) * ab[m][I + c]   (LLaMAMLP / ActivationGating) */
 int rstnet_lm_silu_mul_bf16(const void* ab, void* out, int32_t M, int32_t I, rstnet_stream_t stream);
 /* ---- depth transformer attention at codebook step `step` (keys 0..step, capacity dep_q <= 8, no RoPE):

@@ -28,7 +28,10 @@ SYMBOLS = [
     "rstnet_lm_ring_decode_attention_bf16", "rstnet_lm_silu_mul_bf16", "rstnet_lm_depth_attention_bf16",
     "rstnet_resample_f32", "rstnet_lm_delay_cache_in", "rstnet_lm_delay_cache_out", "rstnet_counter_add_rows",
     "rstnet_lm_cross_entropy_bf16", "rstnet_rows_fill_tail_f32", "rstnet_lm_sample_params_bf16",
+    "rstnet_lm_rope_kv_append_paged_bf16", "rstnet_lm_paged_decode_attention_bf16",
 ]
+
+KV_LOG2_PAGE_MIN, KV_LOG2_PAGE_MAX = 4, 12   # RSTNET_KV_LOG2_PAGE_MIN / _MAX: pages of 16 .. 4096 positions
 
 RESAMPLE_MAX_TABLE_BYTES = 48 * 1024   # RSTNET_RESAMPLE_MAX_TABLE_BYTES
 
@@ -143,6 +146,10 @@ def lib() -> C.CDLL:
     L.rstnet_lm_rope_kv_append_bf16.argtypes = [vp, vp, vp, i64, i32, vp, i32, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]
     L.rstnet_lm_rope_pair_kv_append_bf16.argtypes = [vp, vp, i32, vp, vp, i32, i32, i32, i32, i32, vp, vp]
     L.rstnet_lm_ring_decode_attention_bf16.argtypes = [vp, vp, vp, i32, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp]
+    L.rstnet_lm_rope_kv_append_paged_bf16.argtypes = [vp, vp, vp, i64, i32, vp, i32, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32,
+                                                      vp, i32, i32, vp]
+    L.rstnet_lm_paged_decode_attention_bf16.argtypes = [vp, vp, vp, i32, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp, i32, i32,
+                                                        vp]
     L.rstnet_lm_silu_mul_bf16.argtypes = [vp, vp, i32, i32, vp]
     L.rstnet_lm_depth_attention_bf16.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]
     L.rstnet_resample_f32.argtypes = [vp, i64, i64, i64, vp, vp, i32, i32, i32, i32, vp, i64, i64, i32, vp]

@@ -102,10 +102,15 @@ __global__ void rms_norm_kernel(const bf16* __restrict__ x, const bf16* __restri
 // Row map (ragged prefill of some streams): with row_stream set, row r is stream row_stream[r] at position
 // offset[row_stream[r]] + row_tl[r] instead; row_stream[r] == -1 is a padding row that reads and writes nothing.  A runtime
 // branch, not a second instantiation, so the uniform and the mapped launch run one compiled body (DESIGN.md §6).
+// Page table (paged KV, GPT.streaming(B, kv_pages=N)): the logical ring is unchanged -- position p in slot p % cap -- but
+// slot s of stream b lives in page page_table[b * pages_stride + (s >> log2_page)], row s & (2^log2_page - 1), of a pool
+// kv[n_pages][2][n_kv][2^log2_page][hs].  A page entry of -1 is unmapped: a row whose own slot falls on one behaves like a
+// padding row.  page_table == nullptr is the contiguous ring, again by a runtime branch of the same body.
 __global__ void rope_kv_append_bf16_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ cosb, const bf16* __restrict__ sinb,
                                            const long long* __restrict__ offset, bf16* __restrict__ q_out, bf16* __restrict__ kv,
                                            int ostride, int B, int n_kv, int q_per_kv, int hs, int cap, int rope_n,
-                                           long long rope_rows, const int* __restrict__ row_stream, const int* __restrict__ row_tl) {
+                                           long long rope_rows, const int* __restrict__ row_stream, const int* __restrict__ row_tl,
+                                           const int* __restrict__ page_table, int pages_stride, int log2_page) {
   const int row = blockIdx.x / n_kv, g = blockIdx.x % n_kv;
   int b, tl;
   if (row_stream) {
@@ -118,13 +123,23 @@ __global__ void rope_kv_append_bf16_kernel(const bf16* __restrict__ qkv, const b
   }
   const long long pos = offset[(long long)b * ostride] + tl;   // per-stream counters (ostride 1) or one shared (0)
   const int slot = (int)(pos % cap);
+  bf16* kdst;
+  long long vofs;   // V row of a slot = its K row + vofs
+  if (page_table) {
+    const int page = page_table[(long long)b * pages_stride + (slot >> log2_page)];
+    if (page < 0) return;   // unmapped: nothing read, nothing written
+    kdst = kv + ((((long long)page * 2 * n_kv + g) << log2_page) + (slot & ((1 << log2_page) - 1))) * hs;
+    vofs = ((long long)n_kv << log2_page) * hs;
+  } else {
+    kdst = kv + (((long long)b * n_kv + g) * cap + slot) * hs;
+    vofs = (long long)B * n_kv * cap * hs;
+  }
+  bf16* vdst = kdst + vofs;
   const bool bad = pos >= rope_rows;
   if (bad && threadIdx.x == 0) atomicOr(&g_lm_dev_err, 2u);
   const bf16* base = qkv + ((long long)row * n_kv + g) * (q_per_kv + 2) * hs;
   const bf16* c = cosb + (bad ? 0 : pos) * rope_n;
   const bf16* s = sinb + (bad ? 0 : pos) * rope_n;
-  bf16* kdst = kv + (((long long)b * n_kv + g) * cap + slot) * hs;
-  bf16* vdst = kv + (long long)B * n_kv * cap * hs + (((long long)b * n_kv + g) * cap + slot) * hs;
   const int half = rope_n / 2;
   const bf16 nan = f2b(__int_as_float(0x7fc00000));
   for (int i = threadIdx.x; i < (q_per_kv + 1) * hs; i += blockDim.x) {
@@ -192,6 +207,10 @@ __global__ void rope_pair_kv_append_bf16_kernel(const bf16* __restrict__ qkv, co
 // The K/V rows travel through a per-lane cp.async ring in shared memory, ATT_STAGES - 1 sweeps (of 32 keys per CTA) in
 // flight per warp -- every lane copies and reads back only its own 16-byte pieces, so cp.async.wait_group is the only
 // synchronisation.
+// Page table: slot addressing of rope_kv_append_bf16_kernel.  A row whose own slot is on an unmapped page writes zeros; a
+// key slot on an unmapped page is never read (its cp.async copies 0 bytes and fills zeros) -- callers keep every key of a
+// window mapped (GPT.streaming's host guard), so that never enters a real result.  Keys are visited in the same order
+// and summed in the same order as in the contiguous ring: only the addresses differ.
 constexpr int ATT_STAGES = 4;
 constexpr int ATT_WARPS = 8;
 template <int HS, int G>
@@ -199,7 +218,8 @@ __global__ void __launch_bounds__(ATT_WARPS * 32, (G == 1 ? 3 : 2)) ring_decode_
                                                                     const long long* __restrict__ offset, bf16* __restrict__ out,
                                                                     int ostride, int B, int nh, int n_kv, int cap, int context,
                                                                     float scale, const int* __restrict__ row_stream,
-                                                                    const int* __restrict__ row_tl) {
+                                                                    const int* __restrict__ row_tl, const int* __restrict__ page_table,
+                                                                    int pages_stride, int log2_page) {
   constexpr int ST = ATT_STAGES;
   constexpr int DPL = HS / 8;  // dims per lane
   __shared__ float sm_m[G][ATT_WARPS], sm_l[G][ATT_WARPS], sm_acc[G][ATT_WARPS][HS];
@@ -224,8 +244,24 @@ __global__ void __launch_bounds__(ATT_WARPS * 32, (G == 1 ? 3 : 2)) ring_decode_
   if (lo < 0) lo = 0;
   if (lo < pos + 2 - cap) lo = pos + 2 - cap;  // ring quirk: the oldest slot is labelled end_offset and masked
   const long long nkeys = pos - lo + 1;
-  const bf16* Kb = kv + ((long long)b * n_kv + g) * cap * HS;
-  const bf16* Vb = Kb + (long long)B * n_kv * cap * HS;
+  // K row of slot s: Kb + r(s) * HS with r(s) = s (contiguous) or page(s) * page_rows + (s & pmask); V row = K row + vofs
+  const int* pt = nullptr;
+  const bf16* Kb;
+  long long vofs, page_rows = 0;
+  const int pmask = (1 << log2_page) - 1;
+  if (page_table) {
+    pt = page_table + (long long)b * pages_stride;
+    if (pt[(int)(pos % cap) >> log2_page] < 0) {   // the query's own position is unmapped: a finite, all-zero output
+      for (int idx = threadIdx.x; idx < G * HS; idx += blockDim.x) out[((long long)row * nh + h0) * HS + idx] = f2b(0.f);
+      return;
+    }
+    Kb = kv + ((long long)g << log2_page) * HS;
+    vofs = ((long long)n_kv << log2_page) * HS;
+    page_rows = (2LL * n_kv) << log2_page;
+  } else {
+    Kb = kv + ((long long)b * n_kv + g) * cap * HS;
+    vofs = (long long)B * n_kv * cap * HS;
+  }
   float qf[G][DPL];
 #pragma unroll
   for (int u = 0; u < G; ++u) {
@@ -250,12 +286,19 @@ __global__ void __launch_bounds__(ATT_WARPS * 32, (G == 1 ? 3 : 2)) ring_decode_
   auto issue_rows = [&](long long j0, int s) {
     const long long j = j0 + grp;
     const int slot = (int)((lo + (j < nkeys ? j : 0)) % cap);
-    const uint4* kp = reinterpret_cast<const uint4*>(Kb + (long long)slot * HS) + sub;
-    const uint4* vp = reinterpret_cast<const uint4*>(Vb + (long long)slot * HS) + sub;
+    long long r = slot;
+    int bytes = 16;
+    if (pt) {
+      const int page = pt[slot >> log2_page];
+      bytes = page < 0 ? 0 : 16;
+      r = page < 0 ? 0 : page * page_rows + (slot & pmask);
+    }
+    const uint4* kp = reinterpret_cast<const uint4*>(Kb + r * HS) + sub;
+    const uint4* vp = reinterpret_cast<const uint4*>(Kb + vofs + r * HS) + sub;
 #pragma unroll
     for (int i = 0; i < CH; ++i) {
-      cp_async16(&ring[(s * 2 * CH + i) * 32 + lane], kp + i * 8, 16);
-      cp_async16(&ring[(s * 2 * CH + CH + i) * 32 + lane], vp + i * 8, 16);
+      cp_async16(&ring[(s * 2 * CH + i) * 32 + lane], kp + i * 8, bytes);
+      cp_async16(&ring[(s * 2 * CH + CH + i) * 32 + lane], vp + i * 8, bytes);
     }
   };
   const long long jstep = (long long)nwarps * 4;
@@ -354,12 +397,13 @@ __global__ void __launch_bounds__(ATT_WARPS * 32, (G == 1 ? 3 : 2)) ring_decode_
 template <int HS, int G>
 void launch_ring_decode_attention(cudaStream_t st, const bf16* q, const bf16* kv, const long long* offset, bf16* out, int ostride,
                                   int rows, int B, int nh, int n_kv, int cap, int context, float scale, const int* row_stream,
-                                  const int* row_tl) {
+                                  const int* row_tl, const int* page_table, int pages_stride, int log2_page) {
   constexpr int smem = ATT_STAGES * ATT_WARPS * 32 * (HS / 64) * 2 * 16;
   static unsigned long long attr = 0;
   smem_optin(ring_decode_attention_kernel<HS, G>, smem, attr);
   ring_decode_attention_kernel<HS, G><<<rows * (nh / G), ATT_WARPS * 32, smem, st>>>(q, kv, offset, out, ostride, B, nh, n_kv, cap, context, scale,
-                                                                                                    row_stream, row_tl);
+                                                                                                    row_stream, row_tl, page_table, pages_stride,
+                                                                                                    log2_page);
 }
 
 // ---------------------------------------------------------------- SiLU gating: out = silu(a) * b  (bf16 roundings as eager)
@@ -868,10 +912,20 @@ extern "C" int rstnet_lm_rms_norm_bf16(const void* x, const void* w, void* y, in
   return check_launch("lm_rms_norm");
 }
 
-extern "C" int rstnet_lm_rope_kv_append_bf16(const void* qkv, const void* cos_tab, const void* sin_tab, int64_t rope_rows,
-                                             int32_t rope_n, const int64_t* offset, int32_t offset_stride, const int32_t* row_stream,
-                                             const int32_t* row_tl, void* q_out, void* kv, int32_t rows, int32_t B, int32_t n_head,
-                                             int32_t n_kv, int32_t hs, int32_t cap, rstnet_stream_t stream) {
+// the page-table arguments of the paged entry points, checked before any launch
+static int check_pages(const char* who, const int32_t* page_table, int32_t pages_stride, int32_t log2_page, int32_t cap) {
+  RSTNET_REQUIRE(page_table, "%s: null page table", who);
+  RSTNET_REQUIRE(log2_page >= RSTNET_KV_LOG2_PAGE_MIN && log2_page <= RSTNET_KV_LOG2_PAGE_MAX,
+                 "%s: log2_page (%d) outside [%d, %d]", who, log2_page, RSTNET_KV_LOG2_PAGE_MIN, RSTNET_KV_LOG2_PAGE_MAX);
+  RSTNET_REQUIRE(cap > 0 && pages_stride > 0 && ((long long)pages_stride << log2_page) >= cap,
+                 "%s: pages_stride (%d) pages of %d positions do not cover the ring of %d", who, pages_stride, 1 << log2_page, cap);
+  return 0;
+}
+
+static int rope_kv_append(const void* qkv, const void* cos_tab, const void* sin_tab, int64_t rope_rows, int32_t rope_n,
+                          const int64_t* offset, int32_t offset_stride, const int32_t* row_stream, const int32_t* row_tl, void* q_out,
+                          void* kv, int32_t rows, int32_t B, int32_t n_head, int32_t n_kv, int32_t hs, int32_t cap,
+                          const int32_t* page_table, int32_t pages_stride, int32_t log2_page, rstnet_stream_t stream) {
   RSTNET_REQUIRE(qkv && cos_tab && sin_tab && offset && q_out && kv, "lm_rope_kv_append: null pointer");
   RSTNET_REQUIRE(!row_stream == !row_tl, "lm_rope_kv_append: row_stream and row_tl go together");
   RSTNET_REQUIRE(!row_stream || offset_stride, "lm_rope_kv_append: a row map needs per-stream offsets (offset_stride 1)");
@@ -881,9 +935,29 @@ extern "C" int rstnet_lm_rope_kv_append_bf16(const void* qkv, const void* cos_ta
   RSTNET_REQUIRE(rope_n >= 0 && rope_n <= hs && rope_n % 2 == 0 && rope_rows > 0, "lm_rope_kv_append: bad rope table (%d of %d dims)", rope_n, hs);
   rope_kv_append_bf16_kernel<<<dim3(rows * n_kv), dim3(64), 0, (cudaStream_t)stream>>>((const bf16*)qkv, (const bf16*)cos_tab,
              (const bf16*)sin_tab, (const long long*)offset, (bf16*)q_out, (bf16*)kv, offset_stride ? 1 : 0, B, n_kv, n_head / n_kv, hs,
-             cap, rope_n, (long long)rope_rows, (const int*)row_stream, (const int*)row_tl);
+             cap, rope_n, (long long)rope_rows, (const int*)row_stream, (const int*)row_tl, (const int*)page_table, pages_stride,
+             log2_page);
   count_launch();
   return check_launch("lm_rope_kv_append");
+}
+
+extern "C" int rstnet_lm_rope_kv_append_bf16(const void* qkv, const void* cos_tab, const void* sin_tab, int64_t rope_rows,
+                                             int32_t rope_n, const int64_t* offset, int32_t offset_stride, const int32_t* row_stream,
+                                             const int32_t* row_tl, void* q_out, void* kv, int32_t rows, int32_t B, int32_t n_head,
+                                             int32_t n_kv, int32_t hs, int32_t cap, rstnet_stream_t stream) {
+  return rope_kv_append(qkv, cos_tab, sin_tab, rope_rows, rope_n, offset, offset_stride, row_stream, row_tl, q_out, kv, rows, B,
+                        n_head, n_kv, hs, cap, nullptr, 0, 0, stream);
+}
+
+extern "C" int rstnet_lm_rope_kv_append_paged_bf16(const void* qkv, const void* cos_tab, const void* sin_tab, int64_t rope_rows,
+                                                   int32_t rope_n, const int64_t* offset, int32_t offset_stride,
+                                                   const int32_t* row_stream, const int32_t* row_tl, void* q_out, void* kv, int32_t rows,
+                                                   int32_t B, int32_t n_head, int32_t n_kv, int32_t hs, int32_t cap,
+                                                   const int32_t* page_table, int32_t pages_stride, int32_t log2_page,
+                                                   rstnet_stream_t stream) {
+  if (check_pages("lm_rope_kv_append_paged", page_table, pages_stride, log2_page, cap)) return 1;
+  return rope_kv_append(qkv, cos_tab, sin_tab, rope_rows, rope_n, offset, offset_stride, row_stream, row_tl, q_out, kv, rows, B,
+                        n_head, n_kv, hs, cap, page_table, pages_stride, log2_page, stream);
 }
 
 extern "C" int rstnet_lm_rope_pair_kv_append_bf16(const void* qkv, const int64_t* offset, int32_t offset_stride, void* q_out, void* kv,
@@ -897,10 +971,10 @@ extern "C" int rstnet_lm_rope_pair_kv_append_bf16(const void* qkv, const int64_t
   return check_launch("lm_rope_pair_kv_append");
 }
 
-extern "C" int rstnet_lm_ring_decode_attention_bf16(const void* q, const void* kv, const int64_t* offset, int32_t offset_stride,
-                                                    const int32_t* row_stream, const int32_t* row_tl, void* out, int32_t rows,
-                                                    int32_t B, int32_t n_head, int32_t n_kv, int32_t hs, int32_t cap, int32_t context,
-                                                    rstnet_stream_t stream) {
+static int ring_decode_attention(const void* q, const void* kv, const int64_t* offset, int32_t offset_stride,
+                                 const int32_t* row_stream, const int32_t* row_tl, void* out, int32_t rows, int32_t B, int32_t n_head,
+                                 int32_t n_kv, int32_t hs, int32_t cap, int32_t context, const int32_t* page_table,
+                                 int32_t pages_stride, int32_t log2_page, rstnet_stream_t stream) {
   RSTNET_REQUIRE(q && kv && offset && out, "lm_ring_decode_attention: null pointer");
   RSTNET_REQUIRE(!row_stream == !row_tl, "lm_ring_decode_attention: row_stream and row_tl go together");
   RSTNET_REQUIRE(!row_stream || offset_stride, "lm_ring_decode_attention: a row map needs per-stream offsets (offset_stride 1)");
@@ -914,9 +988,27 @@ extern "C" int rstnet_lm_ring_decode_attention_bf16(const void* q, const void* k
   const auto launch = hs == 128 ? (G == 2 ? launch_ring_decode_attention<128, 2> : launch_ring_decode_attention<128, 1>)
                                 : (G == 2 ? launch_ring_decode_attention<64, 2> : launch_ring_decode_attention<64, 1>);
   launch((cudaStream_t)stream, (const bf16*)q, (const bf16*)kv, (const long long*)offset, (bf16*)out, offset_stride ? 1 : 0, rows, B,
-         n_head, n_kv, cap, context, scale, (const int*)row_stream, (const int*)row_tl);
+         n_head, n_kv, cap, context, scale, (const int*)row_stream, (const int*)row_tl, (const int*)page_table, pages_stride, log2_page);
   count_launch();
   return check_launch("lm_ring_decode_attention");
+}
+
+extern "C" int rstnet_lm_ring_decode_attention_bf16(const void* q, const void* kv, const int64_t* offset, int32_t offset_stride,
+                                                    const int32_t* row_stream, const int32_t* row_tl, void* out, int32_t rows,
+                                                    int32_t B, int32_t n_head, int32_t n_kv, int32_t hs, int32_t cap, int32_t context,
+                                                    rstnet_stream_t stream) {
+  return ring_decode_attention(q, kv, offset, offset_stride, row_stream, row_tl, out, rows, B, n_head, n_kv, hs, cap, context, nullptr,
+                               0, 0, stream);
+}
+
+extern "C" int rstnet_lm_paged_decode_attention_bf16(const void* q, const void* kv, const int64_t* offset, int32_t offset_stride,
+                                                     const int32_t* row_stream, const int32_t* row_tl, void* out, int32_t rows,
+                                                     int32_t B, int32_t n_head, int32_t n_kv, int32_t hs, int32_t cap, int32_t context,
+                                                     const int32_t* page_table, int32_t pages_stride, int32_t log2_page,
+                                                     rstnet_stream_t stream) {
+  if (check_pages("lm_paged_decode_attention", page_table, pages_stride, log2_page, cap)) return 1;
+  return ring_decode_attention(q, kv, offset, offset_stride, row_stream, row_tl, out, rows, B, n_head, n_kv, hs, cap, context,
+                               page_table, pages_stride, log2_page, stream);
 }
 
 extern "C" int rstnet_lm_silu_mul_bf16(const void* ab, void* out, int32_t M, int32_t I, rstnet_stream_t stream) {

@@ -30,7 +30,7 @@ import numpy as np
 import torch
 
 from ._lib import RstnetError
-from .lm import GPT, MAX_STREAMS, Sampling
+from .lm import GPT, KV_PAGE, MAX_STREAMS, Sampling
 
 
 def candidate_counts(pre_gen_len: int, minlen: int, g_idx: int, dep_q: int = 8) -> List[int]:
@@ -249,7 +249,8 @@ class InferenceImp(object):
     @torch.no_grad()
     def generate_many(self, items: Iterable[Tuple[object, torch.Tensor]], capacity: int,
                       seeds: Optional[Dict[object, int]] = None, return_frames: bool = False,
-                      sampling: Optional[Dict[object, Sampling]] = None) -> Iterator[Tuple]:
+                      sampling: Optional[Dict[object, Sampling]] = None, kv_pages: Optional[int] = None,
+                      stats: Optional[dict] = None) -> Iterator[Tuple]:
         """Continuous batching over (utt_id, seq [9, L]) items, each in its own TTS layout: yields (utt_id, codes [8, G-1])
         in completion order.  Up to `capacity` utterances decode together, one graph replay per frame; a finished row is
         held until the next utterance is admitted into it (its prompt fed through GPT.prefill_streams while the other
@@ -258,11 +259,29 @@ class InferenceImp(object):
         of generate() on that utterance alone.  return_frames: yield (utt_id, codes, raw frames [G, 9]) as generate does.
         sampling: {utt_id: Sampling} gives those utterances their own settings (the others take the instance's); each
         utterance's codes are then those of generate() on it alone with its settings, whatever the others' settings.
-        The settings are rows of device tables: changing them captures no new graph."""
+        The settings are rows of device tables: changing them captures no new graph.
+
+        The KV cache is paged (GPT.streaming(B, kv_pages=N)): an admitted utterance holds pages for exactly the positions
+        it writes (its prompt and init token feed, then one per generated frame) and frees them when it finishes.
+        kv_pages: the pool size in pages of lm.KV_PAGE positions; None gives every row a whole ring (capacity x
+        ceil(context / KV_PAGE) pages), so admissions and completion order are those of unpaged rings.  With a smaller
+        pool an utterance waits for pages while a row is free; admission stops at the first utterance that does not fit,
+        so the completion order is fixed for a given pool.  An utterance needing more than the whole pool raises.
+        stats: a dict that receives 'frames' (frames run), 'row_frames' (occupied rows summed over frames) and
+        'wait_frames' (frames run while an utterance waited for pages with a row free)."""
         self._check_task()
         if not 1 <= capacity <= MAX_STREAMS:
             raise RstnetError(f"capacity must be in [1, {MAX_STREAMS}] (got {capacity})")
         m, seeds = self.model, seeds or {}
+        # GPT always decodes here on paged KV; a stand-in model that offers only the unpaged streaming protocol (no
+        # reserve_kv) runs its own scope
+        paged = hasattr(m, "reserve_kv")
+        if paged and kv_pages is None:
+            kv_pages = capacity * -(-m.config.context // KV_PAGE)
+        if not paged and kv_pages is not None:
+            raise RstnetError(f"{type(m).__name__} has no paged KV scope (kv_pages)")
+        stats = {} if stats is None else stats
+        stats.update(frames=0, row_frames=0, wait_frames=0)
         if sampling is not None:
             default = self.sampling()
             for utt, sp in sampling.items():
@@ -278,25 +297,49 @@ class InferenceImp(object):
         cur = torch.zeros(B, n_cb, 1, dtype=torch.int64, device=dev)
         keys = np.zeros(B, dtype=np.int64)
         active = np.zeros(B, dtype=np.int64)
-        with m.streaming(B):
+        with m.streaming(B, kv_pages=kv_pages) if paged else m.streaming(B):
+            pages = m._state.pages if paged else None   # the scope's allocator, read to decide admissions
             m.set_active_streams(active)
             init = m._get_initial_token()[0].to(dev)
             exhausted = False
+            pending = None   # (utt, seq, P, G) of the next utterance while it waits for pages
+            dirty = set()    # rows whose pages changed on the host since the last upload
             while True:
                 admitted = {}
                 for r in range(B):
-                    if rows[r] is not None or exhausted:
+                    if rows[r] is not None:
                         continue
-                    try:
-                        utt, seq = next(source)
-                    except StopIteration:
-                        exhausted = True
-                        break
-                    P, G = self._layout(seq)
+                    if pending is None:
+                        if exhausted:
+                            break
+                        try:
+                            utt, seq = next(source)
+                        except StopIteration:
+                            exhausted = True
+                            break
+                        P, G = self._layout(seq)
+                        if paged and pages.pages_for(P + G) > pages.n_pages:
+                            raise RstnetError(f"utterance {utt!r} needs {pages.pages_for(P + G)} KV pages ({P + G} positions), "
+                                              f"more than the whole pool of {pages.n_pages}")
+                        pending = (utt, seq, P, G)
+                    utt, seq, P, G = pending
+                    if paged:
+                        if pages.pages_for(P + G) > pages.free:
+                            stats["wait_frames"] += 1
+                            break
+                        # it writes P positions in the prompt feed (init token + all prompt frames but the last) and one
+                        # per generated frame: exactly P + G
+                        pages.reserve([r], P + G)
+                        dirty.add(r)
+                    pending = None
                     feed = torch.cat([init, seq[:, :P].to(device=dev, dtype=torch.int64)], dim=1)
                     admitted[r] = feed
                     rows[r] = dict(utt=utt, P=P, G=G, g=0, start=frame)
                     keys[r] = int(seeds.get(utt, 0))
+                if dirty:
+                    # one upload of the table rows this frame's releases and admissions changed, before any launch
+                    m._state.upload_pages(sorted(dirty))
+                    dirty.clear()
                 if admitted:
                     # the init token + all prompt frames but the last only feed the KV rings; the step on the last prompt
                     # frame yields generated frame 0 (as generate)
@@ -324,6 +367,8 @@ class InferenceImp(object):
                                       top_p_text=self.top_p_text, top_p=self.top_p, sampling=per_row)
                 history[frame] = toks
                 frame += 1
+                stats["frames"] += 1
+                stats["row_frames"] += len(occupied)
                 cur = toks[:, :, None].clone()
                 for r in occupied:
                     st = rows[r]
@@ -331,7 +376,10 @@ class InferenceImp(object):
                     if st["g"] == st["G"]:
                         raw = torch.stack([history[f][r] for f in range(st["start"], frame)])     # [G, 9]
                         rows[r] = None
-                        m.reset_streaming(streams=[r])   # a held row keeps its position: park it at 0
+                        m.reset_streaming(streams=[r])   # a held row keeps its position: park it at 0 ...
+                        if paged:
+                            pages.release([r])           # ... without pages (uploaded before the next launch)
+                            dirty.add(r)
                         codes = reverse_delay(raw[:, 1:])
                         yield (st["utt"], codes, raw) if return_frames else (st["utt"], codes)
                 first = min([st["start"] for st in rows if st is not None], default=frame)

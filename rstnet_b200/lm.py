@@ -21,6 +21,7 @@ dtype recipe of `GPT(config).to(device, bfloat16)` (infer_no_streaming.py:104-10
 from __future__ import annotations
 
 import ctypes as C
+import heapq
 from contextlib import contextmanager
 from dataclasses import dataclass
 from typing import Dict, Optional
@@ -39,6 +40,91 @@ MAX_STREAMS = 256   # streams of one decode scope (one position each): the wides
 ROW_BUCKETS = (16, 32, 64, 128)   # launch widths of a ragged prefill chunk (padding rows fill the rest): one chunk state and
                                   # one set of GEMM plans per width
 SAMPLE_CAND = 1024   # the sampler's largest top_k
+KV_PAGE = 64   # positions per KV page of a paged decode scope (GPT.streaming(B, kv_pages=N))
+
+
+def kv_page_bytes(c: "Config", page: int = KV_PAGE) -> int:
+    """Bytes of one KV page over all layers: K and V of `page` positions, bf16, one row per KV group."""
+    return c.n_layer * 2 * c.n_query_groups * page * c.head_size * 2
+
+
+def kv_pages_for_budget(c: "Config", gib: float, page: int = KV_PAGE) -> int:
+    """The pool that fits in `gib` GiB: floor(gib * 2^30 / kv_page_bytes)."""
+    return int(gib * 2 ** 30 // kv_page_bytes(c, page))
+
+
+class KVPages:
+    """Host side of a paged KV scope: which pool page holds each page of each stream's ring.  The ring itself is the
+    contiguous scope's (position p in slot p % cap); page i of stream s (slots i*page .. (i+1)*page - 1) lives in pool
+    page table[s, i], -1 when unmapped.  A stream holds table[s, :held[s]], and may advance to position limit[s]
+    (unbounded once it holds the whole ring).  Pages are handed out lowest free index first, so a given sequence of
+    reservations always produces the same table."""
+
+    def __init__(self, n_pages: int, streams: int, page: int, cap: int):
+        log2 = int(page).bit_length() - 1
+        if page <= 0 or page != 1 << log2 or not _lib.KV_LOG2_PAGE_MIN <= log2 <= _lib.KV_LOG2_PAGE_MAX:
+            raise RstnetError(f"the KV page must be a power of two in [{1 << _lib.KV_LOG2_PAGE_MIN}, "
+                              f"{1 << _lib.KV_LOG2_PAGE_MAX}] positions (got {page})")
+        if isinstance(n_pages, bool) or not isinstance(n_pages, (int, np.integer)) or n_pages < 1:
+            raise RstnetError(f"kv_pages must be a positive int (got {n_pages!r})")
+        self.n_pages, self.streams, self.page, self.log2_page, self.cap = int(n_pages), streams, page, log2, cap
+        self.stride = -(-cap // page)   # table entries per stream: the whole ring
+        self.table = np.full((streams, self.stride), -1, dtype=np.int32)
+        self.held = np.zeros(streams, dtype=np.int64)
+        self.limit = np.zeros(streams, dtype=np.int64)
+        self._free = list(range(self.n_pages))   # a heap
+
+    @property
+    def free(self) -> int:
+        return len(self._free)
+
+    def pages_for(self, positions: int) -> int:
+        """pages a stream needs to write positions 0 .. positions - 1"""
+        return -(-min(int(positions), self.cap) // self.page)
+
+    def _streams(self, streams):
+        s = [int(x) for x in np.asarray(streams, dtype=np.int64).reshape(-1)]
+        if any(not 0 <= x < self.streams for x in s):
+            raise RstnetError(f"stream index outside [0, {self.streams})")
+        if len(set(s)) != len(s):
+            raise RstnetError("a stream is listed twice")
+        return s
+
+    def reserve(self, streams, positions):
+        """Give each stream pages for min(positions, cap) positions (one count for all, or one per stream), replacing its
+        reservation: it keeps the pages of the positions it still holds, frees the rest, and takes new pages lowest
+        first.  All or nothing: when the pool is short, raise and change nothing.  -> the streams whose table rows changed."""
+        s = self._streams(streams)
+        pos = np.broadcast_to(np.asarray(positions, dtype=np.int64), (len(s),))
+        if (pos < 0).any():
+            raise RstnetError("a reservation needs positions >= 0")
+        need = [self.pages_for(p) for p in pos]
+        grow = sum(max(0, n - int(self.held[x])) for x, n in zip(s, need))
+        shrink = sum(max(0, int(self.held[x]) - n) for x, n in zip(s, need))
+        if grow > len(self._free) + shrink:
+            raise RstnetError(f"the KV pool is short: {grow} more pages wanted, {len(self._free) + shrink} free "
+                              f"(pool of {self.n_pages} pages of {self.page} positions)")
+        for x, n in zip(s, need):
+            for page in self.table[x, n:self.held[x]]:
+                heapq.heappush(self._free, int(page))
+            self.table[x, n:] = -1
+        for x, n, p in zip(s, need, pos):
+            for i in range(int(self.held[x]), n):
+                self.table[x, i] = heapq.heappop(self._free)
+            self.held[x] = n
+            self.limit[x] = p if p < self.cap else np.iinfo(np.int64).max
+        return s
+
+    def release(self, streams):
+        """Free the streams' pages.  -> the streams whose table rows changed."""
+        return self.reserve(streams, 0)
+
+    def check(self, streams, pos, n) -> None:
+        """Raise unless every stream s of `streams` (at position pos[i]) may write n more positions."""
+        for s, p in zip(streams, pos):
+            if int(p) + n > self.limit[s]:
+                raise RstnetError(f"stream {int(s)} would write position {int(p) + n - 1} but holds KV pages for "
+                                  f"{int(self.limit[s])} positions: reserve_kv first")
 
 
 @dataclass(frozen=True)
@@ -415,17 +501,53 @@ class GPT(nn.Module):
         return self._state is not None
 
     @on_own_device
-    def streaming_forever(self, batch_size: int):
+    def streaming_forever(self, batch_size: int, kv_pages: Optional[int] = None, kv_page: int = KV_PAGE):
+        """kv_pages None: every stream owns a contiguous KV ring of `context` positions per layer.  kv_pages N: the layers'
+        KV lives in a shared pool of N pages of kv_page positions (kv_page_bytes each), and a stream holds only the
+        pages reserve_kv gives it -- none at entry.  Both give the same results bit for bit."""
         self._check_runnable()
-        self._state = _LMState(self, batch_size)
+        self._state = _LMState(self, batch_size, kv_pages=kv_pages, kv_page=kv_page)
 
     @contextmanager
-    def streaming(self, batch_size: int):
-        self.streaming_forever(batch_size)
+    def streaming(self, batch_size: int, kv_pages: Optional[int] = None, kv_page: int = KV_PAGE):
+        self.streaming_forever(batch_size, kv_pages=kv_pages, kv_page=kv_page)
         try:
             yield
         finally:
             self._state = None
+
+    def _paged(self) -> "_LMState":
+        st = self._state
+        if st is None:
+            raise RstnetError("the model is not streaming")
+        if st.pages is None:
+            raise RstnetError("this streaming scope keeps contiguous KV rings: enter gpt.streaming(B, kv_pages=N) for pages")
+        return st
+
+    @on_own_device
+    def reserve_kv(self, streams, positions) -> None:
+        """Paged scope: give each listed stream KV pages for min(positions, context) positions from position 0 (one count
+        for all, or one per stream), replacing its reservation (the pages of the positions it keeps stay, with their
+        contents).  An active stream cannot advance past its reservation: the step raises before any launch.  If the
+        pool is short this raises RstnetError and changes nothing."""
+        st = self._paged()
+        st.upload_pages(st.pages.reserve(streams, positions))
+
+    @on_own_device
+    def release_kv(self, streams) -> None:
+        """Paged scope: return the listed streams' KV pages to the pool (a stream without pages may still be held)."""
+        st = self._paged()
+        st.upload_pages(st.pages.release(streams))
+
+    @property
+    def kv_pages_free(self) -> int:
+        """Paged scope: pages of the pool no stream holds."""
+        return self._paged().pages.free
+
+    @property
+    def kv_page_bytes(self) -> int:
+        """Paged scope: bytes of one KV page over all layers (K and V, bf16)."""
+        return kv_page_bytes(self.config, self._paged().pages.page)
 
     @on_own_device
     def reset_streaming(self, streams=None):
@@ -686,9 +808,10 @@ class _LMState:
     only holds the depth transformer (forward_local)."""
 
     def __init__(self, m: GPT, B: int, tn: int = 1, parent: Optional["_LMState"] = None, parts=("temporal", "depth"),
-                 rows: Optional[int] = None):
+                 rows: Optional[int] = None, kv_pages: Optional[int] = None, kv_page: int = KV_PAGE):
         """rows: a ragged prefill chunk of that many rows (with `parent`): row r is stream row_stream[r] at position
-        offset + row_tl[r] (-1: padding), and the counters advance by `delta` per stream."""
+        offset + row_tl[r] (-1: padding), and the counters advance by `delta` per stream.  kv_pages: a paged KV pool of
+        that many pages of kv_page positions instead of contiguous rings (a child shares its parent's)."""
         c, dev = m.config, m.device
         self.m, self.B, self.c, self.tn = m, B, c, tn
         M = self.M = B * tn if rows is None else rows
@@ -735,6 +858,9 @@ class _LMState:
         self.row_children: Dict[int, "_LMState"] = {}
         self.has_temporal = "temporal" in parts
         self.row_mapped = rows is not None
+        self.pages: Optional[KVPages] = None        # paged scope: the host allocator
+        self.page_table: Optional[torch.Tensor] = None   # ... and its device table int32 [B, pages.stride]
+        self._kv_pages = (kv_pages, kv_page)
         if self.row_mapped:
             self.row_stream, self.row_tl = z(M, dtype=torch.int32), z(M, dtype=torch.int32)
             self.delta = z(B, dtype=torch.int64)
@@ -811,8 +937,15 @@ class _LMState:
             # advance flags: a stream with 0 is HELD by the next steps (frame scheduler rows without input)
             self.active = torch.ones(B, dtype=torch.int64, device=dev)
             self.active_host = np.ones(B, dtype=np.int64)
-            # KV rings, one K/V row per KV GROUP: [2, B, n_kv, cap, hs] (lit_model.py:607-615 stores n_head copies)
-            self.kv = [z(2, B, nkv, self.cap, hs) for _ in range(c.n_layer)]
+            # KV rings, one K/V row per KV GROUP: [2, B, n_kv, cap, hs] (lit_model.py:607-615 stores n_head copies), or the
+            # paged pool [n_pages, 2, n_kv, page, hs] per layer, one table for all layers
+            n_pages, page = self._kv_pages
+            if n_pages is None:
+                self.kv = [z(2, B, nkv, self.cap, hs) for _ in range(c.n_layer)]
+            else:
+                self.pages = KVPages(n_pages, B, page, self.cap)
+                self.page_table = torch.full((B, self.pages.stride), -1, dtype=torch.int32, device=dev)
+                self.kv = [z(self.pages.n_pages, 2, nkv, page, hs) for _ in range(c.n_layer)]
             # RoPE tables in the model dtype (the reference's buffers are cast by .to(bfloat16)); lit_model.py:441-488
             n = c.rope_n_elem
             theta = 1.0 / (c.rope_base ** (torch.arange(0, n, 2).float() / n))
@@ -827,6 +960,7 @@ class _LMState:
         else:
             self.offset, self.pos_host, self.kv, self.cos, self.sin = parent.offset, parent.pos_host, parent.kv, parent.cos, parent.sin
             self.active, self.active_host = parent.active, parent.active_host
+            self.pages, self.page_table = parent.pages, parent.page_table
         self.tables = [P[f"input_emb.{i}.weight"] for i in range(c.n_q)]
         self.table_ptrs = torch.tensor([t.data_ptr() for t in self.tables], dtype=torch.int64, device=dev)
         self.wte = P["transformer.wte.weight"]
@@ -876,19 +1010,23 @@ class _LMState:
         # a row map always indexes the position counters per stream (offset_stride 1), even with B == 1
         rs, rt = (self.row_stream.data_ptr(), self.row_tl.data_ptr()) if self.row_mapped else (None, None)
         ost = 1 if self.row_mapped or self.offset.numel() > 1 else 0
+        # a paged scope runs the same kernels through their paged entry points: the page table as three more arguments
+        if self.pages is None:
+            rope, attention, pg = L.rstnet_lm_rope_kv_append_bf16, L.rstnet_lm_ring_decode_attention_bf16, ()
+        else:
+            rope, attention = L.rstnet_lm_rope_kv_append_paged_bf16, L.rstnet_lm_paged_decode_attention_bf16
+            pg = (self.page_table.data_ptr(), self.pages.stride, self.pages.log2_page)
         _lib.check(L.rstnet_lm_embed_sum_bf16(self.seq.data_ptr(), c.n_q + 1, self.wte.data_ptr(), self.wte.shape[0],
                                               self.table_ptrs.data_ptr(), self.tables[0].shape[0], c.n_q, E, self.x.data_ptr(), M, st),
                    "lm_embed_sum")
         _lib.check(L.rstnet_lm_rms_norm_bf16(self.x.data_ptr(), self.n1_first.data_ptr(), self.xn.data_ptr(), M, E, c.norm_eps, 0, st), "rms")
         for l, ly in enumerate(self.layers):
             ly["qkv"].run()
-            _lib.check(L.rstnet_lm_rope_kv_append_bf16(self.qkv.data_ptr(), self.cos.data_ptr(), self.sin.data_ptr(), self.cos.shape[0],
-                                                       c.rope_n_elem, self.offset.data_ptr(), ost, rs, rt, self.q.data_ptr(),
-                                                       self.kv[l].data_ptr(), M, B, c.n_head, c.n_query_groups, c.head_size, self.cap, st),
-                       "rope_kv")
-            _lib.check(L.rstnet_lm_ring_decode_attention_bf16(self.q.data_ptr(), self.kv[l].data_ptr(), self.offset.data_ptr(), ost,
-                                                              rs, rt, self.att.data_ptr(), M, B, c.n_head, c.n_query_groups,
-                                                              c.head_size, self.cap, c.context, st), "attention")
+            _lib.check(rope(self.qkv.data_ptr(), self.cos.data_ptr(), self.sin.data_ptr(), self.cos.shape[0], c.rope_n_elem,
+                            self.offset.data_ptr(), ost, rs, rt, self.q.data_ptr(), self.kv[l].data_ptr(), M, B, c.n_head,
+                            c.n_query_groups, c.head_size, self.cap, *pg, st), "rope_kv")
+            _lib.check(attention(self.q.data_ptr(), self.kv[l].data_ptr(), self.offset.data_ptr(), ost, rs, rt, self.att.data_ptr(),
+                                 M, B, c.n_head, c.n_query_groups, c.head_size, self.cap, c.context, *pg, st), "attention")
             ly["proj"].run()   # + residual + norm_2 -> xn
             ly["fc"].run()     # + SiLU gating -> hmid
             ly["down"].run()   # + residual + next pre-norm -> xn (last layer: ln_f -> transformer_out)
@@ -980,7 +1118,21 @@ class _LMState:
         if int(self.pos_host.max()) + n > self.cos.shape[0]:
             raise IndexError(f"position {int(self.pos_host.max()) + n - 1} is beyond block_size = {self.cos.shape[0]} "
                              "(RoPE table exhausted; reset the stream or raise Config.block_size)")
+        if self.pages is not None:
+            # paged scope: an active stream writes only where it holds pages (held streams advance nothing)
+            act = np.flatnonzero(self.active_host)
+            self.pages.check(act, self.pos_host[act], n)
         self.pos_host += n * self.active_host
+
+    def upload_pages(self, streams) -> None:
+        """Copy the listed streams' rows of the host page table to the device table (stream-ordered: frames already
+        enqueued read the old rows, later ones the new; outside any graph, so a captured frame keeps serving).  The rows
+        go through pinned copies, so the host does not wait for the frames in flight."""
+        if len(streams):
+            idx = np.asarray(streams, dtype=np.int64)
+            dev = self.page_table.device
+            rows = torch.from_numpy(self.pages.table[idx]).pin_memory().to(dev, non_blocking=True)
+            self.page_table.index_copy_(0, torch.from_numpy(idx).pin_memory().to(dev, non_blocking=True), rows)
 
     def set_active(self, mask):
         """mask [B]: streams with 0 are held by the next steps (they run through the kernels, but their position does not
@@ -1011,6 +1163,9 @@ class _LMState:
         # than MAX_ROWS streams go one position per pass through the decode state).
         # A multi-position chunk appends all its keys before any of its queries run, so it must not overwrite a ring slot
         # one of those queries still needs: tn > 1 only while the ring does not wrap inside the chunk.
+        if self.pages is not None:   # the whole prefill fits each active stream's reservation, or nothing is launched
+            act = np.flatnonzero(self.active_host)
+            self.pages.check(act, self.pos_host[act], T)
         outs, logits = [], []
         per = max(1, MAX_ROWS // B)
         t = 0
@@ -1054,6 +1209,8 @@ class _LMState:
             if int(self.pos_host[s]) + p.shape[1] > self.cos.shape[0]:
                 raise IndexError(f"position {int(self.pos_host[s]) + p.shape[1] - 1} of stream {s} is beyond block_size = "
                                  f"{self.cos.shape[0]} (RoPE table exhausted; reset the stream or raise Config.block_size)")
+            if self.pages is not None:
+                self.pages.check([s], [self.pos_host[s]], p.shape[1])
             if p.shape[1] > 0:
                 todo.append([s, p.to(device=dev, dtype=torch.int64).t(), 0])
         while todo:

@@ -35,13 +35,14 @@ import argparse
 import os
 import sys
 from collections import defaultdict
-from typing import Dict, Iterable, Tuple
+from typing import Dict, Iterable, Optional, Tuple
 
 import numpy as np
 import torch
 
 from .audio import Resample
 from .codec import MimiCodec
+from .lm import kv_pages_for_budget
 
 
 def _as_row(wav: torch.Tensor) -> torch.Tensor:
@@ -177,10 +178,13 @@ def reconstruct_corpus(codec: MimiCodec, src: str, dst: str, capacity: int = 128
 
 
 @torch.no_grad()
-def synthesize(imp, corpus: Dict[str, torch.Tensor], capacity: int = 32, seeds=None) -> Dict[str, torch.Tensor]:
-    """{utt_id: int16 [8, T]} for every utterance of `corpus` ({utt_id: int64 [9, L]}), through imp.generate_many."""
+def synthesize(imp, corpus: Dict[str, torch.Tensor], capacity: int = 32, seeds=None,
+               kv_gb: Optional[float] = None) -> Dict[str, torch.Tensor]:
+    """{utt_id: int16 [8, T]} for every utterance of `corpus` ({utt_id: int64 [9, L]}), through imp.generate_many.
+    kv_gb: the KV cache's budget in GiB (a pool of floor(kv_gb * 2^30 / kv_page_bytes) pages); None: a whole ring per row."""
     items = ((utt, torch.as_tensor(seq, dtype=torch.int64)) for utt, seq in corpus.items())
-    return {utt: codes.to(torch.int16).cpu() for utt, codes in imp.generate_many(items, capacity, seeds=seeds)}
+    kv_pages = None if kv_gb is None else kv_pages_for_budget(imp.model.config, kv_gb)
+    return {utt: codes.to(torch.int16).cpu() for utt, codes in imp.generate_many(items, capacity, seeds=seeds, kv_pages=kv_pages)}
 
 
 @torch.no_grad()
@@ -198,6 +202,13 @@ def write_codes_wav(codec: MimiCodec, codes: Dict[str, torch.Tensor], dst: str, 
             for u, w in zip(part, wav):
                 write_wav(os.path.join(dst, f"{u}_sample.wav"), w[0], codec.sample_rate)
     return sum(len(u) for u in by_len.values())
+
+
+def _positive_float(text: str) -> float:
+    v = float(text)
+    if not (v > 0 and np.isfinite(v)):
+        raise argparse.ArgumentTypeError(f"must be a positive number (got {text})")
+    return v
 
 
 def _load_gpt(config_path: str, checkpoint: str, device: str):
@@ -220,7 +231,7 @@ def _synthesize_cli(args) -> int:
     if args.top_p or args.top_p_text:
         imp.sampling()   # validates a nucleus run's settings before the model runs
     corpus = torch.load(args.input, map_location="cpu")
-    codes = synthesize(imp, corpus, args.capacity)
+    codes = synthesize(imp, corpus, args.capacity, kv_gb=args.kv_gb)
     save_tokens(codes, args.output_file)
     print(f"synthesized {len(codes)} utterances -> {args.output_file}")
     if args.wav_dir:
@@ -320,6 +331,9 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--checkpoint", required=True, help="training checkpoint ({'model': state_dict})")
     p.add_argument("--output-file", required=True, help="torch.save'd dict utt_id -> int16 [8, T]")
     p.add_argument("--capacity", type=int, default=32, help="utterances decoded together (<= 256)")
+    p.add_argument("--kv-gb", type=_positive_float, default=None,
+                   help="KV cache budget in GiB: each utterance holds pages for only the positions it writes and waits for "
+                        "pages when the budget is spent (default: a whole context ring per row)")
     p.add_argument("--use-sampling", action=argparse.BooleanOptionalAction, default=True,
                    help="sample (the reference hard-codes this); --no-use-sampling decodes by argmax")
     p.add_argument("--temp", type=float, default=0.8)

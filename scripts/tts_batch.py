@@ -3,13 +3,17 @@
 
   * frames/s and tokens/s (9 tokens per generated frame: text + 8 audio) of the whole corpus at each capacity;
   * row occupancy: generated frames / (decode steps x capacity);
+  * the paged KV pool of each run (--kv-gb: a pool of floor(X * 2^30 / kv_page_bytes) pages shared by every capacity;
+    without it each capacity gets a whole ring per row) and the frames run while an utterance waited for pages;
+  * whether every capacity produced the same codes;
   * the share of the time spent in ragged prefill (GPT.prefill_streams), timed with device events;
   * the ceiling: uniform InferenceImp.generate at B = 32 (every row the same layout, as cfg4_infer);
   * the serial rate: InferenceImp.generate at B = 1 on a few utterances, extrapolated to the corpus.
 
-usage: python scripts/tts_batch.py [--utts 256] [--capacities 32,48] [--seed 0] [--out FILE]
+usage: python scripts/tts_batch.py [--utts 256] [--capacities 32,48] [--kv-gb X] [--seed 0] [--no-baselines] [--out FILE]
 """
 import argparse
+import hashlib
 import json
 import os
 import sys
@@ -19,7 +23,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from rstnet_b200.infer import InferenceImp   # noqa: E402
-from rstnet_b200.lm import GPT, Config      # noqa: E402
+from rstnet_b200.lm import GPT, KV_PAGE, Config, kv_page_bytes, kv_pages_for_budget   # noqa: E402
 
 TEXT_EMPTY = 128002
 
@@ -68,7 +72,7 @@ class PrefillTimer:
         return sum(a.elapsed_time(b) for a, b in self.events) * 1e-3
 
 
-def run_many(imp, items, capacity, dev):
+def run_many(imp, items, capacity, dev, kv_pages=None):
     m = imp.model
     steps = [0]
     orig = m.forward_step
@@ -82,13 +86,14 @@ def run_many(imp, items, capacity, dev):
         with PrefillTimer(m) as pt:
             torch.cuda.synchronize()
             t0 = time.perf_counter()
-            out = dict(imp.generate_many(((u, s.to(dev)) for u, s in items), capacity))
+            stats = {}
+            out = dict(imp.generate_many(((u, s.to(dev)) for u, s in items), capacity, kv_pages=kv_pages, stats=stats))
             torch.cuda.synchronize()
             wall = time.perf_counter() - t0
             prefill = pt.seconds()
     finally:
         del m.forward_step
-    return out, wall, prefill, steps[0]
+    return out, wall, prefill, steps[0], stats
 
 
 def main():
@@ -97,6 +102,9 @@ def main():
     ap.add_argument("--capacities", default="32,48")
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--serial-utts", type=int, default=3)
+    ap.add_argument("--kv-gb", type=float, default=None, help="KV budget in GiB, the same paged pool at every capacity")
+    ap.add_argument("--baselines", action=argparse.BooleanOptionalAction, default=True,
+                    help="also time uniform generate at B = 32 and serial B = 1")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -107,7 +115,8 @@ def main():
     items = corpus(args.utts, args.seed)
     frames = sum(int((s[0] == TEXT_EMPTY).sum()) for _, s in items)
     res = {"model": "7B shapes, random init, bf16, context 2048", "utterances": len(items), "generated_frames": frames,
-           "gpu": torch.cuda.get_device_name(dev), "batched": {}}
+           "gpu": torch.cuda.get_device_name(dev), "batched": {}, "kv_page_positions": KV_PAGE,
+           "kv_page_bytes": kv_page_bytes(m.config), "kv_gb": args.kv_gb}
     try:
         import subprocess
         res["power_limit"] = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"],
@@ -116,12 +125,23 @@ def main():
         res["power_limit"] = f"unknown ({e})"
     # warm-up (plans, chunk states, the frame graph of each width) on the corpus' prompts with 8 frames to generate
     warm = [(u, s[:, :s.shape[1] - int((s[0] == TEXT_EMPTY).sum()) + 8]) for u, s in items]
+    pool = None if args.kv_gb is None else kv_pages_for_budget(m.config, args.kv_gb)
+    digests = set()
     for cap in [int(c) for c in args.capacities.split(",")]:
-        run_many(imp, warm[:2 * cap], cap, dev)
-        _, wall, prefill, steps = run_many(imp, items, cap, dev)
+        run_many(imp, warm[:2 * cap], cap, dev, pool)
+        out, wall, prefill, steps, stats = run_many(imp, items, cap, dev, pool)
+        digest = hashlib.sha256(b"".join(out[u].cpu().numpy().tobytes() for u, _ in items)).hexdigest()
+        digests.add(digest)
         res["batched"][str(cap)] = {"seconds": wall, "frames_per_s": frames / wall, "tokens_per_s": 9 * frames / wall,
                                     "decode_steps": steps, "row_occupancy": frames / (steps * cap),
-                                    "prefill_share": prefill / wall}
+                                    "prefill_share": prefill / wall, "wait_frames": stats["wait_frames"],
+                                    "kv_pages": pool if pool is not None else cap * -(-m.config.context // KV_PAGE),
+                                    "codes_sha256": digest}
+        del out
+        torch.cuda.empty_cache()
+    res["codes_identical_across_capacities"] = len(digests) == 1
+    if not args.baselines:
+        return finish(res, args.out)
     # ceiling: every row the same layout (cfg4_infer's shape), B = 32
     P, G, B = 70, 550, 32
     seq = items[0][1][:, :P + G].clone()
@@ -148,10 +168,14 @@ def main():
     wall = time.perf_counter() - t0
     res["serial_B1_extrapolated"] = {"measured_utterances": len(sub), "frames_per_s": sub_frames / wall,
                                      "tokens_per_s": 9 * sub_frames / wall, "corpus_seconds_extrapolated": frames / (sub_frames / wall)}
+    finish(res, args.out)
+
+
+def finish(res, out):
     line = json.dumps(res)
     print(line)
-    if args.out:
-        with open(args.out, "w") as f:
+    if out:
+        with open(out, "w") as f:
             f.write(line + "\n")
 
 

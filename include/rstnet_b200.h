@@ -82,7 +82,8 @@ int rstnet_gemm_rows_f32(const rstnet_gemm_rows_args* args, rstnet_stream_t stre
  * rstnet_tc_gemm_create) is applied to A in registers as the operand fragments are built.
  * precision 0 = 3xTF32 split (fp32-equivalent, for RVQ-index exactness; W must already be rounded to
  * TF32 and W_lo = tf32(w - W) supplied -- see rstnet_tf32_split_f32), 1 = single TF32 pass.
- * The kernel is persistent (at most one CTA per SM walking the 128 x 32 or 128 x 64 output tiles).  ELU, as pre- and
+ * The kernel is persistent (at most one CTA per SM walking the 128 x 32 or 128 x 64 output tiles, or 64-row tiles in
+ * K-pair mode, below).  ELU, as pre- and
  * post-activation, is evaluated with ex2.approx.
  * Same reference call sites as rstnet_gemm_rows_f32. */
 typedef struct rstnet_tc_plan rstnet_tc_plan;
@@ -109,8 +110,17 @@ typedef struct {
 int rstnet_tc_gemm_create(const rstnet_tc_gemm_desc* desc, rstnet_tc_plan** out);
 int rstnet_tc_gemm_run(const rstnet_tc_plan* plan, rstnet_stream_t stream);
 void rstnet_tc_gemm_destroy(rstnet_tc_plan* plan);
-/* the plan's tile grid: M tiles (I tiles x O_out), N tiles, tile width */
+/* the plan's tile grid: 128-row M tiles (I tiles x O_out), N tiles, tile width */
 int rstnet_tc_gemm_grid(const rstnet_tc_plan* plan, int32_t* grid_x, int32_t* grid_y, int32_t* tile_n);
+/* K-pair mode: 64-row tiles whose promotion chunks (K = 128) alternate between the CTA's two consumer warpgroups, one
+ * warpgroup adding the other's chunk sums in chunk order, so the output is bit-identical to the 128-row form.
+ * rstnet_tc_gemm_create picks it for the few-tile, long-K launches: when the 128-row tiles fit in one round of the
+ * SMs (tiles128 <= SMs) and
+ *   ceil(tiles64 / SMs) * ceil(chunks / 2) * 4  <  taps * Kc / 32
+ * (rounds times serial K stages per tile); a tie keeps 128-row tiles.  rstnet_tc_gemm_create_ex takes the choice explicitly:
+ * kpair = -1 (the same rule), 0 (128-row tiles) or 1 (K-pair).  rstnet_tc_gemm_kpair reports the plan's mode. */
+int rstnet_tc_gemm_create_ex(const rstnet_tc_gemm_desc* desc, int32_t kpair, rstnet_tc_plan** out);
+int rstnet_tc_gemm_kpair(const rstnet_tc_plan* plan, int32_t* on);
 /* ---- one SEANet residual block (modules/seanet.py SEANetResnetBlock, kernel 3, compress 2) of C = 64 or 128 channels
  * on the tensor cores, as one plan and one launch:
  *   h[i, t] = ELU(b1 + sum_{tap<3} W1[:, tap*C:(tap+1)*C] ELU(y[i, t - 2 + tap]))        (C -> C/2)

@@ -17,6 +17,7 @@ ACT_NONE, ACT_ELU, ACT_GELU = 0, 1, 2
 SYMBOLS = [
     "rstnet_version", "rstnet_last_error", "rstnet_launch_count", "rstnet_device_error_flags",
     "rstnet_gemm_rows_f32", "rstnet_tc_gemm_create", "rstnet_tc_gemm_run", "rstnet_tc_gemm_destroy", "rstnet_tc_gemm_grid",
+    "rstnet_tc_gemm_create_ex", "rstnet_tc_gemm_kpair",
     "rstnet_tc_resblock_create", "rstnet_tc_resblock_run", "rstnet_tc_resblock_destroy", "rstnet_tf32_split_f32", "rstnet_conv1d_cin1_f32", "rstnet_conv1d_cout1_f32",
     "rstnet_convtr1d_depthwise_f32", "rstnet_rows_fill_f32", "rstnet_rows_copy_table_f32",
     "rstnet_counter_add", "rstnet_layer_norm_f32", "rstnet_rope_kv_append_f32",
@@ -111,6 +112,8 @@ def lib() -> C.CDLL:
     L.rstnet_tc_gemm_destroy.argtypes = [vp]
     L.rstnet_tc_gemm_destroy.restype = None
     L.rstnet_tc_gemm_grid.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)]
+    L.rstnet_tc_gemm_create_ex.argtypes = [C.POINTER(TcGemmDesc), i32, C.POINTER(C.c_void_p)]
+    L.rstnet_tc_gemm_kpair.argtypes = [vp, C.POINTER(i32)]
     L.rstnet_tc_resblock_create.argtypes = [C.POINTER(TcResblockDesc), C.POINTER(C.c_void_p)]
     L.rstnet_tc_resblock_run.argtypes = [vp, vp]
     L.rstnet_tc_resblock_destroy.argtypes = [vp]

@@ -16,6 +16,14 @@
 // (hi only; the tensor core reads the top 19 bits of the fp32 weights).
 // Every chunk of TC_CHUNK_STAGES stages (K = 128) starts fresh wgmma accumulators that are then added into fp32 registers
 // with round-to-nearest, so the error of the tensor core's internal accumulation is bounded by one chunk, whatever K is.
+//
+// K-pair mode (a per-plan choice for launches with too few 128-row tiles to fill the SMs and a long K): a tile is 64 x BN
+// and both consumer warpgroups hold the same 64 rows.  Warpgroup 0 computes the promotion chunks 0, 2, 4, ..., warpgroup
+// 1 the chunks 1, 3, 5, ... and hands each chunk's d0 + d1, thread for thread, to warpgroup 0 through a two-slot
+// shared-memory queue.  Warpgroup 0 adds the chunks into acc in chunk order, so every fp32 addition into acc is the one
+// the 128-row mode makes and the output is bit-identical; it alone runs the epilogue.  The stage ring is split into one
+// ring of S / 2 slots per warpgroup (a warpgroup that skipped the other's stages in one shared ring could wait on a
+// slot two phases ahead), and the queue lives in the A halves the 64-row boxes leave unused.
 #include <cstdlib>
 
 #include "common.cuh"
@@ -47,6 +55,7 @@ struct TcParams {
   int taps, tap_di, tap_do, o_mul, kchunks;
   int pre_act, post_act, i_tiles;
   int m_tiles, n_tiles;  // (I tiles x O_out) and N tiles
+  int kpair;             // 1: 64-row tiles, promotion chunks alternating between the consumer warpgroups (host side)
 };
 
 template <int BN, int PREC>
@@ -56,6 +65,10 @@ struct TcCfg {
   static constexpr int STAGE_BYTES = TC_A_BYTES + B_BYTES * (SPLIT ? 2 : 1);
   static constexpr int STAGES = (200 * 1024 / STAGE_BYTES) > 8 ? 8 : (200 * 1024 / STAGE_BYTES);
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  // K-pair queue: a slot holds a 64 x BN fp32 chunk in Q_PIECES 8 KB pieces, piece h of slot q in the unused second half
+  // of stage slot q * Q_PIECES + h's A tile
+  static constexpr int Q_PIECES = BN / 32;
+  static_assert(STAGES % 2 == 0 && 2 * Q_PIECES <= STAGES, "K-pair rings and queue");
 };
 
 // round-to-nearest (ties away) TF32 on the integer pipe: add half an ulp of the 10-bit mantissa to
@@ -134,7 +147,10 @@ __device__ __forceinline__ void tc_mma_stage(float (&d0)[BN / 2], float (&d1)[BN
   }
 }
 
-template <int BN, int PREC, bool PRE_ELU>
+// KP: K-pair mode.  A template parameter, so that the 128-row form carries none of K-pair's branches (as a runtime flag
+// they cost it about 10 %); the promotion adds and the epilogue are the same source in both forms, and
+// tests/test_gemm_tc_kpair_gpu.py holds the two to equal bits.
+template <int BN, int PREC, bool PRE_ELU, bool KP>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
                const __grid_constant__ CUtensorMap tmWlo, const TcParams p) {
@@ -147,15 +163,23 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   // would demote every later access through `smem` to generic LD / ST)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + S * Cfg::STAGE_BYTES);   // [S] TMA landed
-  uint64_t* empty = full + S;                                                  // [S] every consumer warp is done with it
+  uint64_t* empty = full + S;                                                  // [S] every consumer warp reading it is done
+  uint64_t* qfull = empty + S;                                                 // [2] K-pair: warpgroup 1's chunk is in the slot
+  uint64_t* qempty = qfull + 2;                                                // [2] K-pair: warpgroup 0 has added it
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   const int total_k = p.taps * p.kchunks;
   const int total_tiles = p.m_tiles * p.n_tiles;
+  const int bm = KP ? TC_BM / 2 : TC_BM;   // tile rows
+  const int R = KP ? S / 2 : S;            // slots per ring: K-pair, slots [0, S/2) feed warpgroup 0, the rest 1
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < S; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], TC_CONSUMER_WARPS);
+      mbar_init(&empty[s], KP ? TC_CONSUMER_WARPS / 2 : TC_CONSUMER_WARPS);   // K-pair: one warpgroup reads a stage
+    }
+    for (int q = 0; q < 2; ++q) {
+      mbar_init(&qfull[q], 128);
+      mbar_init(&qempty[q], 128);
     }
     fence_barrier_init();
   }
@@ -167,16 +191,21 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       tma_prefetch_desc(&tmA);
       tma_prefetch_desc(&tmW);
       if (Cfg::SPLIT) tma_prefetch_desc(&tmWlo);
-      int g = 0;
+      int pos0 = 0, ph0 = 0, pos1 = 0, ph1 = 0;   // next slot and its phase parity, per ring
       for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
         const int nt = t % p.n_tiles, mt = t / p.n_tiles;
-        const int i0 = (mt % p.i_tiles) * TC_BM, ot = mt / p.i_tiles, n0 = nt * BN;
-        for (int kit = 0; kit < total_k; ++kit, ++g) {
-          const int s = g % S;
-          mbar_wait(&empty[s], ((g / S) & 1) ^ 1);
+        const int i0 = (mt % p.i_tiles) * bm, ot = mt / p.i_tiles, n0 = nt * BN;
+        for (int kit = 0; kit < total_k; ++kit) {
+          const int w = KP ? (kit / TC_CHUNK_STAGES) & 1 : 0;   // the ring of the warpgroup that reads the stage
+          const int pos = w ? pos1 : pos0, ph = w ? ph1 : ph0;
+          const int s = w * R + pos;
+          const int npos = pos + 1 == R ? 0 : pos + 1, nph = ph ^ (npos == 0);
+          if (w) { pos1 = npos; ph1 = nph; } else { pos0 = npos; ph0 = nph; }
+          mbar_wait(&empty[s], ph ^ 1);
           const int tap = kit / p.kchunks, kc = kit % p.kchunks;
           uint8_t* st = smem + s * Cfg::STAGE_BYTES;
-          mbar_arrive_expect_tx(&full[s], Cfg::STAGE_BYTES);
+          // the A box is bm rows (the plan's tensor map); in K-pair mode the slot's second 64 A rows stay unused
+          mbar_arrive_expect_tx(&full[s], Cfg::STAGE_BYTES - (TC_BM - bm) * 128);
           tma_load_3d(st, &tmA, &full[s], kc * TC_BKE, i0 + tap * p.tap_di, ot * p.o_mul + tap * p.tap_do);
           tma_load_2d(st + TC_A_BYTES, &tmW, &full[s], kit * TC_BKE, n0);   // tap * Kc + kc * 32 == kit * 32
           if (Cfg::SPLIT) tma_load_2d(st + TC_A_BYTES + Cfg::B_BYTES, &tmWlo, &full[s], kit * TC_BKE, n0);
@@ -188,9 +217,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 
   // ================= consumers.  Thread (warp wq of warpgroup wg, lane = 4 gq + tq) holds A rows r0 and r0 + 8 of the
   // tile, columns tq and tq + 4 of every 8-wide K step (the wgmma register fragment); the accumulator fragment covers the
-  // same two rows, columns 8 b + 2 tq and 8 b + 2 tq + 1 of every 8-column block b.
+  // same two rows, columns 8 b + 2 tq and 8 b + 2 tq + 1 of every 8-column block b.  In K-pair mode both warpgroups
+  // hold rows 0..63, so thread t of warpgroup 1 holds the accumulator elements of thread t of warpgroup 0.
   const int wg = warp / 4, wq = warp % 4, gq = lane / 4, tq = lane % 4;
-  const int r0 = wg * 64 + wq * 16 + gq;
+  const int r0 = (KP ? 0 : wg * 64) + wq * 16 + gq;
   // element (r, c) of a stage's swizzled [128][32] fp32 A tile sits at byte r * 128 + ((c / 4) ^ (r % 8)) * 16 + (c % 4) * 4;
   // rows r0 and r0 + 8 share r % 8
   const uint32_t a_row = (uint32_t)r0 * 128u + (uint32_t)tq * 4u, a_sw = (uint32_t)(r0 & 7);
@@ -198,20 +228,39 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   float acc[NR], d0[NR], d1[NR];
 #pragma unroll
   for (int j = 0; j < NR; ++j) d0[j] = d1[j] = 0.f;
-  int g = 0;
+  const int nch = (total_k + CH - 1) / CH;
+  const bool sender = KP && wg == 1;   // K-pair: this warpgroup's chunks go through the queue
+  // this thread's element j of queue slot q: 8 KB pieces of 16 x 128 fp32, element j * 128 + (thread in warpgroup)
+  auto qel = [&](int q, int j) {
+    return reinterpret_cast<float*>(smem + (q * Cfg::Q_PIECES + j / 16) * Cfg::STAGE_BYTES + TC_A_BYTES / 2) +
+           (j % 16) * 128 + (threadIdx.x & 127);
+  };
+  int qn = 0;                               // chunks queued so far (slot qn & 1, use qn >> 1 of it)
+  // warpgroup 0 adds the chunk warpgroup 1 queued, as acc += (d0 + d1) of that chunk
+  auto take_queued = [&]() {
+    mbar_wait(&qfull[qn & 1], (qn >> 1) & 1);
+#pragma unroll
+    for (int j = 0; j < NR; ++j) acc[j] += *qel(qn & 1, j);
+    mbar_arrive(&qempty[qn & 1]);
+    ++qn;
+  };
+  // this warpgroup's ring: every stage in the 128-row mode, its own chunks' stages in K-pair mode
+  const int base = KP ? wg * R : 0;
+  int pos = 0, ph = 0;
   for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
     const int nt = t % p.n_tiles, mt = t / p.n_tiles;
-    const int i0 = (mt % p.i_tiles) * TC_BM, ot = mt / p.i_tiles, n0 = nt * BN;
+    const int i0 = (mt % p.i_tiles) * bm, ot = mt / p.i_tiles, n0 = nt * BN;
 #pragma unroll
     for (int j = 0; j < NR; ++j) acc[j] = 0.f;
     // K in chunks of up to CH stages, each chunk's accumulators promoted after it.  Every wgmma wait sits outside any
     // branch, so ptxas needs no serialising warpgroup waits of its own.  The two consumer warpgroups overlap each other:
     // one builds fragments while the other's wgmmas run.
-    for (int k0 = 0; k0 < total_k; k0 += CH) {
+    for (int c = KP ? wg : 0; c < nch; c += KP ? 2 : 1) {
+      const int k0 = c * CH;
       const int nst = total_k - k0 < CH ? total_k - k0 : CH;
-      for (int u = 0; u < nst; ++u, ++g) {
-        const int s = g % S;
-        mbar_wait(&full[s], (g / S) & 1);
+      for (int u = 0; u < nst; ++u) {
+        const int s = base + pos;
+        mbar_wait(&full[s], ph);
         const uint32_t st = smem0 + (uint32_t)(s * Cfg::STAGE_BYTES);
         uint32_t ah[4][4], al[4][4];
         tc_build_a<Cfg::SPLIT, PRE_ELU>(st, a_row, a_sw, ah, al);
@@ -224,12 +273,25 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         wgmma_wait<0>();
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty[s]);   // this warp's wgmmas have read the stage
+        pos = pos + 1 == R ? 0 : pos + 1;
+        ph ^= pos == 0;
       }
       fence_acc(d0);
       if (Cfg::SPLIT) fence_acc(d1);
+      if (sender) {
+        mbar_wait(&qempty[qn & 1], ((qn >> 1) & 1) ^ 1);
 #pragma unroll
-      for (int j = 0; j < NR; ++j) acc[j] += Cfg::SPLIT ? d0[j] + d1[j] : d0[j];
+        for (int j = 0; j < NR; ++j) *qel(qn & 1, j) = Cfg::SPLIT ? d0[j] + d1[j] : d0[j];
+        mbar_arrive(&qfull[qn & 1]);
+        ++qn;
+      } else {
+        if (KP && c > 0) take_queued();   // chunk c - 1 first
+#pragma unroll
+        for (int j = 0; j < NR; ++j) acc[j] += Cfg::SPLIT ? d0[j] + d1[j] : d0[j];
+      }
     }
+    if (KP && !sender && nch % 2 == 0) take_queued();   // the tile's last chunk is warpgroup 1's
+    if (sender) continue;   // warpgroup 0 writes the tile
     // ---- epilogue: bias, LayerScale, residual, activation -> global (8-byte stores: 4 lanes = one 32-byte sector)
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -512,18 +574,26 @@ struct rstnet_tc_plan {
   int bn, prec;
 };
 
-template <int BN, int PREC, bool PRE_ELU>
+template <int BN, int PREC, bool PRE_ELU, bool KP>
 static int tc_launch(const rstnet_tc_plan* pl, cudaStream_t st) {
   using Cfg = TcCfg<BN, PREC>;
   static unsigned long long attr = 0;
-  smem_optin(gemm_tc_kernel<BN, PREC, PRE_ELU>, Cfg::SMEM_BYTES, attr);
-  gemm_tc_kernel<BN, PREC, PRE_ELU><<<pl->grid, TC_THREADS, Cfg::SMEM_BYTES, st>>>(pl->tmA, pl->tmW, pl->tmWlo, pl->p);
+  smem_optin(gemm_tc_kernel<BN, PREC, PRE_ELU, KP>, Cfg::SMEM_BYTES, attr);
+  gemm_tc_kernel<BN, PREC, PRE_ELU, KP><<<pl->grid, TC_THREADS, Cfg::SMEM_BYTES, st>>>(pl->tmA, pl->tmW, pl->tmWlo, pl->p);
   count_launch();
   return check_launch("gemm_tc");
 }
 
-extern "C" int rstnet_tc_gemm_create(const rstnet_tc_gemm_desc* d, rstnet_tc_plan** out) {
+template <int BN, int PREC>
+static int tc_launch_mode(const rstnet_tc_plan* pl, cudaStream_t st) {
+  const bool elu = pl->p.pre_act == ACT_ELU;
+  if (pl->p.kpair) return elu ? tc_launch<BN, PREC, true, true>(pl, st) : tc_launch<BN, PREC, false, true>(pl, st);
+  return elu ? tc_launch<BN, PREC, true, false>(pl, st) : tc_launch<BN, PREC, false, false>(pl, st);
+}
+
+extern "C" int rstnet_tc_gemm_create_ex(const rstnet_tc_gemm_desc* d, int32_t kpair, rstnet_tc_plan** out) {
   RSTNET_REQUIRE(d && out, "tc_gemm_create: null argument");
+  RSTNET_REQUIRE(kpair >= -1 && kpair <= 1, "tc_gemm_create: kpair must be -1 (auto), 0 or 1 (got %d)", kpair);
   RSTNET_REQUIRE(d->A && d->W && d->C, "tc_gemm_create: null tensor pointer");
   RSTNET_REQUIRE(d->precision != 0 || d->W_lo, "tc_gemm_create: precision 0 (3xTF32) needs W_lo");
   RSTNET_REQUIRE(d->Kc > 0 && d->Kc % TC_BKE == 0, "tc_gemm_create: Kc (%d) must be a multiple of %d", d->Kc, TC_BKE);
@@ -550,10 +620,22 @@ extern "C" int rstnet_tc_gemm_create(const rstnet_tc_gemm_desc* d, rstnet_tc_pla
     if (pl->bn == 64 && ((t32 + sms - 1) / sms) * 2 <= ((t64 + sms - 1) / sms) * 3) pl->bn = 32;
   }
   pl->prec = d->precision;
+  const int n_tiles = ceil_div(N, pl->bn);
+  if (kpair < 0) {
+    // K-pair (64-row tiles, the promotion chunks split between the two consumer warpgroups) for the few-tile, long-K
+    // launches: when the 128-row tiles fit in one round of the SMs and K-pair takes fewer rounds times serial K stages.
+    // A tie keeps 128-row tiles.  Past one round the per-tile cost decides: at 3 840 tiles of K = 256 (the 12.5 kHz
+    // decoder's transposed conv) the rule alone would pick K-pair, which ran 1.6x slower there.
+    const long long total_k = (long long)d->taps * (d->Kc / TC_BKE);
+    const long long t128 = (long long)i_tiles * d->O_out * n_tiles, t64 = (long long)ceil_div(d->I_out, TC_BM / 2) * d->O_out * n_tiles;
+    const long long pair_k = (total_k + 2 * TC_CHUNK_STAGES - 1) / (2 * TC_CHUNK_STAGES) * TC_CHUNK_STAGES;
+    kpair = t128 <= sms && ((t64 + sms - 1) / sms) * pair_k < total_k;
+  }
+  const int bm = kpair ? TC_BM / 2 : TC_BM;
   {
     cuuint64_t gdim[3] = {(cuuint64_t)d->a_c_extent, (cuuint64_t)d->a_i_extent, (cuuint64_t)d->a_o_extent};
     cuuint64_t gstr[2] = {(cuuint64_t)d->a_i_stride * 4, (cuuint64_t)d->a_o_stride * 4};
-    cuuint32_t box[3] = {TC_BKE, TC_BM, 1};
+    cuuint32_t box[3] = {TC_BKE, (cuuint32_t)bm, 1};
     cuuint32_t estr[3] = {1, 1, 1};
     CUresult r = enc(&pl->tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, (void*)d->A, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -588,25 +670,26 @@ extern "C" int rstnet_tc_gemm_create(const rstnet_tc_gemm_desc* d, rstnet_tc_pla
   p.bias = d->bias; p.scale = d->scale; p.n_split = d->n_split;
   p.I_out = d->I_out; p.O_out = d->O_out; p.N = N; p.Kc = d->Kc;
   p.taps = d->taps; p.tap_di = d->tap_di; p.tap_do = d->tap_do; p.o_mul = d->o_mul; p.kchunks = d->Kc / TC_BKE;
-  p.pre_act = d->pre_act; p.post_act = d->post_act; p.i_tiles = i_tiles;
-  p.m_tiles = i_tiles * d->O_out;
-  p.n_tiles = ceil_div(N, pl->bn);
+  p.pre_act = d->pre_act; p.post_act = d->post_act;
+  p.kpair = kpair;
+  p.i_tiles = ceil_div(d->I_out, bm);
+  p.m_tiles = p.i_tiles * d->O_out;
+  p.n_tiles = n_tiles;
   const long long tiles = (long long)p.m_tiles * p.n_tiles;
   pl->grid = dim3((unsigned)(tiles < sms ? tiles : sms));
   *out = pl;
   return 0;
 }
 
+extern "C" int rstnet_tc_gemm_create(const rstnet_tc_gemm_desc* d, rstnet_tc_plan** out) {
+  return rstnet_tc_gemm_create_ex(d, -1, out);
+}
+
 extern "C" int rstnet_tc_gemm_run(const rstnet_tc_plan* pl, rstnet_stream_t stream) {
   RSTNET_REQUIRE(pl != nullptr, "tc_gemm_run: null plan");
   cudaStream_t st = (cudaStream_t)stream;
-  const bool elu = pl->p.pre_act == ACT_ELU;
-  if (pl->prec == 0) {
-    if (pl->bn == 64) return elu ? tc_launch<64, 0, true>(pl, st) : tc_launch<64, 0, false>(pl, st);
-    return elu ? tc_launch<32, 0, true>(pl, st) : tc_launch<32, 0, false>(pl, st);
-  }
-  if (pl->bn == 64) return elu ? tc_launch<64, 1, true>(pl, st) : tc_launch<64, 1, false>(pl, st);
-  return elu ? tc_launch<32, 1, true>(pl, st) : tc_launch<32, 1, false>(pl, st);
+  if (pl->prec == 0) return pl->bn == 64 ? tc_launch_mode<64, 0>(pl, st) : tc_launch_mode<32, 0>(pl, st);
+  return pl->bn == 64 ? tc_launch_mode<64, 1>(pl, st) : tc_launch_mode<32, 1>(pl, st);
 }
 
 extern "C" void rstnet_tc_gemm_destroy(rstnet_tc_plan* pl) { delete pl; }
@@ -690,7 +773,12 @@ extern "C" int rstnet_tc_resblock_run(const rstnet_tc_resblock_plan* pl, rstnet_
 extern "C" void rstnet_tc_resblock_destroy(rstnet_tc_resblock_plan* pl) { delete pl; }
 extern "C" int rstnet_tc_gemm_grid(const rstnet_tc_plan* pl, int32_t* gx, int32_t* gy, int32_t* bn) {
   if (!pl) return 1;
-  *gx = pl->p.m_tiles; *gy = pl->p.n_tiles; *bn = pl->bn;
+  *gx = ceil_div(pl->p.I_out, TC_BM) * pl->p.O_out; *gy = pl->p.n_tiles; *bn = pl->bn;
+  return 0;
+}
+extern "C" int rstnet_tc_gemm_kpair(const rstnet_tc_plan* pl, int32_t* on) {
+  if (!pl) return 1;
+  *on = pl->p.kpair;
   return 0;
 }
 

@@ -295,6 +295,42 @@ int rstnet_resample_f32(const float* x, int64_t x_row_stride, int64_t x_len, int
                         const int32_t* start, int32_t n, int32_t o, int32_t S, int32_t start_max, float* out,
                         int64_t out_row_stride, int64_t out_len, int32_t rows, rstnet_stream_t stream);
 
+/* ---- codec evaluation over ragged batches of clips.  Clip c of a pack is ref[offsets[c] .. + lengths[c]) and
+ * deg[offsets[c] .. + lengths[c]) (device fp32 buffers, device int64 offsets / lengths; the length is already
+ * min(len_ref, len_deg)).  Each clip is tiled on its own, from its own frame or sample 0, into fp64 partials in `ws`, and
+ * a second launch sums each clip's partials in an order fixed by its length: a clip's sums are the same bytes whatever
+ * else is in the pack, where it sits and what the pack's capacity is.  No atomics.  A clip whose length lies outside the
+ * host's [min_len, max_len] gets NaN sums; so does a clip with a non-finite sample, and no other clip.
+ *
+ * The loss sums of one resolution of STFTLoss (Evaluation/codec/compute_ms_stft_loss.py:17-73): torch.stft(x, n_fft, hop,
+ * win, hann_window(win)) with center=True, reflect padding (t < 0 -> -t, t >= L -> 2(L-1) - t), the window zero-padded
+ * centred to n_fft, onesided; T = sqrt(max(|STFT ref|^2, 1e-7)) ("true"), P the same of deg ("fake").  Frames
+ * f = 0 .. L / hop, bins k = 0 .. n_fft / 2.  For each clip c:
+ *   sums[(c * n_res + res) * 3 + 0] = sum (T - P)^2      (SpectralConvergence numerator squared, :31)
+ *   sums[(c * n_res + res) * 3 + 1] = sum T^2            (its denominator squared, :32)
+ *   sums[(c * n_res + res) * 3 + 2] = sum |log P - log T| (LogSTFTMagnitude, :43-45, before the mean), as 0.5 log of the
+ *                                                          clamped squares
+ * One n_fft-point complex FFT of z = w r + i w d per frame gives both spectra; a frame whose two inputs are equal takes T
+ * for P (so a signal against itself gives sums 0 and 2 of exactly 0).  twiddle: device fp32 [n_fft / 2][2],
+ * (cos, -sin)(2 pi k / n_fft); window: device fp32 [win], torch.hann_window(win) (periodic); both computed in fp64 and
+ * rounded once.  Limits: n_fft a power of two in [64, 4096], 1 <= win <= n_fft, hop >= 1, min_len > n_fft / 2 (torch.stft's
+ * reflect padding), clips <= 65535.  ws: rstnet_stft_loss_workspace(clips, max_len, hop) bytes.  Two launches. */
+#define RSTNET_STFT_FRAMES_PER_BLOCK 16
+int64_t rstnet_stft_loss_workspace(int32_t clips, int64_t max_len, int32_t hop);
+int rstnet_stft_loss_sums_f32(const float* ref, const float* deg, const int64_t* offsets, const int64_t* lengths,
+                              int32_t clips, int64_t min_len, int64_t max_len, int32_t n_fft, int32_t hop, int32_t win,
+                              const float* twiddle, const float* window, double* sums, int32_t n_res, int32_t res,
+                              void* ws, int64_t ws_bytes, rstnet_stream_t stream);
+
+/* The moments of SI-SNR (the metric that Evaluation/codec/compute_sisnr.py:11,21 imports as estimate_si_sdr from a
+ * module the reference does not ship), per clip in fp64: moments[c * 5 + k] = sum r, sum d, sum r^2, sum d^2, sum r d for
+ * k = 0..4 (zeros for an empty clip).  ws: rstnet_sisnr_moments_workspace(clips, max_len) bytes.  Two launches. */
+#define RSTNET_SISNR_SAMPLES_PER_BLOCK 8192
+int64_t rstnet_sisnr_moments_workspace(int32_t clips, int64_t max_len);
+int rstnet_sisnr_moments_f32(const float* ref, const float* deg, const int64_t* offsets, const int64_t* lengths,
+                             int32_t clips, int64_t max_len, double* moments, void* ws, int64_t ws_bytes,
+                             rstnet_stream_t stream);
+
 /* ======================================================================================
  * Speech-text LM decode step (MLLM_v2/models/llama_streaming.py GPT under `with gpt.streaming(B)`),
  * bf16 activations / weights, fp32 accumulation.  One token per stream: rows are streams.

@@ -30,11 +30,15 @@ SYMBOLS = [
     "rstnet_resample_f32", "rstnet_lm_delay_cache_in", "rstnet_lm_delay_cache_out", "rstnet_counter_add_rows",
     "rstnet_lm_cross_entropy_bf16", "rstnet_rows_fill_tail_f32", "rstnet_lm_sample_params_bf16",
     "rstnet_lm_rope_kv_append_paged_bf16", "rstnet_lm_paged_decode_attention_bf16",
+    "rstnet_stft_loss_workspace", "rstnet_stft_loss_sums_f32", "rstnet_sisnr_moments_workspace", "rstnet_sisnr_moments_f32",
 ]
 
 KV_LOG2_PAGE_MIN, KV_LOG2_PAGE_MAX = 4, 12   # RSTNET_KV_LOG2_PAGE_MIN / _MAX: pages of 16 .. 4096 positions
 
 RESAMPLE_MAX_TABLE_BYTES = 48 * 1024   # RSTNET_RESAMPLE_MAX_TABLE_BYTES
+
+STFT_FRAMES_PER_BLOCK = 16             # RSTNET_STFT_FRAMES_PER_BLOCK
+SISNR_SAMPLES_PER_BLOCK = 8192         # RSTNET_SISNR_SAMPLES_PER_BLOCK
 
 
 class GemmRowsArgs(C.Structure):
@@ -162,6 +166,12 @@ def lib() -> C.CDLL:
     L.rstnet_lm_cross_entropy_bf16.argtypes = [vp, i64, i32, i32, i32, vp, vp, vp, vp, i32, vp, vp, vp, vp]
     L.rstnet_lm_sample_params_bf16.argtypes = [vp, i32, i32, i32, vp, i32, i32, f32, f32, vp, vp, vp, i32, C.c_uint32, vp, vp, vp,
                                                vp, i32, vp]
+    L.rstnet_stft_loss_workspace.argtypes = [i32, i64, i32]
+    L.rstnet_stft_loss_workspace.restype = i64
+    L.rstnet_stft_loss_sums_f32.argtypes = [vp, vp, vp, vp, i32, i64, i64, i32, i32, i32, vp, vp, vp, i32, i32, vp, i64, vp]
+    L.rstnet_sisnr_moments_workspace.argtypes = [i32, i64]
+    L.rstnet_sisnr_moments_workspace.restype = i64
+    L.rstnet_sisnr_moments_f32.argtypes = [vp, vp, vp, vp, i32, i64, vp, vp, i64, vp]
     for name in SYMBOLS:
         fn = getattr(L, name)
         if fn.restype is C.c_int and name not in ("rstnet_version",):

@@ -281,8 +281,46 @@ def _load_codec(args) -> MimiCodec:
     return m.to(args.device).eval()
 
 
+def pair_files(ref_dir: str, deg_dir: str):
+    """[(name, ref_path, deg_path)] for every *.wav of deg_dir, paired by basename with ref_dir (compute_ms_stft_loss.py:108,
+    123); a degraded file without a reference is an error that names the files."""
+    names = sorted(n for n in os.listdir(deg_dir) if n.endswith(".wav"))
+    if not names:
+        raise FileNotFoundError(f"found no wavs in {deg_dir}")
+    missing = [n for n in names if not os.path.isfile(os.path.join(ref_dir, n))]
+    if missing:
+        shown = ", ".join(missing[:10]) + (f" and {len(missing) - 10} more" if len(missing) > 10 else "")
+        raise FileNotFoundError(f"{len(missing)} degraded file(s) of {deg_dir} have no reference in {ref_dir}: {shown}")
+    return [(n, os.path.join(ref_dir, n), os.path.join(deg_dir, n)) for n in names]
+
+
+def _evaluate_cli(args) -> int:
+    import json
+    from . import metrics as M
+    pairs = pair_files(args.ref_dir, args.deg_dir)
+
+    def items():
+        for name, rp, dp in pairs:
+            ref, rsr = read_wav(rp)
+            deg, dsr = read_wav(dp)
+            yield name, ref, rsr, deg, dsr
+    capacity = max(1, int(round(args.capacity_seconds * args.sample_rate)))
+    per_clip = dict(M.evaluate_pairs(items(), args.sample_rate, capacity, device=args.device))
+    summary = M.corpus_summary(per_clip)
+    with open(args.output_file, "w") as f:
+        json.dump({"sample_rate": args.sample_rate, "summary": summary, "clips": per_clip}, f, indent=1)
+    print(f"MS-STFT-Loss: {summary['ms_stft']}")
+    print(f"SI-SNR: {summary['sisnr']}")
+    if summary["stft_skipped"] or summary["sisnr_skipped"]:
+        print(f"skipped: {summary['stft_skipped']} clip(s) too short for the STFT loss, {summary['sisnr_skipped']} without an "
+              "SI-SNR (empty or constant reference)", file=sys.stderr)
+    return 0
+
+
 def main(argv=None) -> int:
     args = build_parser().parse_args(argv)
+    if args.cmd == "evaluate":
+        return _evaluate_cli(args)
     if args.cmd == "synthesize":
         return _synthesize_cli(args)
     if args.cmd == "score":
@@ -352,6 +390,15 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--checkpoint", required=True, help="training checkpoint ({'model': state_dict})")
     p.add_argument("--output-file", required=True, help="json file of per-utterance metrics")
     p.add_argument("--capacity", type=int, default=8, help="utterances packed into the same chunks (<= 256)")
+    p.add_argument("--device", default="cuda")
+    p = sub.add_parser("evaluate", help="multi-resolution STFT loss and SI-SNR of degraded wavs against references "
+                                        "(Evaluation/codec/compute_ms_stft_loss.py, compute_sisnr.py)")
+    p.add_argument("--ref-dir", required=True, help="reference wavs")
+    p.add_argument("--deg-dir", required=True, help="degraded wavs, paired with --ref-dir by file name")
+    p.add_argument("--sample-rate", type=int, default=16000, help="both signals are resampled to this rate (default 16000)")
+    p.add_argument("--capacity-seconds", type=_positive_float, default=600.0,
+                   help="audio per launch at --sample-rate (a longer clip runs alone)")
+    p.add_argument("--output-file", default="metrics.json", help="json: per-clip metrics, corpus means, skipped counts")
     p.add_argument("--device", default="cuda")
     return ap
 

@@ -262,3 +262,29 @@ def rvq_decode_gather(codes, E, q, N, T, n_q, ns, dim, bins, time_major=False):
     _cuda(codes, E, q)
     _lib.check(_lib.lib().rstnet_rvq_decode_gather_f32(codes.data_ptr(), E.data_ptr(), q.data_ptr(), N, T, n_q, ns, dim,
                                                        bins, int(time_major), _stream()), "rvq_decode_gather")
+
+
+def stft_loss_workspace(clips, max_len, hop) -> int:
+    return int(_lib.lib().rstnet_stft_loss_workspace(clips, max_len, hop))
+
+
+def stft_loss_sums(ref, deg, offsets, lengths, clips, min_len, max_len, n_fft, hop, win, twiddle, window, sums, n_res, res,
+                   ws):
+    """sums[c, res, 0:3] = (sum (T - P)^2, sum T^2, sum |log P - log T|) of one STFT resolution for every clip of a pack."""
+    _cuda(ref, deg, offsets, lengths, twiddle, window, sums, ws)
+    _lib.check(_lib.lib().rstnet_stft_loss_sums_f32(ref.data_ptr(), deg.data_ptr(), offsets.data_ptr(), lengths.data_ptr(),
+                                                    clips, min_len, max_len, n_fft, hop, win, twiddle.data_ptr(),
+                                                    window.data_ptr(), sums.data_ptr(), n_res, res, ws.data_ptr(),
+                                                    ws.numel() * ws.element_size(), _stream()), "stft_loss_sums")
+
+
+def sisnr_moments_workspace(clips, max_len) -> int:
+    return int(_lib.lib().rstnet_sisnr_moments_workspace(clips, max_len))
+
+
+def sisnr_moments(ref, deg, offsets, lengths, clips, max_len, moments, ws):
+    """moments[c, 0:5] = (sum r, sum d, sum r^2, sum d^2, sum r d) in fp64 for every clip of a pack."""
+    _cuda(ref, deg, offsets, lengths, moments, ws)
+    _lib.check(_lib.lib().rstnet_sisnr_moments_f32(ref.data_ptr(), deg.data_ptr(), offsets.data_ptr(), lengths.data_ptr(),
+                                                   clips, max_len, moments.data_ptr(), ws.data_ptr(),
+                                                   ws.numel() * ws.element_size(), _stream()), "sisnr_moments")

@@ -414,6 +414,13 @@ int rstnet_lm_rope_kv_append_paged_bf16(const void* qkv, const void* cos_tab, co
 int rstnet_lm_rope_pair_kv_append_bf16(const void* qkv, const int64_t* offset, int32_t offset_stride, void* q_out, void* kv,
                                        int32_t rows, int32_t B, int32_t H, int32_t hd, int32_t cap, const float* freqs,
                                        rstnet_stream_t stream);
+/* ---- the Kyutai pair-RoPE append over a paged pool kv[n_pages][2][H][P][hd] (page table, its checks and the unmapped
+ * rule as rstnet_lm_rope_kv_append_paged_bf16): a row whose own slot is on an unmapped page writes neither q_out nor K/V.
+ * Every stored byte equals the contiguous form's; both run the same kernel. */
+int rstnet_lm_rope_pair_kv_append_paged_bf16(const void* qkv, const int64_t* offset, int32_t offset_stride, void* q_out, void* kv,
+                                             int32_t rows, int32_t B, int32_t H, int32_t hd, int32_t cap, const float* freqs,
+                                             const int32_t* page_table, int32_t pages_stride, int32_t log2_page,
+                                             rstnet_stream_t stream);
 /* ---- one query position per row over the ring with RingKVCache.complete's position labels and the
  * (pos_k>=0)&(delta>=0)&(delta<context) mask (llama_streaming.py:983-992), fp32 softmax. HBM-bound.  Rows and row map as
  * rstnet_lm_rope_kv_append_bf16 (padding rows write no output); every position of the launch must already be in the ring

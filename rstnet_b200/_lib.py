@@ -29,7 +29,7 @@ SYMBOLS = [
     "rstnet_lm_ring_decode_attention_bf16", "rstnet_lm_silu_mul_bf16", "rstnet_lm_depth_attention_bf16",
     "rstnet_resample_f32", "rstnet_lm_delay_cache_in", "rstnet_lm_delay_cache_out", "rstnet_counter_add_rows",
     "rstnet_lm_cross_entropy_bf16", "rstnet_rows_fill_tail_f32", "rstnet_lm_sample_params_bf16",
-    "rstnet_lm_rope_kv_append_paged_bf16", "rstnet_lm_paged_decode_attention_bf16",
+    "rstnet_lm_rope_kv_append_paged_bf16", "rstnet_lm_paged_decode_attention_bf16", "rstnet_lm_rope_pair_kv_append_paged_bf16",
     "rstnet_stft_loss_workspace", "rstnet_stft_loss_sums_f32", "rstnet_sisnr_moments_workspace", "rstnet_sisnr_moments_f32",
 ]
 
@@ -152,6 +152,7 @@ def lib() -> C.CDLL:
     L.rstnet_lm_rms_norm_bf16.argtypes = [vp, vp, vp, i32, i32, f32, i32, vp]
     L.rstnet_lm_rope_kv_append_bf16.argtypes = [vp, vp, vp, i64, i32, vp, i32, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]
     L.rstnet_lm_rope_pair_kv_append_bf16.argtypes = [vp, vp, i32, vp, vp, i32, i32, i32, i32, i32, vp, vp]
+    L.rstnet_lm_rope_pair_kv_append_paged_bf16.argtypes = [vp, vp, i32, vp, vp, i32, i32, i32, i32, i32, vp, vp, i32, i32, vp]
     L.rstnet_lm_ring_decode_attention_bf16.argtypes = [vp, vp, vp, i32, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp]
     L.rstnet_lm_rope_kv_append_paged_bf16.argtypes = [vp, vp, vp, i64, i32, vp, i32, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32,
                                                       vp, i32, i32, vp]

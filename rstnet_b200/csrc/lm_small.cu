@@ -167,9 +167,13 @@ __global__ void rope_kv_append_bf16_kernel(const bf16* __restrict__ qkv, const b
 // qkv [row][3][H][hd] ((p h d) layout, transformer.py:391-393); (even, odd) pairs of q and k rotate by
 // freqs[d/2] * (offset + tl) with everything in fp32 and ONE rounding to bf16 at the end (modules/rope.py:36-66);
 // rotated q -> q_out [row][H*hd], rotated k and v -> kv[2][B][H][cap][hd] at slot pos % cap.
+// Page table (paged KV, LMModel.streaming(B, kv_pages=N)): as rope_kv_append_bf16_kernel's -- slot s of stream b lives in
+// page page_table[b * pages_stride + (s >> log2_page)], row s & (2^log2_page - 1), of a pool kv[n_pages][2][H][2^log2_page][hd],
+// and a row whose own slot falls on an unmapped page (-1) writes nothing, q_out included.  A runtime branch of the same body.
 __global__ void rope_pair_kv_append_bf16_kernel(const bf16* __restrict__ qkv, const long long* __restrict__ offset, int ostride,
                                                 bf16* __restrict__ q_out, bf16* __restrict__ kv, int B, int H, int hd, int cap,
-                                                const float* __restrict__ freqs) {
+                                                const float* __restrict__ freqs, const int* __restrict__ page_table,
+                                                int pages_stride, int log2_page) {
   const int row = blockIdx.x / H, h = blockIdx.x % H;
   const int b = row % B;
   const long long off = offset[(long long)b * ostride];
@@ -179,8 +183,18 @@ __global__ void rope_pair_kv_append_bf16_kernel(const bf16* __restrict__ qkv, co
   const bf16* q = qkv + (long long)row * 3 * HD + h * hd;
   const bf16* k = q + HD;
   const bf16* v = q + 2 * HD;
-  bf16* kdst = kv + (((long long)b * H + h) * cap + slot) * hd;
-  bf16* vdst = kv + (long long)B * H * cap * hd + (((long long)b * H + h) * cap + slot) * hd;
+  bf16* kdst;
+  long long vofs;   // V row of a slot = its K row + vofs
+  if (page_table) {
+    const int page = page_table[(long long)b * pages_stride + (slot >> log2_page)];
+    if (page < 0) return;   // unmapped: nothing read, nothing written
+    kdst = kv + ((((long long)page * 2 * H + h) << log2_page) + (slot & ((1 << log2_page) - 1))) * hd;
+    vofs = ((long long)H << log2_page) * hd;
+  } else {
+    kdst = kv + (((long long)b * H + h) * cap + slot) * hd;
+    vofs = (long long)B * H * cap * hd;
+  }
+  bf16* vdst = kdst + vofs;
   const float ts = __fadd_rn((float)off, (float)(row / B));     // offset.float() + arange(T) in fp32 (rope.py:37)
   for (int pr = threadIdx.x; pr < hd / 2; pr += blockDim.x) {
     const float ang = __fmul_rn(freqs[pr], ts);     // freqs = exp(ds * (-ln(max_period) * 2 / hd)) from the host (rope.py:35-36)
@@ -960,15 +974,31 @@ extern "C" int rstnet_lm_rope_kv_append_paged_bf16(const void* qkv, const void* 
                         n_head, n_kv, hs, cap, page_table, pages_stride, log2_page, stream);
 }
 
-extern "C" int rstnet_lm_rope_pair_kv_append_bf16(const void* qkv, const int64_t* offset, int32_t offset_stride, void* q_out, void* kv,
-                                                  int32_t rows, int32_t B, int32_t H, int32_t hd, int32_t cap, const float* freqs,
-                                                  rstnet_stream_t stream) {
+static int rope_pair_kv_append(const void* qkv, const int64_t* offset, int32_t offset_stride, void* q_out, void* kv, int32_t rows,
+                               int32_t B, int32_t H, int32_t hd, int32_t cap, const float* freqs, const int32_t* page_table,
+                               int32_t pages_stride, int32_t log2_page, rstnet_stream_t stream) {
   RSTNET_REQUIRE(qkv && offset && q_out && kv && freqs, "lm_rope_pair_kv_append: null pointer");
   RSTNET_REQUIRE(rows > 0 && B > 0 && rows % B == 0 && H > 0 && hd > 0 && hd % 2 == 0 && cap > 0, "lm_rope_pair_kv_append: bad shape");
   rope_pair_kv_append_bf16_kernel<<<dim3(rows * H), dim3(64), 0, (cudaStream_t)stream>>>((const bf16*)qkv,
-             (const long long*)offset, offset_stride ? 1 : 0, (bf16*)q_out, (bf16*)kv, B, H, hd, cap, freqs);
+             (const long long*)offset, offset_stride ? 1 : 0, (bf16*)q_out, (bf16*)kv, B, H, hd, cap, freqs, (const int*)page_table,
+             pages_stride, log2_page);
   count_launch();
   return check_launch("lm_rope_pair_kv_append");
+}
+
+extern "C" int rstnet_lm_rope_pair_kv_append_bf16(const void* qkv, const int64_t* offset, int32_t offset_stride, void* q_out, void* kv,
+                                                  int32_t rows, int32_t B, int32_t H, int32_t hd, int32_t cap, const float* freqs,
+                                                  rstnet_stream_t stream) {
+  return rope_pair_kv_append(qkv, offset, offset_stride, q_out, kv, rows, B, H, hd, cap, freqs, nullptr, 0, 0, stream);
+}
+
+extern "C" int rstnet_lm_rope_pair_kv_append_paged_bf16(const void* qkv, const int64_t* offset, int32_t offset_stride, void* q_out,
+                                                        void* kv, int32_t rows, int32_t B, int32_t H, int32_t hd, int32_t cap,
+                                                        const float* freqs, const int32_t* page_table, int32_t pages_stride,
+                                                        int32_t log2_page, rstnet_stream_t stream) {
+  if (check_pages("lm_rope_pair_kv_append_paged", page_table, pages_stride, log2_page, cap)) return 1;
+  return rope_pair_kv_append(qkv, offset, offset_stride, q_out, kv, rows, B, H, hd, cap, freqs, page_table, pages_stride, log2_page,
+                             stream);
 }
 
 static int ring_decode_attention(const void* q, const void* kv, const int64_t* offset, int32_t offset_stride,

@@ -324,7 +324,45 @@ def merge_lora_weights(model: "GPT") -> None:
     return None
 
 
-class GPT(nn.Module):
+class PagedKVModel:
+    """The paged-KV methods of a decode model whose streaming scope (`_state`, an `_LMState`) may keep its KV in pages:
+    `GPT` and the Moshi twin's `LMModel` (rstnet_b200.moshi)."""
+
+    def _paged(self) -> "_LMState":
+        st = self._state
+        if st is None:
+            raise RstnetError("the model is not streaming")
+        if st.pages is None:
+            raise RstnetError("this streaming scope keeps contiguous KV rings: enter streaming(B, kv_pages=N) for pages")
+        return st
+
+    @on_own_device
+    def reserve_kv(self, streams, positions) -> None:
+        """Paged scope: give each listed stream KV pages for min(positions, context) positions from position 0 (one count
+        for all, or one per stream), replacing its reservation (the pages of the positions it keeps stay, with their
+        contents).  An active stream cannot advance past its reservation: the step raises before any launch.  If the
+        pool is short this raises RstnetError and changes nothing."""
+        st = self._paged()
+        st.upload_pages(st.pages.reserve(streams, positions))
+
+    @on_own_device
+    def release_kv(self, streams) -> None:
+        """Paged scope: return the listed streams' KV pages to the pool (a stream without pages may still be held)."""
+        st = self._paged()
+        st.upload_pages(st.pages.release(streams))
+
+    @property
+    def kv_pages_free(self) -> int:
+        """Paged scope: pages of the pool no stream holds."""
+        return self._paged().pages.free
+
+    @property
+    def kv_page_bytes(self) -> int:
+        """Paged scope: bytes of one KV page over all layers (K and V, bf16)."""
+        return kv_page_bytes(self.config, self._paged().pages.page)
+
+
+class GPT(PagedKVModel, nn.Module):
     def __init__(self, config: Config, device=None, dtype=None):
         """device/dtype: create the (random-init) parameters directly there (a 7B model in bf16 on the GPU
         without a 28 GB fp32 host copy); default = CPU fp32 like the reference constructor."""
@@ -515,39 +553,6 @@ class GPT(nn.Module):
             yield
         finally:
             self._state = None
-
-    def _paged(self) -> "_LMState":
-        st = self._state
-        if st is None:
-            raise RstnetError("the model is not streaming")
-        if st.pages is None:
-            raise RstnetError("this streaming scope keeps contiguous KV rings: enter gpt.streaming(B, kv_pages=N) for pages")
-        return st
-
-    @on_own_device
-    def reserve_kv(self, streams, positions) -> None:
-        """Paged scope: give each listed stream KV pages for min(positions, context) positions from position 0 (one count
-        for all, or one per stream), replacing its reservation (the pages of the positions it keeps stay, with their
-        contents).  An active stream cannot advance past its reservation: the step raises before any launch.  If the
-        pool is short this raises RstnetError and changes nothing."""
-        st = self._paged()
-        st.upload_pages(st.pages.reserve(streams, positions))
-
-    @on_own_device
-    def release_kv(self, streams) -> None:
-        """Paged scope: return the listed streams' KV pages to the pool (a stream without pages may still be held)."""
-        st = self._paged()
-        st.upload_pages(st.pages.release(streams))
-
-    @property
-    def kv_pages_free(self) -> int:
-        """Paged scope: pages of the pool no stream holds."""
-        return self._paged().pages.free
-
-    @property
-    def kv_page_bytes(self) -> int:
-        """Paged scope: bytes of one KV page over all layers (K and V, bf16)."""
-        return kv_page_bytes(self.config, self._paged().pages.page)
 
     @on_own_device
     def reset_streaming(self, streams=None):

@@ -34,7 +34,7 @@ from torch import nn
 from . import _lib, ops
 from ._lib import RstnetError
 from .codec import _register, on_own_device
-from .lm import GPT, Sampling, SkinnyGemm, _DepthScope, _LMState, _head_mode  # noqa: F401
+from .lm import GPT, KV_PAGE, KVPages, PagedKVModel, Sampling, SkinnyGemm, _DepthScope, _LMState, _head_mode  # noqa: F401
 
 
 class _MoshiState(_LMState):
@@ -58,7 +58,14 @@ class _MoshiState(_LMState):
         self.pos_host = np.zeros(B, dtype=np.int64)
         self.active = torch.ones(B, dtype=torch.int64, device=dev)
         self.active_host = np.ones(B, dtype=np.int64)
-        self.kv = [z(2, B, nh, self.cap, hs) for _ in range(c.n_layer)]
+        # contiguous rings [2, B, H, cap, hd] per layer, or the paged pool [n_pages, 2, H, page, hd] per layer with one table
+        n_pages, page = self._kv_pages
+        if n_pages is None:
+            self.kv = [z(2, B, nh, self.cap, hs) for _ in range(c.n_layer)]
+        else:
+            self.pages = KVPages(n_pages, B, page, self.cap)
+            self.page_table = torch.full((B, self.pages.stride), -1, dtype=torch.int32, device=dev)
+            self.kv = [z(self.pages.n_pages, 2, nh, page, hs) for _ in range(c.n_layer)]
         # freqs exactly as modules/rope.py:35-36 evaluates them (fp32 tensor * python scalar, then exp)
         ds = torch.arange(hs // 2, dtype=torch.float32)
         self.freqs = torch.exp(ds * (-math.log(m.max_period) * 2 / hs)).to(dev)
@@ -90,18 +97,22 @@ class _MoshiState(_LMState):
         c, B, M, L = self.c, self.B, self.M, _lib.lib()
         st = ops._stream()
         E = c.n_embd
+        # a paged scope runs the same kernels through their paged entry points: the page table as three more arguments
+        if self.pages is None:
+            rope, attention, pg = L.rstnet_lm_rope_pair_kv_append_bf16, L.rstnet_lm_ring_decode_attention_bf16, ()
+        else:
+            rope, attention = L.rstnet_lm_rope_pair_kv_append_paged_bf16, L.rstnet_lm_paged_decode_attention_bf16
+            pg = (self.page_table.data_ptr(), self.pages.stride, self.pages.log2_page)
         _lib.check(L.rstnet_lm_embed_sum_bf16(self.seq.data_ptr(), c.n_q + 1, self.wte.data_ptr(), self.wte.shape[0],
                                               self.table_ptrs.data_ptr(), self.tables[0].shape[0], c.n_q, E, self.x.data_ptr(), M, st),
                    "lm_embed_sum")
         _lib.check(L.rstnet_lm_rms_norm_bf16(self.x.data_ptr(), self.n1_first.data_ptr(), self.xn.data_ptr(), M, E, 1e-8, 1, st), "rms")
         for l, ly in enumerate(self.layers):
             ly["qkv"].run()
-            _lib.check(L.rstnet_lm_rope_pair_kv_append_bf16(self.qkv.data_ptr(), self.offset.data_ptr(), 1, self.q.data_ptr(),
-                                                            self.kv[l].data_ptr(), M, B, c.n_head, c.head_size, self.cap,
-                                                            self.freqs.data_ptr(), st), "rope_pair_kv")
-            _lib.check(L.rstnet_lm_ring_decode_attention_bf16(self.q.data_ptr(), self.kv[l].data_ptr(), self.offset.data_ptr(), 1,
-                                                              None, None, self.att.data_ptr(), M, B, c.n_head, c.n_head, c.head_size,
-                                                              self.cap, c.context, st), "attention")
+            _lib.check(rope(self.qkv.data_ptr(), self.offset.data_ptr(), 1, self.q.data_ptr(), self.kv[l].data_ptr(), M, B, c.n_head,
+                            c.head_size, self.cap, self.freqs.data_ptr(), *pg, st), "rope_pair_kv")
+            _lib.check(attention(self.q.data_ptr(), self.kv[l].data_ptr(), self.offset.data_ptr(), 1, None, None, self.att.data_ptr(),
+                                 M, B, c.n_head, c.n_head, c.head_size, self.cap, c.context, *pg, st), "attention")
             ly["proj"].run()
             ly["fc"].run()
             ly["down"].run()
@@ -110,10 +121,15 @@ class _MoshiState(_LMState):
         ops.counter_add(self.offset, self.tn, self.active)
 
     def _advance_host(self, n: int):
-        self.pos_host += n * self.active_host      # positions enter the RoPE as fp32 angles: no table to run out of
+        # positions enter the RoPE as fp32 angles: no table to run out of.  A paged scope raises, before any launch and
+        # with the counters unchanged, when an active stream would write past its pages (held streams advance nothing).
+        if self.pages is not None:
+            act = np.flatnonzero(self.active_host)
+            self.pages.check(act, self.pos_host[act], n)
+        self.pos_host += n * self.active_host
 
 
-class LMModel(nn.Module):
+class LMModel(PagedKVModel, nn.Module):
     """Drop-in for ``models.model.LMModel`` on the streaming decode path (same constructor arguments / defaults)."""
 
     _DN = dict(din="depformer_in.{}.weight", demb="depformer_emb.{}.weight", dtext="depformer_text_emb.weight",
@@ -276,16 +292,19 @@ class LMModel(nn.Module):
         return self._state is not None
 
     @on_own_device
-    def streaming_forever(self, batch_size: int):
+    def streaming_forever(self, batch_size: int, kv_pages: Optional[int] = None, kv_page: int = KV_PAGE):
+        """kv_pages None: every stream owns a contiguous KV ring of `context` positions per layer.  kv_pages N: a shared
+        pool of N pages of kv_page positions per layer, and a stream holds only the pages reserve_kv gives it -- none at
+        entry (as GPT.streaming_forever).  Both give the same results bit for bit."""
         if self.device.type != "cuda":
             raise RstnetError("LMModel decode runs on CUDA only (sm_90a kernels; the CPU path is the reference itself)")
         if next(self.parameters()).dtype != torch.bfloat16:
             raise RstnetError("LMModel decode runs in bfloat16: call .to(device, torch.bfloat16)")
-        self._state = _MoshiState(self, batch_size)
+        self._state = _MoshiState(self, batch_size, kv_pages=kv_pages, kv_page=kv_page)
 
     @contextmanager
-    def streaming(self, batch_size: int):
-        self.streaming_forever(batch_size)
+    def streaming(self, batch_size: int, kv_pages: Optional[int] = None, kv_page: int = KV_PAGE):
+        self.streaming_forever(batch_size, kv_pages=kv_pages, kv_page=kv_page)
         try:
             yield
         finally:
@@ -381,15 +400,17 @@ class LMGen(nn.Module):
     def is_streaming(self) -> bool:
         return self._st is not None
 
-    def streaming_forever(self, batch_size: int):
+    def streaming_forever(self, batch_size: int, kv_pages: Optional[int] = None, kv_page: int = KV_PAGE):
+        """kv_pages / kv_page: the LMModel scope's KV (LMModel.streaming_forever); a paged scope's rows hold the pages
+        reserve_kv gives them."""
         lm = self.lm_model
-        lm.streaming_forever(batch_size)
+        lm.streaming_forever(batch_size, kv_pages=kv_pages, kv_page=kv_page)
         self._st = _GenState(self, lm._st(), batch_size)
         self._row_sampling = None
 
     @contextmanager
-    def streaming(self, batch_size: int):
-        self.streaming_forever(batch_size)
+    def streaming(self, batch_size: int, kv_pages: Optional[int] = None, kv_page: int = KV_PAGE):
+        self.streaming_forever(batch_size, kv_pages=kv_pages, kv_page=kv_page)
         try:
             yield
         finally:
@@ -400,6 +421,21 @@ class LMGen(nn.Module):
         if self._st is None:
             raise ValueError("the generator is not streaming")
         return self._st
+
+    # ---- paged KV (LMGen.streaming(B, kv_pages=N)): the LMModel's methods
+    def reserve_kv(self, streams, positions) -> None:
+        self.lm_model.reserve_kv(streams, positions)
+
+    def release_kv(self, streams) -> None:
+        self.lm_model.release_kv(streams)
+
+    @property
+    def kv_pages_free(self) -> int:
+        return self.lm_model.kv_pages_free
+
+    @property
+    def kv_page_bytes(self) -> int:
+        return self.lm_model.kv_page_bytes
 
     def reset_streaming(self, streams=None):
         """Restart every row, or (extension) only the rows in `streams`: their cache back to ungenerated, their step count

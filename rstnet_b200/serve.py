@@ -15,6 +15,11 @@ sessions push and receive PCM at their own rate.
 `FrameScheduler` is pure host logic over an engine object with `reset_rows(rows)` and `step(pcm_rows, active) ->
 {row: (tokens, pcm)}`; `DuplexEngine` is that engine for a MimiCodec + GPT pair on a GPU, `MoshiDuplexEngine` for the
 MimiCodec + `LMGen(LMModel)` pair server.py itself runs (rstnet_b200.moshi).
+
+Paged KV (`kv_pages=N` on either engine): the LM scope keeps its KV in a shared pool of N pages, and a session holds pages
+only for the frames it has run -- one at admission, one more each time it crosses a page boundary, all returned when it
+ends.  The engine then also has `grow_kv(rows)`, `release_rows(rows)` and `kv_pages_free` (`_PagedRows`), and the
+scheduler admits on free pages and evicts a session whose next page the pool cannot give.
 """
 from __future__ import annotations
 
@@ -28,7 +33,7 @@ import torch
 
 from ._lib import RstnetError
 from .audio import StreamingResampler
-from .lm import MAX_STREAMS, Sampling
+from .lm import KV_PAGE, MAX_STREAMS, Sampling
 
 FRAME_SAMPLES = 1920       # 80 ms at 24 kHz = one 12.5 Hz frame (moshi/server.py:57: sample_rate / frame_rate)
 FRAME_SECONDS = 0.08
@@ -47,13 +52,23 @@ def check_client_rate(sample_rate) -> int:
 
 class FrameScheduler:
     """Rows of a fixed-capacity batch are leased to sessions.  Every `tick()` steps the engine once for all rows that
-    have a full frame of audio queued; the others are held."""
+    have a full frame of audio queued; the others are held.
 
-    def __init__(self, engine, capacity: int):
+    On an engine with paged KV (its `kv_pages` is not None) a session also holds KV pages: admission takes its first page
+    and refuses while fewer than 1 + kv_headroom pages are free (kv_headroom: pages left for the live sessions to grow
+    into); every tick first grows the ready sessions oldest first, and one whose next page the pool cannot give is
+    evicted -- its row and pages returned, its queued frames dropped, not stepped -- and reported by `take_evicted()`."""
+
+    def __init__(self, engine, capacity: int, kv_headroom: int = 0):
         self.engine, self.capacity = engine, capacity
-        self._row_of: Dict[Hashable, int] = {}
+        self.paged = getattr(engine, "kv_pages", None) is not None
+        if isinstance(kv_headroom, bool) or not isinstance(kv_headroom, int) or kv_headroom < 0:
+            raise RstnetError(f"kv_headroom must be an int >= 0 (got {kv_headroom!r})")
+        self.kv_headroom = kv_headroom
+        self._row_of: Dict[Hashable, int] = {}     # in admission order
         self._free: List[int] = list(range(capacity))
         self._queue: Dict[Hashable, Deque] = {}
+        self._evicted: List[Hashable] = []
         self.ticks = 0
 
     # ---- session lifecycle
@@ -67,6 +82,9 @@ class FrameScheduler:
             raise RuntimeError(f"session {session!r} is already admitted")
         if not self._free:
             raise RuntimeError("no free row: the batch is full")
+        if self.paged and self.engine.kv_pages_free < 1 + self.kv_headroom:
+            raise RuntimeError(f"the KV pool is short: {self.engine.kv_pages_free} pages free, admission needs "
+                               f"1 + {self.kv_headroom} (kv_headroom)")
         self._free.sort()
         row = self._free.pop(0)
         self._row_of[session] = row
@@ -81,6 +99,13 @@ class FrameScheduler:
         row = self._row_of.pop(session)
         self._queue.pop(session, None)
         self._free.append(row)
+        if self.paged:
+            self.engine.release_rows([row])
+
+    def take_evicted(self) -> List[Hashable]:
+        """The sessions evicted since the last call (paged KV: the pool had no page for their next frame), oldest first."""
+        out, self._evicted = self._evicted, []
+        return out
 
     def sessions(self) -> Dict[Hashable, int]:
         return dict(self._row_of)
@@ -97,6 +122,12 @@ class FrameScheduler:
         """One scheduler period: step every session that has a frame queued; returns {session: (tokens, pcm)}."""
         ready = {s: r for s, r in self._row_of.items() if self._queue[s]}
         self.ticks += 1
+        if self.paged and ready:
+            short = set(self.engine.grow_kv(list(ready.values())))     # admission order: the oldest sessions grow first
+            for s in [s for s, r in ready.items() if r in short]:
+                del ready[s]
+                self.release(s)
+                self._evicted.append(s)
         if not ready:
             return {}
         pcm_rows = {r: self._queue[s].popleft() for s, r in ready.items()}
@@ -104,7 +135,52 @@ class FrameScheduler:
         return {s: out[r] for s, r in ready.items()}
 
 
-class DuplexEngine:
+class _PagedRows:
+    """The paged-KV policy of both duplex engines, over the LM whose scope holds the pages (`_kv_lm`: a GPT, or the
+    LMGen's LMModel; None: contiguous rings).  Positions come from the scope's host mirror, so no call here waits on
+    the GPU, and every table change is uploaded outside graph replay (PagedKVModel.reserve_kv)."""
+
+    kv_pages: Optional[int] = None
+    _kv_lm = None
+
+    def _reserve_first_page(self, rows) -> None:
+        """A restarted row returns its old pages and holds its first page (its other pages go back to the pool)."""
+        if self._kv_lm is not None:
+            self._kv_lm.reserve_kv(list(rows), self._kv_lm._paged().pages.page)
+
+    def grow_kv(self, rows) -> List[int]:
+        """Walk `rows` in order: a row whose next position lies past its pages gets one more page while the pool has
+        one.  A row that holds its whole ring needs none.  -> the rows that could not get their page (unchanged)."""
+        st = self._kv_lm._paged()
+        kp = st.pages
+        grow, want, short = [], [], []
+        free = kp.free
+        for r in rows:
+            r = int(r)
+            if st.pos_host[r] + 1 <= kp.limit[r]:
+                continue
+            positions = (int(kp.held[r]) + 1) * kp.page
+            extra = kp.pages_for(positions) - int(kp.held[r])    # 0: the last page of the ring is already held
+            if extra > free:
+                short.append(r)
+                continue
+            free -= extra
+            grow.append(r)
+            want.append(positions)
+        if grow:
+            self._kv_lm.reserve_kv(grow, want)      # one reservation and one table upload, pages handed out in row order
+        return short
+
+    def release_rows(self, rows) -> None:
+        """Return the rows' pages to the pool (the rows stay in the batch, held until they are restarted)."""
+        self._kv_lm.release_kv(list(rows))
+
+    @property
+    def kv_pages_free(self) -> int:
+        return self._kv_lm.kv_pages_free
+
+
+class DuplexEngine(_PagedRows):
     """One streaming scope of a MimiCodec and a GPT for `capacity` sessions: per tick, for all rows at once,
     encode the sessions' 80 ms chunks -> one LM frame (temporal step + 8 depth steps + sampling) -> decode the generated
     codes (the three calls of server.py:128-136).  The LM input frame of a row is [its previous text token, the 8 codes of
@@ -112,10 +188,14 @@ class DuplexEngine:
 
     `sample_rate` is the sessions' PCM rate (see `check_client_rate`): each pushes and receives sample_rate * 0.08 samples
     per tick.  At any rate other than 24000 two StreamingResamplers run for all rows at once, r -> 24 kHz before the
-    encode and 24 kHz -> r after the decode; row resets and the held-row mask apply to both."""
+    encode and 24 kHz -> r after the decode; row resets and the held-row mask apply to both.
+
+    kv_pages N: the GPT scope keeps its KV in a pool of N pages of kv_page positions (see `_PagedRows`); a restarted row
+    holds one page.  None: contiguous rings."""
 
     def __init__(self, codec, gpt, capacity: int, *, use_sampling: bool = True, temp_text: float = 0.7, top_k_text: int = 25,
-                 temp: float = 0.8, top_k: int = 30, sample_rate: int = CODEC_RATE, top_p_text: float = 0.0, top_p: float = 0.0):
+                 temp: float = 0.8, top_k: int = 30, sample_rate: int = CODEC_RATE, top_p_text: float = 0.0, top_p: float = 0.0,
+                 kv_pages: Optional[int] = None, kv_page: int = KV_PAGE):
         self.sample_rate = check_client_rate(sample_rate)
         self.frame_samples = self.sample_rate * 2 // 25                       # 80 ms at the client rate
         if capacity > MAX_STREAMS:
@@ -132,7 +212,11 @@ class DuplexEngine:
         self._keys_dirty = False
         self._valid_table = None
         codec.streaming_forever(capacity)
-        gpt.streaming_forever(capacity)
+        if kv_pages is None:
+            gpt.streaming_forever(capacity)
+        else:
+            gpt.streaming_forever(capacity, kv_pages=kv_pages, kv_page=kv_page)
+            self.kv_pages, self._kv_lm = kv_pages, gpt
         F = self.frame_samples
         self.pcm_in = torch.zeros(capacity, 1, F, dtype=torch.float32).pin_memory()
         self.pcm_dev = torch.zeros(capacity, 1, FRAME_SAMPLES, dtype=torch.float32, device=self.dev)
@@ -164,6 +248,7 @@ class DuplexEngine:
                 self.row_sampling[r] = sampling if sampling is not None else default
                 self.row_keys[r] = int(seed or 0) & 0xFFFFFFFF
             self._keys_dirty = True
+        self._reserve_first_page(rows)
         self.codec.reset_streaming(streams=list(rows))
         self.gpt.reset_streaming(streams=list(rows))
         self.prev_text[list(rows)] = self.gpt.text_initial_token_id
@@ -209,7 +294,7 @@ class DuplexEngine:
         return {r: (self.tok_host[r].clone(), self.pcm_host[r, 0].clone()) for r in active}
 
 
-class MoshiDuplexEngine:
+class MoshiDuplexEngine(_PagedRows):
     """The serving loop of server.py:128-136 -- `mimi.encode -> lm_gen.step(codes) -> mimi.decode(tokens[:, 1:])` --
     for `capacity` sessions in one streaming scope of a MimiCodec and an `LMGen` (rstnet_b200.moshi).
 
@@ -217,9 +302,11 @@ class MoshiDuplexEngine:
     the codec's decoder is held for that row (the reference does not call `mimi.decode` then) while its encoder advances.
     `step` returns {row: (tokens, pcm)}, tokens = int64 [dep_q + 1] (text token, then the audio codes that were decoded),
     pcm = float32 [sample_rate * 0.08]; a row in its warm-up gets (None, None), as the reference's `lm_gen.step` returns
-    None.  Text-piece decoding and the transport stay with the caller.  `sample_rate` as for `DuplexEngine`."""
+    None.  Text-piece decoding and the transport stay with the caller.  `sample_rate` and `kv_pages` / `kv_page` as for
+    `DuplexEngine` (the pages are the LMGen's LMModel scope's)."""
 
-    def __init__(self, codec, lm_gen, capacity: int, *, sample_rate: int = CODEC_RATE):
+    def __init__(self, codec, lm_gen, capacity: int, *, sample_rate: int = CODEC_RATE, kv_pages: Optional[int] = None,
+                 kv_page: int = KV_PAGE):
         self.sample_rate = check_client_rate(sample_rate)
         self.frame_samples = self.sample_rate * 2 // 25                       # 80 ms at the client rate
         if capacity > MAX_STREAMS:
@@ -232,7 +319,11 @@ class MoshiDuplexEngine:
         self.codec, self.lm_gen, self.B = codec, lm_gen, capacity
         self.dev = lm.device
         codec.streaming_forever(capacity)
-        lm_gen.streaming_forever(capacity)
+        if kv_pages is None:
+            lm_gen.streaming_forever(capacity)
+        else:
+            lm_gen.streaming_forever(capacity, kv_pages=kv_pages, kv_page=kv_page)
+            self.kv_pages, self._kv_lm = kv_pages, lm
         F = self.frame_samples
         pin = self.dev.type == "cuda"                                           # False: host logic under a test's fakes
         self.pcm_in = torch.zeros(capacity, 1, F, dtype=torch.float32, pin_memory=pin)
@@ -252,6 +343,7 @@ class MoshiDuplexEngine:
 
     def reset_rows(self, rows, sampling=None, seed: Optional[int] = None) -> None:
         """Restart `rows`; sampling / seed as DuplexEngine.reset_rows (LMGen.set_stream_sampling)."""
+        self._reserve_first_page(rows)
         self.codec.reset_streaming(streams=list(rows))
         self.lm_gen.reset_streaming(streams=list(rows))
         if sampling is not None or seed is not None or getattr(self.lm_gen, "_row_sampling", None) is not None:

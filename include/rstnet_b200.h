@@ -513,6 +513,25 @@ int rstnet_lm_delay_cache_out(int64_t* cache, int64_t* off, const int64_t* activ
                               const int64_t* tokens, int32_t tok_stride, int64_t* out, int32_t out_stride, int64_t* valid,
                               int32_t B, int32_t K, int32_t dep_q, int32_t CT, int32_t max_delay, rstnet_stream_t stream);
 
+/* ---- segment gather / scatter: one batch row's streaming state <-> a packed staging blob (session suspend / resume).
+ * A segment is `count` pieces of `bytes` at base + i * stride_bytes (device memory); in staging it occupies
+ * [staging_offset, + count * bytes), the pieces back to back.  gather copies every segment into staging, scatter back.
+ * `staging` is pinned host memory (reached through UVA; device memory works too); `table` holds n entries in device
+ * memory or in pinned host memory, which the kernel reads directly (a device table is copied back to the host for the
+ * checks, which synchronises).  One launch of at most `ctas` CTAs.  Accesses are 16 bytes wide where base, stride, piece
+ * size and staging address are 16-byte aligned, else 8, 4 or 1.  Checked before any launch, each an error return: n < 0,
+ * ctas < 1, a null table / staging / base, count, bytes or staging_offset < 0, two segments whose staging ranges
+ * overlap, and (scatter) a segment whose pieces overlap in device memory.  n == 0 launches nothing. */
+typedef struct {
+  void* base;
+  int64_t stride_bytes;
+  int64_t bytes;
+  int32_t count;
+  int64_t staging_offset;
+} rstnet_segment;
+int rstnet_segments_gather(const rstnet_segment* table_dev, int32_t n, void* staging, int32_t ctas, rstnet_stream_t s);
+int rstnet_segments_scatter(const rstnet_segment* table_dev, int32_t n, const void* staging, int32_t ctas, rstnet_stream_t s);
+
 #ifdef __cplusplus
 }
 #endif

@@ -31,6 +31,7 @@ SYMBOLS = [
     "rstnet_lm_cross_entropy_bf16", "rstnet_rows_fill_tail_f32", "rstnet_lm_sample_params_bf16",
     "rstnet_lm_rope_kv_append_paged_bf16", "rstnet_lm_paged_decode_attention_bf16", "rstnet_lm_rope_pair_kv_append_paged_bf16",
     "rstnet_stft_loss_workspace", "rstnet_stft_loss_sums_f32", "rstnet_sisnr_moments_workspace", "rstnet_sisnr_moments_f32",
+    "rstnet_segments_gather", "rstnet_segments_scatter",
 ]
 
 KV_LOG2_PAGE_MIN, KV_LOG2_PAGE_MAX = 4, 12   # RSTNET_KV_LOG2_PAGE_MIN / _MAX: pages of 16 .. 4096 positions
@@ -79,6 +80,12 @@ class TcResblockDesc(C.Structure):
 class RowCopy(C.Structure):
     _fields_ = [("buf", C.c_void_p), ("batch_stride", C.c_int64), ("C", C.c_int32), ("src_row", C.c_int32),
                 ("dst_row", C.c_int32), ("nrows", C.c_int32), ("cps", C.c_int32), ("reserved", C.c_int32)]
+
+
+class Segment(C.Structure):
+    """rstnet_segment: count pieces of `bytes` at base + i * stride_bytes <-> staging[staging_offset, + count * bytes)"""
+    _fields_ = [("base", C.c_void_p), ("stride_bytes", C.c_int64), ("bytes", C.c_int64), ("count", C.c_int32),
+                ("staging_offset", C.c_int64)]
 
 
 class RstnetError(RuntimeError):
@@ -173,6 +180,8 @@ def lib() -> C.CDLL:
     L.rstnet_sisnr_moments_workspace.argtypes = [i32, i64]
     L.rstnet_sisnr_moments_workspace.restype = i64
     L.rstnet_sisnr_moments_f32.argtypes = [vp, vp, vp, vp, i32, i64, vp, vp, i64, vp]
+    L.rstnet_segments_gather.argtypes = [vp, i32, vp, i32, vp]
+    L.rstnet_segments_scatter.argtypes = [vp, i32, vp, i32, vp]
     for name in SYMBOLS:
         fn = getattr(L, name)
         if fn.restype is C.c_int and name not in ("rstnet_version",):

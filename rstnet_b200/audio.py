@@ -259,6 +259,14 @@ class StreamingResampler:
         ops.rows_copy_table(self._copy_table, self._copy_entries, self.B, self.active)
         return out
 
+    def row_segments(self, b: int, chunk: int):
+        """Row b's state as row_state regions: its carry of `carry` input samples (the buffer for `chunk`-sample calls is
+        built here if no call has built it yet)."""
+        from .row_state import segs
+        self._ensure(chunk)
+        n = self.carry * self._buf.element_size()
+        return [("carry", segs((self._buf[b].data_ptr(), n, n, 1)))]
+
     def reset(self, rows=None) -> None:
         """Zero the carry of `rows` (None = all): those streams restart as fresh streams."""
         if self._buf is None:

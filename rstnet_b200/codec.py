@@ -27,6 +27,7 @@ from torch import nn
 
 from . import ops
 from ._lib import ACT_ELU, ACT_GELU, ACT_NONE, RstnetError
+from .row_state import segs, tensor_segs
 
 
 def on_own_device(fn):
@@ -398,6 +399,17 @@ class _Buf:
             else:
                 self.t[streams, :self.ctx] = 0.0
 
+    def row_segments(self, b: int) -> np.ndarray:
+        """The carry rows [0, ctx) of stream b as state segments (row_state): ctx rows of C floats, row after row, in
+        either layout."""
+        if not self.ctx:
+            return segs()
+        e = self.t.element_size()
+        if self.tbc:
+            return segs((self.t.data_ptr() + b * self.bs * e, self.ts * e, self.C * e, self.ctx))
+        n = self.ctx * self.C * e
+        return segs((self.t.data_ptr() + b * self.bs * e, n, n, 1))
+
     def carry_entry(self):
         """row-copy table entry that moves the last ctx rows to the front (streaming carry)."""
         if self.tbc:
@@ -761,6 +773,16 @@ class _Plan:
         self.add(lambda: ops.rows_copy_table(table, n, nb, self.active))
         self.add(lambda: ops.counter_add(self.offset, F, self.active))
 
+    def row_segments(self, b: int):
+        """Stream b's state in this streaming plan, as row_state regions: the carry rows of every buffer, every layer's
+        transformer ring kv[l][:, b] (all `cap` slots: unwritten ones are masked by the position), the position counter."""
+        regions = [(f"carry{i}", buf.row_segments(b)) for i, buf in enumerate(self.carries) if buf.ctx]
+        for l, kv in enumerate(self.kv):
+            e = kv.element_size()
+            regions.append((f"ring{l}", segs((kv[0, b].data_ptr(), kv.stride(0) * e, kv[0, b].numel() * e, 2))))
+        regions.append(("offset", tensor_segs(self.offset[b:b + 1])))
+        return regions
+
     def reset(self, streams=None):
         assert self.streaming
         for b in self.carries:
@@ -974,21 +996,33 @@ class _StreamState:
             raise RstnetError(f"streaming batch size is {self.B}, got {B}")
         if L == 0:
             return torch.empty((B, self.eng.m.n_q, 0), dtype=torch.int64, device=self.eng.device)
+        return self._enc_plan(L).run(x, self.eng.m.use_cuda_graphs).clone()
+
+    def _enc_plan(self, L: int) -> "_EncPlan":
         if L not in self.enc:
             if self.enc:
                 raise RstnetError("the chunk size must stay constant within one streaming scope")
-            self.enc[L] = _EncPlan(self.eng, B, L, True, self.eng.m.streaming_tensor_cores, active=self.active)
-        return self.enc[L].run(x, self.eng.m.use_cuda_graphs).clone()
+            self.enc[L] = _EncPlan(self.eng, self.B, L, True, self.eng.m.streaming_tensor_cores, active=self.active)
+        return self.enc[L]
+
+    def _dec_plan(self, T: int, K: int) -> "_DecPlan":
+        if T not in self.dec:
+            if self.dec:
+                raise RstnetError("the chunk size must stay constant within one streaming scope")
+            self.dec[T] = _DecPlan(self.eng, self.B, T, True, self.eng.m.streaming_tensor_cores, n_codes=K, active=self.active)
+        return self.dec[T]
+
+    def row_segments(self, b: int, chunk: int, frames: int, n_codes: int):
+        """Stream b's state as row_state regions: the encoder plan of `chunk` samples and the decoder plan of `frames`
+        frames of n_codes codes (built here if no step has built them yet, as encode / decode would)."""
+        enc, dec = self._enc_plan(chunk), self._dec_plan(frames, n_codes)
+        return [("enc." + n, s) for n, s in enc.row_segments(b)] + [("dec." + n, s) for n, s in dec.row_segments(b)]
 
     def decode(self, codes: torch.Tensor) -> torch.Tensor:
         B, K, T = codes.shape
         if B != self.B:
             raise RstnetError(f"streaming batch size is {self.B}, got {B}")
-        if T not in self.dec:
-            if self.dec:
-                raise RstnetError("the chunk size must stay constant within one streaming scope")
-            self.dec[T] = _DecPlan(self.eng, B, T, True, self.eng.m.streaming_tensor_cores, n_codes=K, active=self.active)
-        return self.dec[T].run(codes, self.eng.m.use_cuda_graphs).clone()
+        return self._dec_plan(T, K).run(codes, self.eng.m.use_cuda_graphs).clone()
 
     def set_active(self, mask):
         """mask [B] (bool / int): streams with 0 are HELD by the next steps -- they still run through the kernels (the

@@ -24,7 +24,7 @@ import ctypes as C
 import heapq
 from contextlib import contextmanager
 from dataclasses import dataclass
-from typing import Dict, Optional
+from typing import Dict, List, Optional
 
 import numpy as np
 import torch
@@ -118,6 +118,19 @@ class KVPages:
     def release(self, streams):
         """Free the streams' pages.  -> the streams whose table rows changed."""
         return self.reserve(streams, 0)
+
+    def detach(self, stream: int) -> List[int]:
+        """Unmap the stream's pages WITHOUT returning them to the pool (their contents are still being read); -> the
+        pages, which `give_back` returns later."""
+        s = self._streams([stream])[0]
+        pages = [int(p) for p in self.table[s, :self.held[s]]]
+        self.table[s] = -1
+        self.held[s] = self.limit[s] = 0
+        return pages
+
+    def give_back(self, pages) -> None:
+        for p in pages:
+            heapq.heappush(self._free, int(p))
 
     def check(self, streams, pos, n) -> None:
         """Raise unless every stream s of `streams` (at position pos[i]) may write n more positions."""
@@ -1128,6 +1141,37 @@ class _LMState:
             act = np.flatnonzero(self.active_host)
             self.pages.check(act, self.pos_host[act], n)
         self.pos_host += n * self.active_host
+
+    def row_segments(self, b: int, positions: int):
+        """Stream b's state as row_state regions for a stream that has run `positions` positions: the KV it wrote, in
+        canonical slot order [layer][k/v][group][slot][hs] over slots < min(positions, cap) -- the same bytes from
+        contiguous rings or from pages, wherever the pages lie (a paged stream must hold them) -- then the position
+        counter and the per-row sampler's step counter and key.  Depth KV and activations are rewritten by every frame
+        before they are read, so they are not state."""
+        from .row_state import segs, tensor_segs
+        c = self.c
+        nkv, hs = c.n_query_groups, c.head_size
+        n = min(int(positions), self.cap)
+        e = self.kv[0].element_size()
+        if n == 0:
+            kv = segs()
+        elif self.pages is None:
+            kv = segs(*[(t[i, b].data_ptr(), self.cap * hs * e, n * hs * e, nkv) for t in self.kv for i in range(2)])
+        else:
+            P = self.pages.page
+            npg = self.pages.pages_for(n)
+            pid = self.pages.table[b, :npg].astype(np.int64)
+            if (pid < 0).any():
+                raise RstnetError(f"stream {b} does not hold KV pages for its {n} positions")
+            cnt = np.minimum(P, n - np.arange(npg) * P)
+            off = ((pid[None, None, :] * 2 + np.arange(2)[:, None, None]) * nkv + np.arange(nkv)[None, :, None]) * P * hs * e
+            base = np.array([t.data_ptr() for t in self.kv], dtype=np.int64)[:, None, None, None] + off[None]
+            nb = np.broadcast_to(cnt * hs * e, base.shape).reshape(-1)
+            kv = np.stack([base.reshape(-1), nb, nb, np.ones_like(nb)], axis=1)
+        regions = [("kv", kv), ("offset", tensor_segs(self.offset[b:b + 1]))]
+        if hasattr(self, "row_step"):
+            regions += [("row_step", tensor_segs(self.row_step[b:b + 1])), ("row_key", tensor_segs(self.row_key[b:b + 1]))]
+        return regions
 
     def upload_pages(self, streams) -> None:
         """Copy the listed streams' rows of the host page table to the device table (stream-ordered: frames already

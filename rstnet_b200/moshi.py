@@ -367,6 +367,13 @@ class _GenState:
         self.off_host = np.zeros(B, dtype=np.int64)
         self.stepped = np.zeros(B, dtype=bool)      # rows that were active in the last step
 
+    def row_segments(self, b: int):
+        """Row b's delay-cache state as row_state regions: its cache columns, step count and valid flag (`out` and `user`
+        are rewritten by every step before they are read)."""
+        from .row_state import tensor_segs
+        return [("cache", tensor_segs(self.cache[b])), ("off", tensor_segs(self.off[b:b + 1])),
+                ("valid", tensor_segs(self.valid[b:b + 1]))]
+
     @property
     def offset(self) -> int:
         """The reference's single step count; defined while every row is at the same step (see `off_host`)."""

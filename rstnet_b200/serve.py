@@ -20,6 +20,12 @@ Paged KV (`kv_pages=N` on either engine): the LM scope keeps its KV in a shared 
 only for the frames it has run -- one at admission, one more each time it crosses a page boundary, all returned when it
 ends.  The engine then also has `grow_kv(rows)`, `release_rows(rows)` and `kv_pages_free` (`_PagedRows`), and the
 scheduler admits on free pages and evicts a session whose next page the pool cannot give.
+
+Suspend / resume (`suspend_rows(rows)` / `resume_rows(rows, states)` on either engine, paged or not; `_SessionRows`): a
+session's state -- codec carries and rings, resampler carries, the KV it wrote, counters, sampling settings -- is packed
+into pinned host memory (row_state.SessionState), which frees its row and its pages; later it is unpacked into any free
+row of a compatible engine, and the session goes on with the bytes an uninterrupted run would have produced.
+`FrameScheduler(on_short="suspend")` suspends a session the pool cannot grow instead of evicting it.
 """
 from __future__ import annotations
 
@@ -31,6 +37,7 @@ from typing import Deque, Dict, Hashable, List, Optional, Tuple
 import numpy as np
 import torch
 
+from . import row_state
 from ._lib import RstnetError
 from .audio import StreamingResampler
 from .lm import KV_PAGE, MAX_STREAMS, Sampling
@@ -57,14 +64,27 @@ class FrameScheduler:
     On an engine with paged KV (its `kv_pages` is not None) a session also holds KV pages: admission takes its first page
     and refuses while fewer than 1 + kv_headroom pages are free (kv_headroom: pages left for the live sessions to grow
     into); every tick first grows the ready sessions oldest first, and one whose next page the pool cannot give is
-    evicted -- its row and pages returned, its queued frames dropped, not stepped -- and reported by `take_evicted()`."""
+    evicted -- its row and pages returned, its queued frames dropped, not stepped -- and reported by `take_evicted()`.
 
-    def __init__(self, engine, capacity: int, kv_headroom: int = 0):
+    Suspension (an engine with suspend_rows / resume_rows): `suspend(session)` packs the session's state into host
+    memory and frees its row and pages; its queue stays, and `push` keeps queueing to it.  `resume(session)` unpacks it
+    into the lowest free row.  With on_short="suspend" a session whose next page the pool cannot give is suspended
+    instead of evicted, and every tick first resumes suspended sessions, oldest first, while a row and
+    pages_for(its positions) + 1 + kv_headroom pages are free.  A resumed session still steps one frame per tick, so it
+    lags by the ticks it spent suspended (its queue holds the frames pushed meanwhile); `lag` records them per session."""
+
+    def __init__(self, engine, capacity: int, kv_headroom: int = 0, on_short: str = "evict"):
         self.engine, self.capacity = engine, capacity
         self.paged = getattr(engine, "kv_pages", None) is not None
         if isinstance(kv_headroom, bool) or not isinstance(kv_headroom, int) or kv_headroom < 0:
             raise RstnetError(f"kv_headroom must be an int >= 0 (got {kv_headroom!r})")
-        self.kv_headroom = kv_headroom
+        if on_short not in ("evict", "suspend"):
+            raise RstnetError(f"on_short must be 'evict' or 'suspend' (got {on_short!r})")
+        self.kv_headroom, self.on_short = kv_headroom, on_short
+        self._suspended: Dict[Hashable, object] = {}   # session -> SessionState, in suspension order
+        self._suspended_at: Dict[Hashable, int] = {}
+        self.lag: Dict[Hashable, int] = {}              # ticks each session has spent suspended
+        self.suspensions = self.resumes = 0
         self._row_of: Dict[Hashable, int] = {}     # in admission order
         self._free: List[int] = list(range(capacity))
         self._queue: Dict[Hashable, Deque] = {}
@@ -96,6 +116,10 @@ class FrameScheduler:
         return row
 
     def release(self, session: Hashable) -> None:
+        if session in self._suspended:       # its state and queue are dropped; it holds no row or pages
+            del self._suspended[session], self._suspended_at[session]
+            self._queue.pop(session, None)
+            return
         row = self._row_of.pop(session)
         self._queue.pop(session, None)
         self._free.append(row)
@@ -106,6 +130,51 @@ class FrameScheduler:
         """The sessions evicted since the last call (paged KV: the pool had no page for their next frame), oldest first."""
         out, self._evicted = self._evicted, []
         return out
+
+    def suspend(self, session: Hashable):
+        """Pack the session's state into host memory (engine.suspend_rows) and free its row and pages; its queue stays.
+        -> its SessionState."""
+        row = self._row_of[session]
+        state = self.engine.suspend_rows([row])[0]
+        del self._row_of[session]
+        self._free.append(row)
+        self._suspended[session], self._suspended_at[session] = state, self.ticks
+        self.suspensions += 1
+        return state
+
+    def resume(self, session: Hashable) -> int:
+        """Unpack a suspended session into the lowest free row (engine.resume_rows; a short pool raises and changes
+        nothing).  -> the row."""
+        if session not in self._suspended:
+            raise RuntimeError(f"session {session!r} is not suspended")
+        if not self._free:
+            raise RuntimeError("no free row: the batch is full")
+        self._free.sort()
+        row = self._free[0]
+        self.engine.resume_rows([row], [self._suspended[session]])
+        self._free.pop(0)
+        del self._suspended[session]
+        self.lag[session] = self.lag.get(session, 0) + self.ticks - self._suspended_at.pop(session)
+        self._row_of[session] = row
+        self.resumes += 1
+        return row
+
+    def suspended(self) -> List[Hashable]:
+        """The suspended sessions, oldest suspension first."""
+        return list(self._suspended)
+
+    def _resume_waiting(self) -> None:
+        """on_short="suspend": resume suspended sessions, oldest first, while a row and their pages (+ 1 + kv_headroom)
+        are free."""
+        if self.paged:
+            self.engine.reclaim()
+        for s in list(self._suspended):
+            if not self._free:
+                return
+            if self.paged and self.engine.kv_pages_free < (self.engine.kv_pages_for(max(self._suspended[s].positions, 1)) + 1
+                                                            + self.kv_headroom):
+                return
+            self.resume(s)
 
     def sessions(self) -> Dict[Hashable, int]:
         return dict(self._row_of)
@@ -120,14 +189,19 @@ class FrameScheduler:
 
     def tick(self) -> Dict[Hashable, Tuple]:
         """One scheduler period: step every session that has a frame queued; returns {session: (tokens, pcm)}."""
+        if self.on_short == "suspend" and self._suspended:
+            self._resume_waiting()
         ready = {s: r for s, r in self._row_of.items() if self._queue[s]}
         self.ticks += 1
         if self.paged and ready:
             short = set(self.engine.grow_kv(list(ready.values())))     # admission order: the oldest sessions grow first
             for s in [s for s, r in ready.items() if r in short]:
                 del ready[s]
-                self.release(s)
-                self._evicted.append(s)
+                if self.on_short == "suspend":
+                    self.suspend(s)
+                else:
+                    self.release(s)
+                    self._evicted.append(s)
         if not ready:
             return {}
         pcm_rows = {r: self._queue[s].popleft() for s, r in ready.items()}
@@ -151,6 +225,7 @@ class _PagedRows:
     def grow_kv(self, rows) -> List[int]:
         """Walk `rows` in order: a row whose next position lies past its pages gets one more page while the pool has
         one.  A row that holds its whole ring needs none.  -> the rows that could not get their page (unchanged)."""
+        self.reclaim()
         st = self._kv_lm._paged()
         kp = st.pages
         grow, want, short = [], [], []
@@ -177,10 +252,237 @@ class _PagedRows:
 
     @property
     def kv_pages_free(self) -> int:
+        """Pages no row holds, without the pages of suspended rows whose gather is still in flight."""
         return self._kv_lm.kv_pages_free
 
+    def kv_pages_for(self, positions: int) -> int:
+        return self._kv_lm._paged().pages.pages_for(positions)
 
-class DuplexEngine(_PagedRows):
+    def reclaim(self) -> int:
+        """Return the pages of suspended rows whose gather has completed to the pool (no wait).  -> pages returned."""
+        n = 0
+        for item in list(getattr(self, "_in_flight", ())):
+            if item[0].query():
+                self._kv_lm._paged().pages.give_back(item[1])
+                self._in_flight.remove(item)
+                n += len(item[1])
+        return n
+
+
+class _SessionRows:
+    """Suspend / resume of both duplex engines.  The engine lists a row's state as row_state regions (`_row_regions`) and
+    host fields (`_row_host` / `_set_row_host`); this class moves them with one segment gather / scatter launch per row on
+    a side stream of at most `swap_ctas` CTAs.
+
+    Ordering, with no host synchronise on the tick path:
+      * suspend: the gather waits (an event) for the ticks already enqueued; the row then stays held -- a held row's
+        state does not advance -- and its pages are unmapped but stay out of the pool until the gather's completion
+        event has passed (`reclaim`, or the next tick).
+      * resume: the scatter waits for the ticks already enqueued, for the state's gather and for any swap still touching
+        the row; the next tick makes the main stream wait for the scatter (every tick runs every row of the batch, held
+        ones included, so no tick may touch the row before its state has landed).
+      * reset_rows of a row makes the main stream wait for every gather or scatter still touching it, so a session
+        admitted into a row whose previous session was just suspended (or resumed and released) starts clean.
+    Host memory: the pinned blob and table of every swap are kept by the engine until the swap has completed, so a
+    caller may drop a SessionState at any time.  The blob of a resumed state returns to the engine's pool once its
+    scatter has completed (the state is then consumed), and later suspends reuse pooled blobs (best fit) before they
+    allocate; `pin_host_blobs` fills the pool up front so that suspension allocates nothing on the tick path.
+    Sampling: a resumed session draws from its own key and frame count, so resume_rows switches the engine to per-row
+    random streams, exactly as reset_rows(seed=...) does; sessions restore bit for bit when they were admitted with a
+    seed or settings (per-row streams from the start).  Resuming into an engine of another capacity is allowed but its
+    results are not promised bit for bit (the LM GEMM's split-K count depends on the batch)."""
+
+    swap_ctas = 16
+    _swap_stream: Optional[torch.cuda.Stream] = None
+
+    def _swap_init(self) -> None:
+        self._row_swaps: Dict[int, torch.cuda.Event] = {}   # row -> the last gather / scatter touching it
+        self._scatters: List[torch.cuda.Event] = []         # scatters the next tick waits for
+        self._in_flight: List[Tuple[torch.cuda.Event, List[int]]] = []
+        self._keep: List[tuple] = []                        # (event, objects a swap reads / writes, blob to pool or None)
+        self._blob_pool: List[torch.Tensor] = []
+
+    def _prune(self) -> None:
+        """drop the host memory of completed swaps; the blobs of completed resumes go back to the pool"""
+        keep = []
+        for item in self._keep:
+            if item[0].query():
+                if item[2] is not None:
+                    self._blob_pool.append(item[2])
+            else:
+                keep.append(item)
+        self._keep = keep
+
+    def _before_tick(self) -> None:
+        """the tick waits for the scatters enqueued since the last one; finished swaps give back their host memory and
+        pages"""
+        self._wait_scatters()
+        if self._keep:
+            self._prune()
+        if self.kv_pages is not None:
+            self.reclaim()
+
+    def pin_host_blobs(self, count: int, nbytes: int) -> None:
+        """Add `count` pinned blobs of `nbytes` bytes to the pool suspensions draw from (row_bytes(positions) gives a
+        session's size), so that suspending allocates no pinned memory while the engine serves."""
+        for _ in range(int(count)):
+            self._blob_pool.append(torch.empty(max(int(nbytes), 1), dtype=torch.uint8, pin_memory=True))
+
+    def drop_host_blobs(self) -> None:
+        """Free the pooled blobs (blobs of live SessionStates are not pooled)."""
+        self._prune()
+        self._blob_pool = []
+
+    def _take_blob(self, nbytes: int) -> torch.Tensor:
+        fit = [i for i, b in enumerate(self._blob_pool) if b.numel() >= nbytes]
+        if fit:
+            return self._blob_pool.pop(min(fit, key=lambda i: self._blob_pool[i].numel()))
+        return torch.empty(max(nbytes, 1), dtype=torch.uint8, pin_memory=True)
+
+    def row_bytes(self, positions: int) -> int:
+        """the blob size of a session that has run `positions` LM positions"""
+        c = self._lm_config()
+        kv = c.n_layer * 2 * c.n_query_groups * min(int(positions), c.context) * c.head_size * 2
+        return row_state.layout(self._row_regions(0, dict(self._row_host(0), pos=0)))[1] + -(-kv // row_state.ALIGN) * row_state.ALIGN
+
+    def _side(self) -> torch.cuda.Stream:
+        if self._swap_stream is None:
+            self._swap_stream = torch.cuda.Stream(device=self.dev)
+        return self._swap_stream
+
+    def _wait_rows(self, rows) -> None:
+        """the main stream waits for the gathers and scatters still touching these rows"""
+        for r in rows:
+            ev = self._row_swaps.pop(int(r), None)
+            if ev is not None:
+                torch.cuda.current_stream(self.dev).wait_event(ev)
+
+    def _wait_scatters(self) -> None:
+        if self._scatters:
+            main = torch.cuda.current_stream(self.dev)
+            for ev in self._scatters:
+                main.wait_event(ev)
+            self._scatters = []
+
+    def session_key(self) -> Tuple:
+        """what a SessionState must match to restore here: engine kind, LM and codec shapes, client rate, KV page"""
+        cfg = self._lm_config()
+        cfg = sorted((vars(cfg) if not hasattr(cfg, "__dataclass_fields__") else
+                      {k: getattr(cfg, k) for k in cfg.__dataclass_fields__}).items())
+        m = self.codec
+        codec = (m.sample_rate, m.n_filters, tuple(m.ratios), m.compress, m.latent_dim, m.codebook_size, m.codebook_dim, m.n_q,
+                 m.num_heads, m.num_layers, m.context)
+        page = self._kv_lm._paged().pages.page if self.kv_pages is not None else self._kv_page
+        return (type(self).__name__, repr(cfg), codec, self.sample_rate, page)
+
+    def _common_regions(self, row: int, positions: int):
+        regions = [("codec." + n, sg) for n, sg in self.codec._stream_state.row_segments(row, FRAME_SAMPLES, 1, self._n_codes)]
+        if self.up is not None:
+            regions += [("up." + n, sg) for n, sg in self.up.row_segments(row, self.frame_samples)]
+            regions += [("down." + n, sg) for n, sg in self.down.row_segments(row, FRAME_SAMPLES)]
+        regions += [("lm." + n, sg) for n, sg in self._lm_state().row_segments(row, positions)]
+        return regions
+
+    @torch.no_grad()
+    def suspend_rows(self, rows, ctas: Optional[int] = None) -> List[row_state.SessionState]:
+        """Pack each row's state into a pinned host blob (one gather per row on the side stream, after the ticks already
+        enqueued) and free the row: it stays held, and on a paged engine its pages return to the pool once the gather
+        has completed.  -> one SessionState per row.  The caller no longer steps these rows (a FrameScheduler frees
+        them); they are restarted by reset_rows or resume_rows."""
+        rows = [int(r) for r in rows]
+        if len(set(rows)) != len(rows) or any(not 0 <= r < self.B for r in rows):
+            raise RstnetError(f"rows must be distinct and in [0, {self.B})")
+        # every row's segments first (this may build the codec plans or resampler buffers, on the main stream), so that a
+        # row that cannot be listed raises before anything changes, and the gathers are ordered after those writes
+        key, plans = self.session_key(), []
+        for r in rows:
+            host = self._row_host(r)
+            regions = self._row_regions(r, host)
+            table, nbytes = row_state.layout(regions)
+            plans.append((r, host, row_state.signature(regions), table, nbytes))
+        if self._keep:
+            self._prune()
+        main, side = torch.cuda.current_stream(self.dev), self._side()
+        side.wait_stream(main)
+        states = []
+        for r, host, sig, table, nbytes in plans:
+            blob = self._take_blob(nbytes)
+            tab = row_state.pinned_table(table)
+            row_state.run("gather", tab, len(table), blob, side, ctas or self.swap_ctas)
+            done = torch.cuda.Event()
+            done.record(side)
+            self._row_swaps[r] = done
+            self._keep.append((done, (tab, blob), None))    # the gather writes the blob: alive until it completed
+            states.append(row_state.SessionState(key, sig, blob, nbytes, host, done, tab))
+            if self.kv_pages is not None:
+                st = self._kv_lm._paged()
+                self._in_flight.append((done, st.pages.detach(r)))
+                st.upload_pages([r])          # stream-ordered: later ticks write nothing to the pages of this row
+        return states
+
+    @torch.no_grad()
+    def resume_rows(self, rows, states, ctas: Optional[int] = None) -> None:
+        """Unpack each state into its row (a free row: on a paged engine, one that holds no pages).  A paged engine first
+        reserves pages for the state's positions (a short pool raises and changes nothing).  The scatter runs on the
+        side stream after the ticks already enqueued and after the state's gather; the next tick waits for it.  An
+        incompatible state (other engine kind, LM or codec shapes, client rate or KV page) raises RstnetError."""
+        rows = [int(r) for r in rows]
+        states = list(states)
+        if len(rows) != len(states) or len(set(rows)) != len(rows) or any(not 0 <= r < self.B for r in rows):
+            raise RstnetError(f"rows must be distinct, in [0, {self.B}), one per state")
+        key = self.session_key()
+        for s in states:
+            if not isinstance(s, row_state.SessionState):
+                raise RstnetError(f"expected a SessionState, got {type(s).__name__}")
+            if s.key != key:
+                row_state.check_compatible(s, key, ())
+            if s.blob is None:
+                raise RstnetError("this session state was already resumed")
+        if len({id(s) for s in states}) != len(states):
+            raise RstnetError("a session state is listed twice")
+        if self.kv_pages is not None:
+            pages = self._kv_lm._paged().pages
+            if any(pages.held[r] for r in rows):
+                raise RstnetError("resume_rows needs free rows: a listed row holds KV pages")
+            self.reclaim()
+            # positions up to the page boundary (at least the first page), as growth and admission reserve
+            P = pages.page
+            self._kv_lm.reserve_kv(rows, [max(P, -(-s.positions // P) * P) for s in states])
+        try:
+            plans = []
+            for r, s in zip(rows, states):
+                regions = self._row_regions(r, s.host)
+                row_state.check_compatible(s, key, regions)
+                plans.append(row_state.layout(regions)[0])
+        except Exception:
+            if self.kv_pages is not None:
+                self._kv_lm.release_kv(rows)
+            raise
+        self._per_row_sampling()              # before the scatters: a first switch rewrites every row's key
+        if self._keep:
+            self._prune()
+        main, side = torch.cuda.current_stream(self.dev), self._side()
+        side.wait_stream(main)
+        for r, s, table in zip(rows, states, plans):
+            if s.ready is not None:
+                side.wait_event(s.ready)
+            prev = self._row_swaps.get(r)
+            if prev is not None:
+                side.wait_event(prev)
+            tab = row_state.pinned_table(table)
+            row_state.run("scatter", tab, len(table), s.blob, side, ctas or self.swap_ctas)
+            done = torch.cuda.Event()
+            done.record(side)
+            self._scatters.append(done)
+            self._row_swaps[r] = done        # a reset_rows of this row before the next tick waits for it too
+            # the scatter reads the blob (and the gather's table may still be referenced): kept until it completed, then
+            # the blob joins the pool and the state is consumed
+            self._keep.append((done, (tab, s._table), s.blob))
+            s.blob, s._table = None, None
+            self._set_row_host(r, s.host)
+
+
+class DuplexEngine(_SessionRows, _PagedRows):
     """One streaming scope of a MimiCodec and a GPT for `capacity` sessions: per tick, for all rows at once,
     encode the sessions' 80 ms chunks -> one LM frame (temporal step + 8 depth steps + sampling) -> decode the generated
     codes (the three calls of server.py:128-136).  The LM input frame of a row is [its previous text token, the 8 codes of
@@ -231,6 +533,32 @@ class DuplexEngine(_PagedRows):
         self.pcm_host = torch.zeros(capacity, 1, F, dtype=torch.float32).pin_memory()
         self.mask_host = torch.zeros(capacity, dtype=torch.int64).pin_memory()
         self.latencies_ms: List[float] = []
+        self._kv_page, self._n_codes = kv_page, gpt.config.dep_q
+        self._swap_init()
+
+    # ---- the row state of suspend_rows / resume_rows (_SessionRows)
+    def _lm_config(self):
+        return self.gpt.config
+
+    def _lm_state(self):
+        return self.gpt._state
+
+    def _row_host(self, r: int) -> dict:
+        return {"pos": int(self.gpt._state.pos_host[r]), "key": int(self.row_keys[r]),
+                "sampling": None if self.row_sampling is None else self.row_sampling[r]}
+
+    def _row_regions(self, r: int, host: dict):
+        return self._common_regions(r, host["pos"]) + [("prev_text", row_state.tensor_segs(self.prev_text[r]))]
+
+    def _per_row_sampling(self) -> None:
+        if self.row_sampling is None:
+            self.row_sampling = [Sampling(*self._defaults)] * self.B
+
+    def _set_row_host(self, r: int, host: dict) -> None:
+        self.gpt._state.pos_host[r] = host["pos"]
+        self.row_sampling[r] = host["sampling"] if host["sampling"] is not None else Sampling(*self._defaults)
+        self.row_keys[r] = host["key"]
+        self._keys_dirty = True
 
     def reset_rows(self, rows, sampling=None, seed: Optional[int] = None) -> None:
         """Restart `rows`.  sampling / seed give them their own settings and random stream (keyed by the seed and the
@@ -248,6 +576,7 @@ class DuplexEngine(_PagedRows):
                 self.row_sampling[r] = sampling if sampling is not None else default
                 self.row_keys[r] = int(seed or 0) & 0xFFFFFFFF
             self._keys_dirty = True
+        self._wait_rows(rows)
         self._reserve_first_page(rows)
         self.codec.reset_streaming(streams=list(rows))
         self.gpt.reset_streaming(streams=list(rows))
@@ -259,6 +588,7 @@ class DuplexEngine(_PagedRows):
     @torch.no_grad()
     def step(self, pcm_rows: Dict[int, torch.Tensor], active: List[int]):
         t0 = time.perf_counter()
+        self._before_tick()
         self.mask_host.zero_()
         for r, chunk in pcm_rows.items():
             self.pcm_in[r, 0].copy_(torch.as_tensor(chunk, dtype=torch.float32).reshape(self.frame_samples))
@@ -294,7 +624,7 @@ class DuplexEngine(_PagedRows):
         return {r: (self.tok_host[r].clone(), self.pcm_host[r, 0].clone()) for r in active}
 
 
-class MoshiDuplexEngine(_PagedRows):
+class MoshiDuplexEngine(_SessionRows, _PagedRows):
     """The serving loop of server.py:128-136 -- `mimi.encode -> lm_gen.step(codes) -> mimi.decode(tokens[:, 1:])` --
     for `capacity` sessions in one streaming scope of a MimiCodec and an `LMGen` (rstnet_b200.moshi).
 
@@ -340,9 +670,38 @@ class MoshiDuplexEngine(_PagedRows):
         self.dec_mask_host = torch.zeros(capacity, dtype=torch.int64, pin_memory=pin)
         self.dec_mask_dev = torch.zeros(capacity, dtype=torch.int64, device=self.dev)
         self.latencies_ms: List[float] = []
+        self._kv_page, self._n_codes = kv_page, lm.dep_q
+        self._swap_init()
+
+    # ---- the row state of suspend_rows / resume_rows (_SessionRows): the decoder's warm-up is the delay cache's step
+    # count (off_host: no tokens, and the codec decoder held, for the first max_delay steps)
+    def _lm_config(self):
+        return self.lm_gen.lm_model.config
+
+    def _lm_state(self):
+        return self.lm_gen.lm_model._state
+
+    def _row_host(self, r: int) -> dict:
+        g = self.lm_gen
+        return {"pos": int(g._st.lm.pos_host[r]), "off": int(g._st.off_host[r]), "stepped": bool(g._st.stepped[r]),
+                "sampling": None if g._row_sampling is None else g._row_sampling[r]}
+
+    def _row_regions(self, r: int, host: dict):
+        return self._common_regions(r, host["pos"]) + [("gen." + n, sg) for n, sg in self.lm_gen._st.row_segments(r)]
+
+    def _per_row_sampling(self) -> None:
+        if self.lm_gen._row_sampling is None:
+            self.lm_gen.set_stream_sampling([])
+
+    def _set_row_host(self, r: int, host: dict) -> None:
+        g = self.lm_gen
+        g._st.lm.pos_host[r] = host["pos"]
+        g._st.off_host[r], g._st.stepped[r] = host["off"], host["stepped"]
+        g._row_sampling[r] = host["sampling"] if host["sampling"] is not None else g.default_sampling()
 
     def reset_rows(self, rows, sampling=None, seed: Optional[int] = None) -> None:
         """Restart `rows`; sampling / seed as DuplexEngine.reset_rows (LMGen.set_stream_sampling)."""
+        self._wait_rows(rows)
         self._reserve_first_page(rows)
         self.codec.reset_streaming(streams=list(rows))
         self.lm_gen.reset_streaming(streams=list(rows))
@@ -355,6 +714,7 @@ class MoshiDuplexEngine(_PagedRows):
     @torch.no_grad()
     def step(self, pcm_rows: Dict[int, torch.Tensor], active: List[int]):
         t0 = time.perf_counter()
+        self._before_tick()
         self.mask_host.zero_()
         for r, chunk in pcm_rows.items():
             self.pcm_in[r, 0].copy_(torch.as_tensor(chunk, dtype=torch.float32).reshape(self.frame_samples))

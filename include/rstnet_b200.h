@@ -421,6 +421,16 @@ int rstnet_lm_rope_pair_kv_append_paged_bf16(const void* qkv, const int64_t* off
                                              int32_t rows, int32_t B, int32_t H, int32_t hd, int32_t cap, const float* freqs,
                                              const int32_t* page_table, int32_t pages_stride, int32_t log2_page,
                                              rstnet_stream_t stream);
+/* ---- the Kyutai pair-RoPE append with a row map over contiguous rings (ragged chunks that pack many utterances:
+ * rstnet_b200.moshi.score_many, LMModel.forward): row r is stream row_stream[r] at position offset[row_stream[r]] + row_tl[r]
+ * (offset int64 [B], one counter per stream), and row_stream[r] == -1 marks a padding row that reads and writes nothing,
+ * neither q_out nor K/V.  The angle is fp32(offset) + fp32(tl) times freqs, as in the uniform form, and every stored byte
+ * equals a uniform launch's for the same (stream, position).  Null pointers (either half of the map included), rows < 1 and
+ * bad shapes are error returns before any launch.  Same kernel as rstnet_lm_rope_pair_kv_append_bf16.
+ * Reference call site: models/model.py:364-389 (forward_text over a whole sequence, modules/transformer.py:391-399). */
+int rstnet_lm_rope_pair_kv_append_rows_bf16(const void* qkv, const int64_t* offset, const int32_t* row_stream, const int32_t* row_tl,
+                                            void* q_out, void* kv, int32_t rows, int32_t B, int32_t H, int32_t hd, int32_t cap,
+                                            const float* freqs, rstnet_stream_t stream);
 /* ---- one query position per row over the ring with RingKVCache.complete's position labels and the
  * (pos_k>=0)&(delta>=0)&(delta<context) mask (llama_streaming.py:983-992), fp32 softmax. HBM-bound.  Rows and row map as
  * rstnet_lm_rope_kv_append_bf16 (padding rows write no output); every position of the launch must already be in the ring

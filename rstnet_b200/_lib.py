@@ -31,7 +31,7 @@ SYMBOLS = [
     "rstnet_lm_cross_entropy_bf16", "rstnet_rows_fill_tail_f32", "rstnet_lm_sample_params_bf16",
     "rstnet_lm_rope_kv_append_paged_bf16", "rstnet_lm_paged_decode_attention_bf16", "rstnet_lm_rope_pair_kv_append_paged_bf16",
     "rstnet_stft_loss_workspace", "rstnet_stft_loss_sums_f32", "rstnet_sisnr_moments_workspace", "rstnet_sisnr_moments_f32",
-    "rstnet_segments_gather", "rstnet_segments_scatter",
+    "rstnet_segments_gather", "rstnet_segments_scatter", "rstnet_lm_rope_pair_kv_append_rows_bf16",
 ]
 
 KV_LOG2_PAGE_MIN, KV_LOG2_PAGE_MAX = 4, 12   # RSTNET_KV_LOG2_PAGE_MIN / _MAX: pages of 16 .. 4096 positions
@@ -160,6 +160,7 @@ def lib() -> C.CDLL:
     L.rstnet_lm_rope_kv_append_bf16.argtypes = [vp, vp, vp, i64, i32, vp, i32, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]
     L.rstnet_lm_rope_pair_kv_append_bf16.argtypes = [vp, vp, i32, vp, vp, i32, i32, i32, i32, i32, vp, vp]
     L.rstnet_lm_rope_pair_kv_append_paged_bf16.argtypes = [vp, vp, i32, vp, vp, i32, i32, i32, i32, i32, vp, vp, i32, i32, vp]
+    L.rstnet_lm_rope_pair_kv_append_rows_bf16.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp]
     L.rstnet_lm_ring_decode_attention_bf16.argtypes = [vp, vp, vp, i32, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp]
     L.rstnet_lm_rope_kv_append_paged_bf16.argtypes = [vp, vp, vp, i64, i32, vp, i32, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32,
                                                       vp, i32, i32, vp]

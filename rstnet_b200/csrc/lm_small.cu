@@ -170,14 +170,26 @@ __global__ void rope_kv_append_bf16_kernel(const bf16* __restrict__ qkv, const b
 // Page table (paged KV, LMModel.streaming(B, kv_pages=N)): as rope_kv_append_bf16_kernel's -- slot s of stream b lives in
 // page page_table[b * pages_stride + (s >> log2_page)], row s & (2^log2_page - 1), of a pool kv[n_pages][2][H][2^log2_page][hd],
 // and a row whose own slot falls on an unmapped page (-1) writes nothing, q_out included.  A runtime branch of the same body.
+// Row map (ragged chunks of many streams, LMModel.forward / moshi.score_many): as rope_kv_append_bf16_kernel's -- row r is
+// stream row_stream[r] at position offset[row_stream[r]] + row_tl[r], and row_stream[r] == -1 is a padding row that reads
+// and writes nothing, q_out included.  The angle is fp32(offset) + fp32(tl) either way.  Again a runtime branch.
 __global__ void rope_pair_kv_append_bf16_kernel(const bf16* __restrict__ qkv, const long long* __restrict__ offset, int ostride,
                                                 bf16* __restrict__ q_out, bf16* __restrict__ kv, int B, int H, int hd, int cap,
                                                 const float* __restrict__ freqs, const int* __restrict__ page_table,
-                                                int pages_stride, int log2_page) {
+                                                int pages_stride, int log2_page, const int* __restrict__ row_stream,
+                                                const int* __restrict__ row_tl) {
   const int row = blockIdx.x / H, h = blockIdx.x % H;
-  const int b = row % B;
+  int b, tl;
+  if (row_stream) {
+    b = row_stream[row];
+    if (b < 0) return;
+    tl = row_tl[row];
+  } else {
+    b = row % B;
+    tl = row / B;
+  }
   const long long off = offset[(long long)b * ostride];
-  const long long pos = off + row / B;
+  const long long pos = off + tl;
   const int slot = (int)(pos % cap);
   const int HD = H * hd;
   const bf16* q = qkv + (long long)row * 3 * HD + h * hd;
@@ -195,7 +207,7 @@ __global__ void rope_pair_kv_append_bf16_kernel(const bf16* __restrict__ qkv, co
     vofs = (long long)B * H * cap * hd;
   }
   bf16* vdst = kdst + vofs;
-  const float ts = __fadd_rn((float)off, (float)(row / B));     // offset.float() + arange(T) in fp32 (rope.py:37)
+  const float ts = __fadd_rn((float)off, (float)tl);     // offset.float() + arange(T) in fp32 (rope.py:37)
   for (int pr = threadIdx.x; pr < hd / 2; pr += blockDim.x) {
     const float ang = __fmul_rn(freqs[pr], ts);     // freqs = exp(ds * (-ln(max_period) * 2 / hd)) from the host (rope.py:35-36)
     const float c = cosf(ang), s = sinf(ang);
@@ -976,12 +988,14 @@ extern "C" int rstnet_lm_rope_kv_append_paged_bf16(const void* qkv, const void* 
 
 static int rope_pair_kv_append(const void* qkv, const int64_t* offset, int32_t offset_stride, void* q_out, void* kv, int32_t rows,
                                int32_t B, int32_t H, int32_t hd, int32_t cap, const float* freqs, const int32_t* page_table,
-                               int32_t pages_stride, int32_t log2_page, rstnet_stream_t stream) {
+                               int32_t pages_stride, int32_t log2_page, const int32_t* row_stream, const int32_t* row_tl,
+                               rstnet_stream_t stream) {
   RSTNET_REQUIRE(qkv && offset && q_out && kv && freqs, "lm_rope_pair_kv_append: null pointer");
-  RSTNET_REQUIRE(rows > 0 && B > 0 && rows % B == 0 && H > 0 && hd > 0 && hd % 2 == 0 && cap > 0, "lm_rope_pair_kv_append: bad shape");
+  RSTNET_REQUIRE(rows > 0 && B > 0 && (row_stream || rows % B == 0) && H > 0 && hd > 0 && hd % 2 == 0 && cap > 0,
+                 "lm_rope_pair_kv_append: bad shape");
   rope_pair_kv_append_bf16_kernel<<<dim3(rows * H), dim3(64), 0, (cudaStream_t)stream>>>((const bf16*)qkv,
              (const long long*)offset, offset_stride ? 1 : 0, (bf16*)q_out, (bf16*)kv, B, H, hd, cap, freqs, (const int*)page_table,
-             pages_stride, log2_page);
+             pages_stride, log2_page, (const int*)row_stream, (const int*)row_tl);
   count_launch();
   return check_launch("lm_rope_pair_kv_append");
 }
@@ -989,7 +1003,7 @@ static int rope_pair_kv_append(const void* qkv, const int64_t* offset, int32_t o
 extern "C" int rstnet_lm_rope_pair_kv_append_bf16(const void* qkv, const int64_t* offset, int32_t offset_stride, void* q_out, void* kv,
                                                   int32_t rows, int32_t B, int32_t H, int32_t hd, int32_t cap, const float* freqs,
                                                   rstnet_stream_t stream) {
-  return rope_pair_kv_append(qkv, offset, offset_stride, q_out, kv, rows, B, H, hd, cap, freqs, nullptr, 0, 0, stream);
+  return rope_pair_kv_append(qkv, offset, offset_stride, q_out, kv, rows, B, H, hd, cap, freqs, nullptr, 0, 0, nullptr, nullptr, stream);
 }
 
 extern "C" int rstnet_lm_rope_pair_kv_append_paged_bf16(const void* qkv, const int64_t* offset, int32_t offset_stride, void* q_out,
@@ -998,7 +1012,14 @@ extern "C" int rstnet_lm_rope_pair_kv_append_paged_bf16(const void* qkv, const i
                                                         int32_t log2_page, rstnet_stream_t stream) {
   if (check_pages("lm_rope_pair_kv_append_paged", page_table, pages_stride, log2_page, cap)) return 1;
   return rope_pair_kv_append(qkv, offset, offset_stride, q_out, kv, rows, B, H, hd, cap, freqs, page_table, pages_stride, log2_page,
-                             stream);
+                             nullptr, nullptr, stream);
+}
+
+extern "C" int rstnet_lm_rope_pair_kv_append_rows_bf16(const void* qkv, const int64_t* offset, const int32_t* row_stream,
+                                                       const int32_t* row_tl, void* q_out, void* kv, int32_t rows, int32_t B, int32_t H,
+                                                       int32_t hd, int32_t cap, const float* freqs, rstnet_stream_t stream) {
+  RSTNET_REQUIRE(row_stream && row_tl, "lm_rope_pair_kv_append_rows: null row map");
+  return rope_pair_kv_append(qkv, offset, 1, q_out, kv, rows, B, H, hd, cap, freqs, nullptr, 0, 0, row_stream, row_tl, stream);
 }
 
 static int ring_decode_attention(const void* q, const void* kv, const int64_t* offset, int32_t offset_stride,

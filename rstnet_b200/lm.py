@@ -375,7 +375,53 @@ class PagedKVModel:
         return kv_page_bytes(self.config, self._paged().pages.page)
 
 
-class GPT(PagedKVModel, nn.Module):
+class DepthLocalModel:
+    """The non-streaming depth transformer (`forward_local`, and the depth-only states teacher-forced scoring runs) and the
+    device error check, shared by `GPT` and the Moshi twin's `LMModel` (rstnet_b200.moshi): the depth transformer is the
+    same module in both, read through the parameter names of `_DN`.  A model provides `_make_state(B, **kw)` (its scope
+    class), `_check_runnable()` and a `_local_states` dict."""
+
+    def check_device_errors(self, clear: bool = True) -> None:
+        """Raise if a kernel met an input the reference would have raised on (out-of-range token id, position beyond
+        block_size): device code cannot raise, it poisons its output and sets a sticky flag (synchronises)."""
+        with torch.cuda.device(self.device):
+            flags = int(_lib.lib().rstnet_device_error_flags(int(clear)))
+        if flags & 1:
+            raise IndexError("a token id was outside its embedding table (index out of range in self)")
+        if flags & 2:
+            raise IndexError(f"a position reached block_size = {self.config.block_size} (RoPE table exhausted)")
+
+    @torch.no_grad()
+    @on_own_device
+    def forward_local(self, local_start_token: torch.Tensor, sequence: torch.Tensor, transformer_out: torch.Tensor) -> torch.Tensor:
+        """llama_streaming.py:694-725 (GPT) / models/model.py:321-361 (LMModel): the depth transformer over every (stream,
+        frame) row, teacher-forced with `sequence[B, dep_q, T]`, non-streaming (every step sees all earlier keys), step 0
+        from the features local_start_token [B, T, D].  -> logits [B, T, dep_q, card]."""
+        self._check_runnable()
+        c = self.config
+        B, K, S = sequence.shape
+        assert K == c.dep_q, f"Sequence shape {sequence.shape} must match the moshi stream output."
+        rows = B * S
+        start = local_start_token.reshape(rows, -1).to(torch.bfloat16)
+        tout = transformer_out.reshape(rows, -1).to(torch.bfloat16)
+        ids = sequence.permute(0, 2, 1).reshape(rows, K).to(torch.int64)
+        out = torch.empty(rows, c.dep_q, c.audio_card, dtype=torch.bfloat16, device=self.device)
+        for r0 in range(0, rows, MAX_ROWS):
+            n = min(MAX_ROWS, rows - r0)
+            self._depth_state(n).depth_local(start[r0:r0 + n], ids[r0:r0 + n], tout[r0:r0 + n], out[r0:r0 + n])
+        return out.view(B, S, c.dep_q, c.audio_card)
+
+    def _depth_state(self, n: int) -> "_LMState":
+        """the depth-transformer-only state of n rows (forward_local, teacher-forced scoring)"""
+        st = self._local_states.get(n)
+        if st is None:
+            if len(self._local_states) >= 4:
+                self._local_states.clear()
+            st = self._local_states[n] = self._make_state(n, parts=("depth",))
+        return st
+
+
+class GPT(PagedKVModel, DepthLocalModel, nn.Module):
     def __init__(self, config: Config, device=None, dtype=None):
         """device/dtype: create the (random-init) parameters directly there (a 7B model in bf16 on the GPU
         without a 28 GB fp32 host copy); default = CPU fp32 like the reference constructor."""
@@ -539,6 +585,9 @@ class GPT(PagedKVModel, nn.Module):
         y = torch.nn.functional.embedding(ids.clamp(min=0), w)
         return torch.where((ids == self.zero_token_id)[..., None], torch.zeros(1, dtype=y.dtype, device=y.device), y)
 
+    def _make_state(self, B: int, **kw) -> "_LMState":
+        return _LMState(self, B, **kw)
+
     # ---- StreamingModule protocol (modules/streaming.py:33-151)
     def _check_runnable(self):
         dev = self.device
@@ -597,16 +646,6 @@ class GPT(PagedKVModel, nn.Module):
             raise RuntimeError("the streaming state belongs to another model")
         self._state = st
 
-    def check_device_errors(self, clear: bool = True) -> None:
-        """Raise if a kernel met an input the reference would have raised on (out-of-range token id, position beyond
-        block_size): device code cannot raise, it poisons its output and sets a sticky flag (synchronises)."""
-        with torch.cuda.device(self.device):
-            flags = int(_lib.lib().rstnet_device_error_flags(int(clear)))
-        if flags & 1:
-            raise IndexError("a token id was outside its embedding table (index out of range in self)")
-        if flags & 2:
-            raise IndexError(f"a position reached block_size = {self.config.block_size} (RoPE table exhausted)")
-
     # ---- reference API
     @torch.no_grad()
     @on_own_device
@@ -640,34 +679,6 @@ class GPT(PagedKVModel, nn.Module):
             raise RstnetError("forward_codecformer is the streaming form: call it inside `with gpt.streaming(B):` and "
                               "`with gpt.codecformer.streaming(B):` (forward_local is the non-streaming one)")
         return self._state.forward_codecformer(codecformer_cb_index, sequence, transformer_out)
-
-    @torch.no_grad()
-    @on_own_device
-    def forward_local(self, local_start_token: torch.Tensor, sequence: torch.Tensor, transformer_out: torch.Tensor) -> torch.Tensor:
-        """llama_streaming.py:694-725: the depth transformer over every (stream, frame) row, teacher-forced with
-        `sequence[B, dep_q, T]`, non-streaming (every step sees all earlier keys).  -> logits [B, T, dep_q, card]."""
-        self._check_runnable()
-        c = self.config
-        B, K, S = sequence.shape
-        assert K == c.dep_q, f"Sequence shape {sequence.shape} must match the moshi stream output."
-        rows = B * S
-        start = local_start_token.reshape(rows, -1).to(torch.bfloat16)
-        tout = transformer_out.reshape(rows, -1).to(torch.bfloat16)
-        ids = sequence.permute(0, 2, 1).reshape(rows, K).to(torch.int64)
-        out = torch.empty(rows, c.dep_q, c.audio_card, dtype=torch.bfloat16, device=self.device)
-        for r0 in range(0, rows, MAX_ROWS):
-            n = min(MAX_ROWS, rows - r0)
-            self._depth_state(n).depth_local(start[r0:r0 + n], ids[r0:r0 + n], tout[r0:r0 + n], out[r0:r0 + n])
-        return out.view(B, S, c.dep_q, c.audio_card)
-
-    def _depth_state(self, n: int) -> "_LMState":
-        """the depth-transformer-only state of n rows (forward_local, teacher-forced scoring)"""
-        st = self._local_states.get(n)
-        if st is None:
-            if len(self._local_states) >= 4:
-                self._local_states.clear()
-            st = self._local_states[n] = _LMState(self, n, parts=("depth",))
-        return st
 
     @torch.no_grad()
     @on_own_device
@@ -819,6 +830,109 @@ def CrossEntropyAndAccuracy(logits, y, masks, loss_weights, ignore_ids=None):
     return m["loss"], m
 
 
+def score_item(seq, mask, K: int, max_frames: Optional[int] = None):
+    """Host-side checks of one scoring item -> (seq int64 [K, L], mask fp32 [K, L], frames to score).  Trailing frames
+    whose mask is zero in every codebook are dropped: the model is causal, so they change no earlier logit, and their
+    rows add nothing to any sum.  max_frames: the most frames the model can score (None: no limit)."""
+    seq, mask = torch.as_tensor(seq), torch.as_tensor(mask)
+    if seq.dim() != 2 or seq.shape[0] != K:
+        raise RstnetError(f"a scored sequence is [{K}, L], got {tuple(seq.shape)}")
+    if tuple(mask.shape) != tuple(seq.shape):
+        raise RstnetError(f"the mask must have the sequence's shape {tuple(seq.shape)}, got {tuple(mask.shape)}")
+    seq, mask = seq.to("cpu", torch.int64), mask.to("cpu", torch.float32)
+    used = torch.nonzero((mask != 0).any(0))
+    L = int(used[-1]) + 1 if used.numel() else 0
+    if max_frames is not None and L > max_frames:
+        raise RstnetError(f"{L} frames to score (after dropping all-zero-mask frames) > context = {max_frames}: "
+                          "the non-streaming temporal transformer holds at most `context` positions")
+    return seq[:, :L], mask[:, :L], L
+
+
+def score_packed(m, st: "_LMState", items, capacity: int, ignore_text: int, ignore_audio: int, depth_feed: str, check):
+    """Teacher-forced scoring of (utt_id, seq [K, L], mask [K, L]) items in shared ragged chunks: yields (utt_id,
+    sums_audio fp64 [dep_q, 5], sums_text fp64 [1, 5], frames) in completion order (fields CE_FIELDS; the caller turns
+    the sums into its metrics).  The model-independent body of InferenceImp.score_many and rstnet_b200.moshi.score_many.
+
+    st: a temporal scope of `capacity` streams of model m.  Up to `capacity` utterances are live, one stream each; each feeds
+    [initial token, seq[:, :L-1]], and their rows are packed into ragged chunks of at most MAX_ROWS rows (`row_chunk`) run
+    with the text head on.  Each chunk's rows go to the text cross-entropy, through the depth transformer on the same rows,
+    and to the audio cross-entropy; the sums land in the utterance's own accumulator slot.  No [L, V] logits are kept.
+    Codebook 0 is text (ignore id ignore_text), codebooks 1..dep_q audio (ignore_audio).  depth_feed: 'labels' -- depth
+    step k reads token k of the row's label frame (GPT.forward); 'inputs' -- of the row's own input frame (MLLM_v2
+    LMModel.forward).  check(seq, mask) -> (seq, mask, frames): the host-side item checks (score_item)."""
+    if not 1 <= capacity <= MAX_STREAMS:
+        raise RstnetError(f"capacity must be in [1, {MAX_STREAMS}] (got {capacity})")
+    if depth_feed not in ("labels", "inputs"):
+        raise RstnetError(f"depth_feed is 'labels' or 'inputs' (got {depth_feed!r})")
+    dev, c = m.device, m.config
+    Q = c.dep_q
+    G = Q + 1                                    # the scored codebooks: text, then dep_q audio
+    ign_text = torch.tensor([ignore_text], dtype=torch.int64, device=dev)
+    ign_audio = torch.full((Q,), ignore_audio, dtype=torch.int64, device=dev)
+    acc_text = torch.zeros(capacity, 1, 5, dtype=torch.float64, device=dev)
+    acc_audio = torch.zeros(capacity, Q, 5, dtype=torch.float64, device=dev)
+    source = iter(items)
+    free, live, todo = list(range(capacity)), {}, []
+    exhausted = False
+    init = m._get_initial_token()[0]                                   # [K, 1]
+    while True:
+        admitted = []
+        while free and not exhausted:
+            try:
+                utt, seq, mask = next(source)
+            except StopIteration:
+                exhausted = True
+                break
+            seq, mask, L = check(seq, mask)
+            if L == 0:
+                yield utt, torch.zeros(Q, 5, dtype=torch.float64), torch.zeros(1, 5, dtype=torch.float64), 0
+                continue
+            s = free.pop(0)
+            feed = torch.cat([init, seq[:, :L - 1].to(dev)], dim=1)        # [initial token, seq[:, :-1]]
+            todo.append([s, feed.t().contiguous(), 0])
+            live[s] = dict(utt=utt, seq=seq[:G].t().numpy(), mask=mask[:G].t().numpy(), L=L)
+            admitted.append(s)
+        if admitted:
+            st.reset(admitted)
+            acc_text[admitted] = 0
+            acc_audio[admitted] = 0
+        if not todo:
+            break
+        ch, segs = st.row_chunk(todo, head=True)
+        M = ch.M
+        # labels / weights / accumulator slots of the chunk's rows; padding rows: ignore ids, weight 0, slot -1
+        lab = np.empty((M, G), dtype=np.int64)
+        lab[:, 0], lab[:, 1:] = ignore_text, ignore_audio
+        w = np.zeros((M, G), dtype=np.float32)
+        slot = np.full(M, -1, dtype=np.int32)
+        for s, r0, t0, tn in segs:
+            u = live[s]
+            lab[r0:r0 + tn] = u["seq"][t0:t0 + tn]
+            w[r0:r0 + tn] = u["mask"][t0:t0 + tn]
+            slot[r0:r0 + tn] = s
+        lab_d = torch.from_numpy(lab).to(dev)
+        w_d = torch.from_numpy(w).to(dev)
+        slot_d = torch.from_numpy(slot).to(dev)
+        cross_entropy_sums(ch.logits, lab_d[:, 0].contiguous(), w_d[:, 0].contiguous(), 1, ign_text, slot_d, acc_text)
+        dst = m._depth_state(M)
+        if not hasattr(dst, "score_logits"):
+            dst.score_logits = torch.empty(M, Q, c.audio_card, dtype=torch.bfloat16, device=dev)
+        dst.depth_teacher(ch.out, lab_d if depth_feed == "labels" else ch.seq[:, :G], dst.score_logits)
+        cross_entropy_sums(dst.score_logits.view(M * Q, c.audio_card), lab_d[:, 1:].reshape(-1).contiguous(),
+                           w_d[:, 1:].reshape(-1).contiguous(), Q, ign_audio,
+                           slot_d.repeat_interleave(Q).contiguous(), acc_audio)
+        done = [it for it in todo if it[2] == it[1].shape[0]]
+        todo = [it for it in todo if it[2] < it[1].shape[0]]
+        if done:
+            m.check_device_errors()
+            sa, stx = acc_audio.cpu(), acc_text.cpu()
+            for s, _, _ in done:
+                u = live.pop(s)
+                free.append(s)
+                yield u["utt"], sa[s], stx[s], u["L"]
+    m.check_device_errors()
+
+
 class _LMState:
     """Buffers, KV rings, GEMM plans of one `streaming(B)` scope.  Rows of every activation buffer are (position,
     stream) pairs, position-major: row = tl * B + b.  The decode state has tn == 1; a prefill chunk state (`parent` set)
@@ -826,10 +940,12 @@ class _LMState:
     only holds the depth transformer (forward_local)."""
 
     def __init__(self, m: GPT, B: int, tn: int = 1, parent: Optional["_LMState"] = None, parts=("temporal", "depth"),
-                 rows: Optional[int] = None, kv_pages: Optional[int] = None, kv_page: int = KV_PAGE):
+                 rows: Optional[int] = None, kv_pages: Optional[int] = None, kv_page: int = KV_PAGE, cap: Optional[int] = None):
         """rows: a ragged prefill chunk of that many rows (with `parent`): row r is stream row_stream[r] at position
         offset + row_tl[r] (-1: padding), and the counters advance by `delta` per stream.  kv_pages: a paged KV pool of
-        that many pages of kv_page positions instead of contiguous rings (a child shares its parent's)."""
+        that many pages of kv_page positions instead of contiguous rings (a child shares its parent's).  cap: ring slots per
+        stream (default `context`; a child takes its parent's).  A ring of cap > context slots still attends over exactly
+        `context` positions, and lets a chunk of up to cap - context + 1 positions run after the ring has wrapped."""
         c, dev = m.config, m.device
         self.m, self.B, self.c, self.tn = m, B, c, tn
         M = self.M = B * tn if rows is None else rows
@@ -843,7 +959,9 @@ class _LMState:
         P = {k: v for k, v in m.named_parameters()}
         E, V, I, D, H = c.n_embd, c.padded_vocab_size, c.intermediate_size, c.codecformer_dim, c.ff_hidden
         nh, nkv, hs = c.n_head, c.n_query_groups, c.head_size
-        self.cap = c.context
+        self.cap = parent.cap if parent is not None else (c.context if cap is None else int(cap))
+        if self.cap < c.context:
+            raise RstnetError(f"a KV ring of {self.cap} slots cannot hold a window of context = {c.context} positions")
         Hp = -(-H // 64) * 64  # the GEMMs' K granularity: pad the gating hidden size with zero weights
         self.Hp = Hp
 
@@ -1211,7 +1329,8 @@ class _LMState:
         # prefill: chunks of tn consecutive positions for all streams (tn * B <= MAX_ROWS rows per launch sequence; more
         # than MAX_ROWS streams go one position per pass through the decode state).
         # A multi-position chunk appends all its keys before any of its queries run, so it must not overwrite a ring slot
-        # one of those queries still needs: tn > 1 only while the ring does not wrap inside the chunk.
+        # one of those queries still needs: once the ring wraps inside the chunk, tn <= cap - context + 1 (1 for a ring
+        # of `context` slots).
         if self.pages is not None:   # the whole prefill fits each active stream's reservation, or nothing is launched
             act = np.flatnonzero(self.active_host)
             self.pages.check(act, self.pos_host[act], T)
@@ -1221,7 +1340,7 @@ class _LMState:
         while t < T:
             tn = min(per, T - t)
             if tn > 1 and int(self.pos_host.max()) + tn > self.cap:
-                tn = 1
+                tn = min(tn, self.cap - c.context + 1)
             if tn == 1:
                 r = self.forward_global(sequence[:, :, t:t + 1], want_outputs)
                 if want_outputs:
@@ -1231,7 +1350,7 @@ class _LMState:
                 if ch is None:
                     if len(self.children) >= 2:      # keep at most two chunk shapes alive (full chunk + one tail)
                         self.children.pop(next(iter(self.children)))
-                    ch = self.children[tn] = _LMState(self.m, B, tn=tn, parent=self, parts=("temporal",))
+                    ch = self.children[tn] = type(self)(self.m, B, tn=tn, parent=self, parts=("temporal",))
                 self._advance_host(tn)
                 ch.seq.copy_(sequence[:, :, t:t + tn].permute(2, 0, 1).reshape(tn * B, K))
                 ch._temporal(head=want_outputs)
@@ -1282,9 +1401,9 @@ class _LMState:
                 break
             if done >= p.shape[0]:
                 continue
-            # a chunk appends all its keys before any of its queries run: several positions of a stream only while its
-            # ring does not wrap inside the chunk (as forward_global's prefill), one per chunk after that
-            tn = min(p.shape[0] - done, budget, max(1, self.cap - int(self.pos_host[s])))
+            # a chunk appends all its keys before any of its queries run: several positions of a stream while its ring
+            # does not wrap inside the chunk, and after that at most cap - context + 1 (as forward_global's prefill)
+            tn = min(p.shape[0] - done, budget, max(self.cap - int(self.pos_host[s]), self.cap - c.context + 1))
             segs.append((s, len(rs), done, tn))
             rs += [s] * tn
             rt += range(tn)
@@ -1295,7 +1414,7 @@ class _LMState:
         M = next(b for b in ROW_BUCKETS if b >= n)
         ch = self.row_children.get(M)
         if ch is None:
-            ch = self.row_children[M] = _LMState(self.m, self.B, parent=self, parts=("temporal",), rows=M)
+            ch = self.row_children[M] = type(self)(self.m, self.B, parent=self, parts=("temporal",), rows=M)
         pad = M - n
         ch.row_stream.copy_(torch.tensor(rs + [-1] * pad, dtype=torch.int32))
         ch.row_tl.copy_(torch.tensor(rt + [0] * pad, dtype=torch.int32))

@@ -11,6 +11,10 @@ embedding, a text head, and the depth transformer with per-codebook-step weights
   * ``LMGen(lm, use_sampling, temp, temp_text, top_k, top_k_text).step(input_tokens[B, K_in, 1]) -> [B, dep_q+1, 1] | None``
     with the delay cache of :490-562 (acoustic delays, initial tokens, `max_delay` warm-up frames returning None).
 
+Outside a streaming scope, the evaluation forward of the same file (:297-389): ``forward_text`` over whole sequences,
+``forward_local`` and ``forward(sequence, masks) -> (audio_logits, text_logits)``, with the non-streaming attention
+window of `context` positions at any length; ``score_many`` runs the reference trainer's `validate_model` over a corpus.
+
 Extensions for serving a batch of sessions (rstnet_b200.serve.MoshiDuplexEngine): the delay cache keeps one step count per
 row, so `LMGen.reset_streaming(streams=...)` restarts single rows and `LMGen.set_active_streams(mask)` holds rows, each
 with its own warm-up (`LMGen.valid_rows()`).
@@ -34,7 +38,8 @@ from torch import nn
 from . import _lib, ops
 from ._lib import RstnetError
 from .codec import _register, on_own_device
-from .lm import GPT, KV_PAGE, KVPages, PagedKVModel, Sampling, SkinnyGemm, _DepthScope, _LMState, _head_mode  # noqa: F401
+from .lm import (GPT, KV_PAGE, MAX_ROWS, MAX_STREAMS, DepthLocalModel, KVPages, PagedKVModel, Sampling, SkinnyGemm,  # noqa: F401
+                 _DepthScope, _LMState, _head_mode, combine_sums, score_item, score_packed)
 
 
 class _MoshiState(_LMState):
@@ -52,20 +57,24 @@ class _MoshiState(_LMState):
         self.x, self.xn, self.q, self.att = z(M, E), z(M, E), z(M, E), z(M, E)
         self.qkv, self.hmid = z(M, 3 * E), z(M, I)
         self.out, self.logits = z(M, E), z(M, V)
-        if parent is not None:
-            raise RstnetError("the Moshi twin streams one position per call (LMGen.step)")
-        self.offset = z(B, dtype=torch.int64)
-        self.pos_host = np.zeros(B, dtype=np.int64)
-        self.active = torch.ones(B, dtype=torch.int64, device=dev)
-        self.active_host = np.ones(B, dtype=np.int64)
-        # contiguous rings [2, B, H, cap, hd] per layer, or the paged pool [n_pages, 2, H, page, hd] per layer with one table
-        n_pages, page = self._kv_pages
-        if n_pages is None:
-            self.kv = [z(2, B, nh, self.cap, hs) for _ in range(c.n_layer)]
+        if parent is None:
+            self.offset = z(B, dtype=torch.int64)
+            self.pos_host = np.zeros(B, dtype=np.int64)
+            self.active = torch.ones(B, dtype=torch.int64, device=dev)
+            self.active_host = np.ones(B, dtype=np.int64)
+            # contiguous rings [2, B, H, cap, hd] per layer, or the paged pool [n_pages, 2, H, page, hd] per layer with one table
+            n_pages, page = self._kv_pages
+            if n_pages is None:
+                self.kv = [z(2, B, nh, self.cap, hs) for _ in range(c.n_layer)]
+            else:
+                self.pages = KVPages(n_pages, B, page, self.cap)
+                self.page_table = torch.full((B, self.pages.stride), -1, dtype=torch.int32, device=dev)
+                self.kv = [z(self.pages.n_pages, 2, nh, page, hs) for _ in range(c.n_layer)]
         else:
-            self.pages = KVPages(n_pages, B, page, self.cap)
-            self.page_table = torch.full((B, self.pages.stride), -1, dtype=torch.int32, device=dev)
-            self.kv = [z(self.pages.n_pages, 2, nh, page, hs) for _ in range(c.n_layer)]
+            # a chunk of the non-streaming pass: B x tn time-major rows, or a row map (row_chunk); the parent's rings and counters
+            self.offset, self.pos_host, self.kv = parent.offset, parent.pos_host, parent.kv
+            self.active, self.active_host = parent.active, parent.active_host
+            self.pages, self.page_table = parent.pages, parent.page_table
         # freqs exactly as modules/rope.py:35-36 evaluates them (fp32 tensor * python scalar, then exp)
         ds = torch.arange(hs // 2, dtype=torch.float32)
         self.freqs = torch.exp(ds * (-math.log(m.max_period) * 2 / hs)).to(dev)
@@ -97,7 +106,9 @@ class _MoshiState(_LMState):
         c, B, M, L = self.c, self.B, self.M, _lib.lib()
         st = ops._stream()
         E = c.n_embd
-        # a paged scope runs the same kernels through their paged entry points: the page table as three more arguments
+        # a paged scope runs the same kernels through their paged entry points: the page table as three more arguments.  A
+        # row-mapped chunk (row_chunk, contiguous rings only) runs the pair-RoPE append's row-map entry point
+        rs, rt = (self.row_stream.data_ptr(), self.row_tl.data_ptr()) if self.row_mapped else (None, None)
         if self.pages is None:
             rope, attention, pg = L.rstnet_lm_rope_pair_kv_append_bf16, L.rstnet_lm_ring_decode_attention_bf16, ()
         else:
@@ -109,16 +120,24 @@ class _MoshiState(_LMState):
         _lib.check(L.rstnet_lm_rms_norm_bf16(self.x.data_ptr(), self.n1_first.data_ptr(), self.xn.data_ptr(), M, E, 1e-8, 1, st), "rms")
         for l, ly in enumerate(self.layers):
             ly["qkv"].run()
-            _lib.check(rope(self.qkv.data_ptr(), self.offset.data_ptr(), 1, self.q.data_ptr(), self.kv[l].data_ptr(), M, B, c.n_head,
-                            c.head_size, self.cap, self.freqs.data_ptr(), *pg, st), "rope_pair_kv")
-            _lib.check(attention(self.q.data_ptr(), self.kv[l].data_ptr(), self.offset.data_ptr(), 1, None, None, self.att.data_ptr(),
+            if self.row_mapped:
+                _lib.check(L.rstnet_lm_rope_pair_kv_append_rows_bf16(self.qkv.data_ptr(), self.offset.data_ptr(), rs, rt, self.q.data_ptr(),
+                                                                     self.kv[l].data_ptr(), M, B, c.n_head, c.head_size, self.cap,
+                                                                     self.freqs.data_ptr(), st), "rope_pair_kv_rows")
+            else:
+                _lib.check(rope(self.qkv.data_ptr(), self.offset.data_ptr(), 1, self.q.data_ptr(), self.kv[l].data_ptr(), M, B, c.n_head,
+                                c.head_size, self.cap, self.freqs.data_ptr(), *pg, st), "rope_pair_kv")
+            _lib.check(attention(self.q.data_ptr(), self.kv[l].data_ptr(), self.offset.data_ptr(), 1, rs, rt, self.att.data_ptr(),
                                  M, B, c.n_head, c.n_head, c.head_size, self.cap, c.context, *pg, st), "attention")
             ly["proj"].run()
             ly["fc"].run()
             ly["down"].run()
         if head:
             self.head.run()
-        ops.counter_add(self.offset, self.tn, self.active)
+        if self.row_mapped:
+            _lib.check(L.rstnet_counter_add_rows(self.offset.data_ptr(), self.delta.data_ptr(), B, st), "counter_add_rows")
+        else:
+            ops.counter_add(self.offset, self.tn, self.active)
 
     def _advance_host(self, n: int):
         # positions enter the RoPE as fp32 angles: no table to run out of.  A paged scope raises, before any launch and
@@ -129,8 +148,9 @@ class _MoshiState(_LMState):
         self.pos_host += n * self.active_host
 
 
-class LMModel(PagedKVModel, nn.Module):
-    """Drop-in for ``models.model.LMModel`` on the streaming decode path (same constructor arguments / defaults)."""
+class LMModel(PagedKVModel, DepthLocalModel, nn.Module):
+    """Drop-in for ``models.model.LMModel`` (same constructor arguments / defaults): the streaming decode path, and the
+    non-streaming evaluation forward (forward_text over whole sequences, forward_local, forward)."""
 
     _DN = dict(din="depformer_in.{}.weight", demb="depformer_emb.{}.weight", dtext="depformer_text_emb.weight",
                dlayer="depformer_.layers.{}", dhead="linears.{}.weight")
@@ -213,6 +233,8 @@ class LMModel(PagedKVModel, nn.Module):
         self.depformer = _DepthScope(self)
         self._state: Optional[_MoshiState] = None
         self._packed = None
+        self._local_states = {}                          # depth-only states of forward_local / scoring, by row count
+        self._ns_state: Optional[_MoshiState] = None     # scratch scope of the non-streaming forward_text
         self.use_cuda_graphs = True
 
     # ---- state_dict keys identical to the reference (`depformer.` lives under a private name: `depformer` is an API object)
@@ -234,11 +256,28 @@ class LMModel(PagedKVModel, nn.Module):
                     k = src + k[len(dst):]
             sd[k] = v
         self._packed = None
+        self._local_states, self._ns_state = {}, None
         return super().load_state_dict(sd, strict=strict, **kw)
 
     def _apply(self, fn, *a, **kw):
         self._packed = None
+        self._local_states, self._ns_state = {}, None
         return super()._apply(fn, *a, **kw)
+
+    def _make_state(self, B: int, **kw) -> _MoshiState:
+        return _MoshiState(self, B, **kw)
+
+    def _scratch_state(self, B: int) -> _MoshiState:
+        """A temporal scope of B streams for the non-streaming pass: rings of context + MAX_ROWS - 1 slots, so a chunk of up
+        to MAX_ROWS consecutive positions never overwrites a key an earlier row of the same chunk still needs, and the
+        window of `context` positions is exact at any length.  Attention runs with this cap and the model's context."""
+        return _MoshiState(self, B, parts=("temporal",), cap=self.context + MAX_ROWS - 1)
+
+    def _check_runnable(self):
+        if self.device.type != "cuda":
+            raise RstnetError("LMModel decode runs on CUDA only (sm_90a kernels; the CPU path is the reference itself)")
+        if next(self.parameters()).dtype != torch.bfloat16:
+            raise RstnetError("LMModel decode runs in bfloat16: call .to(device, torch.bfloat16)")
 
     # ---- token conventions (models/model.py:226-288)
     @property
@@ -296,10 +335,7 @@ class LMModel(PagedKVModel, nn.Module):
         """kv_pages None: every stream owns a contiguous KV ring of `context` positions per layer.  kv_pages N: a shared
         pool of N pages of kv_page positions per layer, and a stream holds only the pages reserve_kv gives it -- none at
         entry (as GPT.streaming_forever).  Both give the same results bit for bit."""
-        if self.device.type != "cuda":
-            raise RstnetError("LMModel decode runs on CUDA only (sm_90a kernels; the CPU path is the reference itself)")
-        if next(self.parameters()).dtype != torch.bfloat16:
-            raise RstnetError("LMModel decode runs in bfloat16: call .to(device, torch.bfloat16)")
+        self._check_runnable()
         self._state = _MoshiState(self, batch_size, kv_pages=kv_pages, kv_page=kv_page)
 
     @contextmanager
@@ -331,8 +367,21 @@ class LMModel(PagedKVModel, nn.Module):
     @torch.no_grad()
     @on_own_device
     def forward_text(self, sequence: torch.Tensor):
+        """models/model.py:364-389.  Inside a streaming scope: one frame per call (the decode step).  Outside: the
+        non-streaming form over positions 0..S-1 from scratch, nothing kept, each position attending over the last
+        `context` positions (modules/transformer.py:399-405) at any S.  -> (transformer_out [B, S, dim], text_logits
+        [B, 1, S, text_card]), bf16."""
         B, K, S = sequence.shape
         assert K == self.num_codebooks, f"Sequence shape {sequence.shape} must match the number of codebooks."
+        if self._state is None:
+            self._check_runnable()
+            st = self._ns_state
+            if st is None or st.B != B:
+                self._ns_state = None                    # free the old rings before the new ones are allocated
+                st = self._ns_state = self._scratch_state(B)
+            st.reset()
+            out, logits = st.forward_global(sequence.to(device=self.device, dtype=torch.int64))
+            return out, logits[:, None]
         if S != 1:
             raise RstnetError("streaming forward_text takes one frame per call")
         out, logits = self._st().forward_global(sequence)
@@ -347,8 +396,28 @@ class LMModel(PagedKVModel, nn.Module):
         assert transformer_out.shape[1] == 1, "Transformer out should be a for a single step."
         return self._st().forward_codecformer(depformer_cb_index, sequence, transformer_out)
 
-    def forward(self, *a, **kw):
-        raise NotImplementedError("training forward is out of scope; use LMGen.step / forward_text / forward_depformer")
+    @torch.no_grad()
+    @on_own_device
+    def forward(self, sequence: torch.Tensor, masks: Optional[torch.Tensor] = None):
+        """models/model.py (MLLM_v2) :297-319, the teacher-forced forward: forward_text over [initial token,
+        sequence[:, :, :-1]], then forward_local started from depformer_text_emb of each INPUT frame's text token and fed
+        the input frames' audio tokens 1..dep_q.  sequence [B, K, S] -> (audio_logits [B, S, dep_q, card], text_logits
+        [B, S, text_card]) in bf16, at any S (the attention window is `context` positions).  masks is accepted and unused,
+        as upstream.  Evaluation only: no gradients."""
+        if self._state is not None:
+            raise RstnetError("LMModel.forward is the non-streaming teacher-forced form: call it outside a streaming scope")
+        B, K, S = sequence.shape
+        sequence = sequence.to(device=self.device, dtype=torch.int64)
+        start = self._get_initial_token().repeat(B, 1, 1)
+        inputs = torch.cat([start, sequence[:, :, :-1]], dim=2)
+        transformer_out, text_logits = self.forward_text(inputs)
+        text_logits = text_logits.squeeze(1)
+        ids = inputs[:, 0, :]
+        w = dict(self.named_parameters())["depformer_text_emb.weight"]
+        local_start = torch.nn.functional.embedding(ids.clamp(min=0), w)
+        local_start = torch.where((ids == self.zero_token_id)[..., None], torch.zeros(1, dtype=w.dtype, device=w.device), local_start)
+        audio_logits = self.forward_local(local_start, inputs[:, 1:self.dep_q + 1, :], transformer_out)
+        return audio_logits, text_logits
 
 
 class _GenState:
@@ -565,3 +634,41 @@ class LMGen(nn.Module):
         if not (st.off_host > self.max_delay).any():
             return None
         return st.out[:, :, None].clone()
+
+
+# ------------------------------------------------------------------------------------------- teacher-forced scoring
+AUDIO_WEIGHTS = (100, 1, 1, 1, 1, 1, 1, 1)   # validate_model's audio loss weights (MLLM/trainer/finetuning_full_fsdp.py:274-297)
+
+
+def _score_metrics(sums_audio: torch.Tensor, sums_text: torch.Tensor, frames: int, audio_weights) -> dict:
+    a, t = combine_sums(sums_audio, audio_weights), combine_sums(sums_text, [1])
+    return {"frames": frames, "loss_audio": float(a["loss"]), "loss_text": float(t["loss"]),
+            "acc_audio": float(a["acc_all"]), "acc_text": float(t["acc_all"]),
+            "acc_target_audio": float(a["acc_target"]), "acc_target_text": float(t["acc_target"]),
+            "sums_audio": sums_audio.tolist(), "sums_text": sums_text.tolist()}
+
+
+@torch.no_grad()
+def score_many(lm: LMModel, items, capacity: int = 8, audio_weights=AUDIO_WEIGHTS, ignore_audio: int = 2048,
+               ignore_text: int = 32000):
+    """validate_model (MLLM/trainer/finetuning_full_fsdp.py:274-297) over a corpus of (utt_id, seq [K, L], mask [K, L])
+    items, K = n_q + 1: yields (utt_id, metrics) in completion order, each utterance scored as
+    CrossEntropyAndAccuracy(LMModel.forward(seq)) on it alone.  metrics: loss_audio (sum_k w_k * loss_k over the dep_q
+    audio codebooks with audio_weights, NOT divided by dep_q), loss_text, acc_audio / acc_text (acc_all), acc_target_audio /
+    acc_target_text, frames scored, and the per-codebook sums sums_audio [dep_q][5], sums_text [1][5] (lm.CE_FIELDS).
+    Trailing all-zero-mask frames are dropped; there is no length limit.  A codebook whose mask is zero throughout gives
+    NaN, as upstream.  The depth transformer reads each row's own input frame (MLLM_v2's forward).
+
+    Up to `capacity` utterances are live, one stream each of a scratch scope whose rings hold context + MAX_ROWS - 1
+    positions (about 1.64 GB per stream at 7B shapes, freed when scoring ends); their frames are packed into ragged chunks
+    of at most MAX_ROWS rows (lm.score_packed)."""
+    if len(audio_weights) != lm.dep_q:
+        raise RstnetError(f"{len(audio_weights)} audio loss weights for dep_q = {lm.dep_q} codebooks")
+    if not 1 <= capacity <= MAX_STREAMS:
+        raise RstnetError(f"capacity must be in [1, {MAX_STREAMS}] (got {capacity})")
+    lm._check_runnable()
+    K = lm.num_codebooks
+    st = lm._scratch_state(capacity)
+    for utt, sa, stx, L in score_packed(lm, st, items, capacity, ignore_text, ignore_audio, "inputs",
+                                        lambda seq, mask: score_item(seq, mask, K)):
+        yield utt, _score_metrics(sa, stx, L, audio_weights)

@@ -17,7 +17,9 @@
   * `score` / `python -m rstnet_b200.offline score`: infer_no_streaming.py main() with --inference_mode teacher-force
     (:174-182) over a corpus (`torch.save`d dict utt_id -> {"seq": int64 [9, L], "mask": float [9, L]}) with
     InferenceImp.score_many: per-utterance losses / accuracies to a json file, and one json line with the mean
-    loss_audio / 8, perplexity_audio = exp(that mean) and the mean text loss.
+    loss_audio / 8, perplexity_audio = exp(that mean) and the mean text loss.  `score --model moshi` scores a Moshi
+    fine-tune (the LMModel of rstnet_b200.moshi) as the reference trainer's validate_model does, with moshi.score_many over
+    [n_q + 1, L] seq / mask items.
   * `synthesize` / `python -m rstnet_b200.offline synthesize`: the TTS loop of infer_no_streaming.py main() (:119-143) over a
     whole corpus (`torch.save`d dict utt_id -> int64 [9, L]) with InferenceImp.generate_many: utterances of any prompt and
     generation length decode together, a finished row taking the next utterance.  Writes utt_id -> int16 codes [8, T] and,
@@ -259,9 +261,46 @@ def score_summary(metrics: Dict[str, dict]) -> dict:
     return {"utterances": n, "loss_audio": la, "perplexity_audio": math.exp(la) if la == la else float("nan"), "loss_text": lt}
 
 
+def _load_moshi(config_path: str, checkpoint: str, device: str):
+    """moshi.LMModel(**json) with the checkpoint's weights (a state_dict, or {'model': state_dict}; `module.` prefixes
+    stripped), in bf16 on `device`."""
+    import json
+    from .moshi import LMModel
+    m = LMModel(**json.load(open(config_path)))
+    sd = torch.load(checkpoint, map_location="cpu")
+    sd = sd["model"] if isinstance(sd, dict) and "model" in sd and isinstance(sd["model"], dict) else sd
+    m.load_state_dict({k.split("module.")[-1] if k.startswith("module.") else k: v for k, v in sd.items()})
+    return m.to(device, torch.bfloat16).eval()
+
+
+def moshi_score_summary(metrics: Dict[str, dict], audio_weights=None) -> dict:
+    """Corpus metrics of `score --model moshi`, pooled from the summed per-codebook sums: every scored token weighs the
+    same, whatever its utterance (loss_k = sum of mask * nll over the corpus / count of non-zero mask entries).  The
+    reference trainer's reporter instead averages the per-batch values, so its numbers depend on the batching."""
+    from .lm import combine_sums
+    from .moshi import AUDIO_WEIGHTS
+    aw = AUDIO_WEIGHTS if audio_weights is None else audio_weights
+    sa = sum((torch.tensor(m["sums_audio"], dtype=torch.float64) for m in metrics.values()), torch.zeros(len(aw), 5, dtype=torch.float64))
+    st = sum((torch.tensor(m["sums_text"], dtype=torch.float64) for m in metrics.values()), torch.zeros(1, 5, dtype=torch.float64))
+    a, t = combine_sums(sa, aw), combine_sums(st, [1])
+    return {"utterances": len(metrics), "frames": sum(m["frames"] for m in metrics.values()), "loss_audio": float(a["loss"]),
+            "loss_text": float(t["loss"]), "acc_audio": float(a["acc_all"]), "acc_text": float(t["acc_all"]),
+            "acc_target_audio": float(a["acc_target"]), "acc_target_text": float(t["acc_target"])}
+
+
 def _score_cli(args) -> int:
     import json
     from .infer import InferenceImp
+    if args.model == "moshi":
+        from .moshi import score_many
+        model = _load_moshi(args.config, args.checkpoint, args.device)
+        corpus = torch.load(args.input, map_location="cpu")
+        items = ((utt, torch.as_tensor(d["seq"]), torch.as_tensor(d["mask"])) for utt, d in corpus.items())
+        metrics = dict(score_many(model, items, args.capacity))
+        with open(args.output_file, "w") as f:
+            json.dump(metrics, f)
+        print(json.dumps(moshi_score_summary(metrics)))
+        return 0
     model = _load_gpt(args.config, args.checkpoint, args.device)
     imp = InferenceImp(None, model, "teacher-force", 0.7, 25, 0.8, 30, "TTS")
     corpus = torch.load(args.input, map_location="cpu")
@@ -384,10 +423,15 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--codec-weights", default=None)
     p.add_argument("--codec-config", default=None, help="json with the MimiCodec constructor arguments")
     p.add_argument("--device", default="cuda")
-    p = sub.add_parser("score", help="teacher-forced losses / audio perplexity of a corpus (infer_no_streaming.py teacher-force)")
-    p.add_argument("--input", required=True, help="torch.save'd dict utt_id -> {'seq': int64 [9, L], 'mask': float [9, L]}")
-    p.add_argument("--config", required=True, help="json with the GPT Config fields")
-    p.add_argument("--checkpoint", required=True, help="training checkpoint ({'model': state_dict})")
+    p = sub.add_parser("score", help="teacher-forced losses / audio perplexity of a corpus (infer_no_streaming.py teacher-force; "
+                                     "--model moshi: the Moshi fine-tune trainer's validate_model)")
+    p.add_argument("--input", required=True, help="torch.save'd dict utt_id -> {'seq': int64 [9, L], 'mask': float [9, L]} "
+                                                  "([n_q + 1, L] with --model moshi)")
+    p.add_argument("--model", choices=("gpt", "moshi"), default="gpt",
+                   help="gpt: the speech-text GPT; moshi: the Moshi-style LMModel (--config holds its constructor kwargs)")
+    p.add_argument("--config", required=True, help="json with the GPT Config fields (--model moshi: the LMModel kwargs)")
+    p.add_argument("--checkpoint", required=True, help="training checkpoint ({'model': state_dict}; --model moshi also takes a "
+                                                       "bare state_dict)")
     p.add_argument("--output-file", required=True, help="json file of per-utterance metrics")
     p.add_argument("--capacity", type=int, default=8, help="utterances packed into the same chunks (<= 256)")
     p.add_argument("--device", default="cuda")

@@ -276,12 +276,15 @@ class MimiCodec(nn.Module):
         return self._stream_state is not None
 
     @on_own_device
-    def streaming_forever(self, batch_size: int):
-        self._stream_state = _StreamState(self._eng(), batch_size)
+    def streaming_forever(self, batch_size: int, clip_window: bool = False):
+        """clip_window (extension): the decoder transformer's rings get one step's tokens more than `context`, so every
+        query sees `context` keys as in `decode` of the whole clip, and a stream of steps decodes to exactly that clip's
+        `decode` at any length; False keeps the reference's RingKVCache, which leaves context - 1 keys once it wraps."""
+        self._stream_state = _StreamState(self._eng(), batch_size, clip_window)
 
     @contextmanager
-    def streaming(self, batch_size: int):
-        self.streaming_forever(batch_size)
+    def streaming(self, batch_size: int, clip_window: bool = False):
+        self.streaming_forever(batch_size, clip_window)
         try:
             yield
         finally:
@@ -982,8 +985,8 @@ class _StreamState:
     """Per-`streaming(B)` scope state: one encode plan and one decode plan per chunk size, sharing
     nothing with other scopes (mirrors `_MimiState`, compression.py:37-60)."""
 
-    def __init__(self, eng: _Engine, batch_size: int):
-        self.eng, self.B = eng, batch_size
+    def __init__(self, eng: _Engine, batch_size: int, clip_window: bool = False):
+        self.eng, self.B, self.clip_window = eng, batch_size, clip_window
         self.enc: Dict[int, _EncPlan] = {}
         self.dec: Dict[int, _DecPlan] = {}
         # per-stream "advance" flags read by the carry copy and the position counters of every step (all ones unless a
@@ -1009,7 +1012,8 @@ class _StreamState:
         if T not in self.dec:
             if self.dec:
                 raise RstnetError("the chunk size must stay constant within one streaming scope")
-            self.dec[T] = _DecPlan(self.eng, self.B, T, True, self.eng.m.streaming_tensor_cores, n_codes=K, active=self.active)
+            self.dec[T] = _DecPlan(self.eng, self.B, T, True, self.eng.m.streaming_tensor_cores, n_codes=K, active=self.active,
+                                   corpus=self.clip_window)
         return self.dec[T]
 
     def row_segments(self, b: int, chunk: int, frames: int, n_codes: int):
@@ -1035,9 +1039,11 @@ class _StreamState:
 
     def reset(self, streams=None):
         if streams is not None:
-            streams = torch.as_tensor(streams, dtype=torch.int64, device=self.eng.device).reshape(-1)
+            # checked before the copy to the device, so that a reset does not wait for the device
+            streams = torch.as_tensor(streams, dtype=torch.int64).reshape(-1)
             if streams.numel() and (int(streams.min()) < 0 or int(streams.max()) >= self.B):
                 raise RstnetError(f"stream index outside [0, {self.B})")
+            streams = streams.to(self.eng.device)
         for p in list(self.enc.values()) + list(self.dec.values()):
             p.reset(streams)
 

@@ -24,7 +24,8 @@ utterance.
 """
 from __future__ import annotations
 
-from typing import Dict, Iterable, Iterator, List, Optional, Tuple
+from contextlib import contextmanager
+from typing import Dict, Iterable, Iterator, List, NamedTuple, Optional, Tuple
 
 import numpy as np
 import torch
@@ -167,6 +168,39 @@ class InferenceImp(object):
             raise RstnetError("the sequence has no prompt frames")
         return prefix_len, L - prefix_len
 
+
+    def _check_many(self, capacity: int, kv_pages: Optional[int]) -> None:
+        """the argument checks of generate_many / stream_many / serve.TTSEngine"""
+        self._check_task()
+        if not 1 <= capacity <= MAX_STREAMS:
+            raise RstnetError(f"capacity must be in [1, {MAX_STREAMS}] (got {capacity})")
+        if not hasattr(self.model, "reserve_kv") and kv_pages is not None:
+            raise RstnetError(f"{type(self.model).__name__} has no paged KV scope (kv_pages)")
+
+    @staticmethod
+    def _check_sampling(sampling: Optional[Dict[object, Sampling]]) -> None:
+        if sampling is not None:
+            for utt, sp in sampling.items():
+                if not isinstance(sp, Sampling):
+                    raise RstnetError(f"sampling[{utt!r}] must be a Sampling (got {type(sp).__name__})")
+
+    def _puller(self, items, seeds, sampling):
+        """-> pull(): the next item of `items` as an admission request (utt, seq, P, G, Sampling or None, seed), or None
+        once they are exhausted; items are read one at a time, when a row can take them"""
+        source, seeds, done = iter(items), seeds or {}, []
+
+        def pull():
+            if done:
+                return None
+            try:
+                utt, seq = next(source)
+            except StopIteration:
+                done.append(True)
+                return None
+            P, G = self._layout(seq)
+            return utt, seq, P, G, None if sampling is None else sampling.get(utt), int(seeds.get(utt, 0))
+        return pull
+
     @torch.no_grad()
     def generate_many(self, items: Iterable[Tuple[object, torch.Tensor]], capacity: int,
                       seeds: Optional[Dict[object, int]] = None, return_frames: bool = False,
@@ -190,120 +224,296 @@ class InferenceImp(object):
         so the completion order is fixed for a given pool.  An utterance needing more than the whole pool raises.
         stats: a dict that receives 'frames' (frames run), 'row_frames' (occupied rows summed over frames) and
         'wait_frames' (frames run while an utterance waited for pages with a row free)."""
-        self._check_task()
-        if not 1 <= capacity <= MAX_STREAMS:
-            raise RstnetError(f"capacity must be in [1, {MAX_STREAMS}] (got {capacity})")
-        m, seeds = self.model, seeds or {}
-        # GPT always decodes here on paged KV; a stand-in model that offers only the unpaged streaming protocol (no
-        # reserve_kv) runs its own scope
-        paged = hasattr(m, "reserve_kv")
-        if paged and kv_pages is None:
-            kv_pages = capacity * -(-m.config.context // KV_PAGE)
-        if not paged and kv_pages is not None:
-            raise RstnetError(f"{type(m).__name__} has no paged KV scope (kv_pages)")
+        self._check_many(capacity, kv_pages)
+        m = self.model
         stats = {} if stats is None else stats
         stats.update(frames=0, row_frames=0, wait_frames=0)
-        if sampling is not None:
-            default = self.sampling()
-            for utt, sp in sampling.items():
-                if not isinstance(sp, Sampling):
-                    raise RstnetError(f"sampling[{utt!r}] must be a Sampling (got {type(sp).__name__})")
-        dev, B = m.device, capacity
-        n_cb = m.num_codebooks
-        dep_q = n_cb - 1                 # text + dep_q audio codebooks per frame
-        source = iter(items)
-        rows: List[Optional[dict]] = [None] * B
-        history: Dict[int, torch.Tensor] = {}       # frame -> tokens [B, 9] of every row
-        frame = 0
-        cur = torch.zeros(B, n_cb, 1, dtype=torch.int64, device=dev)
-        keys = np.zeros(B, dtype=np.int64)
-        active = np.zeros(B, dtype=np.int64)
-        with m.streaming(B, kv_pages=kv_pages) if paged else m.streaming(B):
-            pages = m._state.pages if paged else None   # the scope's allocator, read to decide admissions
-            m.set_active_streams(active)
-            init = m._get_initial_token()[0].to(dev)
-            exhausted = False
-            pending = None   # (utt, seq, P, G) of the next utterance while it waits for pages
-            dirty = set()    # rows whose pages changed on the host since the last upload
+        self._check_sampling(sampling)
+        pull = self._puller(items, seeds, sampling)
+        with _tts_scope(m, capacity, kv_pages):
+            rows = _TTSRows(self, capacity, sampling is not None, stats)
             while True:
-                admitted = {}
-                for r in range(B):
-                    if rows[r] is not None:
-                        continue
-                    if pending is None:
-                        if exhausted:
-                            break
-                        try:
-                            utt, seq = next(source)
-                        except StopIteration:
-                            exhausted = True
-                            break
-                        P, G = self._layout(seq)
-                        if paged and pages.pages_for(P + G) > pages.n_pages:
-                            raise RstnetError(f"utterance {utt!r} needs {pages.pages_for(P + G)} KV pages ({P + G} positions), "
-                                              f"more than the whole pool of {pages.n_pages}")
-                        pending = (utt, seq, P, G)
-                    utt, seq, P, G = pending
-                    if paged:
-                        if pages.pages_for(P + G) > pages.free:
-                            stats["wait_frames"] += 1
-                            break
-                        # it writes P positions in the prompt feed (init token + all prompt frames but the last) and one
-                        # per generated frame: exactly P + G
-                        pages.reserve([r], P + G)
-                        dirty.add(r)
-                    pending = None
-                    feed = torch.cat([init, seq[:, :P].to(device=dev, dtype=torch.int64)], dim=1)
-                    admitted[r] = feed
-                    rows[r] = dict(utt=utt, P=P, G=G, g=0, start=frame)
-                    keys[r] = int(seeds.get(utt, 0))
-                if dirty:
-                    # one upload of the table rows this frame's releases and admissions changed, before any launch
-                    m._state.upload_pages(sorted(dirty))
-                    dirty.clear()
-                if admitted:
-                    # the init token + all prompt frames but the last only feed the KV rings; the step on the last prompt
-                    # frame yields generated frame 0 (as generate)
-                    m.reset_streaming(streams=sorted(admitted))
-                    m.prefill_streams({r: f[:, :-1] for r, f in admitted.items()})
-                    for r, f in admitted.items():
-                        cur[r, :, 0] = f[:, -1]
-                occupied = [r for r in range(B) if rows[r] is not None]
-                if not occupied:
+                rows.admit(pull)
+                if not rows.occupied():
                     break
-                mask = np.array([1 if rows[r] is not None else 0 for r in range(B)], dtype=np.int64)
-                if not np.array_equal(mask, active):
-                    active = mask
-                    m.set_active_streams(active)
-                table = torch.full((B, dep_q), 2048, dtype=torch.int32)
-                for r in occupied:
-                    st = rows[r]
-                    table[r] = torch.tensor(candidate_counts(st["P"], st["G"], st["g"], dep_q), dtype=torch.int32)
-                per_row = None
-                if sampling is not None:
-                    per_row = [sampling.get(rows[r]["utt"], default) if rows[r] is not None else default for r in range(B)]
-                toks = m.forward_step(cur, use_sampling=self.use_sampling, temp_text=self.temp_text, top_k_text=self.top_k_text,
-                                      temp=self.temp, top_k=self.top_k, audio_valid=table,
-                                      sample_key=keys if admitted else None, depth_ring_quirk=False,
-                                      top_p_text=self.top_p_text, top_p=self.top_p, sampling=per_row)
-                history[frame] = toks
-                frame += 1
-                stats["frames"] += 1
-                stats["row_frames"] += len(occupied)
-                cur = toks[:, :, None].clone()
-                for r in occupied:
-                    st = rows[r]
-                    st["g"] += 1
-                    if st["g"] == st["G"]:
-                        raw = torch.stack([history[f][r] for f in range(st["start"], frame)])     # [G, 9]
-                        rows[r] = None
-                        m.reset_streaming(streams=[r])   # a held row keeps its position: park it at 0 ...
-                        if paged:
-                            pages.release([r])           # ... without pages (uploaded before the next launch)
-                            dirty.add(r)
-                        codes = reverse_delay(raw[:, 1:])
-                        yield (st["utt"], codes, raw) if return_frames else (st["utt"], codes)
-                first = min([st["start"] for st in rows if st is not None], default=frame)
-                for f in [f for f in history if f < first]:
-                    del history[f]
+                for utt, codes, raw in rows.frame():
+                    yield (utt, codes, raw) if return_frames else (utt, codes)
             m.check_device_errors()
+
+    @torch.no_grad()
+    def stream_many(self, items: Iterable[Tuple[object, torch.Tensor]], capacity: int, codec,
+                    *, seeds: Optional[Dict[object, int]] = None, sampling: Optional[Dict[object, Sampling]] = None,
+                    kv_pages: Optional[int] = None) -> Iterator["TTSChunk"]:
+        """generate_many's corpus, options and admissions, with the audio streamed: every frame also undoes the TTS delay
+        on the device and decodes one codec frame for each row that has one (see `_TTSRows`), and the PCM is yielded as
+        TTSChunk(utt_id, index, pcm [1920] float32 on the host, codes) while the utterances are still generating.  An
+        utterance of G frames gives chunks 0 .. G-2 in order (their concatenation is `codec.decode` of its codes); its
+        last chunk carries its codes [8, G-1] (those generate_many yields; on the host), the others None.  G = 1 gives one
+        chunk of no samples.  The host hands out frame n's chunks while the device runs frame n + 1, so chunks of
+        different utterances interleave in frame order.  codec: a MimiCodec on the model's device; it runs its own
+        streaming scope of `capacity` rows for the duration, with clip_window rings, so that the chunks are the utterance's
+        whole-clip decode at any length."""
+        self._check_many(capacity, kv_pages)
+        self._check_sampling(sampling)
+        pull = self._puller(items, seeds, sampling)
+        with _tts_scope(self.model, capacity, kv_pages), codec.streaming(capacity, clip_window=True):
+            rows = _TTSRows(self, capacity, sampling is not None, {}, codec)
+            while True:
+                chunks = rows.stream_step(pull)
+                if chunks is None:
+                    break
+                yield from chunks
+            self.model.check_device_errors()
+
+
+class TTSChunk(NamedTuple):
+    """One codec frame of streamed TTS audio: `index` counts the utterance's chunks from 0; pcm float32 [1920] (80 ms at
+    24 kHz) on the host; codes: the utterance's codes [8, G-1] on its last chunk, None before."""
+    utt_id: object
+    index: int
+    pcm: torch.Tensor
+    codes: Optional[torch.Tensor]
+
+
+@contextmanager
+def _tts_scope(m, capacity: int, kv_pages: Optional[int]):
+    """The LM scope of batch TTS: GPT decodes on paged KV (None: a whole ring per row, capacity x ceil(context / KV_PAGE)
+    pages); a stand-in model that offers only the unpaged streaming protocol (no reserve_kv) runs its own scope."""
+    if not hasattr(m, "reserve_kv"):
+        with m.streaming(capacity):
+            yield
+        return
+    if kv_pages is None:
+        kv_pages = capacity * -(-m.config.context // KV_PAGE)
+    with m.streaming(capacity, kv_pages=kv_pages):
+        yield
+
+
+class _TTSRows:
+    """The admission and frame loop of batch TTS, shared by generate_many, stream_many and serve.TTSEngine, inside one LM
+    scope of B rows (`_tts_scope`).  `admit(pull)` fills free rows in order with the requests pull() gives -- (utt, seq,
+    P, G, Sampling or None, seed), None when there is none -- and stops at the first one whose KV pages the pool cannot
+    give yet (it waits, in `pending`, for the next call); `frame()` runs one generated frame for every row and returns
+    the utterances it finished as (utt, codes [8, G-1], raw frames [G, 9]).  per_row: every row samples with its own
+    settings (a request's Sampling, else the InferenceImp's) from the per-row tables; False: the instance's scalar settings.
+
+    With a codec (stream_step), every frame also runs, for all B rows, the acoustic-delay cache kernel
+    (_TTSDelay: codec frame f = codebook 0 of generated frame f and codebooks 1-7 of frame f + 1, reverse_delay on the
+    device) and one step of the codec's streaming decoder, holding the rows that have no undelayed frame (a row's first
+    generated frame, free rows); the PCM goes to one of two pinned host slots, and the host waits only for the previous
+    frame's copy before it hands that frame's chunks out.  No eager torch arithmetic runs on this path, except the clamp of
+    the codes to the codebook (ids 2048 / 2049 are LM samples, which the codec's gather clamps alike but flags as errors)."""
+
+    def __init__(self, imp: InferenceImp, B: int, per_row: bool, stats: dict, codec=None):
+        m = imp.model
+        self.imp, self.m, self.B, self.stats = imp, m, B, stats
+        stats.update(frames=0, row_frames=0, wait_frames=0)
+        self.default = None             # the instance's Sampling while rows sample with per-row settings
+        if per_row:
+            self.use_per_row()
+        self.paged = hasattr(m, "reserve_kv")
+        self.pages = m._state.pages if self.paged else None   # the scope's allocator, read to decide admissions
+        self.dev, n_cb = m.device, m.num_codebooks
+        self.dep_q = n_cb - 1                 # text + dep_q audio codebooks per frame
+        self.rows: List[Optional[dict]] = [None] * B
+        self.history: Dict[int, torch.Tensor] = {}       # frame -> tokens [B, 9] of every row
+        self.n = 0                                       # frames run
+        self.cur = torch.zeros(B, n_cb, 1, dtype=torch.int64, device=self.dev)
+        self.keys = np.zeros(B, dtype=np.int64)
+        self.active = np.zeros(B, dtype=np.int64)
+        m.set_active_streams(self.active)
+        self.init = m._get_initial_token()[0].to(self.dev)
+        self.pending = None   # the next request while it waits for pages
+        self.dirty = set()    # rows whose pages changed on the host since the last upload
+        self.admitted = False
+        self.codec = codec
+        if codec is not None:
+            self.delay = _TTSDelay(m, B)
+            self.card = codec.codebook_size
+            cuda = self.dev.type == "cuda"
+            self.pcm = [torch.zeros(B, codec.frame_size, dtype=torch.float32, pin_memory=cuda) for _ in range(2)]
+            self.events = [torch.cuda.Event() for _ in range(2)] if cuda else None
+            self.slot = 0
+            self.in_flight = None         # (slot, chunk records) of the last frame run, not yet handed out
+
+    def use_per_row(self) -> None:
+        """from the next frame on, every row samples with its own settings (per-row tables)"""
+        if self.default is None:
+            self.default = self.imp.sampling()
+
+    def occupied(self) -> List[int]:
+        return [r for r in range(self.B) if self.rows[r] is not None]
+
+    def fits(self, utt, P: int, G: int) -> None:
+        """raise if the utterance needs more KV pages than the whole pool"""
+        if self.paged and self.pages.pages_for(P + G) > self.pages.n_pages:
+            raise RstnetError(f"utterance {utt!r} needs {self.pages.pages_for(P + G)} KV pages ({P + G} positions), "
+                              f"more than the whole pool of {self.pages.n_pages}")
+
+    def admit(self, pull) -> None:
+        m, dev, pages = self.m, self.dev, self.pages
+        admitted = {}
+        for r in range(self.B):
+            if self.rows[r] is not None:
+                continue
+            if self.pending is None:
+                req = pull()
+                if req is None:
+                    break
+                self.fits(req[0], req[2], req[3])
+                self.pending = req
+            utt, seq, P, G, sp, seed = self.pending
+            if self.paged:
+                if pages.pages_for(P + G) > pages.free:
+                    self.stats["wait_frames"] += 1
+                    break
+                # it writes P positions in the prompt feed (init token + all prompt frames but the last) and one
+                # per generated frame: exactly P + G
+                pages.reserve([r], P + G)
+                self.dirty.add(r)
+            self.pending = None
+            feed = torch.cat([self.init, seq[:, :P].to(device=dev, dtype=torch.int64)], dim=1)
+            admitted[r] = feed
+            self.rows[r] = dict(utt=utt, P=P, G=G, g=0, start=self.n, sp=sp)
+            self.keys[r] = seed
+        if self.dirty:
+            # one upload of the table rows this frame's releases and admissions changed, before any launch
+            m._state.upload_pages(sorted(self.dirty))
+            self.dirty.clear()
+        self.admitted = bool(admitted)
+        if admitted:
+            # the init token + all prompt frames but the last only feed the KV rings; the step on the last prompt
+            # frame yields generated frame 0 (as generate)
+            m.reset_streaming(streams=sorted(admitted))
+            if self.codec is not None:
+                self.delay.reset(sorted(admitted))
+                self.codec.reset_streaming(streams=sorted(admitted))
+            m.prefill_streams({r: f[:, :-1] for r, f in admitted.items()})
+            for r, f in admitted.items():
+                self.cur[r, :, 0] = f[:, -1]
+
+    def frame(self, records: Optional[list] = None) -> List[Tuple]:
+        """One generated frame of every row (there must be an occupied row).  records: a list that receives the
+        frame's chunk records (row, utt, index, codes or None) when the codec runs."""
+        imp, m, B, rows = self.imp, self.m, self.B, self.rows
+        occupied = self.occupied()
+        mask = np.array([1 if rows[r] is not None else 0 for r in range(B)], dtype=np.int64)
+        if not np.array_equal(mask, self.active):
+            self.active = mask
+            m.set_active_streams(self.active)
+        table = torch.full((B, self.dep_q), 2048, dtype=torch.int32)
+        for r in occupied:
+            st = rows[r]
+            table[r] = torch.tensor(candidate_counts(st["P"], st["G"], st["g"], self.dep_q), dtype=torch.int32)
+        per_row = None
+        if self.default is not None:
+            default = self.default
+            per_row = [default if rows[r] is None or rows[r]["sp"] is None else rows[r]["sp"] for r in range(B)]
+        toks = m.forward_step(self.cur, use_sampling=imp.use_sampling, temp_text=imp.temp_text, top_k_text=imp.top_k_text,
+                              temp=imp.temp, top_k=imp.top_k, audio_valid=table,
+                              sample_key=self.keys if self.admitted else None, depth_ring_quirk=False,
+                              top_p_text=imp.top_p_text, top_p=imp.top_p, sampling=per_row)
+        if self.codec is not None:
+            self._decode(toks)
+        self.history[self.n] = toks
+        self.n += 1
+        self.stats["frames"] += 1
+        self.stats["row_frames"] += len(occupied)
+        self.cur = toks[:, :, None].clone()
+        done = []
+        for r in occupied:
+            st = rows[r]
+            st["g"] += 1
+            last = st["g"] == st["G"]
+            codes = raw = None
+            if last:
+                raw = torch.stack([self.history[f][r] for f in range(st["start"], self.n)])     # [G, 9]
+                rows[r] = None
+                m.reset_streaming(streams=[r])   # a held row keeps its position: park it at 0 ...
+                if self.paged:
+                    self.pages.release([r])      # ... without pages (uploaded before the next launch)
+                    self.dirty.add(r)
+                codes = reverse_delay(raw[:, 1:])
+                done.append((st["utt"], codes, raw))
+            if records is not None and (st["g"] >= 2 or last):
+                # step g - 1 >= 1 completes codec frame g - 2; an utterance of one frame has no audio
+                records.append((r, st["utt"], max(st["g"] - 2, 0), codes, st["g"] >= 2))
+        if records is not None and done:
+            self.delay.reset([r for r in occupied if rows[r] is None])   # a free row has no frame: the codec holds it
+        first = min([st["start"] for st in rows if st is not None], default=self.n)
+        for f in [f for f in self.history if f < first]:
+            del self.history[f]
+        return done
+
+    def _decode(self, toks: torch.Tensor) -> None:
+        """the codec frame of every row that has one, into PCM slot self.slot"""
+        out, valid = self.delay.step(toks)
+        self.codec.set_active_streams(valid)
+        pcm = self.codec.decode(out[:, 1:, None].clamp(max=self.card - 1))   # [B, 1, 1920]
+        self.pcm[self.slot].copy_(pcm[:, 0], non_blocking=True)
+
+    def stream_step(self, pull) -> Optional[List[TTSChunk]]:
+        """Admit, run one frame with its codec step if a row is occupied, then hand out the previous frame's chunks.
+        -> the chunks, or None when no row is occupied and nothing is left to hand out (nothing was launched)."""
+        self.admit(pull)
+        prev, self.in_flight = self.in_flight, None
+        if self.occupied():
+            records = []
+            self.frame(records)
+            cuda = self.events is not None
+            records = [(r, utt, i, None if c is None else _to_host(c), has_pcm) for r, utt, i, c, has_pcm in records]
+            if cuda:
+                self.events[self.slot].record()
+            self.in_flight, self.slot = (self.slot, records), self.slot ^ 1
+        elif prev is None:
+            return None
+        return [] if prev is None else self._hand_out(*prev)
+
+    def _hand_out(self, slot: int, records) -> List[TTSChunk]:
+        if self.events is not None:
+            self.events[slot].synchronize()
+        pcm = self.pcm[slot].numpy()
+        empty = torch.zeros(0, dtype=torch.float32)
+        return [TTSChunk(utt, i, torch.from_numpy(pcm[r].copy()) if has_pcm else empty, codes)
+                for r, utt, i, codes, has_pcm in records]
+
+
+def _to_host(t: torch.Tensor) -> torch.Tensor:
+    """a host copy with t's strides, enqueued without waiting (pinned memory; valid once the stream has passed it)"""
+    if t.device.type != "cuda":
+        return t
+    return torch.empty_like(t, device="cpu", pin_memory=True).copy_(t, non_blocking=True)
+
+
+class _TTSDelay:
+    """The TTS acoustic delay undone on the device by the Moshi delay-cache kernel (rstnet_lm_delay_cache_out): K = 9
+    codebooks (text + 8 audio), delays [0, 0, 1, ..., 1], max_delay 1, ring of CT = 3 columns per (row, codebook).  After
+    generated frame f of a row, out[row, 1:] is its codec frame f - 1 and valid[row] = 1 (f >= 1).  Rows held by the LM
+    scope (its device `active` flags) keep their ring, step count and valid flag."""
+
+    def __init__(self, m, B: int):
+        dev, K = m.device, m.num_codebooks
+        self.B, self.K, self.dep_q = B, K, K - 1
+        self.delays = torch.tensor([0, 0] + [1] * (K - 2), dtype=torch.int64, device=dev)
+        self.cache = torch.zeros(B, K, 3, dtype=torch.int64, device=dev)
+        self.off = torch.zeros(B, dtype=torch.int64, device=dev)
+        self.valid = torch.zeros(B, dtype=torch.int64, device=dev)
+        self.out = torch.zeros(B, K, dtype=torch.int64, device=dev)
+        self.lm_active = m._state.active
+
+    def reset(self, rows) -> None:
+        """the rows' step counts and valid flags back to 0"""
+        idx = torch.as_tensor(rows, dtype=torch.int64).to(self.off.device)
+        self.off[idx] = 0
+        self.valid[idx] = 0
+
+    def step(self, toks: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+        """toks: the frame's tokens [B, 9] (int64, rows contiguous) -> (out [B, 9], valid [B]), device buffers"""
+        from . import _lib, ops
+        if toks.dtype != torch.int64 or tuple(toks.shape) != (self.B, self.K) or toks.stride(1) != 1:
+            raise RstnetError(f"the TTS delay takes int64 tokens [{self.B}, {self.K}] with contiguous rows")
+        _lib.check(_lib.lib().rstnet_lm_delay_cache_out(
+            self.cache.data_ptr(), self.off.data_ptr(), self.lm_active.data_ptr(), self.delays.data_ptr(), toks.data_ptr(),
+            toks.stride(0), self.out.data_ptr(), self.K, self.valid.data_ptr(), self.B, self.K, self.dep_q, 3, 1,
+            ops._stream()), "delay_cache_out")
+        return self.out, self.valid

@@ -24,6 +24,8 @@
     whole corpus (`torch.save`d dict utt_id -> int64 [9, L]) with InferenceImp.generate_many: utterances of any prompt and
     generation length decode together, a finished row taking the next utterance.  Writes utt_id -> int16 codes [8, T] and,
     with a codec, one 24 kHz 16-bit wav per utterance (Mimi decode of equal-length groups, as main()'s detokenize).
+    `synthesize_stream` / `synthesize --stream`: the same codes through InferenceImp.stream_many, each wav decoded frame by
+    frame during generation and written when its utterance completes.
 
 Audio at any integer sample rate is resampled to 24 kHz on the GPU the way the reference does it,
 torchaudio.transforms.Resample(sr, 24000) with its defaults (mimi_tokenizer.py:40,67; inference.py:24-34 `convert_audio`:
@@ -190,6 +192,25 @@ def synthesize(imp, corpus: Dict[str, torch.Tensor], capacity: int = 32, seeds=N
 
 
 @torch.no_grad()
+def synthesize_stream(imp, codec: MimiCodec, corpus: Dict[str, torch.Tensor], dst: str, capacity: int = 32, seeds=None,
+                      kv_gb: Optional[float] = None) -> Dict[str, torch.Tensor]:
+    """`synthesize` through imp.stream_many: the same {utt_id: int16 [8, T]}, and each utterance's `<utt_id>_sample.wav`
+    (24 kHz 16-bit, as write_codes_wav; none for T = 0) written from its streamed chunks as soon as it completes."""
+    os.makedirs(dst, exist_ok=True)
+    items = ((utt, torch.as_tensor(seq, dtype=torch.int64)) for utt, seq in corpus.items())
+    kv_pages = None if kv_gb is None else kv_pages_for_budget(imp.model.config, kv_gb)
+    parts, out = defaultdict(list), {}
+    for ch in imp.stream_many(items, capacity, codec, seeds=seeds, kv_pages=kv_pages):
+        parts[ch.utt_id].append(ch.pcm)
+        if ch.codes is not None:
+            wav = torch.cat(parts.pop(ch.utt_id))
+            if wav.numel():
+                write_wav(os.path.join(dst, f"{ch.utt_id}_sample.wav"), wav, codec.sample_rate)
+            out[ch.utt_id] = ch.codes.to(torch.int16)
+    return out
+
+
+@torch.no_grad()
 def write_codes_wav(codec: MimiCodec, codes: Dict[str, torch.Tensor], dst: str, batch_size: int = 64) -> int:
     """One `<utt_id>_sample.wav` per utterance (main()'s file name), 24 kHz 16-bit: codes of equal length decode as one batch."""
     os.makedirs(dst, exist_ok=True)
@@ -233,6 +254,14 @@ def _synthesize_cli(args) -> int:
     if args.top_p or args.top_p_text:
         imp.sampling()   # validates a nucleus run's settings before the model runs
     corpus = torch.load(args.input, map_location="cpu")
+    if args.stream:
+        if not (args.wav_dir and args.codec_weights):
+            raise SystemExit("--stream needs --wav-dir and --codec-weights")
+        codec = _load_codec(argparse.Namespace(weights=args.codec_weights, config=args.codec_config, device=args.device))
+        codes = synthesize_stream(imp, codec, corpus, args.wav_dir, args.capacity, kv_gb=args.kv_gb)
+        save_tokens(codes, args.output_file)
+        print(f"synthesized {len(codes)} utterances -> {args.output_file}, streamed their wavs -> {args.wav_dir}")
+        return 0
     codes = synthesize(imp, corpus, args.capacity, kv_gb=args.kv_gb)
     save_tokens(codes, args.output_file)
     print(f"synthesized {len(codes)} utterances -> {args.output_file}")
@@ -422,6 +451,9 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--wav-dir", default=None, help="also write <utt_id>_sample.wav here (needs --codec-weights)")
     p.add_argument("--codec-weights", default=None)
     p.add_argument("--codec-config", default=None, help="json with the MimiCodec constructor arguments")
+    p.add_argument("--stream", action="store_true",
+                   help="with --wav-dir: decode each utterance's audio frame by frame while it generates "
+                        "(InferenceImp.stream_many) and write its wav as it completes; the codes file is the same")
     p.add_argument("--device", default="cuda")
     p = sub.add_parser("score", help="teacher-forced losses / audio perplexity of a corpus (infer_no_streaming.py teacher-force; "
                                      "--model moshi: the Moshi fine-tune trainer's validate_model)")

@@ -745,3 +745,94 @@ class MoshiDuplexEngine(_SessionRows, _PagedRows):
             torch.cuda.current_stream(self.dev).synchronize()
         self.latencies_ms.append(1e3 * (time.perf_counter() - t0))
         return {r: (self.tok_host[r].clone(), self.pcm_host[r, 0].clone()) if valid[r] else (None, None) for r in active}
+
+
+class TTSEngine:
+    """Request-driven streaming TTS: the batch TTS loop of InferenceImp.generate_many (`infer._TTSRows`, shared with
+    stream_many) over one LM scope of `capacity` rows and one codec streaming scope, taking requests while it runs.
+
+    `submit(utt_id, seq)` checks the request's TTS layout (InferenceImp._layout) and queues it; every `step()` admits
+    queued requests in submission order into free rows (waiting for KV pages as generate_many does), runs one generated
+    frame with its codec frame for all rows, and returns the chunks of the frame before it as TTSChunk(utt_id, index,
+    pcm [1920] float32 on the host, codes): an utterance of G frames gives chunks 0 .. G-2, and its last chunk carries
+    its codes [8, G-1] on the host, equal to generate_many's.  The host waits only for that previous frame's PCM copy,
+    so the device always has the current frame queued.  `step()` with nothing admitted or queued returns [] and launches
+    nothing.  The engine holds the model's and the codec's streaming scopes until `close()` (or the end of a `with`)."""
+
+    def __init__(self, imp, codec, capacity: int, *, kv_pages: Optional[int] = None):
+        from contextlib import ExitStack
+        from .infer import _TTSRows, _tts_scope
+        if isinstance(capacity, bool) or not isinstance(capacity, (int, np.integer)):
+            raise RstnetError(f"capacity must be an int (got {capacity!r})")
+        imp._check_many(int(capacity), kv_pages)
+        self.imp, self.codec, self.capacity = imp, codec, int(capacity)
+        self._stack = ExitStack()
+        try:
+            self._stack.enter_context(_tts_scope(imp.model, self.capacity, kv_pages))
+            self._stack.enter_context(codec.streaming(self.capacity, clip_window=True))
+            self._rows = _TTSRows(imp, self.capacity, False, {}, codec)
+        except BaseException:
+            self._stack.close()
+            raise
+        self._queue: Deque[tuple] = deque()
+        self._live: set = set()          # utt ids submitted whose last chunk has not been returned
+        self._closed = False
+
+    def submit(self, utt_id, seq: torch.Tensor, sampling: Optional[Sampling] = None, seed: int = 0) -> None:
+        """Queue one utterance, seq [9, L] in the TTS layout (raises at once on a bad layout, on a request longer than the
+        whole KV pool and on an id still in flight).  sampling: its own settings (from then on every row samples through
+        the per-row tables); seed: its random stream."""
+        if self._closed:
+            raise RstnetError("the engine is closed")
+        if sampling is not None and not isinstance(sampling, Sampling):
+            raise RstnetError(f"sampling must be a Sampling (got {type(sampling).__name__})")
+        if isinstance(seed, bool) or not isinstance(seed, (int, np.integer)):
+            raise RstnetError(f"seed must be an int (got {seed!r})")
+        if utt_id in self._live:
+            raise RstnetError(f"utterance {utt_id!r} is already queued or generating")
+        seq = torch.as_tensor(seq)
+        if seq.dim() != 2 or seq.shape[0] != self._rows.dep_q + 1:
+            raise RstnetError(f"seq must be [{self._rows.dep_q + 1}, L], got {tuple(seq.shape)}")
+        P, G = self.imp._layout(seq)
+        self._rows.fits(utt_id, P, G)
+        if sampling is not None:
+            self._rows.use_per_row()
+        self._live.add(utt_id)
+        self._queue.append((utt_id, seq, P, G, sampling, int(seed)))
+
+    @property
+    def pending(self) -> int:
+        """requests submitted and not yet admitted"""
+        return len(self._queue) + (self._rows.pending is not None)
+
+    @property
+    def active(self) -> int:
+        """admitted utterances whose last chunk has not been returned yet"""
+        return len(self._live) - self.pending
+
+    @torch.no_grad()
+    def step(self) -> List:
+        if self._closed:
+            raise RstnetError("the engine is closed")
+        chunks = self._rows.stream_step(lambda: self._queue.popleft() if self._queue else None) or []
+        for c in chunks:
+            if c.codes is not None:
+                self._live.discard(c.utt_id)
+        return chunks
+
+    def close(self) -> None:
+        """Leave the scopes (the chunks of a frame still in flight are dropped) and check the LM's device error flags."""
+        if self._closed:
+            return
+        self._closed = True
+        try:
+            if self._rows.n:
+                self.imp.model.check_device_errors()
+        finally:
+            self._stack.close()
+
+    def __enter__(self) -> "TTSEngine":
+        return self
+
+    def __exit__(self, *exc) -> None:
+        self.close()

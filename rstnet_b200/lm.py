@@ -337,10 +337,126 @@ def merge_lora_weights(model: "GPT") -> None:
     return None
 
 
-class PagedKVModel:
-    """The paged-KV methods of a decode model whose streaming scope (`_state`, an `_LMState`) may keep its KV in pages:
-    `GPT` and the Moshi twin's `LMModel` (rstnet_b200.moshi)."""
+class _DecodeModel(nn.Module):
+    """What `GPT` and the Moshi twin's `LMModel` (rstnet_b200.moshi) share: state_dict keys renamed through `_RENAME`,
+    the token-id conventions both follow, the streaming protocol over one `_LMState` scope (`_state`; `_make_state` builds
+    the model's scope class), paged KV, the device error check and the non-streaming depth transformer (`forward_local`,
+    and the depth-only states teacher-forced scoring runs): the depth transformer is the same module in both, read through
+    the parameter names of `_DN`.  A model has `config` with the fields `_LMState` reads."""
 
+    # (internal prefix, state_dict prefix): subtrees stored under private names because the public name is an API object
+    _RENAME = ()
+
+    def __init__(self):
+        super().__init__()
+        self._state: Optional["_LMState"] = None
+        self._packed = None
+        self._local_states: Dict[int, "_LMState"] = {}   # depth-only states of forward_local / scoring, by row count
+        self._ns_state: Optional["_LMState"] = None      # scratch scope of the non-streaming temporal pass
+        self.use_cuda_graphs = True
+
+    def state_dict(self, *a, **kw):
+        sd = super().state_dict(*a, **kw)
+        out = type(sd)()
+        for k, v in sd.items():
+            for src, dst in self._RENAME:
+                if k.startswith(src):
+                    k = dst + k[len(src):]
+            out[k] = v
+        return out
+
+    def load_state_dict(self, state_dict, strict: bool = True, **kw):
+        sd = {}
+        for k, v in state_dict.items():
+            for src, dst in self._RENAME:
+                if k.startswith(dst):
+                    k = src + k[len(dst):]
+            sd[k] = v
+        self._packed = None
+        self._local_states, self._ns_state = {}, None
+        return super().load_state_dict(sd, strict=strict, **kw)
+
+    def _apply(self, fn, *a, **kw):
+        self._packed = None
+        self._local_states, self._ns_state = {}, None
+        return super()._apply(fn, *a, **kw)
+
+    # ---- token-id conventions (llama_streaming.py:590-634, models/model.py:226-288)
+    @property
+    def zero_token_id(self) -> int:
+        return -1
+
+    @property
+    def ungenerated_token_id(self) -> int:
+        return -2
+
+    @property
+    def num_codebooks(self) -> int:
+        return self.config.n_q + 1
+
+    @property
+    def num_audio_codebooks(self) -> int:
+        return self.config.n_q
+
+    @property
+    def audio_offset(self) -> int:
+        return 1
+
+    @property
+    def device(self):
+        return next(iter(self.parameters())).device
+
+    def _get_initial_token(self) -> torch.Tensor:
+        tok = torch.full([1, self.num_codebooks, 1], self.initial_token_id, device=self.device, dtype=torch.long)
+        tok[:, 0] = self.text_initial_token_id
+        return tok
+
+    def _make_state(self, B: int, **kw) -> "_LMState":
+        return _LMState(self, B, **kw)
+
+    # ---- StreamingModule protocol (modules/streaming.py:33-151)
+    def _check_runnable(self):
+        name = type(self).__name__
+        if self.device.type != "cuda":
+            raise RstnetError(f"{name} decode runs on CUDA only (sm_90a kernels; the CPU path is the reference itself)")
+        if next(self.parameters()).dtype != torch.bfloat16:
+            raise RstnetError(f"{name} decode runs in bfloat16: call .to(device, torch.bfloat16)")
+
+    @property
+    def is_streaming(self) -> bool:
+        return self._state is not None
+
+    @on_own_device
+    def streaming_forever(self, batch_size: int, kv_pages: Optional[int] = None, kv_page: int = KV_PAGE):
+        """kv_pages None: every stream owns a contiguous KV ring of `context` positions per layer.  kv_pages N: the layers'
+        KV lives in a shared pool of N pages of kv_page positions (kv_page_bytes each), and a stream holds only the
+        pages reserve_kv gives it -- none at entry.  Both give the same results bit for bit."""
+        self._check_runnable()
+        self._state = self._make_state(batch_size, kv_pages=kv_pages, kv_page=kv_page)
+
+    @contextmanager
+    def streaming(self, batch_size: int, kv_pages: Optional[int] = None, kv_page: int = KV_PAGE):
+        self.streaming_forever(batch_size, kv_pages=kv_pages, kv_page=kv_page)
+        try:
+            yield
+        finally:
+            self._state = None
+
+    @on_own_device
+    def reset_streaming(self, streams=None):
+        """reset_streaming (modules/streaming.py:115-126); `streams` (extension) restarts only those batch rows: their
+        position counters go back to 0 (the ring contents need no clearing: the position mask hides them)."""
+        if self._state is None:
+            raise ValueError("Trying to reset streaming, but the model wasn't streaming.")
+        self._state.reset(streams)
+
+    def set_active_streams(self, mask) -> None:
+        """Extension for batched serving: hold the rows whose flag is 0 during the following steps (see codec.py)."""
+        if self._state is None:
+            raise ValueError("the model is not streaming")
+        self._state.set_active(mask)
+
+    # ---- paged KV (streaming(B, kv_pages=N))
     def _paged(self) -> "_LMState":
         st = self._state
         if st is None:
@@ -374,13 +490,7 @@ class PagedKVModel:
         """Paged scope: bytes of one KV page over all layers (K and V, bf16)."""
         return kv_page_bytes(self.config, self._paged().pages.page)
 
-
-class DepthLocalModel:
-    """The non-streaming depth transformer (`forward_local`, and the depth-only states teacher-forced scoring runs) and the
-    device error check, shared by `GPT` and the Moshi twin's `LMModel` (rstnet_b200.moshi): the depth transformer is the
-    same module in both, read through the parameter names of `_DN`.  A model provides `_make_state(B, **kw)` (its scope
-    class), `_check_runnable()` and a `_local_states` dict."""
-
+    # ---- device errors and the non-streaming depth transformer
     def check_device_errors(self, clear: bool = True) -> None:
         """Raise if a kernel met an input the reference would have raised on (out-of-range token id, position beyond
         block_size): device code cannot raise, it poisons its output and sets a sticky flag (synchronises)."""
@@ -421,7 +531,7 @@ class DepthLocalModel:
         return st
 
 
-class GPT(PagedKVModel, DepthLocalModel, nn.Module):
+class GPT(_DecodeModel):
     def __init__(self, config: Config, device=None, dtype=None):
         """device/dtype: create the (random-init) parameters directly there (a 7B model in bf16 on the GPU
         without a 28 GB fp32 host copy); default = CPU fp32 like the reference constructor."""
@@ -469,11 +579,6 @@ class GPT(PagedKVModel, DepthLocalModel, nn.Module):
             _register(self, f"audio_linears.{i}.weight", w_(c.audio_card, D))
         self.max_seq_length = c.block_size
         self.codecformer = _DepthScope(self)
-        self._state: Optional["_LMState"] = None
-        self._packed = None
-        self._local_states: Dict[int, "_LMState"] = {}
-        self._ns_state: Optional["_LMState"] = None      # scratch scope of the non-streaming forward_global
-        self.use_cuda_graphs = True
 
     # parameter names of the depth transformer (the Moshi-style LMModel of rstnet_b200/moshi.py has the same structure under
     # other names, models/model.py:188-224)
@@ -484,24 +589,11 @@ class GPT(PagedKVModel, DepthLocalModel, nn.Module):
     # stored under private attribute names because `codecformer` / `codecformer_text_emb` are API objects here)
     _RENAME = (("codecformer_.", "codecformer."), ("codecformer_text_emb_.", "codecformer_text_emb."))
 
-    def state_dict(self, *a, **kw):
-        sd = super().state_dict(*a, **kw)
-        out = type(sd)()
-        for k, v in sd.items():
-            for src, dst in self._RENAME:
-                if k.startswith(src):
-                    k = dst + k[len(src):]
-            out[k] = v
-        return out
-
     def load_state_dict(self, state_dict, strict: bool = True, **kw):
         sd, lora = {}, {}
         old = {"lm_head.weight": "lm_head.linear.weight"}  # llama_streaming.py:762-766 compatibility mapping
         for k, v in state_dict.items():
             k = old.get(k, k)
-            for src, dst in self._RENAME:
-                if k.startswith(dst):
-                    k = src + k[len(dst):]
             for a, b in ((".attn.weight", ".attn.linear.weight"), (".proj.weight", ".proj.linear.weight"),
                          (".fc_1.weight", ".fc_1.linear.weight"), (".fc_2.weight", ".fc_2.linear.weight")):
                 if k.endswith(a) and k.startswith("transformer.h."):
@@ -511,9 +603,7 @@ class GPT(PagedKVModel, DepthLocalModel, nn.Module):
             else:
                 sd[k] = v
         self._merge_lora(sd, lora)
-        self._packed = None
-        self._local_states, self._ns_state = {}, None
-        return super().load_state_dict(sd, strict=strict, **kw)
+        return super().load_state_dict(sd, strict=strict, **kw)   # -> the internal names of _RENAME
 
     def _merge_lora(self, sd, lora):
         """W += (B @ A) * (lora_alpha / r) for every wrapped linear that carries LoRA factors: LoRALinear.merge /
@@ -537,16 +627,7 @@ class GPT(PagedKVModel, DepthLocalModel, nn.Module):
                 delta = (B @ A) * (c.lora_alpha / r)
             sd[kw_] = (W.float() + delta.to(W.device)).to(W.dtype)   # in-place add into the weight's dtype upstream (:133)
 
-    def _apply(self, fn, *a, **kw):
-        self._packed = None
-        self._local_states, self._ns_state = {}, None
-        return super()._apply(fn, *a, **kw)
-
     # ---- token-id conventions (llama_streaming.py:590-634)
-    @property
-    def zero_token_id(self) -> int:
-        return -1
-
     @property
     def text_initial_token_id(self) -> int:
         return 151655
@@ -555,80 +636,10 @@ class GPT(PagedKVModel, DepthLocalModel, nn.Module):
     def initial_token_id(self) -> int:
         return self.config.audio_card
 
-    @property
-    def num_codebooks(self) -> int:
-        return self.config.n_q + 1
-
-    @property
-    def num_audio_codebooks(self) -> int:
-        return self.config.n_q
-
-    @property
-    def audio_offset(self) -> int:
-        return 1
-
-    @property
-    def ungenerated_token_id(self) -> int:
-        return -2
-
-    @property
-    def device(self):
-        return next(iter(self.parameters())).device
-
-    def _get_initial_token(self) -> torch.Tensor:
-        tok = torch.full([1, self.num_codebooks, 1], self.initial_token_id, device=self.device, dtype=torch.long)
-        tok[:, 0] = self.text_initial_token_id
-        return tok
-
     def codecformer_text_emb(self, ids: torch.Tensor) -> torch.Tensor:
         w = dict(self.named_parameters())["codecformer_text_emb_.weight"]
         y = torch.nn.functional.embedding(ids.clamp(min=0), w)
         return torch.where((ids == self.zero_token_id)[..., None], torch.zeros(1, dtype=y.dtype, device=y.device), y)
-
-    def _make_state(self, B: int, **kw) -> "_LMState":
-        return _LMState(self, B, **kw)
-
-    # ---- StreamingModule protocol (modules/streaming.py:33-151)
-    def _check_runnable(self):
-        dev = self.device
-        if dev.type != "cuda":
-            raise RstnetError("GPT decode runs on CUDA only (sm_90a kernels; the CPU path is the reference itself)")
-        if next(self.parameters()).dtype != torch.bfloat16:
-            raise RstnetError("GPT decode runs in bfloat16: call .to(device, torch.bfloat16) as infer_no_streaming.py:104-105 does")
-
-    @property
-    def is_streaming(self) -> bool:
-        return self._state is not None
-
-    @on_own_device
-    def streaming_forever(self, batch_size: int, kv_pages: Optional[int] = None, kv_page: int = KV_PAGE):
-        """kv_pages None: every stream owns a contiguous KV ring of `context` positions per layer.  kv_pages N: the layers'
-        KV lives in a shared pool of N pages of kv_page positions (kv_page_bytes each), and a stream holds only the
-        pages reserve_kv gives it -- none at entry.  Both give the same results bit for bit."""
-        self._check_runnable()
-        self._state = _LMState(self, batch_size, kv_pages=kv_pages, kv_page=kv_page)
-
-    @contextmanager
-    def streaming(self, batch_size: int, kv_pages: Optional[int] = None, kv_page: int = KV_PAGE):
-        self.streaming_forever(batch_size, kv_pages=kv_pages, kv_page=kv_page)
-        try:
-            yield
-        finally:
-            self._state = None
-
-    @on_own_device
-    def reset_streaming(self, streams=None):
-        """reset_streaming (modules/streaming.py:115-126); `streams` (extension) restarts only those batch rows: their
-        position counters go back to 0 (the ring contents need no clearing: the position mask hides them)."""
-        if self._state is None:
-            raise ValueError("Trying to reset streaming, but the model wasn't streaming.")
-        self._state.reset(streams)
-
-    def set_active_streams(self, mask) -> None:
-        """Extension for batched serving: hold the rows whose flag is 0 during the following steps (see codec.py)."""
-        if self._state is None:
-            raise ValueError("the model is not streaming")
-        self._state.set_active(mask)
 
     def get_streaming_state(self):
         """modules/streaming.py:128-136: name -> state object; the whole LM is one streaming module here."""
@@ -937,9 +948,13 @@ class _LMState:
     """Buffers, KV rings, GEMM plans of one `streaming(B)` scope.  Rows of every activation buffer are (position,
     stream) pairs, position-major: row = tl * B + b.  The decode state has tn == 1; a prefill chunk state (`parent` set)
     has tn > 1 rows per stream and shares the parent's KV rings and position counters; a `parts == ("depth",)` state
-    only holds the depth transformer (forward_local)."""
+    only holds the depth transformer (forward_local).  The temporal weights and RoPE data (`_build_temporal`) and the RoPE
+    / KV append launch (`_rope_kv`) are GPT's; the Moshi twin's subclass (rstnet_b200.moshi) replaces them."""
 
-    def __init__(self, m: GPT, B: int, tn: int = 1, parent: Optional["_LMState"] = None, parts=("temporal", "depth"),
+    cos = sin = None   # the RoPE tables (None: the angles are computed from the positions, as the Moshi twin does)
+    kyutai_norm = 0    # the temporal transformer's first RMSNorm: 1 is Kyutai's rms_norm_f32 flavour
+
+    def __init__(self, m: "_DecodeModel", B: int, tn: int = 1, parent: Optional["_LMState"] = None, parts=("temporal", "depth"),
                  rows: Optional[int] = None, kv_pages: Optional[int] = None, kv_page: int = KV_PAGE, cap: Optional[int] = None):
         """rows: a ragged prefill chunk of that many rows (with `parent`): row r is stream row_stream[r] at position
         offset + row_tl[r] (-1: padding), and the counters advance by `delta` per stream.  kv_pages: a paged KV pool of
@@ -996,12 +1011,36 @@ class _LMState:
         self.row_mapped = rows is not None
         self.pages: Optional[KVPages] = None        # paged scope: the host allocator
         self.page_table: Optional[torch.Tensor] = None   # ... and its device table int32 [B, pages.stride]
-        self._kv_pages = (kv_pages, kv_page)
         if self.row_mapped:
             self.row_stream, self.row_tl = z(M, dtype=torch.int32), z(M, dtype=torch.int32)
             self.delta = z(B, dtype=torch.int64)
 
         if self.has_temporal:
+            self.seq = z(M, c.n_q + 1, dtype=torch.int64)
+            self.x, self.xn, self.q, self.att = z(M, E), z(M, E), z(M, nh * hs), z(M, nh * hs)
+            self.qkv, self.hmid = z(M, (nh + 2 * nkv) * hs), z(M, I)
+            self.out, self.logits = z(M, E), z(M, V)
+            if parent is None:
+                # one position counter per stream (per-stream reset / admission), mirrored on the host for the
+                # block_size check (under graph replay the device cannot raise)
+                self.offset = z(B, dtype=torch.int64)
+                self.pos_host = np.zeros(B, dtype=np.int64)
+                # advance flags: a stream with 0 is HELD by the next steps (frame scheduler rows without input)
+                self.active = torch.ones(B, dtype=torch.int64, device=dev)
+                self.active_host = np.ones(B, dtype=np.int64)
+                # KV rings, one K/V row per KV GROUP: [2, B, n_kv, cap, hs] (lit_model.py:607-615 stores n_head copies), or the
+                # paged pool [n_pages, 2, n_kv, page, hs] per layer, one table for all layers
+                if kv_pages is None:
+                    self.kv = [z(2, B, nkv, self.cap, hs) for _ in range(c.n_layer)]
+                else:
+                    self.pages = KVPages(kv_pages, B, kv_page, self.cap)
+                    self.page_table = torch.full((B, self.pages.stride), -1, dtype=torch.int32, device=dev)
+                    self.kv = [z(self.pages.n_pages, 2, nkv, kv_page, hs) for _ in range(c.n_layer)]
+            else:
+                # a chunk: B x tn time-major rows, or a row map (row_chunk); the parent's KV and counters
+                self.offset, self.pos_host, self.kv = parent.offset, parent.pos_host, parent.kv
+                self.active, self.active_host = parent.active, parent.active_host
+                self.pages, self.page_table = parent.pages, parent.page_table
             self._build_temporal(P, G, z, parent)
 
         if "depth" in parts:
@@ -1057,31 +1096,10 @@ class _LMState:
                 for l in range(c.n_layer)}
 
     def _build_temporal(self, P, G, z, parent):
-        m, c, B, M = self.m, self.c, self.B, self.M
+        """the temporal transformer's weights, GEMM plans and RoPE data"""
+        m, c = self.m, self.c
         dev, bf = m.device, torch.bfloat16
-        E, V, I = c.n_embd, c.padded_vocab_size, c.intermediate_size
-        nh, nkv, hs = c.n_head, c.n_query_groups, c.head_size
-        self.seq = z(M, c.n_q + 1, dtype=torch.int64)
-        self.x, self.xn, self.q, self.att = z(M, E), z(M, E), z(M, nh * hs), z(M, nh * hs)
-        self.qkv, self.hmid = z(M, (nh + 2 * nkv) * hs), z(M, I)
-        self.out, self.logits = z(M, E), z(M, V)
         if parent is None:
-            # one position counter per stream (per-stream reset / admission), mirrored on the host for the
-            # block_size check (under graph replay the device cannot raise)
-            self.offset = z(B, dtype=torch.int64)
-            self.pos_host = np.zeros(B, dtype=np.int64)
-            # advance flags: a stream with 0 is HELD by the next steps (frame scheduler rows without input)
-            self.active = torch.ones(B, dtype=torch.int64, device=dev)
-            self.active_host = np.ones(B, dtype=np.int64)
-            # KV rings, one K/V row per KV GROUP: [2, B, n_kv, cap, hs] (lit_model.py:607-615 stores n_head copies), or the
-            # paged pool [n_pages, 2, n_kv, page, hs] per layer, one table for all layers
-            n_pages, page = self._kv_pages
-            if n_pages is None:
-                self.kv = [z(2, B, nkv, self.cap, hs) for _ in range(c.n_layer)]
-            else:
-                self.pages = KVPages(n_pages, B, page, self.cap)
-                self.page_table = torch.full((B, self.pages.stride), -1, dtype=torch.int32, device=dev)
-                self.kv = [z(self.pages.n_pages, 2, nkv, page, hs) for _ in range(c.n_layer)]
             # RoPE tables in the model dtype (the reference's buffers are cast by .to(bfloat16)); lit_model.py:441-488
             n = c.rope_n_elem
             theta = 1.0 / (c.rope_base ** (torch.arange(0, n, 2).float() / n))
@@ -1094,9 +1112,7 @@ class _LMState:
             idx_theta = torch.outer(torch.arange(c.block_size) / c.rope_condense_ratio, theta).repeat(1, 2)
             self.cos, self.sin = torch.cos(idx_theta).to(bf).to(dev).contiguous(), torch.sin(idx_theta).to(bf).to(dev).contiguous()
         else:
-            self.offset, self.pos_host, self.kv, self.cos, self.sin = parent.offset, parent.pos_host, parent.kv, parent.cos, parent.sin
-            self.active, self.active_host = parent.active, parent.active_host
-            self.pages, self.page_table = parent.pages, parent.page_table
+            self.cos, self.sin = parent.cos, parent.sin
         self.tables = [P[f"input_emb.{i}.weight"] for i in range(c.n_q)]
         self.table_ptrs = torch.tensor([t.data_ptr() for t in self.tables], dtype=torch.int64, device=dev)
         self.wte = P["transformer.wte.weight"]
@@ -1143,24 +1159,22 @@ class _LMState:
         c, B, M, L = self.c, self.B, self.M, _lib.lib()
         st = ops._stream()
         E = c.n_embd
-        # a row map always indexes the position counters per stream (offset_stride 1), even with B == 1
         rs, rt = (self.row_stream.data_ptr(), self.row_tl.data_ptr()) if self.row_mapped else (None, None)
-        ost = 1 if self.row_mapped or self.offset.numel() > 1 else 0
+        ost = self._offset_stride()
         # a paged scope runs the same kernels through their paged entry points: the page table as three more arguments
         if self.pages is None:
-            rope, attention, pg = L.rstnet_lm_rope_kv_append_bf16, L.rstnet_lm_ring_decode_attention_bf16, ()
+            attention, pg = L.rstnet_lm_ring_decode_attention_bf16, ()
         else:
-            rope, attention = L.rstnet_lm_rope_kv_append_paged_bf16, L.rstnet_lm_paged_decode_attention_bf16
+            attention = L.rstnet_lm_paged_decode_attention_bf16
             pg = (self.page_table.data_ptr(), self.pages.stride, self.pages.log2_page)
         _lib.check(L.rstnet_lm_embed_sum_bf16(self.seq.data_ptr(), c.n_q + 1, self.wte.data_ptr(), self.wte.shape[0],
                                               self.table_ptrs.data_ptr(), self.tables[0].shape[0], c.n_q, E, self.x.data_ptr(), M, st),
                    "lm_embed_sum")
-        _lib.check(L.rstnet_lm_rms_norm_bf16(self.x.data_ptr(), self.n1_first.data_ptr(), self.xn.data_ptr(), M, E, c.norm_eps, 0, st), "rms")
+        _lib.check(L.rstnet_lm_rms_norm_bf16(self.x.data_ptr(), self.n1_first.data_ptr(), self.xn.data_ptr(), M, E, c.norm_eps,
+                                             self.kyutai_norm, st), "rms")
         for l, ly in enumerate(self.layers):
             ly["qkv"].run()
-            _lib.check(rope(self.qkv.data_ptr(), self.cos.data_ptr(), self.sin.data_ptr(), self.cos.shape[0], c.rope_n_elem,
-                            self.offset.data_ptr(), ost, rs, rt, self.q.data_ptr(), self.kv[l].data_ptr(), M, B, c.n_head,
-                            c.n_query_groups, c.head_size, self.cap, *pg, st), "rope_kv")
+            self._rope_kv(L, l, ost, rs, rt, pg, st)
             _lib.check(attention(self.q.data_ptr(), self.kv[l].data_ptr(), self.offset.data_ptr(), ost, rs, rt, self.att.data_ptr(),
                                  M, B, c.n_head, c.n_query_groups, c.head_size, self.cap, c.context, *pg, st), "attention")
             ly["proj"].run()   # + residual + norm_2 -> xn
@@ -1172,6 +1186,19 @@ class _LMState:
             _lib.check(L.rstnet_counter_add_rows(self.offset.data_ptr(), self.delta.data_ptr(), B, st), "counter_add_rows")
         else:
             ops.counter_add(self.offset, self.tn, self.active)
+
+    def _offset_stride(self) -> int:
+        """the position counters' stride in the RoPE and attention launches: 0 reads one counter for every row (a row map
+        always indexes them per stream, even with B == 1)"""
+        return 1 if self.row_mapped or self.offset.numel() > 1 else 0
+
+    def _rope_kv(self, L, l: int, ost: int, rs, rt, pg, st) -> None:
+        """layer l's RoPE of q and k from the cos / sin tables, and the K/V append to the ring or the pages"""
+        c = self.c
+        rope = L.rstnet_lm_rope_kv_append_bf16 if self.pages is None else L.rstnet_lm_rope_kv_append_paged_bf16
+        _lib.check(rope(self.qkv.data_ptr(), self.cos.data_ptr(), self.sin.data_ptr(), self.cos.shape[0], c.rope_n_elem,
+                        self.offset.data_ptr(), ost, rs, rt, self.q.data_ptr(), self.kv[l].data_ptr(), self.M, self.B, c.n_head,
+                        c.n_query_groups, c.head_size, self.cap, *pg, st), "rope_kv")
 
     def _depth(self, k: int, ids: Optional[torch.Tensor], id_stride: int, quirk: bool = True):
         """ids None: the step's input embedding is already in self.demb (forward_local passes features for step 0)."""
@@ -1251,7 +1278,7 @@ class _LMState:
     def _advance_host(self, n: int):
         """Host mirror of the position counters: the reference's cos.index_select raises past block_size
         (llama_streaming.py:972-975); a graph replay cannot, so the check happens here, before the launch."""
-        if int(self.pos_host.max()) + n > self.cos.shape[0]:
+        if self.cos is not None and int(self.pos_host.max()) + n > self.cos.shape[0]:
             raise IndexError(f"position {int(self.pos_host.max()) + n - 1} is beyond block_size = {self.cos.shape[0]} "
                              "(RoPE table exhausted; reset the stream or raise Config.block_size)")
         if self.pages is not None:

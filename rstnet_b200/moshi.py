@@ -38,43 +38,21 @@ from torch import nn
 from . import _lib, ops
 from ._lib import RstnetError
 from .codec import _register, on_own_device
-from .lm import (GPT, KV_PAGE, MAX_ROWS, MAX_STREAMS, DepthLocalModel, KVPages, PagedKVModel, Sampling, SkinnyGemm,  # noqa: F401
-                 _DepthScope, _LMState, _head_mode, combine_sums, score_item, score_packed)
+from .lm import (KV_PAGE, MAX_ROWS, MAX_STREAMS, Sampling, _DecodeModel, _DepthScope, _LMState, _head_mode, combine_sums,
+                 score_item, score_packed)
 
 
 class _MoshiState(_LMState):
     """`_LMState` with the Kyutai temporal layer: in_proj (p h d) -> pair-RoPE -> ring attention -> out_proj, gating FFN."""
 
+    kyutai_norm = 1
+
     def _pack_temporal(self, P):
         return {}
 
     def _build_temporal(self, P, G, z, parent):
-        m, c, B, M = self.m, self.c, self.B, self.M
-        dev = m.device
-        E, V, I = c.n_embd, c.padded_vocab_size, c.intermediate_size
-        nh, hs = c.n_head, c.head_size
-        self.seq = z(M, c.n_q + 1, dtype=torch.int64)
-        self.x, self.xn, self.q, self.att = z(M, E), z(M, E), z(M, E), z(M, E)
-        self.qkv, self.hmid = z(M, 3 * E), z(M, I)
-        self.out, self.logits = z(M, E), z(M, V)
-        if parent is None:
-            self.offset = z(B, dtype=torch.int64)
-            self.pos_host = np.zeros(B, dtype=np.int64)
-            self.active = torch.ones(B, dtype=torch.int64, device=dev)
-            self.active_host = np.ones(B, dtype=np.int64)
-            # contiguous rings [2, B, H, cap, hd] per layer, or the paged pool [n_pages, 2, H, page, hd] per layer with one table
-            n_pages, page = self._kv_pages
-            if n_pages is None:
-                self.kv = [z(2, B, nh, self.cap, hs) for _ in range(c.n_layer)]
-            else:
-                self.pages = KVPages(n_pages, B, page, self.cap)
-                self.page_table = torch.full((B, self.pages.stride), -1, dtype=torch.int32, device=dev)
-                self.kv = [z(self.pages.n_pages, 2, nh, page, hs) for _ in range(c.n_layer)]
-        else:
-            # a chunk of the non-streaming pass: B x tn time-major rows, or a row map (row_chunk); the parent's rings and counters
-            self.offset, self.pos_host, self.kv = parent.offset, parent.pos_host, parent.kv
-            self.active, self.active_host = parent.active, parent.active_host
-            self.pages, self.page_table = parent.pages, parent.page_table
+        m, c = self.m, self.c
+        dev, hs = m.device, c.head_size
         # freqs exactly as modules/rope.py:35-36 evaluates them (fp32 tensor * python scalar, then exp)
         ds = torch.arange(hs // 2, dtype=torch.float32)
         self.freqs = torch.exp(ds * (-math.log(m.max_period) * 2 / hs)).to(dev)
@@ -102,53 +80,24 @@ class _MoshiState(_LMState):
                        aux=self.out if last else self.xn, **kw)))
         self.head = G(self.out, P["text_linear.weight"], self.logits)
 
-    def _temporal(self, head: bool = True):
-        c, B, M, L = self.c, self.B, self.M, _lib.lib()
-        st = ops._stream()
-        E = c.n_embd
-        # a paged scope runs the same kernels through their paged entry points: the page table as three more arguments.  A
-        # row-mapped chunk (row_chunk, contiguous rings only) runs the pair-RoPE append's row-map entry point
-        rs, rt = (self.row_stream.data_ptr(), self.row_tl.data_ptr()) if self.row_mapped else (None, None)
-        if self.pages is None:
-            rope, attention, pg = L.rstnet_lm_rope_pair_kv_append_bf16, L.rstnet_lm_ring_decode_attention_bf16, ()
-        else:
-            rope, attention = L.rstnet_lm_rope_pair_kv_append_paged_bf16, L.rstnet_lm_paged_decode_attention_bf16
-            pg = (self.page_table.data_ptr(), self.pages.stride, self.pages.log2_page)
-        _lib.check(L.rstnet_lm_embed_sum_bf16(self.seq.data_ptr(), c.n_q + 1, self.wte.data_ptr(), self.wte.shape[0],
-                                              self.table_ptrs.data_ptr(), self.tables[0].shape[0], c.n_q, E, self.x.data_ptr(), M, st),
-                   "lm_embed_sum")
-        _lib.check(L.rstnet_lm_rms_norm_bf16(self.x.data_ptr(), self.n1_first.data_ptr(), self.xn.data_ptr(), M, E, 1e-8, 1, st), "rms")
-        for l, ly in enumerate(self.layers):
-            ly["qkv"].run()
-            if self.row_mapped:
-                _lib.check(L.rstnet_lm_rope_pair_kv_append_rows_bf16(self.qkv.data_ptr(), self.offset.data_ptr(), rs, rt, self.q.data_ptr(),
-                                                                     self.kv[l].data_ptr(), M, B, c.n_head, c.head_size, self.cap,
-                                                                     self.freqs.data_ptr(), st), "rope_pair_kv_rows")
-            else:
-                _lib.check(rope(self.qkv.data_ptr(), self.offset.data_ptr(), 1, self.q.data_ptr(), self.kv[l].data_ptr(), M, B, c.n_head,
-                                c.head_size, self.cap, self.freqs.data_ptr(), *pg, st), "rope_pair_kv")
-            _lib.check(attention(self.q.data_ptr(), self.kv[l].data_ptr(), self.offset.data_ptr(), 1, rs, rt, self.att.data_ptr(),
-                                 M, B, c.n_head, c.n_head, c.head_size, self.cap, c.context, *pg, st), "attention")
-            ly["proj"].run()
-            ly["fc"].run()
-            ly["down"].run()
-        if head:
-            self.head.run()
+    def _offset_stride(self) -> int:
+        return 1   # the pair-RoPE and attention launches index the counters per stream, even with B == 1
+
+    def _rope_kv(self, L, l: int, ost: int, rs, rt, pg, st) -> None:
+        """layer l's pair-RoPE at the positions' fp32 angles and the K/V append; a row-mapped chunk (row_chunk, contiguous
+        rings only) runs the row-map entry point"""
+        c = self.c
         if self.row_mapped:
-            _lib.check(L.rstnet_counter_add_rows(self.offset.data_ptr(), self.delta.data_ptr(), B, st), "counter_add_rows")
+            _lib.check(L.rstnet_lm_rope_pair_kv_append_rows_bf16(self.qkv.data_ptr(), self.offset.data_ptr(), rs, rt, self.q.data_ptr(),
+                                                                 self.kv[l].data_ptr(), self.M, self.B, c.n_head, c.head_size, self.cap,
+                                                                 self.freqs.data_ptr(), st), "rope_pair_kv_rows")
         else:
-            ops.counter_add(self.offset, self.tn, self.active)
-
-    def _advance_host(self, n: int):
-        # positions enter the RoPE as fp32 angles: no table to run out of.  A paged scope raises, before any launch and
-        # with the counters unchanged, when an active stream would write past its pages (held streams advance nothing).
-        if self.pages is not None:
-            act = np.flatnonzero(self.active_host)
-            self.pages.check(act, self.pos_host[act], n)
-        self.pos_host += n * self.active_host
+            rope = L.rstnet_lm_rope_pair_kv_append_bf16 if self.pages is None else L.rstnet_lm_rope_pair_kv_append_paged_bf16
+            _lib.check(rope(self.qkv.data_ptr(), self.offset.data_ptr(), ost, self.q.data_ptr(), self.kv[l].data_ptr(), self.M, self.B,
+                            c.n_head, c.head_size, self.cap, self.freqs.data_ptr(), *pg, st), "rope_pair_kv")
 
 
-class LMModel(PagedKVModel, DepthLocalModel, nn.Module):
+class LMModel(_DecodeModel):
     """Drop-in for ``models.model.LMModel`` (same constructor arguments / defaults): the streaming decode path, and the
     non-streaming evaluation forward (forward_text over whole sequences, forward_local, forward)."""
 
@@ -231,38 +180,6 @@ class LMModel(PagedKVModel, DepthLocalModel, nn.Module):
                                       n_q=n_q, dep_q=dep_q, audio_card=card, codecformer_dim=D, codecformer_heads=dnh,
                                       codecformer_layers=dnl, ff_hidden=dh, norm_eps=1e-8, block_size=1 << 62, rope_n_elem=0)
         self.depformer = _DepthScope(self)
-        self._state: Optional[_MoshiState] = None
-        self._packed = None
-        self._local_states = {}                          # depth-only states of forward_local / scoring, by row count
-        self._ns_state: Optional[_MoshiState] = None     # scratch scope of the non-streaming forward_text
-        self.use_cuda_graphs = True
-
-    # ---- state_dict keys identical to the reference (`depformer.` lives under a private name: `depformer` is an API object)
-    def state_dict(self, *a, **kw):
-        sd = super().state_dict(*a, **kw)
-        out = type(sd)()
-        for k, v in sd.items():
-            for src, dst in self._RENAME:
-                if k.startswith(src):
-                    k = dst + k[len(src):]
-            out[k] = v
-        return out
-
-    def load_state_dict(self, state_dict, strict: bool = True, **kw):
-        sd = {}
-        for k, v in state_dict.items():
-            for src, dst in self._RENAME:
-                if k.startswith(dst):
-                    k = src + k[len(dst):]
-            sd[k] = v
-        self._packed = None
-        self._local_states, self._ns_state = {}, None
-        return super().load_state_dict(sd, strict=strict, **kw)
-
-    def _apply(self, fn, *a, **kw):
-        self._packed = None
-        self._local_states, self._ns_state = {}, None
-        return super()._apply(fn, *a, **kw)
 
     def _make_state(self, B: int, **kw) -> _MoshiState:
         return _MoshiState(self, B, **kw)
@@ -272,12 +189,6 @@ class LMModel(PagedKVModel, DepthLocalModel, nn.Module):
         to MAX_ROWS consecutive positions never overwrites a key an earlier row of the same chunk still needs, and the
         window of `context` positions is exact at any length.  Attention runs with this cap and the model's context."""
         return _MoshiState(self, B, parts=("temporal",), cap=self.context + MAX_ROWS - 1)
-
-    def _check_runnable(self):
-        if self.device.type != "cuda":
-            raise RstnetError("LMModel decode runs on CUDA only (sm_90a kernels; the CPU path is the reference itself)")
-        if next(self.parameters()).dtype != torch.bfloat16:
-            raise RstnetError("LMModel decode runs in bfloat16: call .to(device, torch.bfloat16)")
 
     # ---- token conventions (models/model.py:226-288)
     @property
@@ -295,68 +206,6 @@ class LMModel(PagedKVModel, DepthLocalModel, nn.Module):
     @property
     def end_of_text_padding_id(self) -> int:
         return 0
-
-    @property
-    def zero_token_id(self) -> int:
-        return -1
-
-    @property
-    def ungenerated_token_id(self) -> int:
-        return -2
-
-    @property
-    def device(self):
-        return next(iter(self.parameters())).device
-
-    @property
-    def num_codebooks(self) -> int:
-        return self.n_q + 1
-
-    @property
-    def num_audio_codebooks(self) -> int:
-        return self.n_q
-
-    @property
-    def audio_offset(self) -> int:
-        return 1
-
-    def _get_initial_token(self) -> torch.Tensor:
-        tok = torch.full([1, self.num_codebooks, 1], self.initial_token_id, device=self.device, dtype=torch.long)
-        tok[:, 0] = self.text_initial_token_id
-        return tok
-
-    # ---- streaming protocol
-    @property
-    def is_streaming(self) -> bool:
-        return self._state is not None
-
-    @on_own_device
-    def streaming_forever(self, batch_size: int, kv_pages: Optional[int] = None, kv_page: int = KV_PAGE):
-        """kv_pages None: every stream owns a contiguous KV ring of `context` positions per layer.  kv_pages N: a shared
-        pool of N pages of kv_page positions per layer, and a stream holds only the pages reserve_kv gives it -- none at
-        entry (as GPT.streaming_forever).  Both give the same results bit for bit."""
-        self._check_runnable()
-        self._state = _MoshiState(self, batch_size, kv_pages=kv_pages, kv_page=kv_page)
-
-    @contextmanager
-    def streaming(self, batch_size: int, kv_pages: Optional[int] = None, kv_page: int = KV_PAGE):
-        self.streaming_forever(batch_size, kv_pages=kv_pages, kv_page=kv_page)
-        try:
-            yield
-        finally:
-            self._state = None
-
-    @on_own_device
-    def reset_streaming(self, streams=None):
-        if self._state is None:
-            raise ValueError("Trying to reset streaming, but the model wasn't streaming.")
-        self._state.reset(streams)
-
-    def set_active_streams(self, mask) -> None:
-        """Extension for batched serving: hold the rows whose flag is 0 during the following steps (as GPT does)."""
-        if self._state is None:
-            raise ValueError("the model is not streaming")
-        self._state.set_active(mask)
 
     def _st(self) -> _MoshiState:
         if self._state is None:

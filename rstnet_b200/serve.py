@@ -21,7 +21,7 @@ only for the frames it has run -- one at admission, one more each time it crosse
 ends.  The engine then also has `grow_kv(rows)`, `release_rows(rows)` and `kv_pages_free` (`_PagedRows`), and the
 scheduler admits on free pages and evicts a session whose next page the pool cannot give.
 
-Suspend / resume (`suspend_rows(rows)` / `resume_rows(rows, states)` on either engine, paged or not; `_SessionRows`): a
+Suspend / resume (`suspend_rows(rows)` / `resume_rows(rows, states)` on either engine, paged or not; `_DuplexCore`): a
 session's state -- codec carries and rings, resampler carries, the KV it wrote, counters, sampling settings -- is packed
 into pinned host memory (row_state.SessionState), which frees its row and its pages; later it is unpacked into any free
 row of a compatible engine, and the session goes on with the bytes an uninterrupted run would have produced.
@@ -212,7 +212,7 @@ class FrameScheduler:
 class _PagedRows:
     """The paged-KV policy of both duplex engines, over the LM whose scope holds the pages (`_kv_lm`: a GPT, or the
     LMGen's LMModel; None: contiguous rings).  Positions come from the scope's host mirror, so no call here waits on
-    the GPU, and every table change is uploaded outside graph replay (PagedKVModel.reserve_kv)."""
+    the GPU, and every table change is uploaded outside graph replay (the model's reserve_kv)."""
 
     kv_pages: Optional[int] = None
     _kv_lm = None
@@ -269,10 +269,15 @@ class _PagedRows:
         return n
 
 
-class _SessionRows:
-    """Suspend / resume of both duplex engines.  The engine lists a row's state as row_state regions (`_row_regions`) and
-    host fields (`_row_host` / `_set_row_host`); this class moves them with one segment gather / scatter launch per row on
-    a side stream of at most `swap_ctas` CTAs.
+class _DuplexCore(_PagedRows):
+    """What both duplex engines share: the client rate and its resamplers, the pinned host buffers, a tick's input half (PCM
+    copy -> upsample -> encode) and output half (decode -> downsample -> D2H -> synchronise -> per-row results), row
+    restarts, and suspend / resume.  An engine adds its LM part: `_reset_lm_rows`, `_lm_step`, and the row state of
+    `_row_host` / `_row_regions` / `_set_row_host` / `_per_row_sampling`.
+
+    Suspend / resume: the engine lists a row's state as row_state regions (`_row_regions`) and host fields (`_row_host` /
+    `_set_row_host`); this class moves them with one segment gather / scatter launch per row on a side stream of at most
+    `swap_ctas` CTAs.
 
     Ordering, with no host synchronise on the tick path:
       * suspend: the gather waits (an event) for the ticks already enqueued; the row then stays held -- a held row's
@@ -294,13 +299,95 @@ class _SessionRows:
 
     swap_ctas = 16
     _swap_stream: Optional[torch.cuda.Stream] = None
+    # True: the LM holds a row's decoder side through its warm-up (no tokens yet), so the codec decode and the downsampler
+    # run under the mask `dec_mask_dev` that `_lm_step` sets; False: under the tick's input mask
+    _lm_holds_decoder = False
 
-    def _swap_init(self) -> None:
+    def __init__(self, codec, lm, model, capacity: int, sample_rate: int, kv_pages: Optional[int], kv_page: int, n_codes: int):
+        """lm: what streams with the codec (a GPT, or an LMGen); model: the LM whose scope holds the KV (the GPT, or the
+        LMGen's LMModel); n_codes: the audio codes of a generated frame."""
+        self.sample_rate = check_client_rate(sample_rate)
+        self.frame_samples = self.sample_rate * 2 // 25                       # 80 ms at the client rate
+        if capacity > MAX_STREAMS:
+            raise RstnetError(f"the LM step takes at most {MAX_STREAMS} streams per scope (one weight-streaming GEMM pass), "
+                              f"got {capacity}")
+        self.codec, self.B, self.dev = codec, capacity, model.device
+        self._lm, self._model = lm, model
+        codec.streaming_forever(capacity)
+        if kv_pages is None:
+            lm.streaming_forever(capacity)
+        else:
+            lm.streaming_forever(capacity, kv_pages=kv_pages, kv_page=kv_page)
+            self.kv_pages, self._kv_lm = kv_pages, model
+        F = self.frame_samples
+        pin = self.dev.type == "cuda"                                           # False: host logic under a test's fakes
+        self.pcm_in = torch.zeros(capacity, 1, F, dtype=torch.float32, pin_memory=pin)
+        self.pcm_dev = torch.zeros(capacity, 1, FRAME_SAMPLES, dtype=torch.float32, device=self.dev)
+        self.up = self.down = None
+        if self.sample_rate != CODEC_RATE:
+            self.up = StreamingResampler(self.sample_rate, CODEC_RATE, capacity, self.dev)
+            self.down = StreamingResampler(CODEC_RATE, self.sample_rate, capacity, self.dev)
+            self.pcm_client_dev = torch.zeros(capacity, 1, F, dtype=torch.float32, device=self.dev)
+            self.pcm_out_dev = torch.zeros(capacity, F, dtype=torch.float32, device=self.dev)
+        self.tok_host = torch.zeros(capacity, n_codes + 1, dtype=torch.int64, pin_memory=pin)
+        self.pcm_host = torch.zeros(capacity, 1, F, dtype=torch.float32, pin_memory=pin)
+        self.mask_host = torch.zeros(capacity, dtype=torch.int64, pin_memory=pin)
+        self.latencies_ms: List[float] = []
+        self._kv_page, self._n_codes = kv_page, n_codes
         self._row_swaps: Dict[int, torch.cuda.Event] = {}   # row -> the last gather / scatter touching it
         self._scatters: List[torch.cuda.Event] = []         # scatters the next tick waits for
         self._in_flight: List[Tuple[torch.cuda.Event, List[int]]] = []
         self._keep: List[tuple] = []                        # (event, objects a swap reads / writes, blob to pool or None)
         self._blob_pool: List[torch.Tensor] = []
+
+    def reset_rows(self, rows, sampling=None, seed: Optional[int] = None) -> None:
+        """Restart `rows`.  sampling / seed give them their own settings and random stream (keyed by the seed and the
+        row's own frame count); from the first such call on, every row samples through per-row tables and keys, so a
+        session's tokens do not depend on its row or its admission tick.  Until then the engine draws exactly as before.
+        A session's random stream is its seed alone (None: 0): two sessions with the same settings, seed and input draw the
+        same tokens, so callers that want them decorrelated pass distinct seeds."""
+        if sampling is not None and not isinstance(sampling, Sampling):
+            raise RstnetError(f"sampling must be a Sampling (got {type(sampling).__name__})")
+        self._wait_rows(rows)
+        self._reserve_first_page(rows)
+        self.codec.reset_streaming(streams=list(rows))
+        self._reset_lm_rows(rows, sampling, seed)
+        if self.up is not None:
+            self.up.reset(rows)
+            self.down.reset(rows)
+
+    @torch.no_grad()
+    def step(self, pcm_rows: Dict[int, torch.Tensor], active: List[int]):
+        t0 = time.perf_counter()
+        self._before_tick()
+        self.mask_host.zero_()
+        for r, chunk in pcm_rows.items():
+            self.pcm_in[r, 0].copy_(torch.as_tensor(chunk, dtype=torch.float32).reshape(self.frame_samples))
+            self.mask_host[r] = 1
+        self.codec.set_active_streams(self.mask_host)
+        self._lm.set_active_streams(self.mask_host)
+        if self.up is None:
+            self.pcm_dev.copy_(self.pcm_in, non_blocking=True)
+        else:
+            self.up.set_active(self.mask_host)
+            if not self._lm_holds_decoder:
+                self.down.set_active(self.mask_host)
+            self.pcm_client_dev.copy_(self.pcm_in, non_blocking=True)
+            self.up(self.pcm_client_dev[:, 0], out=self.pcm_dev[:, 0])                  # r -> 24 kHz, all rows
+        toks, codes, valid = self._lm_step(self.codec.encode(self.pcm_dev))     # encode: [B, 8, 1]
+        if toks is not None:
+            pcm = self.codec.decode(codes)                                        # [B, 1, 1920]
+            if self.down is not None:
+                if self._lm_holds_decoder:
+                    self.down.set_active(self.dec_mask_dev)
+                pcm = self.down(pcm[:, 0], out=self.pcm_out_dev)[:, None]                  # 24 kHz -> r, all rows
+            self.tok_host.copy_(toks, non_blocking=True)
+            self.pcm_host.copy_(pcm, non_blocking=True)
+        if self.dev.type == "cuda":
+            torch.cuda.current_stream(self.dev).synchronize()
+        self.latencies_ms.append(1e3 * (time.perf_counter() - t0))
+        return {r: (self.tok_host[r].clone(), self.pcm_host[r, 0].clone()) if valid is None or valid[r] else (None, None)
+                for r in active}
 
     def _prune(self) -> None:
         """drop the host memory of completed swaps; the blobs of completed resumes go back to the pool"""
@@ -341,7 +428,7 @@ class _SessionRows:
 
     def row_bytes(self, positions: int) -> int:
         """the blob size of a session that has run `positions` LM positions"""
-        c = self._lm_config()
+        c = self._model.config
         kv = c.n_layer * 2 * c.n_query_groups * min(int(positions), c.context) * c.head_size * 2
         return row_state.layout(self._row_regions(0, dict(self._row_host(0), pos=0)))[1] + -(-kv // row_state.ALIGN) * row_state.ALIGN
 
@@ -366,7 +453,7 @@ class _SessionRows:
 
     def session_key(self) -> Tuple:
         """what a SessionState must match to restore here: engine kind, LM and codec shapes, client rate, KV page"""
-        cfg = self._lm_config()
+        cfg = self._model.config
         cfg = sorted((vars(cfg) if not hasattr(cfg, "__dataclass_fields__") else
                       {k: getattr(cfg, k) for k in cfg.__dataclass_fields__}).items())
         m = self.codec
@@ -380,7 +467,7 @@ class _SessionRows:
         if self.up is not None:
             regions += [("up." + n, sg) for n, sg in self.up.row_segments(row, self.frame_samples)]
             regions += [("down." + n, sg) for n, sg in self.down.row_segments(row, FRAME_SAMPLES)]
-        regions += [("lm." + n, sg) for n, sg in self._lm_state().row_segments(row, positions)]
+        regions += [("lm." + n, sg) for n, sg in self._model._state.row_segments(row, positions)]
         return regions
 
     @torch.no_grad()
@@ -482,7 +569,7 @@ class _SessionRows:
             self._set_row_host(r, s.host)
 
 
-class DuplexEngine(_SessionRows, _PagedRows):
+class DuplexEngine(_DuplexCore):
     """One streaming scope of a MimiCodec and a GPT for `capacity` sessions: per tick, for all rows at once,
     encode the sessions' 80 ms chunks -> one LM frame (temporal step + 8 depth steps + sampling) -> decode the generated
     codes (the three calls of server.py:128-136).  The LM input frame of a row is [its previous text token, the 8 codes of
@@ -498,13 +585,8 @@ class DuplexEngine(_SessionRows, _PagedRows):
     def __init__(self, codec, gpt, capacity: int, *, use_sampling: bool = True, temp_text: float = 0.7, top_k_text: int = 25,
                  temp: float = 0.8, top_k: int = 30, sample_rate: int = CODEC_RATE, top_p_text: float = 0.0, top_p: float = 0.0,
                  kv_pages: Optional[int] = None, kv_page: int = KV_PAGE):
-        self.sample_rate = check_client_rate(sample_rate)
-        self.frame_samples = self.sample_rate * 2 // 25                       # 80 ms at the client rate
-        if capacity > MAX_STREAMS:
-            raise RstnetError(f"the LM step takes at most {MAX_STREAMS} streams per scope (one weight-streaming GEMM pass), "
-                              f"got {capacity}")
-        self.codec, self.gpt, self.B = codec, gpt, capacity
-        self.dev = gpt.device
+        super().__init__(codec, gpt, gpt, capacity, sample_rate, kv_pages, kv_page, gpt.config.dep_q)
+        self.gpt = gpt
         self.sampling = dict(use_sampling=use_sampling, temp_text=temp_text, top_k_text=top_k_text, temp=temp, top_k=top_k)
         if top_p_text or top_p:
             self.sampling.update(top_p_text=top_p_text, top_p=top_p)
@@ -513,36 +595,9 @@ class DuplexEngine(_SessionRows, _PagedRows):
         self.row_keys = np.zeros(capacity, dtype=np.int64)
         self._keys_dirty = False
         self._valid_table = None
-        codec.streaming_forever(capacity)
-        if kv_pages is None:
-            gpt.streaming_forever(capacity)
-        else:
-            gpt.streaming_forever(capacity, kv_pages=kv_pages, kv_page=kv_page)
-            self.kv_pages, self._kv_lm = kv_pages, gpt
-        F = self.frame_samples
-        self.pcm_in = torch.zeros(capacity, 1, F, dtype=torch.float32).pin_memory()
-        self.pcm_dev = torch.zeros(capacity, 1, FRAME_SAMPLES, dtype=torch.float32, device=self.dev)
-        self.up = self.down = None
-        if self.sample_rate != CODEC_RATE:
-            self.up = StreamingResampler(self.sample_rate, CODEC_RATE, capacity, self.dev)
-            self.down = StreamingResampler(CODEC_RATE, self.sample_rate, capacity, self.dev)
-            self.pcm_client_dev = torch.zeros(capacity, 1, F, dtype=torch.float32, device=self.dev)
-            self.pcm_out_dev = torch.zeros(capacity, F, dtype=torch.float32, device=self.dev)
         self.prev_text = torch.full((capacity, 1, 1), gpt.text_initial_token_id, dtype=torch.int64, device=self.dev)
-        self.tok_host = torch.zeros(capacity, gpt.config.dep_q + 1, dtype=torch.int64).pin_memory()
-        self.pcm_host = torch.zeros(capacity, 1, F, dtype=torch.float32).pin_memory()
-        self.mask_host = torch.zeros(capacity, dtype=torch.int64).pin_memory()
-        self.latencies_ms: List[float] = []
-        self._kv_page, self._n_codes = kv_page, gpt.config.dep_q
-        self._swap_init()
 
-    # ---- the row state of suspend_rows / resume_rows (_SessionRows)
-    def _lm_config(self):
-        return self.gpt.config
-
-    def _lm_state(self):
-        return self.gpt._state
-
+    # ---- the row state of suspend_rows / resume_rows (_DuplexCore)
     def _row_host(self, r: int) -> dict:
         return {"pos": int(self.gpt._state.pos_host[r]), "key": int(self.row_keys[r]),
                 "sampling": None if self.row_sampling is None else self.row_sampling[r]}
@@ -560,14 +615,7 @@ class DuplexEngine(_SessionRows, _PagedRows):
         self.row_keys[r] = host["key"]
         self._keys_dirty = True
 
-    def reset_rows(self, rows, sampling=None, seed: Optional[int] = None) -> None:
-        """Restart `rows`.  sampling / seed give them their own settings and random stream (keyed by the seed and the
-        row's own frame count); from the first such call on, every row samples through per-row tables and keys, so a
-        session's tokens do not depend on its row or its admission tick.  Until then the engine draws exactly as before.
-        A session's random stream is its seed alone (None: 0): two sessions with the same settings, seed and input draw the
-        same tokens, so callers that want them decorrelated pass distinct seeds."""
-        if sampling is not None and not isinstance(sampling, Sampling):
-            raise RstnetError(f"sampling must be a Sampling (got {type(sampling).__name__})")
+    def _reset_lm_rows(self, rows, sampling, seed) -> None:
         if sampling is not None or seed is not None or self.row_sampling is not None:
             default = Sampling(*self._defaults)
             if self.row_sampling is None:
@@ -576,33 +624,11 @@ class DuplexEngine(_SessionRows, _PagedRows):
                 self.row_sampling[r] = sampling if sampling is not None else default
                 self.row_keys[r] = int(seed or 0) & 0xFFFFFFFF
             self._keys_dirty = True
-        self._wait_rows(rows)
-        self._reserve_first_page(rows)
-        self.codec.reset_streaming(streams=list(rows))
         self.gpt.reset_streaming(streams=list(rows))
         self.prev_text[list(rows)] = self.gpt.text_initial_token_id
-        if self.up is not None:
-            self.up.reset(rows)
-            self.down.reset(rows)
 
-    @torch.no_grad()
-    def step(self, pcm_rows: Dict[int, torch.Tensor], active: List[int]):
-        t0 = time.perf_counter()
-        self._before_tick()
-        self.mask_host.zero_()
-        for r, chunk in pcm_rows.items():
-            self.pcm_in[r, 0].copy_(torch.as_tensor(chunk, dtype=torch.float32).reshape(self.frame_samples))
-            self.mask_host[r] = 1
-        self.codec.set_active_streams(self.mask_host)
-        self.gpt.set_active_streams(self.mask_host)
-        if self.up is None:
-            self.pcm_dev.copy_(self.pcm_in, non_blocking=True)
-        else:
-            self.up.set_active(self.mask_host)
-            self.down.set_active(self.mask_host)
-            self.pcm_client_dev.copy_(self.pcm_in, non_blocking=True)
-            self.up(self.pcm_client_dev[:, 0], out=self.pcm_dev[:, 0])                  # r -> 24 kHz, all rows
-        codes = self.codec.encode(self.pcm_dev)                                   # [B, 8, 1]
+    def _lm_step(self, codes):
+        """-> (tokens [B, dep_q + 1], the codes to decode [B, dep_q, 1], None: every row has tokens)"""
         frame = torch.cat([self.prev_text, codes], dim=1)                        # [B, 9, 1]
         if self.row_sampling is None:
             toks = self.gpt.forward_step(frame, audio_valid=2048, **self.sampling)    # [B, 9]
@@ -614,17 +640,10 @@ class DuplexEngine(_SessionRows, _PagedRows):
             self._keys_dirty = False
         held = (self.mask_host == 0).to(self.dev)
         self.prev_text.copy_(torch.where(held[:, None, None], self.prev_text, toks[:, :1, None]))
-        pcm = self.codec.decode(toks[:, 1:, None].clamp(max=self.codec.codebook_size - 1))   # [B, 1, 1920]
-        if self.down is not None:
-            pcm = self.down(pcm[:, 0], out=self.pcm_out_dev)[:, None]                  # 24 kHz -> r, all rows
-        self.tok_host.copy_(toks, non_blocking=True)
-        self.pcm_host.copy_(pcm, non_blocking=True)
-        torch.cuda.current_stream().synchronize()
-        self.latencies_ms.append(1e3 * (time.perf_counter() - t0))
-        return {r: (self.tok_host[r].clone(), self.pcm_host[r, 0].clone()) for r in active}
+        return toks, toks[:, 1:, None].clamp(max=self.codec.codebook_size - 1), None
 
 
-class MoshiDuplexEngine(_SessionRows, _PagedRows):
+class MoshiDuplexEngine(_DuplexCore):
     """The serving loop of server.py:128-136 -- `mimi.encode -> lm_gen.step(codes) -> mimi.decode(tokens[:, 1:])` --
     for `capacity` sessions in one streaming scope of a MimiCodec and an `LMGen` (rstnet_b200.moshi).
 
@@ -635,52 +654,21 @@ class MoshiDuplexEngine(_SessionRows, _PagedRows):
     None.  Text-piece decoding and the transport stay with the caller.  `sample_rate` and `kv_pages` / `kv_page` as for
     `DuplexEngine` (the pages are the LMGen's LMModel scope's)."""
 
+    _lm_holds_decoder = True
+
     def __init__(self, codec, lm_gen, capacity: int, *, sample_rate: int = CODEC_RATE, kv_pages: Optional[int] = None,
                  kv_page: int = KV_PAGE):
-        self.sample_rate = check_client_rate(sample_rate)
-        self.frame_samples = self.sample_rate * 2 // 25                       # 80 ms at the client rate
-        if capacity > MAX_STREAMS:
-            raise RstnetError(f"the LM step takes at most {MAX_STREAMS} streams per scope (one weight-streaming GEMM pass), "
-                              f"got {capacity}")
         lm = lm_gen.lm_model
         n_user = lm.num_codebooks - lm.dep_q - 1
         if codec.n_q != n_user:
             raise RstnetError(f"the codec emits {codec.n_q} codes per frame, the LM takes {n_user} user codebooks")
-        self.codec, self.lm_gen, self.B = codec, lm_gen, capacity
-        self.dev = lm.device
-        codec.streaming_forever(capacity)
-        if kv_pages is None:
-            lm_gen.streaming_forever(capacity)
-        else:
-            lm_gen.streaming_forever(capacity, kv_pages=kv_pages, kv_page=kv_page)
-            self.kv_pages, self._kv_lm = kv_pages, lm
-        F = self.frame_samples
-        pin = self.dev.type == "cuda"                                           # False: host logic under a test's fakes
-        self.pcm_in = torch.zeros(capacity, 1, F, dtype=torch.float32, pin_memory=pin)
-        self.pcm_dev = torch.zeros(capacity, 1, FRAME_SAMPLES, dtype=torch.float32, device=self.dev)
-        self.up = self.down = None
-        if self.sample_rate != CODEC_RATE:
-            self.up = StreamingResampler(self.sample_rate, CODEC_RATE, capacity, self.dev)
-            self.down = StreamingResampler(CODEC_RATE, self.sample_rate, capacity, self.dev)
-            self.pcm_client_dev = torch.zeros(capacity, 1, F, dtype=torch.float32, device=self.dev)
-            self.pcm_out_dev = torch.zeros(capacity, F, dtype=torch.float32, device=self.dev)
-        self.tok_host = torch.zeros(capacity, lm.dep_q + 1, dtype=torch.int64, pin_memory=pin)
-        self.pcm_host = torch.zeros(capacity, 1, F, dtype=torch.float32, pin_memory=pin)
-        self.mask_host = torch.zeros(capacity, dtype=torch.int64, pin_memory=pin)
-        self.dec_mask_host = torch.zeros(capacity, dtype=torch.int64, pin_memory=pin)
+        super().__init__(codec, lm_gen, lm, capacity, sample_rate, kv_pages, kv_page, lm.dep_q)
+        self.lm_gen = lm_gen
+        self.dec_mask_host = torch.zeros(capacity, dtype=torch.int64, pin_memory=self.dev.type == "cuda")
         self.dec_mask_dev = torch.zeros(capacity, dtype=torch.int64, device=self.dev)
-        self.latencies_ms: List[float] = []
-        self._kv_page, self._n_codes = kv_page, lm.dep_q
-        self._swap_init()
 
-    # ---- the row state of suspend_rows / resume_rows (_SessionRows): the decoder's warm-up is the delay cache's step
+    # ---- the row state of suspend_rows / resume_rows (_DuplexCore): the decoder's warm-up is the delay cache's step
     # count (off_host: no tokens, and the codec decoder held, for the first max_delay steps)
-    def _lm_config(self):
-        return self.lm_gen.lm_model.config
-
-    def _lm_state(self):
-        return self.lm_gen.lm_model._state
-
     def _row_host(self, r: int) -> dict:
         g = self.lm_gen
         return {"pos": int(g._st.lm.pos_host[r]), "off": int(g._st.off_host[r]), "stepped": bool(g._st.stepped[r]),
@@ -699,52 +687,23 @@ class MoshiDuplexEngine(_SessionRows, _PagedRows):
         g._st.off_host[r], g._st.stepped[r] = host["off"], host["stepped"]
         g._row_sampling[r] = host["sampling"] if host["sampling"] is not None else g.default_sampling()
 
-    def reset_rows(self, rows, sampling=None, seed: Optional[int] = None) -> None:
-        """Restart `rows`; sampling / seed as DuplexEngine.reset_rows (LMGen.set_stream_sampling)."""
-        self._wait_rows(rows)
-        self._reserve_first_page(rows)
-        self.codec.reset_streaming(streams=list(rows))
+    def _reset_lm_rows(self, rows, sampling, seed) -> None:
         self.lm_gen.reset_streaming(streams=list(rows))
         if sampling is not None or seed is not None or getattr(self.lm_gen, "_row_sampling", None) is not None:
             self.lm_gen.set_stream_sampling(list(rows), sampling, seed)
-        if self.up is not None:
-            self.up.reset(rows)
-            self.down.reset(rows)
 
-    @torch.no_grad()
-    def step(self, pcm_rows: Dict[int, torch.Tensor], active: List[int]):
-        t0 = time.perf_counter()
-        self._before_tick()
-        self.mask_host.zero_()
-        for r, chunk in pcm_rows.items():
-            self.pcm_in[r, 0].copy_(torch.as_tensor(chunk, dtype=torch.float32).reshape(self.frame_samples))
-            self.mask_host[r] = 1
-        self.codec.set_active_streams(self.mask_host)
-        self.lm_gen.set_active_streams(self.mask_host)
-        if self.up is None:
-            self.pcm_dev.copy_(self.pcm_in, non_blocking=True)
-        else:
-            self.up.set_active(self.mask_host)
-            self.pcm_client_dev.copy_(self.pcm_in, non_blocking=True)
-            self.up(self.pcm_client_dev[:, 0], out=self.pcm_dev[:, 0])                  # r -> 24 kHz, all rows
-        codes = self.codec.encode(self.pcm_dev)                                   # [B, 8, 1]
+    def _lm_step(self, codes):
+        """-> (tokens [B, dep_q + 1], the codes to decode [B, dep_q, 1], the rows past their warm-up), or no tokens and
+        no codes while every row is in its warm-up"""
         toks = self.lm_gen.step(codes)                                           # [B, dep_q + 1, 1] or None
         valid = self.lm_gen.valid_rows()                                         # host mirror: no device sync
-        if toks is not None:
-            # rows in their warm-up keep their decoder state: decode mask = active & valid, a device-to-device copy
-            self.dec_mask_host.copy_(torch.from_numpy(valid.astype("int64")))
-            self.dec_mask_dev.copy_(self.dec_mask_host, non_blocking=True)
-            self.codec.set_active_streams(self.dec_mask_dev)
-            pcm = self.codec.decode(toks[:, 1:].clamp(0, self.codec.codebook_size - 1))   # [B, 1, 1920]
-            if self.down is not None:
-                self.down.set_active(self.dec_mask_dev)
-                pcm = self.down(pcm[:, 0], out=self.pcm_out_dev)[:, None]                  # 24 kHz -> r, all rows
-            self.tok_host.copy_(toks[:, :, 0], non_blocking=True)
-            self.pcm_host.copy_(pcm, non_blocking=True)
-        if self.dev.type == "cuda":
-            torch.cuda.current_stream(self.dev).synchronize()
-        self.latencies_ms.append(1e3 * (time.perf_counter() - t0))
-        return {r: (self.tok_host[r].clone(), self.pcm_host[r, 0].clone()) if valid[r] else (None, None) for r in active}
+        if toks is None:
+            return None, None, valid
+        # rows in their warm-up keep their decoder state: decode mask = active & valid, a device-to-device copy
+        self.dec_mask_host.copy_(torch.from_numpy(valid.astype("int64")))
+        self.dec_mask_dev.copy_(self.dec_mask_host, non_blocking=True)
+        self.codec.set_active_streams(self.dec_mask_dev)
+        return toks[:, :, 0], toks[:, 1:].clamp(0, self.codec.codebook_size - 1), valid
 
 
 class TTSEngine:

@@ -434,7 +434,9 @@ int rstnet_lm_rope_pair_kv_append_rows_bf16(const void* qkv, const int64_t* offs
 /* ---- one query position per row over the ring with RingKVCache.complete's position labels and the
  * (pos_k>=0)&(delta>=0)&(delta<context) mask (llama_streaming.py:983-992), fp32 softmax. HBM-bound.  Rows and row map as
  * rstnet_lm_rope_kv_append_bf16 (padding rows write no output); every position of the launch must already be in the ring
- * and no slot a query needs may have been overwritten (callers keep *offset + Tn <= cap for Tn > 1).  This is the unpaged
+ * and no slot a query needs may have been overwritten (callers bound Tn as rstnet_b200/lm.py's prefill_chunk and
+ * row_chunk_positions do: up to the wrap, then cap - context + 1).  cap < 2 or
+ * context < 1 (an empty window) is an error return before any launch.  This is the unpaged
  * case of rstnet_lm_paged_decode_attention_bf16; both run the same kernel. */
 int rstnet_lm_ring_decode_attention_bf16(const void* q, const void* kv, const int64_t* offset, int32_t offset_stride,
                                          const int32_t* row_stream, const int32_t* row_tl, void* out, int32_t rows, int32_t B,

@@ -974,10 +974,7 @@ def _run_plan(plan, graphs: Optional[bool]) -> None:
             plan.launch()  # eager warm-up steps (also set the kernels' smem attributes)
             return
         torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            plan.launch()  # capture only; nothing executes until replay
-        plan.graph = g
+        plan.graph = ops.capture(plan.launch)  # capture only; nothing executes until replay
     plan.graph.replay()
 
 

@@ -1033,6 +1033,9 @@ static int ring_decode_attention(const void* q, const void* kv, const int64_t* o
   RSTNET_REQUIRE(rows > 0 && B > 0 && (row_stream || rows % B == 0),
                  "lm_ring_decode_attention: rows (%d) must be a multiple of the stream count (%d) without a row map", rows, B);
   RSTNET_REQUIRE(n_kv > 0 && n_head % n_kv == 0, "lm_ring_decode_attention: n_head (%d) must be a multiple of n_kv (%d)", n_head, n_kv);
+  // the window of a query is max(0, pos - context + 1, pos + 2 - cap) .. pos: with cap < 2 or context < 1 it is empty and
+  // every output would be 0 / 0
+  RSTNET_REQUIRE(cap >= 2 && context >= 1, "lm_ring_decode_attention: cap (%d) must be >= 2 and context (%d) >= 1", cap, context);
   const float scale = 1.0f / sqrtf((float)hs);
   const int q_per_kv = n_head / n_kv;
   const int G = q_per_kv % 2 == 0 ? 2 : 1;   // query heads per CTA sharing the K/V rows (the rest of a group hits L2)

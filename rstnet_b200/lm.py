@@ -53,6 +53,25 @@ def kv_pages_for_budget(c: "Config", gib: float, page: int = KV_PAGE) -> int:
     return int(gib * 2 ** 30 // kv_page_bytes(c, page))
 
 
+# A multi-position chunk appends all its keys before any of its queries attend, so it must not overwrite a ring slot one
+# of those queries still needs.  Its first query at position p reads back to max(0, p - context + 1): the chunk may run
+# up to the wrap (cap - p positions) before that, and cap - context + 1 positions once the window starts inside the ring
+# (1 for a ring of `context` slots).
+def prefill_chunk(per: int, left: int, cap: int, context: int, pos_max: int) -> int:
+    """Positions per stream of the next chunk of GPT.forward_global's prefill: `per` = MAX_ROWS // B wanted, `left` still
+    to feed, `pos_max` the furthest stream's next position"""
+    tn = min(per, left)
+    if tn > 1 and pos_max + tn > cap:
+        tn = min(tn, cap - context + 1)
+    return tn
+
+
+def row_chunk_positions(left: int, budget: int, cap: int, context: int, pos: int) -> int:
+    """Positions of one stream in the next ragged chunk (_LMState.row_chunk): `left` still to feed, `budget` rows free in
+    the chunk, `pos` the stream's next position"""
+    return min(left, budget, max(cap - pos, cap - context + 1))
+
+
 class KVPages:
     """Host side of a paged KV scope: which pool page holds each page of each stream's ring.  The ring itself is the
     contiguous scope's (position p in slot p % cap); page i of stream s (slots i*page .. (i+1)*page - 1) lives in pool
@@ -1269,10 +1288,7 @@ class _LMState:
                 fn()
                 return
             torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                fn()
-            self.graphs[key] = g
+            g = self.graphs[key] = ops.capture(fn)
         g.replay()
 
     def _advance_host(self, n: int):
@@ -1354,10 +1370,7 @@ class _LMState:
             self._replay(("temporal_nohead",), lambda: self._temporal(head=False))
             return None
         # prefill: chunks of tn consecutive positions for all streams (tn * B <= MAX_ROWS rows per launch sequence; more
-        # than MAX_ROWS streams go one position per pass through the decode state).
-        # A multi-position chunk appends all its keys before any of its queries run, so it must not overwrite a ring slot
-        # one of those queries still needs: once the ring wraps inside the chunk, tn <= cap - context + 1 (1 for a ring
-        # of `context` slots).
+        # than MAX_ROWS streams go one position per pass through the decode state), as long as prefill_chunk allows.
         if self.pages is not None:   # the whole prefill fits each active stream's reservation, or nothing is launched
             act = np.flatnonzero(self.active_host)
             self.pages.check(act, self.pos_host[act], T)
@@ -1365,9 +1378,7 @@ class _LMState:
         per = max(1, MAX_ROWS // B)
         t = 0
         while t < T:
-            tn = min(per, T - t)
-            if tn > 1 and int(self.pos_host.max()) + tn > self.cap:
-                tn = min(tn, self.cap - c.context + 1)
+            tn = prefill_chunk(per, T - t, self.cap, c.context, int(self.pos_host.max()))
             if tn == 1:
                 r = self.forward_global(sequence[:, :, t:t + 1], want_outputs)
                 if want_outputs:
@@ -1428,9 +1439,7 @@ class _LMState:
                 break
             if done >= p.shape[0]:
                 continue
-            # a chunk appends all its keys before any of its queries run: several positions of a stream while its ring
-            # does not wrap inside the chunk, and after that at most cap - context + 1 (as forward_global's prefill)
-            tn = min(p.shape[0] - done, budget, max(self.cap - int(self.pos_host[s]), self.cap - c.context + 1))
+            tn = row_chunk_positions(p.shape[0] - done, budget, self.cap, c.context, int(self.pos_host[s]))
             segs.append((s, len(rs), done, tn))
             rs += [s] * tn
             rt += range(tn)

@@ -7,6 +7,7 @@ and raises on failure (no fallback path).
 from __future__ import annotations
 
 import ctypes as C
+import gc
 from typing import Optional
 
 import torch
@@ -17,6 +18,22 @@ from ._lib import ACT_ELU, ACT_GELU, ACT_NONE, GemmRowsArgs, RowCopy, TcGemmDesc
 
 def _stream() -> int:
     return torch.cuda.current_stream().cuda_stream
+
+
+def capture(fn) -> torch.cuda.CUDAGraph:
+    """fn() captured into a new CUDA graph, with Python's cyclic garbage collector paused meanwhile: a collection inside
+    the capture may free an unreachable scope's own CUDA graph, and destroying a graph while a stream captures is not
+    permitted -- it invalidates this capture."""
+    g = torch.cuda.CUDAGraph()
+    enabled = gc.isenabled()
+    gc.disable()
+    try:
+        with torch.cuda.graph(g):
+            fn()
+    finally:
+        if enabled:
+            gc.enable()
+    return g
 
 
 def _p(t: Optional[torch.Tensor]) -> Optional[int]:

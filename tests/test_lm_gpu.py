@@ -131,17 +131,9 @@ def test_rope_append_and_ring_decode_attention(hs, cap, context, steps):
 
 
 def test_norms_silu_embed_vs_oracle():
+    """rstnet_lm_silu_mul_bf16 vs torch (RMSNorm is held to the per-element bound in test_lm_kernels_gpu.py)"""
     g = torch.Generator().manual_seed(1)
     lib, st = _lib.lib(), ops._stream()
-    x = (torch.randn(5, 1, 256, generator=g) * 2).to(BF)
-    w = (1 + 0.1 * torch.randn(256, generator=g)).to(BF)
-    for ky, ref in ((0, L.rms_norm(x, w, 1e-5)), (1, L.rms_norm_f32(x, w.view(1, 1, -1), 1e-8))):
-        y = torch.empty(5, 256, dtype=BF, device=DEV)
-        xd, wd = x.to(DEV).contiguous(), w.to(DEV).contiguous()
-        _lib.check(lib.rstnet_lm_rms_norm_bf16(xd.data_ptr(), wd.data_ptr(), y.data_ptr(), 5, 256, 1e-5 if ky == 0 else 1e-8, ky, st))
-        torch.cuda.synchronize()
-        d = (y.float().cpu() - ref[:, 0].float()).abs().max().item()
-        assert d <= 2e-2, (ky, d)  # at most one bf16 ulp at |y| ~ 4
     ab = torch.randn(7, 2 * 96, generator=g).to(BF)
     ref = F.silu(ab[:, :96]) * ab[:, 96:]
     out = torch.empty(7, 96, dtype=BF, device=DEV)
@@ -543,13 +535,13 @@ def test_cfg3_shape_wrapped_ring_vs_reference_eager_on_gpu():
                 assert _rel(a, b_) <= 2e-2
 
 
-@pytest.mark.parametrize("B", [4, 64, 37, 128])
+@pytest.mark.parametrize("B", [4, 64, 37, 128, 256])
 def test_attention_full_window_2047_keys_vs_sdpa(B):
     """ring_decode_attention at capacity 2048, wrapped, vs a float64 softmax over exactly the keys RingKVCache.complete
     leaves attendable, under the per-element bound of test_lm_kernels_gpu.py: MHA, GQA with an even and an odd q_per_kv
     (12 / 4 runs one query head per CTA with n_kv < n_head), MQA, head size 64, and windows shorter than the ring
     (context < cap).  B > 8 puts streams at different fill levels (few keys, partially filled ring, wrapped) in one launch;
-    B = 128 is the most rows one launch takes (lm.MAX_ROWS)."""
+    B = 256 is the most rows one decode launch takes (lm.MAX_STREAMS streams of one position each)."""
     lib, st_ = _lib.lib(), ops._stream()
     cap = 2048
     g = torch.Generator(device=DEV).manual_seed(9)

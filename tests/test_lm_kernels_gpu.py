@@ -177,6 +177,37 @@ def test_skinny_gemm_residual_rmsnorm_finalize(M, N, K, max_splits, kyutai, spre
     check_bound(f"skinny fin_mode 1 aux ({'kyutai' if kyutai else 'lit'}) M {M} N {N}", aux, y, 0.0, 0.999)
 
 
+# ---------------------------------------------------------------------------------------------- standalone RMSNorm
+@pytest.mark.parametrize("kyutai", [False, True])
+@pytest.mark.parametrize("rows", [1, 37, 256])
+@pytest.mark.parametrize("dim", [1000, 1024, 2048, 3072, 4096])
+def test_rms_norm_per_element(dim, rows, kyutai):
+    """rstnet_lm_rms_norm_bf16 (the first pre-norm of every frame, on the residual stream) vs the float64 RMSNorm with the
+    aux check's eps placement and multiplication order, one bf16 ulp and no slack.  Rows are scaled 2^-8 .. 2^8 apart
+    and the last of several rows is all zero, so a row mix-up or a sum taken over the wrong row cannot hide; dim 1000 is
+    not a multiple of the 256-thread block."""
+    g = torch.Generator().manual_seed(dim + rows + kyutai)
+    s = 2.0 ** (torch.arange(rows) % 17 - 8).float()[:, None]
+    x = (torch.randn(rows, dim, generator=g) * s).to(BF)
+    if rows > 1:
+        x[-1] = 0
+    w = (1 + 0.1 * torch.randn(dim, generator=g)).to(BF)
+    eps = 1e-8 if kyutai else 1e-5
+    y = torch.full((rows + 1, dim), NAN, dtype=BF, device=DEV)   # one row past the output must stay untouched
+    xd, wd = x.to(DEV), w.to(DEV)
+    _lib.check(_lib.lib().rstnet_lm_rms_norm_bf16(xd.data_ptr(), wd.data_ptr(), y.data_ptr(), rows, dim, eps, int(kyutai),
+                                                  ops._stream()))
+    torch.cuda.synchronize()
+    assert y[rows].isnan().all()
+    o, w64 = x.to(F64), w.to(F64)
+    eps32 = float(torch.tensor(eps, dtype=torch.float32))
+    ms = (o * o).mean(-1, keepdim=True)
+    ref = o * (w64 * torch.rsqrt(eps32 + ms)) if kyutai else (o * torch.rsqrt(ms + eps32)) * w64
+    check_bound(f"rms norm ({'kyutai' if kyutai else 'lit'}) rows {rows} dim {dim}", y[:rows], ref, 0.0, 0.999)
+    if rows > 1:
+        assert bool((y[rows - 1] == 0).all()), "an all-zero row normalises to zeros"
+
+
 # --------------------------------------------------------------------------------- skinny GEMM, SiLU gating (2 and 3)
 def _gating_chain(a: torch.Tensor, b: torch.Tensor):
     """The documented roundings of the gating, evaluated in float64: bf16(bf16(silu(bf16(a))) * bf16(b)).  Also returns

@@ -261,7 +261,9 @@ int rstnet_rope_ring_attention_f32(const float* qkv, int64_t q_batch_stride, int
  * norms.  Distances follow torch.cdist's matmul form sqrt(max(|x|^2+|e|^2-2x.e, 0)); argmin
  * keeps the first minimum.  codes out: int64 [B][n_q][T] with N == B*T; frame n = b*T + t, or
  * n = t*B + b when time_major != 0 (the streaming plans' [T, B, C] layout).
- * work: scratch of rstnet_rvq_encode_workspace(N, ...) bytes. */
+ * work: scratch of rstnet_rvq_encode_workspace(N, ...) bytes; its contents on entry do not matter.
+ * Requires dim % 16 == 0, bins % 128 == 0, ldx % 4 == 0, N % T == 0, 0 <= n_q_semantic <= n_q; x, E, Et,
+ * enorm and work 16-byte aligned, codes 8-byte aligned (error return otherwise, nothing launched). */
 int64_t rstnet_rvq_encode_workspace(int64_t N, int32_t n_q, int32_t dim, int32_t bins);
 int rstnet_rvq_encode_f32(const float* x, int64_t ldx, const float* E, const float* Et,
                           const float* enorm, int64_t* codes, void* work, int64_t N, int32_t T,
@@ -269,7 +271,8 @@ int rstnet_rvq_encode_f32(const float* x, int64_t ldx, const float* E, const flo
                           int32_t time_major, rstnet_stream_t stream);
 /* ---- SplitResidualVectorQuantizer.decode gather part (vq.py:317-323; core_vq.py:198-206,
  * 378-384): q [N, 2*dim] = [ E0[c0] | sum_{l>=n_q_semantic} E_l[c_l] ]; the two output_proj are
- * then one rstnet_gemm_rows_f32 with K = 2*dim. */
+ * then one rstnet_gemm_rows_f32 with K = 2*dim.  Requires dim % 4 == 0; E and q 16-byte aligned,
+ * codes 8-byte aligned (error return otherwise, nothing launched). */
 int rstnet_rvq_decode_gather_f32(const int64_t* codes, const float* E, float* q, int64_t N, int32_t T,
                                  int32_t n_q, int32_t n_q_semantic, int32_t dim, int32_t bins,
                                  int32_t time_major, rstnet_stream_t stream);

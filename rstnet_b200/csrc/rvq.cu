@@ -93,7 +93,9 @@ __global__ void __launch_bounds__(RQ_NT) rvq_level_kernel(const RvqLevelParams p
         argmin_combine(v, idx, ov, oi);
       }
       if (lane == 0) {
-        code_s[r] = (n < p.N) ? idx : 0;
+        // every d is a number, so the argmin always takes a candidate and idx is in [0, bins); the check keeps the
+        // centroid gather below in bounds should that ever stop holding (the code written out still shows it)
+        code_s[r] = (n < p.N && idx >= 0 && idx < p.bins) ? idx : 0;
         if (blockIdx.y == 0 && n < p.N) {
           const long long nb = p.N / p.T;
           const long long b = p.time_major ? n % nb : n / p.T, t = p.time_major ? n / nb : n % p.T;
@@ -269,6 +271,10 @@ extern "C" int rstnet_rvq_encode_f32(const float* x, int64_t ldx, const float* E
   RSTNET_REQUIRE(N > 0 && T > 0 && N % T == 0, "rvq_encode: N (%lld) must be a positive multiple of T (%d)", (long long)N, T);
   RSTNET_REQUIRE(n_q > 0 && ns >= 0 && ns <= n_q, "rvq_encode: bad level split");
   RSTNET_REQUIRE(dim % 16 == 0 && bins % RQ_BN == 0 && ldx % 4 == 0, "rvq_encode: dim %% 16, bins %% 128, ldx %% 4 required");
+  // the level kernel reads x, the residuals, E and enorm as float4 and streams Et with 16-byte cp.async
+  RSTNET_REQUIRE((uintptr_t)x % 16 == 0 && (uintptr_t)E % 16 == 0 && (uintptr_t)Et % 16 == 0 && (uintptr_t)enorm % 16 == 0 &&
+                     (uintptr_t)work % 16 == 0 && (uintptr_t)codes % 8 == 0,
+                 "rvq_encode: x, E, Et, enorm and work must be 16-byte aligned, codes 8-byte aligned");
   const size_t smem = rvq_smem_bytes(dim);
   RSTNET_REQUIRE(smem <= 220 * 1024, "rvq_encode: dim too large for shared memory");
   static unsigned long long attr = 0;
@@ -325,6 +331,8 @@ extern "C" int rstnet_rvq_decode_gather_f32(const int64_t* codes, const float* E
                                             rstnet_stream_t stream) {
   RSTNET_REQUIRE(codes && E && q, "rvq_decode_gather: null pointer");
   RSTNET_REQUIRE(N > 0 && T > 0 && N % T == 0 && dim % 4 == 0, "rvq_decode_gather: bad shape");
+  RSTNET_REQUIRE((uintptr_t)E % 16 == 0 && (uintptr_t)q % 16 == 0 && (uintptr_t)codes % 8 == 0,
+                 "rvq_decode_gather: E and q must be 16-byte aligned, codes 8-byte aligned");
   const long long total = (long long)N * (dim / 4);
   int gx = ceil_div(total, 256);
   if (gx > sm_count() * 16) gx = sm_count() * 16;

@@ -547,6 +547,20 @@ typedef struct {
 int rstnet_segments_gather(const rstnet_segment* table_dev, int32_t n, void* staging, int32_t ctas, rstnet_stream_t s);
 int rstnet_segments_scatter(const rstnet_segment* table_dev, int32_t n, const void* staging, int32_t ctas, rstnet_stream_t s);
 
+/* ---- batched KV page copy (paged decode scopes; added in version 206): for every pool i < n_pools (pools[i], one per
+ * layer, a host array of device pointers) and every pair j < n_pairs, the page_bytes at pools[i] + pairs[2j] * page_bytes
+ * are copied to pools[i] + pairs[2j + 1] * page_bytes.  `pairs` (int32 (src, dst) pairs) is device memory or pinned host
+ * memory, which the kernel reads directly; a device table is copied back to the host for the checks, which synchronises,
+ * so a launch that a stream captures into a graph takes a pinned host table (its entries are read at every replay).  One
+ * launch of at most `ctas` CTAs; accesses are 16 bytes wide where the pool base and page_bytes are 16-byte aligned, else 8,
+ * 4 or 1.  Checked before any launch, each an error return: a null pools / pairs / pool pointer, n_pools outside
+ * [1, RSTNET_KV_COPY_MAX_POOLS], n_pairs < 0, page_bytes <= 0, ctas < 1, a negative page index, src == dst, a page that
+ * is the dst of two pairs or both a src and a dst.  Page indices are not checked against the pool size (the caller's, as
+ * with the page table).  n_pairs == 0 launches nothing. */
+#define RSTNET_KV_COPY_MAX_POOLS 256
+int rstnet_kv_pages_copy(const void* const* pools, int32_t n_pools, const int32_t* pairs, int32_t n_pairs, int64_t page_bytes,
+                         int32_t ctas, rstnet_stream_t s);
+
 #ifdef __cplusplus
 }
 #endif

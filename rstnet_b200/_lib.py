@@ -32,9 +32,11 @@ SYMBOLS = [
     "rstnet_lm_rope_kv_append_paged_bf16", "rstnet_lm_paged_decode_attention_bf16", "rstnet_lm_rope_pair_kv_append_paged_bf16",
     "rstnet_stft_loss_workspace", "rstnet_stft_loss_sums_f32", "rstnet_sisnr_moments_workspace", "rstnet_sisnr_moments_f32",
     "rstnet_segments_gather", "rstnet_segments_scatter", "rstnet_lm_rope_pair_kv_append_rows_bf16",
+    "rstnet_kv_pages_copy",
 ]
 
 KV_LOG2_PAGE_MIN, KV_LOG2_PAGE_MAX = 4, 12   # RSTNET_KV_LOG2_PAGE_MIN / _MAX: pages of 16 .. 4096 positions
+KV_COPY_MAX_POOLS = 256                      # RSTNET_KV_COPY_MAX_POOLS
 
 RESAMPLE_MAX_TABLE_BYTES = 48 * 1024   # RSTNET_RESAMPLE_MAX_TABLE_BYTES
 
@@ -183,6 +185,7 @@ def lib() -> C.CDLL:
     L.rstnet_sisnr_moments_f32.argtypes = [vp, vp, vp, vp, i32, i64, vp, vp, i64, vp]
     L.rstnet_segments_gather.argtypes = [vp, i32, vp, i32, vp]
     L.rstnet_segments_scatter.argtypes = [vp, i32, vp, i32, vp]
+    L.rstnet_kv_pages_copy.argtypes = [vp, i32, vp, i32, i64, i32, vp]
     for name in SYMBOLS:
         fn = getattr(L, name)
         if fn.restype is C.c_int and name not in ("rstnet_version",):

@@ -41,6 +41,37 @@ def candidate_counts(pre_gen_len: int, minlen: int, g_idx: int, dep_q: int = 8) 
     return [2049 if (g_len == pre_gen_len or (l > 0 and g_len > minlen)) else 2048 for l in range(dep_q)]
 
 
+SEED_STRIDE = 0x9E3779B9   # odd: i -> seed + i * SEED_STRIDE (mod 2^32) is one-to-one
+
+
+def sample_seed(seed: int, i: int) -> int:
+    """The random-stream key of candidate i of an utterance whose seed is `seed` (generate_many(n_samples=N)): seed + i *
+    0x9E3779B9 modulo 2^32, and `seed` itself for i = 0 (the sampler reads a key modulo 2^32), so candidate 0 draws what
+    the utterance draws alone.  The stride is odd, so the N keys of an utterance differ for any N <= 2^32."""
+    seed, i = int(seed), int(i)
+    if i < 0:
+        raise RstnetError(f"a candidate index is >= 0 (got {i})")
+    return seed if i == 0 else (seed + i * SEED_STRIDE) & 0xFFFFFFFF
+
+
+class Candidate(NamedTuple):
+    """One of the n_samples candidates of an utterance (generate_many(n_samples=N)): `index` i (its random stream is
+    sample_seed(seed, i)), codes [8, G-1], the summed log-probabilities of its sampled audio tokens (the 8 audio heads over
+    all G frames) and text tokens under the model's untempered softmax, and its frame count G."""
+    index: int
+    codes: torch.Tensor
+    logprob_audio: float
+    logprob_text: float
+    frames: int
+
+
+def rank_candidates(cands: List[Candidate], rank: Optional[str]) -> List[Candidate]:
+    """rank 'logprob': highest mean audio log-probability per frame first, ties by index; None: index order"""
+    if rank is None:
+        return sorted(cands, key=lambda c: c.index)
+    return sorted(cands, key=lambda c: (-c.logprob_audio / c.frames, c.index))
+
+
 def reverse_delay(x: torch.Tensor) -> torch.Tensor:
     """Undo the one-frame acoustic delay (infer_no_streaming.py:311-323): x [8, L] (or [L, 8]) -> [8, L-1] with
     row 0 kept and rows 1..7 shifted left by one frame."""
@@ -169,13 +200,22 @@ class InferenceImp(object):
         return prefix_len, L - prefix_len
 
 
-    def _check_many(self, capacity: int, kv_pages: Optional[int]) -> None:
+    def _check_many(self, capacity: int, kv_pages: Optional[int], n_samples: int = 1, streamed: bool = False) -> None:
         """the argument checks of generate_many / stream_many / serve.TTSEngine"""
         self._check_task()
         if not 1 <= capacity <= MAX_STREAMS:
             raise RstnetError(f"capacity must be in [1, {MAX_STREAMS}] (got {capacity})")
         if not hasattr(self.model, "reserve_kv") and kv_pages is not None:
             raise RstnetError(f"{type(self.model).__name__} has no paged KV scope (kv_pages)")
+        if isinstance(n_samples, bool) or not isinstance(n_samples, (int, np.integer)) or n_samples < 1:
+            raise RstnetError(f"n_samples must be an int >= 1 (got {n_samples!r})")
+        if n_samples > 1:
+            if streamed:
+                raise RstnetError("streamed TTS takes n_samples = 1: a chunk is handed out before the candidates are ranked")
+            if n_samples > capacity:
+                raise RstnetError(f"n_samples = {n_samples} candidates need as many rows, more than capacity = {capacity}")
+            if not hasattr(self.model, "fork_kv"):
+                raise RstnetError(f"{type(self.model).__name__} has no paged KV scope to fork a prompt into n_samples rows")
 
     @staticmethod
     def _check_sampling(sampling: Optional[Dict[object, Sampling]]) -> None:
@@ -205,7 +245,7 @@ class InferenceImp(object):
     def generate_many(self, items: Iterable[Tuple[object, torch.Tensor]], capacity: int,
                       seeds: Optional[Dict[object, int]] = None, return_frames: bool = False,
                       sampling: Optional[Dict[object, Sampling]] = None, kv_pages: Optional[int] = None,
-                      stats: Optional[dict] = None) -> Iterator[Tuple]:
+                      stats: Optional[dict] = None, n_samples: int = 1, rank: Optional[str] = "logprob") -> Iterator[Tuple]:
         """Continuous batching over (utt_id, seq [9, L]) items, each in its own TTS layout: yields (utt_id, codes [8, G-1])
         in completion order.  Up to `capacity` utterances decode together, one graph replay per frame; a finished row is
         held until the next utterance is admitted into it (its prompt fed through GPT.prefill_streams while the other
@@ -223,27 +263,55 @@ class InferenceImp(object):
         pool an utterance waits for pages while a row is free; admission stops at the first utterance that does not fit,
         so the completion order is fixed for a given pool.  An utterance needing more than the whole pool raises.
         stats: a dict that receives 'frames' (frames run), 'row_frames' (occupied rows summed over frames) and
-        'wait_frames' (frames run while an utterance waited for pages with a row free)."""
-        self._check_many(capacity, kv_pages)
+        'wait_frames' (frames run while an utterance waited for pages with a row free).
+
+        n_samples N > 1 (best-of-N): each utterance is N candidates in N rows, admitted together once N rows and their
+        pages are free.  Its prompt is prefilled into one row and forked into the others (GPT.fork_kv): the candidates
+        share the prompt's full KV pages and hold private pages only for what they write (a shared page is copied when a
+        candidate reaches it again at a ring wrap).  Candidate i samples with the utterance's settings and the random
+        stream sample_seed(seed, i), so its codes are those of the utterance alone with that seed.  The frames run with
+        logprob=True: each candidate's sampled tokens' log-probabilities are summed on the device.  Yields (utt_id,
+        [Candidate]) per utterance, ranked by `rank`: 'logprob' highest mean audio log-probability per frame first (ties
+        by index), None index order.  return_frames is not available there."""
+        self._check_many(capacity, kv_pages, n_samples)
+        if rank not in ("logprob", None):
+            raise RstnetError(f"rank is 'logprob' or None (got {rank!r})")
+        if n_samples > 1 and return_frames:
+            raise RstnetError("return_frames is not available with n_samples > 1")
         m = self.model
         stats = {} if stats is None else stats
         stats.update(frames=0, row_frames=0, wait_frames=0)
         self._check_sampling(sampling)
         pull = self._puller(items, seeds, sampling)
         with _tts_scope(m, capacity, kv_pages):
-            rows = _TTSRows(self, capacity, sampling is not None, stats)
+            rows = _TTSRows(self, capacity, sampling is not None, stats, n_samples=int(n_samples))
+            groups: Dict[object, list] = {}
+            ready = []   # utterances whose candidates all finished in the last frame: their sums are still being copied
             while True:
                 rows.admit(pull)
                 if not rows.occupied():
                     break
-                for utt, codes, raw in rows.frame():
-                    yield (utt, codes, raw) if return_frames else (utt, codes)
+                done = rows.frame()
+                # the sums of the previous frame's finished candidates were copied to the host after that frame, and this
+                # frame is already enqueued: reading them now keeps the device busy while the host waits for the copy
+                for utt, cands in ready:
+                    yield utt, _ranked(cands, rank)
+                ready = []
+                for utt, codes, raw, st in done:
+                    if n_samples == 1:
+                        yield (utt, codes, raw) if return_frames else (utt, codes)
+                        continue
+                    groups.setdefault(st["group"], []).append((st, codes))
+                    if len(groups[st["group"]]) == n_samples:
+                        ready.append((utt, groups.pop(st["group"])))
+            for utt, cands in ready:
+                yield utt, _ranked(cands, rank)
             m.check_device_errors()
 
     @torch.no_grad()
     def stream_many(self, items: Iterable[Tuple[object, torch.Tensor]], capacity: int, codec,
                     *, seeds: Optional[Dict[object, int]] = None, sampling: Optional[Dict[object, Sampling]] = None,
-                    kv_pages: Optional[int] = None) -> Iterator["TTSChunk"]:
+                    kv_pages: Optional[int] = None, n_samples: int = 1) -> Iterator["TTSChunk"]:
         """generate_many's corpus, options and admissions, with the audio streamed: every frame also undoes the TTS delay
         on the device and decodes one codec frame for each row that has one (see `_TTSRows`), and the PCM is yielded as
         TTSChunk(utt_id, index, pcm [1920] float32 on the host, codes) while the utterances are still generating.  An
@@ -252,8 +320,8 @@ class InferenceImp(object):
         chunk of no samples.  The host hands out frame n's chunks while the device runs frame n + 1, so chunks of
         different utterances interleave in frame order.  codec: a MimiCodec on the model's device; it runs its own
         streaming scope of `capacity` rows for the duration, with clip_window rings, so that the chunks are the utterance's
-        whole-clip decode at any length."""
-        self._check_many(capacity, kv_pages)
+        whole-clip decode at any length.  n_samples > 1 raises: a chunk cannot wait for the candidates' ranking."""
+        self._check_many(capacity, kv_pages, n_samples, streamed=True)
         self._check_sampling(sampling)
         pull = self._puller(items, seeds, sampling)
         with _tts_scope(self.model, capacity, kv_pages), codec.streaming(capacity, clip_window=True):
@@ -304,9 +372,11 @@ class _TTSRows:
     frame's copy before it hands that frame's chunks out.  No eager torch arithmetic runs on this path, except the clamp of
     the codes to the codebook (ids 2048 / 2049 are LM samples, which the codec's gather clamps alike but flags as errors)."""
 
-    def __init__(self, imp: InferenceImp, B: int, per_row: bool, stats: dict, codec=None):
+    def __init__(self, imp: InferenceImp, B: int, per_row: bool, stats: dict, codec=None, n_samples: int = 1):
         m = imp.model
         self.imp, self.m, self.B, self.stats = imp, m, B, stats
+        self.n_samples = n_samples      # > 1: each request is that many candidates, forked from one prefill
+        self.groups = 0                 # requests admitted (a candidate's group id)
         stats.update(frames=0, row_frames=0, wait_frames=0)
         self.default = None             # the instance's Sampling while rows sample with per-row settings
         if per_row:
@@ -344,13 +414,24 @@ class _TTSRows:
     def occupied(self) -> List[int]:
         return [r for r in range(self.B) if self.rows[r] is not None]
 
+    def pages_needed(self, P: int, G: int) -> int:
+        """KV pages of one request: its P + G positions, and with n_samples > 1 the N - 1 forked candidates' own pages
+        (the prompt's full pages are shared)"""
+        n = self.pages.pages_for(P + G)
+        if self.n_samples > 1:
+            n += self.pages.share_plan(P, P + G, self.n_samples - 1)[3]
+        return n
+
     def fits(self, utt, P: int, G: int) -> None:
         """raise if the utterance needs more KV pages than the whole pool"""
-        if self.paged and self.pages.pages_for(P + G) > self.pages.n_pages:
-            raise RstnetError(f"utterance {utt!r} needs {self.pages.pages_for(P + G)} KV pages ({P + G} positions), "
+        if self.paged and self.pages_needed(P, G) > self.pages.n_pages:
+            raise RstnetError(f"utterance {utt!r} needs {self.pages_needed(P, G)} KV pages ({P + G} positions"
+                              f"{f' x {self.n_samples} candidates' if self.n_samples > 1 else ''}), "
                               f"more than the whole pool of {self.pages.n_pages}")
 
     def admit(self, pull) -> None:
+        if self.n_samples > 1:
+            return self._admit_groups(pull)
         m, dev, pages = self.m, self.dev, self.pages
         admitted = {}
         for r in range(self.B):
@@ -392,6 +473,56 @@ class _TTSRows:
             for r, f in admitted.items():
                 self.cur[r, :, 0] = f[:, -1]
 
+    def _admit_groups(self, pull) -> None:
+        """admit with n_samples = N > 1: a request takes the N lowest free rows once they and its pages are free; its
+        prompt is prefilled into the first and forked into the others"""
+        m, dev, pages, N = self.m, self.dev, self.pages, self.n_samples
+        st = m._state
+        groups = []
+        forked = 0   # pages the forks of this call's groups will take (they run after the prefill)
+        while True:
+            free = [r for r in range(self.B) if self.rows[r] is None and all(r not in g[0] for g in groups)]
+            if len(free) < N:
+                break
+            if self.pending is None:
+                req = pull()
+                if req is None:
+                    break
+                self.fits(req[0], req[2], req[3])
+                self.pending = req
+            utt, seq, P, G, sp, seed = self.pending
+            if self.pages_needed(P, G) > pages.free - forked:
+                self.stats["wait_frames"] += 1
+                break
+            forked += self.pages_needed(P, G) - pages.pages_for(P + G)
+            rows = free[:N]
+            pages.reserve([rows[0]], P + G)
+            self.dirty.add(rows[0])
+            self.pending = None
+            groups.append((rows, utt, seq, P, G, sp, seed))
+        if self.dirty:
+            st.upload_pages(sorted(self.dirty))
+            self.dirty.clear()
+        self.admitted = bool(groups)
+        if not groups:
+            return
+        all_rows = sorted(r for g in groups for r in g[0])
+        m.reset_streaming(streams=all_rows)
+        if st.lp_acc is None:
+            st.logprob_reset()
+        st.logprob_reset(all_rows)
+        feeds = {}
+        for rows, utt, seq, P, G, sp, seed in groups:
+            feeds[rows[0]] = torch.cat([self.init, seq[:, :P].to(device=dev, dtype=torch.int64)], dim=1)
+        m.prefill_streams({r: f[:, :-1] for r, f in feeds.items()})
+        for rows, utt, seq, P, G, sp, seed in groups:
+            m.fork_kv(rows[0], rows[1:], P + G)
+            gid, self.groups = self.groups, self.groups + 1
+            for i, r in enumerate(rows):
+                self.rows[r] = dict(utt=utt, P=P, G=G, g=0, start=self.n, sp=sp, cand=i, group=gid)
+                self.keys[r] = sample_seed(seed, i)
+                self.cur[r, :, 0] = feeds[rows[0]][:, -1]
+
     def frame(self, records: Optional[list] = None) -> List[Tuple]:
         """One generated frame of every row (there must be an occupied row).  records: a list that receives the
         frame's chunk records (row, utt, index, codes or None) when the codec runs."""
@@ -412,7 +543,8 @@ class _TTSRows:
         toks = m.forward_step(self.cur, use_sampling=imp.use_sampling, temp_text=imp.temp_text, top_k_text=imp.top_k_text,
                               temp=imp.temp, top_k=imp.top_k, audio_valid=table,
                               sample_key=self.keys if self.admitted else None, depth_ring_quirk=False,
-                              top_p_text=imp.top_p_text, top_p=imp.top_p, sampling=per_row)
+                              top_p_text=imp.top_p_text, top_p=imp.top_p, sampling=per_row,
+                              **({"logprob": True} if self.n_samples > 1 else {}))
         if self.codec is not None:
             self._decode(toks)
         self.history[self.n] = toks
@@ -421,6 +553,16 @@ class _TTSRows:
         self.stats["row_frames"] += len(occupied)
         self.cur = toks[:, :, None].clone()
         done = []
+        lp = None
+        if self.n_samples > 1:
+            last = [r for r in occupied if rows[r]["g"] + 1 == rows[r]["G"]]
+            if last:
+                # the log-probability sums of the candidates this frame finishes: one copy to pinned host memory, not
+                # waited for here (generate_many reads it after the next frame is enqueued)
+                host = _to_host(m._state.logprob_sums()[last])
+                ev = torch.cuda.Event()
+                ev.record()
+                lp = {r: (host, i, ev) for i, r in enumerate(last)}
         for r in occupied:
             st = rows[r]
             st["g"] += 1
@@ -428,13 +570,15 @@ class _TTSRows:
             codes = raw = None
             if last:
                 raw = torch.stack([self.history[f][r] for f in range(st["start"], self.n)])     # [G, 9]
+                if lp is not None:
+                    st["lp"] = lp[r]
                 rows[r] = None
                 m.reset_streaming(streams=[r])   # a held row keeps its position: park it at 0 ...
                 if self.paged:
                     self.pages.release([r])      # ... without pages (uploaded before the next launch)
                     self.dirty.add(r)
                 codes = reverse_delay(raw[:, 1:])
-                done.append((st["utt"], codes, raw))
+                done.append((st["utt"], codes, raw, st))
             if records is not None and (st["g"] >= 2 or last):
                 # step g - 1 >= 1 completes codec frame g - 2; an utterance of one frame has no audio
                 records.append((r, st["utt"], max(st["g"] - 2, 0), codes, st["g"] >= 2))
@@ -476,6 +620,17 @@ class _TTSRows:
         empty = torch.zeros(0, dtype=torch.float32)
         return [TTSChunk(utt, i, torch.from_numpy(pcm[r].copy()) if has_pcm else empty, codes)
                 for r, utt, i, codes, has_pcm in records]
+
+
+def _ranked(cands, rank: Optional[str]) -> List[Candidate]:
+    """[(finished row state, codes)] of one utterance -> its Candidates ranked; waits for the copy of their sums"""
+    out = []
+    for st, codes in cands:
+        host, i, ev = st["lp"]
+        ev.synchronize()
+        lp = host[i]
+        out.append(Candidate(st["cand"], codes, float(lp[1:].sum()), float(lp[0]), st["G"]))
+    return rank_candidates(out, rank)
 
 
 def _to_host(t: torch.Tensor) -> torch.Tensor:

@@ -77,7 +77,13 @@ class KVPages:
     contiguous scope's (position p in slot p % cap); page i of stream s (slots i*page .. (i+1)*page - 1) lives in pool
     page table[s, i], -1 when unmapped.  A stream holds table[s, :held[s]], and may advance to position limit[s]
     (unbounded once it holds the whole ring).  Pages are handed out lowest free index first, so a given sequence of
-    reservations always produces the same table."""
+    reservations always produces the same table.
+
+    Sharing (`share`): several streams may map the same pool page.  refs[p] counts the mappings of page p (table entries;
+    a page set aside as a spare counts one), and a page returns to the free heap when its last reference goes.  A page
+    with more than one reference is read-only: before a launch writes into it, the writing stream gets a private copy
+    (`cow`), taken from the spares `share` set aside for that page, or else from the free heap.  Without a `share`, every
+    page has at most one reference, and tables and free lists are exactly those of reservations alone."""
 
     def __init__(self, n_pages: int, streams: int, page: int, cap: int):
         log2 = int(page).bit_length() - 1
@@ -92,10 +98,23 @@ class KVPages:
         self.held = np.zeros(streams, dtype=np.int64)
         self.limit = np.zeros(streams, dtype=np.int64)
         self._free = list(range(self.n_pages))   # a heap
+        self.refs = np.zeros(self.n_pages, dtype=np.int64)
+        self.spares: Dict[int, List[int]] = {}    # shared page -> private pages set aside for its copies
+        self.n_shared = 0                         # pages with more than one reference: writes must check for them
+
+    @property
+    def sharing(self) -> bool:
+        """some page has more than one reference (only then can a write need a copy)"""
+        return self.n_shared > 0
 
     @property
     def free(self) -> int:
         return len(self._free)
+
+    @property
+    def in_use(self) -> int:
+        """pages some stream holds (a shared page counts once) or that are set aside as spares"""
+        return self.n_pages - len(self._free)
 
     def pages_for(self, positions: int) -> int:
         """pages a stream needs to write positions 0 .. positions - 1"""
@@ -109,38 +128,68 @@ class KVPages:
             raise RstnetError("a stream is listed twice")
         return s
 
+    def _take(self) -> int:
+        p = heapq.heappop(self._free)
+        self.refs[p] = 1
+        return p
+
+    def _drop(self, p: int) -> None:
+        """one reference of page p goes; the spares of p that no remaining mapping can need go with it"""
+        p = int(p)
+        self.refs[p] -= 1
+        if self.refs[p] == 1:
+            self.n_shared -= 1
+        elif self.refs[p] == 0:
+            heapq.heappush(self._free, p)
+        sp = self.spares.get(p)
+        while sp and len(sp) > self.refs[p] - 1:
+            self._drop(sp.pop())
+        if sp is not None and not sp:
+            del self.spares[p]
+
+    def _short(self, grow: int, free: int) -> None:
+        if grow > free:
+            raise RstnetError(f"the KV pool is short: {grow} more pages wanted, {free} free "
+                              f"(pool of {self.n_pages} pages of {self.page} positions)")
+
+    def _limit(self, p: int) -> int:
+        return p if p < self.cap else np.iinfo(np.int64).max
+
     def reserve(self, streams, positions):
         """Give each stream pages for min(positions, cap) positions (one count for all, or one per stream), replacing its
-        reservation: it keeps the pages of the positions it still holds, frees the rest, and takes new pages lowest
-        first.  All or nothing: when the pool is short, raise and change nothing.  -> the streams whose table rows changed."""
+        reservation: it keeps the pages of the positions it still holds, drops its references to the rest (a page is
+        freed with its last reference), and takes new pages lowest first.  All or nothing: when the pool is short, raise
+        and change nothing.  -> the streams whose table rows changed."""
         s = self._streams(streams)
         pos = np.broadcast_to(np.asarray(positions, dtype=np.int64), (len(s),))
         if (pos < 0).any():
             raise RstnetError("a reservation needs positions >= 0")
         need = [self.pages_for(p) for p in pos]
         grow = sum(max(0, n - int(self.held[x])) for x, n in zip(s, need))
-        shrink = sum(max(0, int(self.held[x]) - n) for x, n in zip(s, need))
-        if grow > len(self._free) + shrink:
-            raise RstnetError(f"the KV pool is short: {grow} more pages wanted, {len(self._free) + shrink} free "
-                              f"(pool of {self.n_pages} pages of {self.page} positions)")
+        drops: Dict[int, int] = {}
         for x, n in zip(s, need):
             for page in self.table[x, n:self.held[x]]:
-                heapq.heappush(self._free, int(page))
+                drops[int(page)] = drops.get(int(page), 0) + 1
+        shrink = sum(1 for page, d in drops.items() if d >= self.refs[page])   # pages whose last reference goes
+        self._short(grow, len(self._free) + shrink)
+        for x, n in zip(s, need):
+            for page in self.table[x, n:self.held[x]]:
+                self._drop(page)
             self.table[x, n:] = -1
         for x, n, p in zip(s, need, pos):
             for i in range(int(self.held[x]), n):
-                self.table[x, i] = heapq.heappop(self._free)
+                self.table[x, i] = self._take()
             self.held[x] = n
-            self.limit[x] = p if p < self.cap else np.iinfo(np.int64).max
+            self.limit[x] = self._limit(p)
         return s
 
     def release(self, streams):
-        """Free the streams' pages.  -> the streams whose table rows changed."""
+        """Drop the streams' pages.  -> the streams whose table rows changed."""
         return self.reserve(streams, 0)
 
     def detach(self, stream: int) -> List[int]:
-        """Unmap the stream's pages WITHOUT returning them to the pool (their contents are still being read); -> the
-        pages, which `give_back` returns later."""
+        """Unmap the stream's pages WITHOUT dropping their references (their contents are still being read); -> the
+        pages, whose references `give_back` drops later."""
         s = self._streams([stream])[0]
         pages = [int(p) for p in self.table[s, :self.held[s]]]
         self.table[s] = -1
@@ -149,7 +198,7 @@ class KVPages:
 
     def give_back(self, pages) -> None:
         for p in pages:
-            heapq.heappush(self._free, int(p))
+            self._drop(p)
 
     def check(self, streams, pos, n) -> None:
         """Raise unless every stream s of `streams` (at position pos[i]) may write n more positions."""
@@ -157,6 +206,114 @@ class KVPages:
             if int(p) + n > self.limit[s]:
                 raise RstnetError(f"stream {int(s)} would write position {int(p) + n - 1} but holds KV pages for "
                                   f"{int(self.limit[s])} positions: reserve_kv first")
+
+    def written_pages(self, start: int, end: int) -> List[int]:
+        """the table indices of the pages a stream writes over positions start .. end - 1 (ring slots p % cap)"""
+        if end - start >= self.cap:
+            return list(range(self.stride))
+        out, p = set(), int(start)
+        while p < end:
+            slot = p % self.cap
+            out.add(slot >> self.log2_page)
+            p += min(self.page - (slot & (self.page - 1)), self.cap - slot)
+        return sorted(out)
+
+    def share_plan(self, written: int, positions: int, n_dsts: int):
+        """What share() of a stream that has written `written` positions into n_dsts streams reserving `positions` each
+        takes: -> (shared table indices, the index copied at once or None, {shared index: spares}, pages taken from the
+        free heap).  Every holder, the src included, is counted as writing positions written .. positions - 1."""
+        nsh = self.pages_for(written)
+        now = (int(written) % self.cap) >> self.log2_page
+        now = now if now < nsh else None
+        # a page all 1 + n_dsts holders write is copied by every writer but the last: n_dsts spares
+        spares = {i: n_dsts for i in self.written_pages(written, positions) if i < nsh and i != now}
+        take = n_dsts * (self.pages_for(positions) - nsh + (now is not None)) + sum(spares.values())
+        return nsh, now, spares, take
+
+    def share(self, src: int, dsts, positions, written: int):
+        """Map stream src's pages of its `written` positions into every stream of `dsts` (which hold no pages), one
+        reference per mapping; each dst gets a private copy of the page it writes first (src's partial page) and new
+        pages of its own up to min(positions, cap) positions (reserve's `limit`).  Pages a dst or src will reach again at
+        a ring wrap before position `positions` stay shared until then: `cow` gives the writer its copy, from spares set
+        aside here (share_plan: the same count whatever src's own reservation; a copy past `positions` comes from the free
+        heap, or raises before the launch if the pool is short).  All or nothing: when the pool is short, raise and change
+        nothing.  -> ([(src page, dst page)] to copy now, the streams
+        whose table rows changed)."""
+        s = self._streams([src] + list(np.asarray(dsts, dtype=np.int64).reshape(-1)))
+        src, dsts = s[0], s[1:]
+        written, positions = int(written), int(positions)
+        if any(self.held[d] for d in dsts):
+            raise RstnetError("a stream forked into must hold no KV pages")
+        if not 0 <= written <= positions:
+            raise RstnetError(f"a fork needs 0 <= written ({written}) <= positions ({positions})")
+        nsh, now, spares, take = self.share_plan(written, positions, len(dsts))
+        if int(self.held[src]) < nsh:
+            raise RstnetError(f"stream {src} holds {int(self.held[src])} KV pages, fewer than its {written} positions need")
+        self._short(take, len(self._free))
+        pairs = []
+        need = self.pages_for(positions)
+        for d in dsts:
+            for i in range(nsh):
+                pg = int(self.table[src, i])
+                if i == now:
+                    new = self._take()
+                    pairs.append((pg, new))
+                    self.table[d, i] = new
+                else:
+                    self.refs[pg] += 1
+                    self.n_shared += int(self.refs[pg] == 2)
+                    self.table[d, i] = pg
+            for i in range(nsh, need):
+                self.table[d, i] = self._take()
+            self.held[d] = need
+            self.limit[d] = self._limit(positions)
+        for i, k in spares.items():
+            self.spares.setdefault(int(self.table[src, i]), []).extend(self._take() for _ in range(k))
+        return pairs, dsts
+
+    def cow(self, streams, pos, n):
+        """Copy-on-write before a launch: every listed stream (at position pos[i], writing n[i] positions -- one count for
+        all, or one per stream) that would write into a page it shares gets a private copy mapped in its place (a spare of
+        that page, else the lowest free page).  All or nothing.  -> ([(shared page, private page)] to copy, the streams
+        whose table rows changed)."""
+        if not self.sharing:
+            return [], []
+        s = [int(x) for x in np.asarray(streams, dtype=np.int64).reshape(-1)]
+        pos = np.broadcast_to(np.asarray(pos, dtype=np.int64), (len(s),))
+        cnt = np.broadcast_to(np.asarray(n, dtype=np.int64), (len(s),))
+        todo = []
+        for x, p, k in zip(s, pos, cnt):
+            if k > 0 and self.held[x]:
+                todo += [(x, i) for i in self.written_pages(int(p), int(p) + int(k))
+                         if i < self.held[x] and self.refs[self.table[x, i]] > 1]
+        if not todo:
+            return [], []
+        # the last holders of a page need no copy; count what the spares do not cover
+        refs, left, heap = {}, {}, 0
+        for x, i in todo:
+            pg = int(self.table[x, i])
+            r = refs.setdefault(pg, int(self.refs[pg]))
+            if r > 1:
+                refs[pg] = r - 1
+                sp = left.setdefault(pg, len(self.spares.get(pg, ())))
+                if sp:
+                    left[pg] = sp - 1
+                else:
+                    heap += 1
+        self._short(heap, len(self._free))
+        pairs, rows = [], []
+        for x, i in todo:
+            pg = int(self.table[x, i])
+            if self.refs[pg] <= 1:
+                continue
+            sp = self.spares.get(pg)
+            new = sp.pop() if sp else self._take()
+            self._drop(pg)
+            self.table[x, i] = new
+            pairs.append((pg, new))
+            if x not in rows:
+                rows.append(x)
+        return pairs, rows
 
 
 @dataclass(frozen=True)
@@ -494,6 +651,15 @@ class _DecodeModel(nn.Module):
         st.upload_pages(st.pages.reserve(streams, positions))
 
     @on_own_device
+    def fork_kv(self, src_stream: int, dst_streams, positions: int) -> None:
+        """Paged scope: start every stream of dst_streams (which hold no pages) where src_stream is -- its position counter
+        and the KV of its positions -- without copying the KV: the dsts map src's pages (KVPages.share), each with a
+        private copy of the page it writes first and pages of its own up to min(positions, context) positions; a page
+        still shared when a stream reaches it again at a ring wrap is copied before that write.  One page-copy launch and
+        one upload of the dsts' table rows.  If the pool is short this raises RstnetError and changes nothing."""
+        self._paged().fork(src_stream, dst_streams, positions)
+
+    @on_own_device
     def release_kv(self, streams) -> None:
         """Paged scope: return the listed streams' KV pages to the pool (a stream without pages may still be held)."""
         st = self._paged()
@@ -714,7 +880,8 @@ class GPT(_DecodeModel):
     @on_own_device
     def forward_step(self, sequence: torch.Tensor, *, use_sampling: bool = True, temp_text: float = 0.7, top_k_text: int = 25,
                      temp: float = 0.8, top_k: int = 30, audio_valid=2049, depth_ring_quirk: bool = True, sample_key=None,
-                     sample_step=None, top_p_text: float = 0.0, top_p: float = 0.0, sampling=None) -> torch.Tensor:
+                     sample_step=None, top_p_text: float = 0.0, top_p: float = 0.0, sampling=None,
+                     logprob: bool = False) -> torch.Tensor:
         """One generated frame: temporal step on sequence[B,9,1], text token, then the 8 depth steps, each sampled
         on the device (sample_token / sample_token_audio[_2048], utils/sampling.py:85-154: use_sampling False ->
         argmax over the whole card; True -> temperature + top-k (top_k == 0: plain multinomial) over ids <
@@ -733,13 +900,18 @@ class GPT(_DecodeModel):
 
         Per-row settings: sampling, a list of B `Sampling` (with a per-row audio_valid table), replaces the scalar settings
         (use_sampling .. top_k, top_p_text, top_p) by each row's own.  They live in device tables of the scope, written
-        only when they change, so changing a row's settings replays the same graph."""
+        only when they change, so changing a row's settings replays the same graph.
+
+        logprob: also add, for every active row, the log-probability of each sampled token under the head's untempered
+        softmax over all its ids (whatever the temperature, top-k / top-p and candidate counts) into the scope's per-row
+        sums (`logprob_sums`, zeroed by `logprob_reset`), one cross-entropy launch per head inside the frame: a graph of its
+        own, next to the one without."""
         if self._state is None:
             raise RstnetError("forward_step is a streaming call: use it inside `with gpt.streaming(B):`")
         if sampling is None and (top_p_text or top_p):
             Sampling(use_sampling, temp_text, top_k_text, top_p_text, temp, top_k, top_p)   # validates a nucleus frame's settings
         return self._state.forward_step(sequence, use_sampling, temp_text, top_k_text, temp, top_k, audio_valid, depth_ring_quirk,
-                                        sample_key, sample_step, top_p_text, top_p, sampling)
+                                        sample_key, sample_step, top_p_text, top_p, sampling, logprob)
 
     @torch.no_grad()
     @on_own_device
@@ -1030,6 +1202,8 @@ class _LMState:
         self.row_mapped = rows is not None
         self.pages: Optional[KVPages] = None        # paged scope: the host allocator
         self.page_table: Optional[torch.Tensor] = None   # ... and its device table int32 [B, pages.stride]
+        self._copy_pending = None   # (pinned pairs, event) of the last page copy: kept until the copy has read them
+        self.lp_acc = None          # forward_step(logprob=True): per-row sums of the sampled tokens' log-probabilities
         if self.row_mapped:
             self.row_stream, self.row_tl = z(M, dtype=torch.int32), z(M, dtype=torch.int32)
             self.delta = z(B, dtype=torch.int64)
@@ -1301,6 +1475,8 @@ class _LMState:
             # paged scope: an active stream writes only where it holds pages (held streams advance nothing)
             act = np.flatnonzero(self.active_host)
             self.pages.check(act, self.pos_host[act], n)
+            # every stream, held ones too, writes its next n slots: none of them may be a shared page
+            self._cow(np.arange(self.B), self.pos_host, n)
         self.pos_host += n * self.active_host
 
     def row_segments(self, b: int, positions: int):
@@ -1334,6 +1510,43 @@ class _LMState:
             regions += [("row_step", tensor_segs(self.row_step[b:b + 1])), ("row_key", tensor_segs(self.row_key[b:b + 1]))]
         return regions
 
+    def _cow(self, streams, pos, n) -> None:
+        """copy-on-write (KVPages.cow) of the pages the streams are about to write, before the launch that writes them"""
+        if self.pages is not None and self.pages.sharing:
+            pairs, rows = self.pages.cow(streams, pos, n)
+            self.copy_pages(pairs)
+            self.upload_pages(rows)
+
+    def copy_pages(self, pairs) -> None:
+        """One rstnet_kv_pages_copy launch: pool page src -> dst in every layer for each (src, dst) pair.  The pairs go
+        from pinned memory, kept alive until the copy has read them."""
+        if not pairs:
+            return
+        if self._copy_pending is not None:
+            self._copy_pending[1].synchronize()
+        t = torch.tensor(pairs, dtype=torch.int32).pin_memory()
+        pools = (C.c_void_p * len(self.kv))(*[k.data_ptr() for k in self.kv])
+        page_bytes = self.kv[0][0].numel() * self.kv[0].element_size()
+        ctas = torch.cuda.get_device_properties(self.kv[0].device).multi_processor_count
+        _lib.check(_lib.lib().rstnet_kv_pages_copy(pools, len(self.kv), t.data_ptr(), len(pairs), page_bytes, ctas,
+                                                   ops._stream()), "kv_pages_copy")
+        ev = torch.cuda.Event()
+        ev.record()
+        self._copy_pending = (t, ev)
+
+    def fork(self, src: int, dsts, positions: int) -> None:
+        """fork_kv: src's position counter -> the dsts (device and host), KVPages.share, the copies it asks for, one
+        upload of the changed table rows"""
+        src = int(src)
+        if not 0 <= src < self.B:
+            raise RstnetError(f"stream index {src} outside [0, {self.B})")
+        pairs, rows = self.pages.share(src, dsts, positions, int(self.pos_host[src]))
+        if rows:
+            self.offset[torch.tensor(rows, dtype=torch.int64, device=self.offset.device)] = self.offset[src].clone()
+            self.pos_host[rows] = self.pos_host[src]
+        self.copy_pages(pairs)
+        self.upload_pages(rows)
+
     def upload_pages(self, streams) -> None:
         """Copy the listed streams' rows of the host page table to the device table (stream-ordered: frames already
         enqueued read the old rows, later ones the new; outside any graph, so a captured frame keeps serving).  The rows
@@ -1354,6 +1567,8 @@ class _LMState:
             mk = torch.as_tensor(mask).to(dtype=torch.int64).reshape(self.B).cpu()
             self.active_host[:] = mk.numpy()
             self.active.copy_(mk.to(self.active.device))
+        if self.lp_acc is not None:
+            self._logprob_slots()
 
     # ---- API ----------------------------------------------------------------------------------
     def forward_global(self, sequence: torch.Tensor, want_outputs: bool = True):
@@ -1419,6 +1634,8 @@ class _LMState:
                 self.pages.check([s], [self.pos_host[s]], p.shape[1])
             if p.shape[1] > 0:
                 todo.append([s, p.to(device=dev, dtype=torch.int64).t(), 0])
+        if todo:
+            self._cow([it[0] for it in todo], self.pos_host[[it[0] for it in todo]], [it[1].shape[0] for it in todo])
         while todo:
             self.row_chunk(todo)
             todo = [it for it in todo if it[2] < it[1].shape[0]]
@@ -1499,7 +1716,7 @@ class _LMState:
             out[:, k].copy_(self.dlogits)
 
     def forward_step(self, sequence, use_sampling, temp_text, top_k_text, temp, top_k, audio_valid, quirk=True, sample_key=None,
-                     sample_step=None, top_p_text=0.0, top_p=0.0, sampling=None):
+                     sample_step=None, top_p_text=0.0, top_p=0.0, sampling=None, logprob=False):
         c = self.c
         if sequence.shape[0] != self.B or sequence.shape[2] != 1:
             raise RstnetError(f"forward_step takes sequence [{self.B}, {c.n_q + 1}, 1], got {tuple(sequence.shape)}")
@@ -1530,15 +1747,54 @@ class _LMState:
             valid = tuple(audio_valid) if isinstance(audio_valid, (tuple, list)) else (audio_valid,) * c.dep_q
         modes = None if sampling is not None else (_head_mode(use_sampling, temp_text, top_k_text, top_p_text),
                                                    _head_mode(use_sampling, temp, top_k, top_p))
-        self._replay(*self._frame(modes, valid, per_row, quirk))
+        if logprob and self.lp_acc is None:
+            self.logprob_reset()
+        self._replay(*self._frame(modes, valid, per_row, quirk, bool(logprob)))
         return self.tokens.clone()
 
-    def _frame(self, modes, valid, per_row_rng: bool, quirk):
+    # ---- log-probabilities of the sampled tokens (forward_step(logprob=True))
+    def _logprob_slots(self) -> None:
+        """accumulator slot of each row: its own index while active, -1 (not read, adds nothing) while held"""
+        slot = np.where(self.active_host[:self.M] != 0, np.arange(self.M), -1).astype(np.int32)
+        self.lp_slot.copy_(torch.from_numpy(slot).pin_memory(), non_blocking=True)
+
+    def logprob_reset(self, rows=None) -> None:
+        """zero the log-probability sums of `rows` (None: all); the first call allocates them"""
+        c, dev, M = self.c, self.m.device, self.M
+        if self.lp_acc is None:
+            G = c.dep_q + 1
+            self.lp_acc = torch.zeros(G, M, 1, 5, dtype=torch.float64, device=dev)   # [head, row, group 0, CE_FIELDS]
+            self.lp_lab = torch.zeros(G, M, dtype=torch.int64, device=dev)
+            self.lp_w = torch.ones(M, dtype=torch.float32, device=dev)
+            self.lp_nll = torch.zeros(M, dtype=torch.float32, device=dev)
+            self.lp_pred = torch.zeros(M, dtype=torch.int32, device=dev)
+            self.lp_slot = torch.zeros(M, dtype=torch.int32, device=dev)
+            self._logprob_slots()
+        elif rows is None:
+            self.lp_acc.zero_()
+        else:
+            self.lp_acc[:, torch.as_tensor(rows, dtype=torch.int64).to(dev)] = 0
+
+    def logprob_sums(self) -> torch.Tensor:
+        """fp64 [M, 1 + dep_q] on the device: per row, the summed log-probability of its sampled tokens per head (text,
+        then the audio heads) over the frames run with logprob=True since its last logprob_reset"""
+        return -self.lp_acc[:, :, 0, 0].t()
+
+    def _logprob(self, col: int) -> None:
+        """head col's log-softmax at the token just sampled, added into each active row's slot: the cross-entropy kernel
+        over the head's logits with the sampled ids as labels (the sampler only draws ids < V, so every label is covered;
+        a NaN logit gives a NaN sum and no device error)"""
+        logits = self.logits if col == 0 else self.dlogits
+        self.lp_lab[col].copy_(self.tokens[:, col])
+        cross_entropy_sums(logits, self.lp_lab[col], self.lp_w, 1, None, self.lp_slot, self.lp_acc[col], self.lp_nll, self.lp_pred)
+
+    def _frame(self, modes, valid, per_row_rng: bool, quirk, logprob: bool = False):
         """(graph key, launch sequence) of one generated frame from the ids in self.seq to the tokens in self.tokens.
         modes: ((top_k, temp, top_p) of the text head, (...) of the audio heads) for every row, as _head_mode gives them, or
         None: each row's own from the row_topk / row_temp / row_topp tables.  valid: the dep_q audio heads' candidate
         counts for every row, or None: each row's own from row_valid.  per_row_rng: the RNG keyed by (row_step, row_key)
-        in place of (frame_counter, row); the frame advances the counter it keys by."""
+        in place of (frame_counter, row); the frame advances the counter it keys by.  logprob: after each head's sampler,
+        add the log-probability of the sampled tokens into the rows' sums (logprob_sums); a graph of its own."""
         c = self.c
         if modes is not None and modes[1][0] == 0:
             valid = (c.audio_card,) * c.dep_q   # the 2048 / 2049 masks exist on the sampling path only (sampling.py:107-154)
@@ -1547,13 +1803,18 @@ class _LMState:
         def frame():
             self._temporal()
             self._sample(0, text, c.padded_vocab_size, per_row_rng)
+            if logprob:
+                self._logprob(0)
             self.tout.copy_(self.out)
             for k in range(c.dep_q):
                 self._depth(k, self.tokens[:, k], c.dep_q + 1, quirk=quirk)
                 self._sample(k + 1, audio, None if valid is None else min(valid[k], c.audio_card), per_row_rng)
+                if logprob:
+                    self._logprob(k + 1)
             if per_row_rng:
                 ops.counter_add(self.row_step, 1, self.active)
             else:
                 ops.counter_add(self.frame_counter, 1)
 
-        return ("frame", "tables" if modes is None else modes, "rows" if valid is None else valid, per_row_rng, bool(quirk)), frame
+        key = ("frame", "tables" if modes is None else modes, "rows" if valid is None else valid, per_row_rng, bool(quirk))
+        return (key + ("logprob",) if logprob else key), frame

@@ -183,12 +183,22 @@ def reconstruct_corpus(codec: MimiCodec, src: str, dst: str, capacity: int = 128
 
 @torch.no_grad()
 def synthesize(imp, corpus: Dict[str, torch.Tensor], capacity: int = 32, seeds=None,
-               kv_gb: Optional[float] = None) -> Dict[str, torch.Tensor]:
+               kv_gb: Optional[float] = None, n_samples: int = 1, all_samples: bool = False) -> Dict[str, torch.Tensor]:
     """{utt_id: int16 [8, T]} for every utterance of `corpus` ({utt_id: int64 [9, L]}), through imp.generate_many.
-    kv_gb: the KV cache's budget in GiB (a pool of floor(kv_gb * 2^30 / kv_page_bytes) pages); None: a whole ring per row."""
+    kv_gb: the KV cache's budget in GiB (a pool of floor(kv_gb * 2^30 / kv_page_bytes) pages); None: a whole ring per row.
+    n_samples N > 1: best-of-N, the codes of each utterance's candidate with the highest mean audio log-probability per
+    frame; all_samples also returns candidate i's codes as `<utt_id>_s<i>`."""
     items = ((utt, torch.as_tensor(seq, dtype=torch.int64)) for utt, seq in corpus.items())
     kv_pages = None if kv_gb is None else kv_pages_for_budget(imp.model.config, kv_gb)
-    return {utt: codes.to(torch.int16).cpu() for utt, codes in imp.generate_many(items, capacity, seeds=seeds, kv_pages=kv_pages)}
+    if n_samples == 1:
+        return {utt: codes.to(torch.int16).cpu() for utt, codes in imp.generate_many(items, capacity, seeds=seeds, kv_pages=kv_pages)}
+    out = {}
+    for utt, cands in imp.generate_many(items, capacity, seeds=seeds, kv_pages=kv_pages, n_samples=n_samples):
+        out[utt] = cands[0].codes.to(torch.int16).cpu()
+        if all_samples:
+            for c in sorted(cands, key=lambda c: c.index):
+                out[f"{utt}_s{c.index}"] = c.codes.to(torch.int16).cpu()
+    return out
 
 
 @torch.no_grad()
@@ -254,7 +264,11 @@ def _synthesize_cli(args) -> int:
     if args.top_p or args.top_p_text:
         imp.sampling()   # validates a nucleus run's settings before the model runs
     corpus = torch.load(args.input, map_location="cpu")
+    if args.all_samples and args.n_samples == 1:
+        raise SystemExit("--all-samples needs --n-samples > 1")
     if args.stream:
+        if args.n_samples != 1:
+            raise SystemExit("--stream takes --n-samples 1: a streamed chunk cannot wait for the candidates' ranking")
         if not (args.wav_dir and args.codec_weights):
             raise SystemExit("--stream needs --wav-dir and --codec-weights")
         codec = _load_codec(argparse.Namespace(weights=args.codec_weights, config=args.codec_config, device=args.device))
@@ -262,7 +276,7 @@ def _synthesize_cli(args) -> int:
         save_tokens(codes, args.output_file)
         print(f"synthesized {len(codes)} utterances -> {args.output_file}, streamed their wavs -> {args.wav_dir}")
         return 0
-    codes = synthesize(imp, corpus, args.capacity, kv_gb=args.kv_gb)
+    codes = synthesize(imp, corpus, args.capacity, kv_gb=args.kv_gb, n_samples=args.n_samples, all_samples=args.all_samples)
     save_tokens(codes, args.output_file)
     print(f"synthesized {len(codes)} utterances -> {args.output_file}")
     if args.wav_dir:
@@ -454,6 +468,10 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--stream", action="store_true",
                    help="with --wav-dir: decode each utterance's audio frame by frame while it generates "
                         "(InferenceImp.stream_many) and write its wav as it completes; the codes file is the same")
+    p.add_argument("--n-samples", type=int, default=1,
+                   help="best-of-N: sample N candidates of each utterance from one prompt prefill (sharing its KV pages) and "
+                        "keep the one with the highest mean audio log-probability per frame")
+    p.add_argument("--all-samples", action="store_true", help="with --n-samples: also write candidate i as <utt_id>_s<i>")
     p.add_argument("--device", default="cuda")
     p = sub.add_parser("score", help="teacher-forced losses / audio perplexity of a corpus (infer_no_streaming.py teacher-force; "
                                      "--model moshi: the Moshi fine-tune trainer's validate_model)")

@@ -718,12 +718,13 @@ class TTSEngine:
     so the device always has the current frame queued.  `step()` with nothing admitted or queued returns [] and launches
     nothing.  The engine holds the model's and the codec's streaming scopes until `close()` (or the end of a `with`)."""
 
-    def __init__(self, imp, codec, capacity: int, *, kv_pages: Optional[int] = None):
+    def __init__(self, imp, codec, capacity: int, *, kv_pages: Optional[int] = None, n_samples: int = 1):
+        """n_samples > 1 raises: a streamed chunk cannot wait for the ranking of best-of-N candidates."""
         from contextlib import ExitStack
         from .infer import _TTSRows, _tts_scope
         if isinstance(capacity, bool) or not isinstance(capacity, (int, np.integer)):
             raise RstnetError(f"capacity must be an int (got {capacity!r})")
-        imp._check_many(int(capacity), kv_pages)
+        imp._check_many(int(capacity), kv_pages, n_samples, streamed=True)
         self.imp, self.codec, self.capacity = imp, codec, int(capacity)
         self._stack = ExitStack()
         try:

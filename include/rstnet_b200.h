@@ -561,6 +561,25 @@ int rstnet_segments_scatter(const rstnet_segment* table_dev, int32_t n, const vo
 int rstnet_kv_pages_copy(const void* const* pools, int32_t n_pools, const int32_t* pairs, int32_t n_pairs, int64_t page_bytes,
                          int32_t ctas, rstnet_stream_t s);
 
+/* ---- generation window of the batch generation loop, advanced after the last depth sample of a frame (graph-capturable;
+ * MLLM_v2/infer_no_streaming.py:264-292).  rec [B][RSTNET_GEN_REC] int32 (device): {pre_gen_len, minlen, maxlen, g_idx,
+ * mode}; g_idx is the frame these tokens are; mode & 3 is RSTNET_GEN_HELD / _FIXED / _WINDOWED, | RSTNET_GEN_ARGMAX for a
+ * row that takes the whole card.  tokens [B][tok_stride] int64 (text, then audio codebooks 0 .. dep_q - 1).  Per row:
+ *   held:                                               status = IDLE; nothing else is written;
+ *   windowed, g_idx > minlen and a token >= 2048 in audio codebooks 3 .. 7: status = STOPPED (the frame is dropped), the
+ *                                                       row becomes held;
+ *   otherwise g_idx + 1 >= maxlen:                      status = LAST (the frame is kept), the row becomes held;
+ *   otherwise:                                          status = RUNNING, g_idx += 1, and row_valid[b][0 .. dep_q) gets
+ *     the next frame's candidate counts: `card` for an argmax row, else 2049 for l > 0 when pre_gen_len + g_idx > minlen,
+ *     2048 otherwise.
+ * status [B] int32 (device).  Checked before any launch, each an error return: a null pointer, B < 1, dep_q < 1,
+ * card < 2049, tok_stride < dep_q + 1, valid_stride < dep_q. */
+#define RSTNET_GEN_REC 5
+enum { RSTNET_GEN_HELD = 0, RSTNET_GEN_FIXED = 1, RSTNET_GEN_WINDOWED = 2, RSTNET_GEN_ARGMAX = 4 };
+enum { RSTNET_GEN_RUNNING = 0, RSTNET_GEN_LAST = 1, RSTNET_GEN_STOPPED = 2, RSTNET_GEN_IDLE = 3 };
+int rstnet_lm_gen_rows_advance(const int64_t* tokens, int32_t tok_stride, int32_t* rec, int32_t* row_valid, int32_t valid_stride,
+                               int32_t* status, int32_t B, int32_t dep_q, int32_t card, rstnet_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

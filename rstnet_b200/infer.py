@@ -9,7 +9,9 @@ CUDA-graph replay).  The arithmetic per frame is the reference's: upstream evalu
 NON-streaming ``forward_local`` (every depth step sees all earlier keys), so ``forward_step`` runs with
 ``depth_ring_quirk=False`` here; the temporal transformer's non-streaming form equals the streamed one while the
 sequence is shorter than ``config.context`` (tests/test_lm_gpu.py checks the loop against the reference's own tokens).
-Only the 'TTS' task is runnable upstream (the other branches reference undefined variables); same here.
+All four tasks of the reference loop run (``TASKS``; upstream only TTS returns, the other branches raise after their
+loop at an unbound ``gt_audio``): each has its own layout (``InferenceImp._layout``) and a window (minlen, maxlen) with
+the reference's early stop, which the device decides per row inside the frame graph (rstnet_lm_gen_rows_advance).
 
 ``InferenceImp.generate_many`` runs a corpus of utterances, each with its own prompt and generation length, as one
 continuously batched scope: a row that finishes is refilled with the next utterance (ragged prefill of that row alone,
@@ -30,8 +32,13 @@ from typing import Dict, Iterable, Iterator, List, NamedTuple, Optional, Tuple
 import numpy as np
 import torch
 
+from . import _lib
 from ._lib import RstnetError
 from .lm import GPT, KV_PAGE, MAX_STREAMS, Sampling, score_item, score_packed
+
+TASKS = ("TTS", "audio_only", "text_only", "ASR")   # infer_no_streaming.py:184-226
+AUDIO_TASKS = ("TTS", "audio_only")                 # the tasks whose generated frames are audio to stream
+SEMANTIC_PAD = 2049                                 # the semantic pad id: audio_only / TTS strip trailing frames by it
 
 
 def candidate_counts(pre_gen_len: int, minlen: int, g_idx: int, dep_q: int = 8) -> List[int]:
@@ -56,8 +63,9 @@ def sample_seed(seed: int, i: int) -> int:
 
 class Candidate(NamedTuple):
     """One of the n_samples candidates of an utterance (generate_many(n_samples=N)): `index` i (its random stream is
-    sample_seed(seed, i)), codes [8, G-1], the summed log-probabilities of its sampled audio tokens (the 8 audio heads over
-    all G frames) and text tokens under the model's untempered softmax, and its frame count G."""
+    sample_seed(seed, i)), codes [8, G-1] (the generated frames [G, 9] for a task other than TTS), the summed
+    log-probabilities of its sampled audio tokens (the 8 audio heads over all G frames) and text tokens under the model's
+    untempered softmax, and its frame count G (the frames it kept, when its window stopped it)."""
     index: int
     codes: torch.Tensor
     logprob_audio: float
@@ -66,10 +74,30 @@ class Candidate(NamedTuple):
 
 
 def rank_candidates(cands: List[Candidate], rank: Optional[str]) -> List[Candidate]:
-    """rank 'logprob': highest mean audio log-probability per frame first, ties by index; None: index order"""
+    """rank 'logprob': highest mean audio log-probability per frame first, ties by index (a candidate that stopped before
+    its first frame last); None: index order"""
     if rank is None:
         return sorted(cands, key=lambda c: c.index)
-    return sorted(cands, key=lambda c: (-c.logprob_audio / c.frames, c.index))
+    return sorted(cands, key=lambda c: (-c.logprob_audio / c.frames if c.frames else float("inf"), c.index))
+
+
+def continuation_codes(seq: torch.Tensor, frames: torch.Tensor) -> torch.Tensor:
+    """The clip of an audio_only item: its prompt audio (the first L // 2 frames of seq [9, L] after the pad frames are
+    stripped, as _layout does) followed by its generated frames [G', 9], with the one-frame acoustic delay undone over the
+    whole -> codes [8, P + G' - 1].  The prompt's last frame takes codebooks 1..7 from the first generated frame, so the
+    clip decodes without a seam at the join (the reference concatenates the two, :301-302)."""
+    pad_len = int(seq[1].eq(SEMANTIC_PAD).int().sum().item())
+    P = (seq.shape[1] - pad_len) // 2
+    audio = torch.cat([seq[1:, :P].to(frames.device, torch.int64), frames[:, 1:].t().to(torch.int64)], dim=1)
+    return reverse_delay_rows(audio)
+
+
+def reverse_delay_rows(x: torch.Tensor) -> torch.Tensor:
+    """reverse_delay of codes already laid out [8, L] (no orientation guess: any L)"""
+    out = torch.empty_like(x[:, :-1])
+    out[0] = x[0, :-1]
+    out[1:] = x[1:, 1:]
+    return out
 
 
 def reverse_delay(x: torch.Tensor) -> torch.Tensor:
@@ -90,7 +118,7 @@ class InferenceImp(object):
         self.task_name = task_name
         self.text_pad_token = 128003
         self.acoustic_pad_token = 2049
-        self.semantic_pad_token = 2049
+        self.semantic_pad_token = SEMANTIC_PAD
         self.text_empty_token = 128002
         self.mode = mode
         self.use_sampling = True          # upstream hard-codes True (:162); set the attribute to False for argmax decoding
@@ -103,7 +131,8 @@ class InferenceImp(object):
 
     @torch.no_grad()
     def __call__(self, seq: torch.Tensor, mask: torch.Tensor):
-        """seq [9, L] (one utterance, as upstream) -> codes [8, T'] after reverse_delay.  In mode 'teacher-force'
+        """seq [9, L] (one utterance, as upstream) -> codes [8, T'] after reverse_delay (task 'TTS'), or the generated
+        frames [G', 9] (the other tasks).  In mode 'teacher-force'
         (infer_no_streaming.py:172-182, before any padding removal or task check) -> (loss_audio / 8, loss_text) as 0-dim
         fp64 tensors: score_many on this one utterance."""
         if self.mode == "teacher-force":
@@ -114,11 +143,20 @@ class InferenceImp(object):
     @torch.no_grad()
     def generate(self, seq: torch.Tensor, return_frames: bool = False):
         """Batched form: seq [B, 9, L], all rows in the same TTS layout (same prompt length and number of frames to
-        generate; row 0 defines them, as upstream reads `seq[0]`).  -> codes [B, 8, T'] (and the raw frames [B, G, 9])."""
+        generate; row 0 defines them, as upstream reads `seq[0]`).  -> codes [B, 8, T'] (and the raw frames [B, G, 9]).
+        The other tasks: -> a list of B generated frames [G'_b, 9] (rows may stop at different frames), run by
+        generate_many with row b's random stream keyed b, as this loop keys row b (return_frames raises: the frames
+        are the result)."""
         self._check_task()
+        if self.task_name != "TTS":
+            if return_frames:
+                raise RstnetError(f"task {self.task_name!r} returns its generated frames: return_frames is for TTS")
+            got = dict(self.generate_many(((b, seq[b]) for b in range(seq.shape[0])), seq.shape[0],
+                                          seeds={b: b for b in range(seq.shape[0])}))
+            return [got[b] for b in range(seq.shape[0])]
         m = self.model
         dev = seq.device
-        prefix_len, maxlen = self._layout(seq[0])
+        prefix_len, _, maxlen = self._layout(seq[0])
         prefix = seq[:, :, :prefix_len]
         minlen = maxlen
         B = prefix.shape[0]
@@ -146,9 +184,10 @@ class InferenceImp(object):
         codes = torch.stack([reverse_delay(raw[b, :, 1:]) for b in range(B)], 0)
         return (codes, raw) if return_frames else codes
 
-    def _check_task(self):
-        if self.task_name != "TTS":
-            raise NotImplementedError("only task 'TTS' is runnable in the reference loop (infer_no_streaming.py:184-226)")
+    def _check_task(self, task: Optional[str] = None):
+        task = self.task_name if task is None else task
+        if task not in TASKS:
+            raise NotImplementedError(f"task {task!r}: the reference loop runs {', '.join(TASKS)} (infer_no_streaming.py:184-226)")
         if self.mode == "teacher-force":
             raise NotImplementedError("teacher-force mode scores sequences (__call__ / score_many), it does not generate")
 
@@ -187,22 +226,56 @@ class InferenceImp(object):
                                                 "labels", self._score_item):
                 yield utt, self._score_metrics(sa, stx, L)
 
-    def _layout(self, seq: torch.Tensor) -> Tuple[int, int]:
-        """seq [9, L] -> (prompt length P, frames to generate G) after stripping the pad frames
-        (infer_no_streaming.py:184-226)."""
-        pad_len = int(seq[1].eq(self.semantic_pad_token).int().sum().item())
-        L = seq.shape[1] - pad_len
-        prefix_len = L - int(seq[0, :L].eq(self.text_empty_token).int().sum().item())
+    def _layout(self, seq: torch.Tensor, task: Optional[str] = None) -> Tuple[int, int, int]:
+        """seq [9, L] -> (prompt length P, minlen, maxlen) of `task` (default the instance's) after stripping the pad
+        frames (infer_no_streaming.py:184-226):
+          * text_only / ASR strip as many trailing frames as row 0 holds text pads, audio_only / TTS as many as row 1
+            holds semantic pads;
+          * text_only / audio_only: P = L // 2, minlen = maxlen = P;
+          * TTS: P = L - G with G the text-empty frames, minlen = maxlen = G;
+          * ASR: with e text-empty frames, P = e + 1 (at most L), maxlen = L - e + 13, minlen = L - e - 13.
+        At most maxlen frames are generated; from g_idx > minlen on, a frame with an id >= 2048 in audio codebooks 3..7
+        ends the utterance and is dropped, so an utterance whose maxlen - 1 <= minlen always runs maxlen frames."""
+        task = self.task_name if task is None else task
+        self._check_task(task)
+        pad_row, pad = (0, self.text_pad_token) if task in ("text_only", "ASR") else (1, self.semantic_pad_token)
+        L = seq.shape[1] - int(seq[pad_row].eq(pad).int().sum().item())
+        if task in ("text_only", "audio_only"):
+            if L < 2:
+                raise RstnetError(f"a {task} item needs 2 frames or more after its pad frames (got {L})")
+            return L // 2, L // 2, L // 2
+        empty = int(seq[0, :max(L, 0)].eq(self.text_empty_token).int().sum().item())
+        if task == "ASR":
+            if L < 1:
+                raise RstnetError("the ASR item has no frames after its pad frames")
+            return min(empty + 1, L), L - empty - 13, L - empty + 13
+        prefix_len = L - empty
         if L - prefix_len <= 0:
             raise RstnetError("nothing to generate: the sequence has no text-empty frames")
         if prefix_len <= 0:
             raise RstnetError("the sequence has no prompt frames")
-        return prefix_len, L - prefix_len
+        return prefix_len, L - prefix_len, L - prefix_len
+
+    def _request(self, utt, seq, sp, seed, task=None, lengths=None) -> tuple:
+        """an admission request (utt, seq, P, G, Sampling or None, seed, task, minlen, windowed): G = maxlen, the frames it
+        may run; windowed: its window can stop it (maxlen - 1 > minlen), so the device decides its status every frame"""
+        task = self.task_name if task is None else task
+        P, minlen, maxlen = self._layout(seq, task)
+        if lengths is not None:
+            if (not isinstance(lengths, (tuple, list)) or len(lengths) != 2
+                    or not all(isinstance(v, (int, np.integer)) and not isinstance(v, bool) for v in lengths)):
+                raise RstnetError(f"lengths[{utt!r}] is (min_frames, max_frames), two ints (got {lengths!r})")
+            minlen, maxlen = int(lengths[0]), int(lengths[1])
+            if not 1 <= maxlen < 2 ** 31 or not -2 ** 31 <= minlen < 2 ** 31:
+                raise RstnetError(f"lengths[{utt!r}]: max_frames must be in [1, 2^31) and min_frames an int32 (got {lengths!r})")
+        return utt, seq, P, maxlen, sp, seed, task, minlen, maxlen - 1 > minlen
 
 
     def _check_many(self, capacity: int, kv_pages: Optional[int], n_samples: int = 1, streamed: bool = False) -> None:
         """the argument checks of generate_many / stream_many / serve.TTSEngine"""
         self._check_task()
+        if streamed and self.task_name not in AUDIO_TASKS:
+            raise NotImplementedError(f"streamed generation runs {AUDIO_TASKS} (the instance's task is {self.task_name!r})")
         if not 1 <= capacity <= MAX_STREAMS:
             raise RstnetError(f"capacity must be in [1, {MAX_STREAMS}] (got {capacity})")
         if not hasattr(self.model, "reserve_kv") and kv_pages is not None:
@@ -218,16 +291,24 @@ class InferenceImp(object):
                 raise RstnetError(f"{type(self.model).__name__} has no paged KV scope to fork a prompt into n_samples rows")
 
     @staticmethod
+    def _check_streamed(req: tuple) -> None:
+        """streamed generation runs the audio tasks (their generated frames decode to audio)"""
+        utt, task = req[0], req[6]
+        if task not in AUDIO_TASKS:
+            raise RstnetError(f"utterance {utt!r}: task {task!r} generates text; streamed generation runs {AUDIO_TASKS}")
+
+    @staticmethod
     def _check_sampling(sampling: Optional[Dict[object, Sampling]]) -> None:
         if sampling is not None:
             for utt, sp in sampling.items():
                 if not isinstance(sp, Sampling):
                     raise RstnetError(f"sampling[{utt!r}] must be a Sampling (got {type(sp).__name__})")
 
-    def _puller(self, items, seeds, sampling):
-        """-> pull(): the next item of `items` as an admission request (utt, seq, P, G, Sampling or None, seed), or None
-        once they are exhausted; items are read one at a time, when a row can take them"""
+    def _puller(self, items, seeds, sampling, tasks=None, lengths=None, streamed=False):
+        """-> pull(): the next item of `items` as an admission request (_request), or None once they are exhausted; items
+        are read one at a time, when a row can take them.  streamed: the text tasks raise (their frames are no audio)."""
         source, seeds, done = iter(items), seeds or {}, []
+        tasks, lengths = tasks or {}, lengths or {}
 
         def pull():
             if done:
@@ -237,15 +318,20 @@ class InferenceImp(object):
             except StopIteration:
                 done.append(True)
                 return None
-            P, G = self._layout(seq)
-            return utt, seq, P, G, None if sampling is None else sampling.get(utt), int(seeds.get(utt, 0))
+            req = self._request(utt, seq, None if sampling is None else sampling.get(utt), int(seeds.get(utt, 0)),
+                                tasks.get(utt, self.task_name), lengths.get(utt))
+            if streamed:
+                self._check_streamed(req)
+            return req
         return pull
 
     @torch.no_grad()
     def generate_many(self, items: Iterable[Tuple[object, torch.Tensor]], capacity: int,
                       seeds: Optional[Dict[object, int]] = None, return_frames: bool = False,
                       sampling: Optional[Dict[object, Sampling]] = None, kv_pages: Optional[int] = None,
-                      stats: Optional[dict] = None, n_samples: int = 1, rank: Optional[str] = "logprob") -> Iterator[Tuple]:
+                      stats: Optional[dict] = None, n_samples: int = 1, rank: Optional[str] = "logprob",
+                      tasks: Optional[Dict[object, str]] = None,
+                      lengths: Optional[Dict[object, Tuple[int, int]]] = None) -> Iterator[Tuple]:
         """Continuous batching over (utt_id, seq [9, L]) items, each in its own TTS layout: yields (utt_id, codes [8, G-1])
         in completion order.  Up to `capacity` utterances decode together, one graph replay per frame; a finished row is
         held until the next utterance is admitted into it (its prompt fed through GPT.prefill_streams while the other
@@ -272,7 +358,17 @@ class InferenceImp(object):
         stream sample_seed(seed, i), so its codes are those of the utterance alone with that seed.  The frames run with
         logprob=True: each candidate's sampled tokens' log-probabilities are summed on the device.  Yields (utt_id,
         [Candidate]) per utterance, ranked by `rank`: 'logprob' highest mean audio log-probability per frame first (ties
-        by index), None index order.  return_frames is not available there."""
+        by index), None index order.  return_frames is not available there.
+
+        tasks: {utt_id: task} runs those items as another of TASKS than the instance's task_name, in that task's layout
+        (_layout); an item of a task other than TTS yields (utt_id, frames [G', 9]): its generated frames (text token,
+        audio codebooks 0..7), as the reference builds them (the text row of its `prefix`, the audio rows of its
+        `final_results`).  lengths: {utt_id: (min_frames, max_frames)} replaces an item's window (minlen, maxlen) -- on TTS
+        the open-length mode: at most max_frames frames, and from frame min_frames + 1 on the reference's stop rule (an id
+        >= 2048 in audio codebooks 3..7; that frame is dropped).  A row whose window can stop is decided on the device
+        (rstnet_lm_gen_rows_advance in the frame graph); the host reads frame n's statuses after it has enqueued frame
+        n + 1, so such a row runs one frame past its stop before it is released.  It reserves KV pages for P + max_frames
+        positions: that extra frame is at most frame max_frames - 1.  With no such row in the batch, no status is read."""
         self._check_many(capacity, kv_pages, n_samples)
         if rank not in ("logprob", None):
             raise RstnetError(f"rank is 'logprob' or None (got {rank!r})")
@@ -282,16 +378,15 @@ class InferenceImp(object):
         stats = {} if stats is None else stats
         stats.update(frames=0, row_frames=0, wait_frames=0)
         self._check_sampling(sampling)
-        pull = self._puller(items, seeds, sampling)
+        pull = self._puller(items, seeds, sampling, tasks, lengths)
         with _tts_scope(m, capacity, kv_pages):
             rows = _TTSRows(self, capacity, sampling is not None, stats, n_samples=int(n_samples))
             groups: Dict[object, list] = {}
             ready = []   # utterances whose candidates all finished in the last frame: their sums are still being copied
             while True:
                 rows.admit(pull)
-                if not rows.occupied():
-                    break
-                done = rows.frame()
+                last = not rows.occupied()
+                done = rows.settle() if last else rows.frame()
                 # the sums of the previous frame's finished candidates were copied to the host after that frame, and this
                 # frame is already enqueued: reading them now keeps the device busy while the host waits for the copy
                 for utt, cands in ready:
@@ -299,11 +394,16 @@ class InferenceImp(object):
                 ready = []
                 for utt, codes, raw, st in done:
                     if n_samples == 1:
-                        yield (utt, codes, raw) if return_frames else (utt, codes)
+                        if st["task"] != "TTS":
+                            yield utt, raw
+                        else:
+                            yield (utt, codes, raw) if return_frames else (utt, codes)
                         continue
-                    groups.setdefault(st["group"], []).append((st, codes))
+                    groups.setdefault(st["group"], []).append((st, codes if st["task"] == "TTS" else raw))
                     if len(groups[st["group"]]) == n_samples:
                         ready.append((utt, groups.pop(st["group"])))
+                if last:
+                    break
             for utt, cands in ready:
                 yield utt, _ranked(cands, rank)
             m.check_device_errors()
@@ -311,7 +411,8 @@ class InferenceImp(object):
     @torch.no_grad()
     def stream_many(self, items: Iterable[Tuple[object, torch.Tensor]], capacity: int, codec,
                     *, seeds: Optional[Dict[object, int]] = None, sampling: Optional[Dict[object, Sampling]] = None,
-                    kv_pages: Optional[int] = None, n_samples: int = 1) -> Iterator["TTSChunk"]:
+                    kv_pages: Optional[int] = None, n_samples: int = 1, tasks: Optional[Dict[object, str]] = None,
+                    lengths: Optional[Dict[object, Tuple[int, int]]] = None) -> Iterator["TTSChunk"]:
         """generate_many's corpus, options and admissions, with the audio streamed: every frame also undoes the TTS delay
         on the device and decodes one codec frame for each row that has one (see `_TTSRows`), and the PCM is yielded as
         TTSChunk(utt_id, index, pcm [1920] float32 on the host, codes) while the utterances are still generating.  An
@@ -320,10 +421,17 @@ class InferenceImp(object):
         chunk of no samples.  The host hands out frame n's chunks while the device runs frame n + 1, so chunks of
         different utterances interleave in frame order.  codec: a MimiCodec on the model's device; it runs its own
         streaming scope of `capacity` rows for the duration, with clip_window rings, so that the chunks are the utterance's
-        whole-clip decode at any length.  n_samples > 1 raises: a chunk cannot wait for the candidates' ranking."""
+        whole-clip decode at any length.  n_samples > 1 raises: a chunk cannot wait for the candidates' ranking.
+
+        tasks / lengths as generate_many, for the audio tasks (TTS, audio_only; a text task raises): an audio_only item
+        streams its continuation, codes [8, G'-1] the delay undone over its generated frames.  A row whose window can stop
+        it has each chunk handed out once its frame's status is known (one frame later than a fixed row's): the chunk of
+        the frame its stop fired on, which would decode the dropped frame, is not handed out; an empty chunk at that index
+        carries the codes instead, so its chunks are 0 .. G'-2 with audio and G'-1 empty.  Chunks of the frame it ran
+        after its stop are dropped."""
         self._check_many(capacity, kv_pages, n_samples, streamed=True)
         self._check_sampling(sampling)
-        pull = self._puller(items, seeds, sampling)
+        pull = self._puller(items, seeds, sampling, tasks, lengths, streamed=True)
         with _tts_scope(self.model, capacity, kv_pages), codec.streaming(capacity, clip_window=True):
             rows = _TTSRows(self, capacity, sampling is not None, {}, codec)
             while True:
@@ -396,6 +504,14 @@ class _TTSRows:
         self.pending = None   # the next request while it waits for pages
         self.dirty = set()    # rows whose pages changed on the host since the last upload
         self.admitted = False
+        # rows whose window can stop them (`win`) run with the device's generation records (forward_step(gen_rows=True)):
+        self.gen = False      # the last frame ran them
+        self.fresh = set()    # rows admitted since the last frame (their records are uploaded before it)
+        self.awaiting = []    # (row, state) of windowed rows that ran their last frame, until its status is read
+        self.lagged = None    # (frame, slot, event, {row: state}) of the last frame's statuses, copied, not yet read
+        self.status = None    # two pinned host slots for the statuses [B] int32, allocated on the first windowed frame
+        self.status_slot = 0
+        self.lp_frames: Dict[int, torch.Tensor] = {}   # best-of-N: windowed frame -> every row's sums after it (host)
         self.codec = codec
         if codec is not None:
             self.delay = _TTSDelay(m, B)
@@ -443,20 +559,22 @@ class _TTSRows:
                     break
                 self.fits(req[0], req[2], req[3])
                 self.pending = req
-            utt, seq, P, G, sp, seed = self.pending
+            utt, seq, P, G, sp, seed, task, minlen, win = self.pending
             if self.paged:
                 if pages.pages_for(P + G) > pages.free:
                     self.stats["wait_frames"] += 1
                     break
                 # it writes P positions in the prompt feed (init token + all prompt frames but the last) and one
-                # per generated frame: exactly P + G
+                # per generated frame: at most P + G (G = maxlen; a row that stops runs one frame past its stop, at
+                # most frame maxlen - 1)
                 pages.reserve([r], P + G)
                 self.dirty.add(r)
             self.pending = None
             feed = torch.cat([self.init, seq[:, :P].to(device=dev, dtype=torch.int64)], dim=1)
             admitted[r] = feed
-            self.rows[r] = dict(utt=utt, P=P, G=G, g=0, start=self.n, sp=sp)
+            self.rows[r] = dict(utt=utt, P=P, G=G, g=0, start=self.n, sp=sp, task=task, minlen=minlen, win=win)
             self.keys[r] = seed
+            self.fresh.add(r)
         if self.dirty:
             # one upload of the table rows this frame's releases and admissions changed, before any launch
             m._state.upload_pages(sorted(self.dirty))
@@ -490,7 +608,7 @@ class _TTSRows:
                     break
                 self.fits(req[0], req[2], req[3])
                 self.pending = req
-            utt, seq, P, G, sp, seed = self.pending
+            utt, seq, P, G, sp, seed, task, minlen, win = self.pending
             if self.pages_needed(P, G) > pages.free - forked:
                 self.stats["wait_frames"] += 1
                 break
@@ -499,7 +617,7 @@ class _TTSRows:
             pages.reserve([rows[0]], P + G)
             self.dirty.add(rows[0])
             self.pending = None
-            groups.append((rows, utt, seq, P, G, sp, seed))
+            groups.append((rows, utt, seq, P, G, sp, seed, (task, minlen, win)))
         if self.dirty:
             st.upload_pages(sorted(self.dirty))
             self.dirty.clear()
@@ -512,39 +630,84 @@ class _TTSRows:
             st.logprob_reset()
         st.logprob_reset(all_rows)
         feeds = {}
-        for rows, utt, seq, P, G, sp, seed in groups:
+        for rows, utt, seq, P, G, sp, seed, _ in groups:
             feeds[rows[0]] = torch.cat([self.init, seq[:, :P].to(device=dev, dtype=torch.int64)], dim=1)
         m.prefill_streams({r: f[:, :-1] for r, f in feeds.items()})
-        for rows, utt, seq, P, G, sp, seed in groups:
+        for rows, utt, seq, P, G, sp, seed, (task, minlen, win) in groups:
             m.fork_kv(rows[0], rows[1:], P + G)
             gid, self.groups = self.groups, self.groups + 1
             for i, r in enumerate(rows):
-                self.rows[r] = dict(utt=utt, P=P, G=G, g=0, start=self.n, sp=sp, cand=i, group=gid)
+                self.rows[r] = dict(utt=utt, P=P, G=G, g=0, start=self.n, sp=sp, cand=i, group=gid, task=task, minlen=minlen,
+                                    win=win)
+                self.fresh.add(r)
                 self.keys[r] = sample_seed(seed, i)
                 self.cur[r, :, 0] = feeds[rows[0]][:, -1]
 
+    def _argmax(self, st: dict) -> bool:
+        """the row's audio heads take the argmax (no candidate masks: the whole card)"""
+        sp = st["sp"] if st["sp"] is not None else (self.default or self.imp.sampling())
+        return sp.heads()[1][0] == 0
+
+    def _upload_records(self, rows: List[int]) -> None:
+        """the generation records and next-frame candidate counts of these occupied rows, from the host's state"""
+        recs, valid = [], []
+        for r in rows:
+            st = self.rows[r]
+            argmax = self._argmax(st)
+            kind = _lib.GEN_WINDOWED if st["win"] else _lib.GEN_FIXED
+            recs.append([st["P"], st["minlen"], st["G"], st["g"], kind | (_lib.GEN_ARGMAX if argmax else 0)])
+            valid.append([self.m.config.audio_card] * self.dep_q if argmax else
+                         candidate_counts(st["P"], st["minlen"], st["g"], self.dep_q))
+        self.m._state.gen_rows_set(rows, recs, valid)
+
     def frame(self, records: Optional[list] = None) -> List[Tuple]:
         """One generated frame of every row (there must be an occupied row).  records: a list that receives the
-        frame's chunk records (row, utt, index, codes or None) when the codec runs."""
+        frame's chunk records (row, utt, index, codes or None) when the codec runs.  -> the utterances finished:
+        (utt, codes or None, raw frames [G', 9], row state)."""
         imp, m, B, rows = self.imp, self.m, self.B, self.rows
         occupied = self.occupied()
         mask = np.array([1 if rows[r] is not None else 0 for r in range(B)], dtype=np.int64)
         if not np.array_equal(mask, self.active):
             self.active = mask
             m.set_active_streams(self.active)
-        table = torch.full((B, self.dep_q), 2048, dtype=torch.int32)
-        for r in occupied:
-            st = rows[r]
-            table[r] = torch.tensor(candidate_counts(st["P"], st["G"], st["g"], self.dep_q), dtype=torch.int32)
+        gen = any(rows[r]["win"] for r in occupied)
+        table = None
+        if gen:
+            # a row whose window can stop it is in the batch: the device keeps every row's window and candidate counts
+            fresh = occupied if not self.gen else sorted(self.fresh)
+            if fresh:
+                self._upload_records(fresh)
+        else:
+            table = torch.full((B, self.dep_q), 2048, dtype=torch.int32)
+            for r in occupied:
+                st = rows[r]
+                table[r] = torch.tensor(candidate_counts(st["P"], st["minlen"], st["g"], self.dep_q), dtype=torch.int32)
+        self.gen = gen
+        self.fresh.clear()
         per_row = None
         if self.default is not None:
             default = self.default
             per_row = [default if rows[r] is None or rows[r]["sp"] is None else rows[r]["sp"] for r in range(B)]
+        extra = {"gen_rows": True} if gen else {}
+        if self.n_samples > 1:
+            extra["logprob"] = True
         toks = m.forward_step(self.cur, use_sampling=imp.use_sampling, temp_text=imp.temp_text, top_k_text=imp.top_k_text,
                               temp=imp.temp, top_k=imp.top_k, audio_valid=table,
                               sample_key=self.keys if self.admitted else None, depth_ring_quirk=False,
-                              top_p_text=imp.top_p_text, top_p=imp.top_p, sampling=per_row,
-                              **({"logprob": True} if self.n_samples > 1 else {}))
+                              top_p_text=imp.top_p_text, top_p=imp.top_p, sampling=per_row, **extra)
+        lagged = None
+        if gen:
+            # the frame's statuses: one copy to pinned host memory behind an event, read after the next frame is enqueued
+            if self.status is None:
+                cuda = self.dev.type == "cuda"
+                self.status = [torch.zeros(B, dtype=torch.int32, pin_memory=cuda) for _ in range(2)]
+            slot, self.status_slot = self.status_slot, self.status_slot ^ 1
+            self.status[slot].copy_(m._state.gen_status[:B], non_blocking=True)
+            lp = _to_host(m._state.logprob_sums()) if self.n_samples > 1 else None
+            ev = torch.cuda.Event() if self.dev.type == "cuda" else None
+            if ev is not None:
+                ev.record()
+            lagged = (self.n, slot, ev, {r: rows[r] for r in occupied if rows[r]["win"]}, lp)
         if self.codec is not None:
             self._decode(toks)
         self.history[self.n] = toks
@@ -552,10 +715,12 @@ class _TTSRows:
         self.stats["frames"] += 1
         self.stats["row_frames"] += len(occupied)
         self.cur = toks[:, :, None].clone()
-        done = []
+        # the statuses of the frame before this one: the device has this frame queued while the host waits for them
+        done = self.settle(keep_open=True)
+        self.lagged = lagged
         lp = None
         if self.n_samples > 1:
-            last = [r for r in occupied if rows[r]["g"] + 1 == rows[r]["G"]]
+            last = [r for r in occupied if rows[r] is not None and not rows[r]["win"] and rows[r]["g"] + 1 == rows[r]["G"]]
             if last:
                 # the log-probability sums of the candidates this frame finishes: one copy to pinned host memory, not
                 # waited for here (generate_many reads it after the next frame is enqueued)
@@ -565,29 +730,103 @@ class _TTSRows:
                 lp = {r: (host, i, ev) for i, r in enumerate(last)}
         for r in occupied:
             st = rows[r]
+            if st is None or st["start"] >= self.n:
+                continue   # released above (it stopped at the frame before), or admitted after this frame
             st["g"] += 1
             last = st["g"] == st["G"]
             codes = raw = None
             if last:
-                raw = torch.stack([self.history[f][r] for f in range(st["start"], self.n)])     # [G, 9]
-                if lp is not None:
-                    st["lp"] = lp[r]
-                rows[r] = None
-                m.reset_streaming(streams=[r])   # a held row keeps its position: park it at 0 ...
-                if self.paged:
-                    self.pages.release([r])      # ... without pages (uploaded before the next launch)
-                    self.dirty.add(r)
-                codes = reverse_delay(raw[:, 1:])
-                done.append((st["utt"], codes, raw, st))
-            if records is not None and (st["g"] >= 2 or last):
+                self._release(r)
+                if st["win"]:
+                    # its status of this frame (kept, or stopped and dropped) is read with the next frame's
+                    self.awaiting.append((r, st))
+                else:
+                    if lp is not None:
+                        st["lp"] = lp[r]
+                    st["frames"] = st["G"]
+                    raw, codes = self._result(st, r, self.n)
+                    done.append((st["utt"], codes, raw, st))
+            if records is not None and st["win"]:
+                # a windowed row's chunk is decided when it is handed out, once this frame's status has been read
+                records.append((r, st["utt"], max(st["g"] - 2, 0), st, st["g"] >= 2, self.n - 1))
+            elif records is not None and (st["g"] >= 2 or last):
                 # step g - 1 >= 1 completes codec frame g - 2; an utterance of one frame has no audio
                 records.append((r, st["utt"], max(st["g"] - 2, 0), codes, st["g"] >= 2))
-        if records is not None and done:
-            self.delay.reset([r for r in occupied if rows[r] is None])   # a free row has no frame: the codec holds it
-        first = min([st["start"] for st in rows if st is not None], default=self.n)
+        freed = [r for r in occupied if rows[r] is None]
+        if records is not None and freed:
+            self.delay.reset(freed)   # a free row has no frame: the codec holds it
+        self._prune()
+        return done
+
+    def _release(self, r: int) -> None:
+        """free row r: park it at position 0 without pages (uploaded before the next launch)"""
+        self.rows[r] = None
+        self.m.reset_streaming(streams=[r])
+        if self.paged:
+            self.pages.release([r])
+            self.dirty.add(r)
+
+    def _result(self, st: dict, r: int, end: int):
+        """(raw frames [G', 9] of frames start .. end - 1 of row r, codes [8, G' - 1] for the audio tasks else None)"""
+        if end > st["start"]:
+            raw = torch.stack([self.history[f][r] for f in range(st["start"], end)])
+        else:
+            raw = torch.zeros(0, self.dep_q + 1, dtype=torch.int64, device=self.dev)
+        return raw, (reverse_delay(raw[:, 1:]) if st["task"] in AUDIO_TASKS else None)
+
+    def _prune(self) -> None:
+        live = [st for st in self.rows if st is not None] + [st for _, st in self.awaiting]
+        first = min([st["start"] for st in live], default=self.n)
         for f in [f for f in self.history if f < first]:
             del self.history[f]
+
+    def settle(self, keep_open: bool = False) -> List[Tuple]:
+        """Read the statuses of the last windowed frame (waits for its copy) and finish the rows they end: a row that
+        stopped there (the frame and the one it ran after are dropped; it is released) and the rows that ran their last
+        frame there.  keep_open: called from frame(), whose own statuses are still being copied."""
+        lagged, self.lagged = self.lagged, None
+        done = []
+        if lagged is None:
+            return done
+        f, slot, ev, snap, lp = lagged
+        if ev is not None:
+            ev.synchronize()
+        status = self.status[slot].numpy()
+        if lp is not None:
+            # best-of-N: each windowed frame's sums, kept while a row that ran it may still end there
+            self.lp_frames = {k: v for k, v in self.lp_frames.items() if k >= f - 1}
+            self.lp_frames[f] = lp
+        awaiting = {id(st): r for r, st in self.awaiting}
+        for r, st in snap.items():
+            stopped = int(status[r]) == _lib.GEN_STOPPED
+            if self.rows[r] is st:
+                if not stopped:
+                    continue
+                self._release(r)
+            elif id(st) not in awaiting:
+                continue
+            end = f if stopped else f + 1
+            st["frames"] = end - st["start"]
+            st["stopped"] = stopped
+            if lp is not None:
+                # the sums after frame end - 1: this frame's copy if it is kept, else the one before (or none)
+                st["lp"] = self._lp_at(end - 1, st, r)
+            raw, codes = self._result(st, r, end)
+            st["end"], st["codes"] = end, codes
+            if stopped:
+                st["dropped"] = self.history[f][r]     # the frame its stop rule fired on (not part of the result)
+            done.append((st["utt"], codes, raw, st))
+        self.awaiting = [(r, st) for r, st in self.awaiting if "frames" not in st]
+        if not keep_open:
+            self._prune()
         return done
+
+    def _lp_at(self, frame: int, st: dict, r: int):
+        """(host sums, row, event) of row r's log-probability sums after `frame` (zeros before its first frame); the
+        copies were read by settle(), so no event is left to wait for"""
+        if frame < st["start"]:
+            return (torch.zeros(1, self.dep_q + 1, dtype=torch.float64), 0, None)
+        return (self.lp_frames[frame], r, None)
 
     def _decode(self, toks: torch.Tensor) -> None:
         """the codec frame of every row that has one, into PCM slot self.slot"""
@@ -605,12 +844,15 @@ class _TTSRows:
             records = []
             self.frame(records)
             cuda = self.events is not None
-            records = [(r, utt, i, None if c is None else _to_host(c), has_pcm) for r, utt, i, c, has_pcm in records]
+            records = [rec if len(rec) == 6 else rec[:3] + (None if rec[3] is None else _to_host(rec[3]), rec[4])
+                       for rec in records]
             if cuda:
                 self.events[self.slot].record()
             self.in_flight, self.slot = (self.slot, records), self.slot ^ 1
         elif prev is None:
             return None
+        else:
+            self.settle()   # the last frame's statuses, which decide its windowed rows' chunks
         return [] if prev is None else self._hand_out(*prev)
 
     def _hand_out(self, slot: int, records) -> List[TTSChunk]:
@@ -618,8 +860,25 @@ class _TTSRows:
             self.events[slot].synchronize()
         pcm = self.pcm[slot].numpy()
         empty = torch.zeros(0, dtype=torch.float32)
-        return [TTSChunk(utt, i, torch.from_numpy(pcm[r].copy()) if has_pcm else empty, codes)
-                for r, utt, i, codes, has_pcm in records]
+        out = []
+        for rec in records:
+            if len(rec) == 5:
+                r, utt, i, codes, has_pcm = rec
+                out.append(TTSChunk(utt, i, torch.from_numpy(pcm[r].copy()) if has_pcm else empty, codes))
+                continue
+            # a windowed row's frame f, whose status is known by now: kept (running, or its last frame, which carries the
+            # codes), the frame its stop fired on (its chunk would decode the dropped frame: an empty last chunk carries
+            # the codes instead), or the frame it ran after its stop (nothing)
+            r, utt, i, st, has_pcm, f = rec
+            end = st.get("end")
+            if end is None or f < end - 1:
+                if has_pcm:
+                    out.append(TTSChunk(utt, i, torch.from_numpy(pcm[r].copy()), None))
+            elif f == end - 1:
+                out.append(TTSChunk(utt, i, torch.from_numpy(pcm[r].copy()) if has_pcm else empty, st["codes"].cpu()))
+            elif f == end:
+                out.append(TTSChunk(utt, i, empty, st["codes"].cpu()))
+        return out
 
 
 def _ranked(cands, rank: Optional[str]) -> List[Candidate]:
@@ -627,9 +886,10 @@ def _ranked(cands, rank: Optional[str]) -> List[Candidate]:
     out = []
     for st, codes in cands:
         host, i, ev = st["lp"]
-        ev.synchronize()
+        if ev is not None:
+            ev.synchronize()
         lp = host[i]
-        out.append(Candidate(st["cand"], codes, float(lp[1:].sum()), float(lp[0]), st["G"]))
+        out.append(Candidate(st["cand"], codes, float(lp[1:].sum()), float(lp[0]), st["frames"]))
     return rank_candidates(out, rank)
 
 

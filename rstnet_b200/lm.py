@@ -881,7 +881,7 @@ class GPT(_DecodeModel):
     def forward_step(self, sequence: torch.Tensor, *, use_sampling: bool = True, temp_text: float = 0.7, top_k_text: int = 25,
                      temp: float = 0.8, top_k: int = 30, audio_valid=2049, depth_ring_quirk: bool = True, sample_key=None,
                      sample_step=None, top_p_text: float = 0.0, top_p: float = 0.0, sampling=None,
-                     logprob: bool = False) -> torch.Tensor:
+                     logprob: bool = False, gen_rows: bool = False) -> torch.Tensor:
         """One generated frame: temporal step on sequence[B,9,1], text token, then the 8 depth steps, each sampled
         on the device (sample_token / sample_token_audio[_2048], utils/sampling.py:85-154: use_sampling False ->
         argmax over the whole card; True -> temperature + top-k (top_k == 0: plain multinomial) over ids <
@@ -905,13 +905,18 @@ class GPT(_DecodeModel):
         logprob: also add, for every active row, the log-probability of each sampled token under the head's untempered
         softmax over all its ids (whatever the temperature, top-k / top-p and candidate counts) into the scope's per-row
         sums (`logprob_sums`, zeroed by `logprob_reset`), one cross-entropy launch per head inside the frame: a graph of its
-        own, next to the one without."""
+        own, next to the one without.
+
+        gen_rows (with audio_valid=None): the per-row candidate counts are the scope's device table row_valid, kept by the
+        rows' generation windows (`_LMState.gen_rows_set`): after the last depth sample, rstnet_lm_gen_rows_advance decides
+        each row's status for this frame (running, last, stopped by the reference's stop rule, idle) into
+        `_state.gen_status` and writes the next frame's counts.  A graph of its own."""
         if self._state is None:
             raise RstnetError("forward_step is a streaming call: use it inside `with gpt.streaming(B):`")
         if sampling is None and (top_p_text or top_p):
             Sampling(use_sampling, temp_text, top_k_text, top_p_text, temp, top_k, top_p)   # validates a nucleus frame's settings
         return self._state.forward_step(sequence, use_sampling, temp_text, top_k_text, temp, top_k, audio_valid, depth_ring_quirk,
-                                        sample_key, sample_step, top_p_text, top_p, sampling, logprob)
+                                        sample_key, sample_step, top_p_text, top_p, sampling, logprob, gen_rows)
 
     @torch.no_grad()
     @on_own_device
@@ -1245,6 +1250,9 @@ class _LMState:
             self.frame_counter = z(1, dtype=torch.int64)
             # per-row sampling (forward_step with an audio_valid table): candidate counts, RNG keys, step counters
             self.row_valid = z(M, c.dep_q, dtype=torch.int32)
+            # forward_step(gen_rows=True): per-row generation windows (rstnet_lm_gen_rows_advance) and each frame's status
+            self.gen_rec = z(M, _lib.GEN_REC, dtype=torch.int32)
+            self.gen_status = z(M, dtype=torch.int32)
             self.row_key = z(M, dtype=torch.int32)
             self.row_step = z(M, dtype=torch.int64)
             # per-row settings (forward_step(sampling=...)): column 0 the text head, column 1 the audio heads
@@ -1716,10 +1724,15 @@ class _LMState:
             out[:, k].copy_(self.dlogits)
 
     def forward_step(self, sequence, use_sampling, temp_text, top_k_text, temp, top_k, audio_valid, quirk=True, sample_key=None,
-                     sample_step=None, top_p_text=0.0, top_p=0.0, sampling=None, logprob=False):
+                     sample_step=None, top_p_text=0.0, top_p=0.0, sampling=None, logprob=False, gen_rows=False):
         c = self.c
         if sequence.shape[0] != self.B or sequence.shape[2] != 1:
             raise RstnetError(f"forward_step takes sequence [{self.B}, {c.n_q + 1}, 1], got {tuple(sequence.shape)}")
+        if gen_rows:
+            if audio_valid is not None:
+                raise RstnetError("gen_rows=True reads the candidate counts the device keeps in row_valid: pass audio_valid=None")
+            # the per-row path with the table already on the device (argmax rows carry the whole card in their record)
+            audio_valid = self.row_valid[:self.B]
         per_row = torch.is_tensor(audio_valid)
         if sampling is not None and not per_row:
             raise RstnetError("per-row sampling settings go with per-row candidate counts: pass audio_valid as a [B, dep_q] tensor")
@@ -1735,13 +1748,14 @@ class _LMState:
             raise RstnetError("sample_key / sample_step select per-row sampling: pass audio_valid as a [B, dep_q] tensor")
         if sampling is not None:
             argmax = self.set_row_sampling(sampling)
-            if argmax is not None:
+            if argmax is not None and not gen_rows:
                 # the 2048 / 2049 candidate sets exist on the sampling path only: argmax rows take the whole card
                 audio_valid = torch.where(argmax, c.audio_card, audio_valid.to(argmax.device))
         self._advance_host(1)
         self.seq.copy_(sequence[:, :, 0])
         if per_row:
-            self.row_valid.copy_(audio_valid)
+            if not gen_rows:
+                self.row_valid.copy_(audio_valid)
             valid = None
         else:
             valid = tuple(audio_valid) if isinstance(audio_valid, (tuple, list)) else (audio_valid,) * c.dep_q
@@ -1749,8 +1763,19 @@ class _LMState:
                                                    _head_mode(use_sampling, temp, top_k, top_p))
         if logprob and self.lp_acc is None:
             self.logprob_reset()
-        self._replay(*self._frame(modes, valid, per_row, quirk, bool(logprob)))
+        self._replay(*self._frame(modes, valid, per_row, quirk, bool(logprob), bool(gen_rows)))
         return self.tokens.clone()
+
+    # ---- per-row generation windows (forward_step(gen_rows=True))
+    def gen_rows_set(self, rows, records, valid) -> None:
+        """rows' generation records (int32 [n, GEN_REC]: pre_gen_len, minlen, maxlen, g_idx, mode) and the candidate
+        counts of their next frame (int32 [n, dep_q]), uploaded from pinned memory without a synchronise"""
+        idx = torch.as_tensor(rows, dtype=torch.int64).to(self.gen_rec.device)
+        rec = torch.as_tensor(np.asarray(records, dtype=np.int32).reshape(len(rows), _lib.GEN_REC)).pin_memory()
+        val = torch.as_tensor(np.asarray(valid, dtype=np.int32).reshape(len(rows), self.c.dep_q)).pin_memory()
+        self.gen_rec.index_copy_(0, idx, rec.to(self.gen_rec.device, non_blocking=True))
+        self.row_valid.index_copy_(0, idx, val.to(self.row_valid.device, non_blocking=True))
+
 
     # ---- log-probabilities of the sampled tokens (forward_step(logprob=True))
     def _logprob_slots(self) -> None:
@@ -1788,13 +1813,14 @@ class _LMState:
         self.lp_lab[col].copy_(self.tokens[:, col])
         cross_entropy_sums(logits, self.lp_lab[col], self.lp_w, 1, None, self.lp_slot, self.lp_acc[col], self.lp_nll, self.lp_pred)
 
-    def _frame(self, modes, valid, per_row_rng: bool, quirk, logprob: bool = False):
+    def _frame(self, modes, valid, per_row_rng: bool, quirk, logprob: bool = False, gen: bool = False):
         """(graph key, launch sequence) of one generated frame from the ids in self.seq to the tokens in self.tokens.
         modes: ((top_k, temp, top_p) of the text head, (...) of the audio heads) for every row, as _head_mode gives them, or
         None: each row's own from the row_topk / row_temp / row_topp tables.  valid: the dep_q audio heads' candidate
         counts for every row, or None: each row's own from row_valid.  per_row_rng: the RNG keyed by (row_step, row_key)
         in place of (frame_counter, row); the frame advances the counter it keys by.  logprob: after each head's sampler,
-        add the log-probability of the sampled tokens into the rows' sums (logprob_sums); a graph of its own."""
+        add the log-probability of the sampled tokens into the rows' sums (logprob_sums); a graph of its own.  gen: then
+        advance the rows' generation windows (gen_rows): status, next frame's row_valid; a graph of its own."""
         c = self.c
         if modes is not None and modes[1][0] == 0:
             valid = (c.audio_card,) * c.dep_q   # the 2048 / 2049 masks exist on the sampling path only (sampling.py:107-154)
@@ -1817,4 +1843,11 @@ class _LMState:
                 ops.counter_add(self.frame_counter, 1)
 
         key = ("frame", "tables" if modes is None else modes, "rows" if valid is None else valid, per_row_rng, bool(quirk))
-        return (key + ("logprob",) if logprob else key), frame
+        key = key + ("logprob",) if logprob else key
+        if not gen:
+            return key, frame
+
+        def gen_frame():
+            frame()
+            ops.gen_rows_advance(self.tokens, self.gen_rec, self.row_valid, self.gen_status, c.audio_card)
+        return key + ("gen",), gen_frame

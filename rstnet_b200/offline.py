@@ -183,34 +183,52 @@ def reconstruct_corpus(codec: MimiCodec, src: str, dst: str, capacity: int = 128
 
 @torch.no_grad()
 def synthesize(imp, corpus: Dict[str, torch.Tensor], capacity: int = 32, seeds=None,
-               kv_gb: Optional[float] = None, n_samples: int = 1, all_samples: bool = False) -> Dict[str, torch.Tensor]:
+               kv_gb: Optional[float] = None, n_samples: int = 1, all_samples: bool = False,
+               lengths: Optional[Tuple[int, int]] = None) -> Dict[str, torch.Tensor]:
     """{utt_id: int16 [8, T]} for every utterance of `corpus` ({utt_id: int64 [9, L]}), through imp.generate_many.
     kv_gb: the KV cache's budget in GiB (a pool of floor(kv_gb * 2^30 / kv_page_bytes) pages); None: a whole ring per row.
     n_samples N > 1: best-of-N, the codes of each utterance's candidate with the highest mean audio log-probability per
-    frame; all_samples also returns candidate i's codes as `<utt_id>_s<i>`."""
-    items = ((utt, torch.as_tensor(seq, dtype=torch.int64)) for utt, seq in corpus.items())
+    frame; all_samples also returns candidate i's codes as `<utt_id>_s<i>`.
+    imp.task_name other than TTS: audio_only gives each item's prompt audio and continuation as one clip
+    (infer.continuation_codes), int16 [8, P + G' - 1]; text_only and ASR the generated text token ids, int64 [G'].
+    lengths: (min_frames, max_frames) replaces every item's window (generate_many's `lengths`)."""
+    from .infer import continuation_codes
+    corpus = {utt: torch.as_tensor(seq, dtype=torch.int64) for utt, seq in corpus.items()}
     kv_pages = None if kv_gb is None else kv_pages_for_budget(imp.model.config, kv_gb)
-    if n_samples == 1:
-        return {utt: codes.to(torch.int16).cpu() for utt, codes in imp.generate_many(items, capacity, seeds=seeds, kv_pages=kv_pages)}
+    lens = None if lengths is None else {utt: tuple(lengths) for utt in corpus}
+    task = imp.task_name
+
+    def result(utt, out):
+        if task == "TTS":
+            return out.to(torch.int16).cpu()
+        if task == "audio_only":
+            return continuation_codes(corpus[utt], out).to(torch.int16).cpu()
+        return out[:, 0].cpu()
+
     out = {}
-    for utt, cands in imp.generate_many(items, capacity, seeds=seeds, kv_pages=kv_pages, n_samples=n_samples):
-        out[utt] = cands[0].codes.to(torch.int16).cpu()
+    for utt, res in imp.generate_many(iter(corpus.items()), capacity, seeds=seeds, kv_pages=kv_pages, n_samples=n_samples,
+                                      lengths=lens):
+        if n_samples == 1:
+            out[utt] = result(utt, res)
+            continue
+        out[utt] = result(utt, res[0].codes)
         if all_samples:
-            for c in sorted(cands, key=lambda c: c.index):
-                out[f"{utt}_s{c.index}"] = c.codes.to(torch.int16).cpu()
+            for c in sorted(res, key=lambda c: c.index):
+                out[f"{utt}_s{c.index}"] = result(utt, c.codes)
     return out
 
 
 @torch.no_grad()
 def synthesize_stream(imp, codec: MimiCodec, corpus: Dict[str, torch.Tensor], dst: str, capacity: int = 32, seeds=None,
-                      kv_gb: Optional[float] = None) -> Dict[str, torch.Tensor]:
+                      kv_gb: Optional[float] = None, lengths: Optional[Tuple[int, int]] = None) -> Dict[str, torch.Tensor]:
     """`synthesize` through imp.stream_many: the same {utt_id: int16 [8, T]}, and each utterance's `<utt_id>_sample.wav`
     (24 kHz 16-bit, as write_codes_wav; none for T = 0) written from its streamed chunks as soon as it completes."""
     os.makedirs(dst, exist_ok=True)
     items = ((utt, torch.as_tensor(seq, dtype=torch.int64)) for utt, seq in corpus.items())
     kv_pages = None if kv_gb is None else kv_pages_for_budget(imp.model.config, kv_gb)
     parts, out = defaultdict(list), {}
-    for ch in imp.stream_many(items, capacity, codec, seeds=seeds, kv_pages=kv_pages):
+    lens = None if lengths is None else {utt: tuple(lengths) for utt in corpus}
+    for ch in imp.stream_many(items, capacity, codec, seeds=seeds, kv_pages=kv_pages, lengths=lens):
         parts[ch.utt_id].append(ch.pcm)
         if ch.codes is not None:
             wav = torch.cat(parts.pop(ch.utt_id))
@@ -258,7 +276,14 @@ def _load_gpt(config_path: str, checkpoint: str, device: str):
 def _synthesize_cli(args) -> int:
     from .infer import InferenceImp
     model = _load_gpt(args.config, args.checkpoint, args.device)
-    imp = InferenceImp(None, model, "sampling", args.temp_text, args.top_k_text, args.temp, args.top_k, "TTS")
+    imp = InferenceImp(None, model, "sampling", args.temp_text, args.top_k_text, args.temp, args.top_k, args.task)
+    if (args.min_frames is None) != (args.max_frames is None):
+        raise SystemExit("--min-frames and --max-frames go together")
+    lengths = None if args.min_frames is None else (args.min_frames, args.max_frames)
+    if args.task in ("text_only", "ASR") and (args.stream or args.wav_dir):
+        raise SystemExit(f"--task {args.task} writes text token ids: no --stream / --wav-dir")
+    if args.task == "audio_only" and args.stream:
+        raise SystemExit("--stream decodes the generated frames only; audio_only writes prompt + continuation: drop --stream")
     imp.use_sampling = args.use_sampling
     imp.top_p, imp.top_p_text = args.top_p, args.top_p_text
     if args.top_p or args.top_p_text:
@@ -272,11 +297,12 @@ def _synthesize_cli(args) -> int:
         if not (args.wav_dir and args.codec_weights):
             raise SystemExit("--stream needs --wav-dir and --codec-weights")
         codec = _load_codec(argparse.Namespace(weights=args.codec_weights, config=args.codec_config, device=args.device))
-        codes = synthesize_stream(imp, codec, corpus, args.wav_dir, args.capacity, kv_gb=args.kv_gb)
+        codes = synthesize_stream(imp, codec, corpus, args.wav_dir, args.capacity, kv_gb=args.kv_gb, lengths=lengths)
         save_tokens(codes, args.output_file)
         print(f"synthesized {len(codes)} utterances -> {args.output_file}, streamed their wavs -> {args.wav_dir}")
         return 0
-    codes = synthesize(imp, corpus, args.capacity, kv_gb=args.kv_gb, n_samples=args.n_samples, all_samples=args.all_samples)
+    codes = synthesize(imp, corpus, args.capacity, kv_gb=args.kv_gb, n_samples=args.n_samples, all_samples=args.all_samples,
+                       lengths=lengths)
     save_tokens(codes, args.output_file)
     print(f"synthesized {len(codes)} utterances -> {args.output_file}")
     if args.wav_dir:
@@ -472,6 +498,12 @@ def build_parser() -> argparse.ArgumentParser:
                    help="best-of-N: sample N candidates of each utterance from one prompt prefill (sharing its KV pages) and "
                         "keep the one with the highest mean audio log-probability per frame")
     p.add_argument("--all-samples", action="store_true", help="with --n-samples: also write candidate i as <utt_id>_s<i>")
+    p.add_argument("--task", choices=("TTS", "audio_only", "text_only", "ASR"), default="TTS",
+                   help="the reference loop's task and layout; audio_only writes prompt + continuation codes, text_only and "
+                        "ASR the generated text token ids (int64 [G'])")
+    p.add_argument("--min-frames", type=int, default=None,
+                   help="with --max-frames: every item's window (minlen): the stop rule applies from frame min + 1 on")
+    p.add_argument("--max-frames", type=int, default=None, help="with --min-frames: at most this many generated frames")
     p.add_argument("--device", default="cuda")
     p = sub.add_parser("score", help="teacher-forced losses / audio perplexity of a corpus (infer_no_streaming.py teacher-force; "
                                      "--model moshi: the Moshi fine-tune trainer's validate_model)")

@@ -233,6 +233,16 @@ def counter_add(counter: torch.Tensor, delta: int, active: Optional[torch.Tensor
     _lib.check(_lib.lib().rstnet_counter_add(counter.data_ptr(), delta, counter.numel(), _p(active), _stream()), "counter_add")
 
 
+def gen_rows_advance(tokens: torch.Tensor, rec: torch.Tensor, row_valid: torch.Tensor, status: torch.Tensor, card: int):
+    """rstnet_lm_gen_rows_advance over the rows of rec (int32 [B, GEN_REC]): the stop rule and maxlen on the frame's
+    tokens (int64 [>= B, dep_q + 1]) into status (int32 [B]), the next frame's candidate counts into row_valid (int32
+    [>= B, dep_q]) of the rows still running (`card` for argmax rows)"""
+    B, dep_q = rec.shape[0], row_valid.shape[1]
+    _lib.check(_lib.lib().rstnet_lm_gen_rows_advance(tokens.data_ptr(), tokens.stride(0), rec.data_ptr(), row_valid.data_ptr(),
+                                                     row_valid.stride(0), status.data_ptr(), B, dep_q, card,
+                                                     _stream()), "lm_gen_rows_advance")
+
+
 def _ostride(offset: torch.Tensor) -> int:
     return 1 if offset.numel() > 1 else 0
 

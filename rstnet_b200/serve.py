@@ -738,10 +738,13 @@ class TTSEngine:
         self._live: set = set()          # utt ids submitted whose last chunk has not been returned
         self._closed = False
 
-    def submit(self, utt_id, seq: torch.Tensor, sampling: Optional[Sampling] = None, seed: int = 0) -> None:
-        """Queue one utterance, seq [9, L] in the TTS layout (raises at once on a bad layout, on a request longer than the
-        whole KV pool and on an id still in flight).  sampling: its own settings (from then on every row samples through
-        the per-row tables); seed: its random stream."""
+    def submit(self, utt_id, seq: torch.Tensor, sampling: Optional[Sampling] = None, seed: int = 0, *,
+               task: str = "TTS", lengths: Optional[Tuple[int, int]] = None) -> None:
+        """Queue one utterance, seq [9, L] in the layout of `task` (TTS or audio_only; raises at once on a text task, a bad
+        layout, a request longer than the whole KV pool and on an id still in flight).  sampling: its own settings (from
+        then on every row samples through the per-row tables); seed: its random stream; lengths: (min_frames,
+        max_frames), its window as in InferenceImp.generate_many -- an utterance that stops ends with an empty chunk
+        carrying its codes (InferenceImp.stream_many)."""
         if self._closed:
             raise RstnetError("the engine is closed")
         if sampling is not None and not isinstance(sampling, Sampling):
@@ -753,12 +756,13 @@ class TTSEngine:
         seq = torch.as_tensor(seq)
         if seq.dim() != 2 or seq.shape[0] != self._rows.dep_q + 1:
             raise RstnetError(f"seq must be [{self._rows.dep_q + 1}, L], got {tuple(seq.shape)}")
-        P, G = self.imp._layout(seq)
-        self._rows.fits(utt_id, P, G)
+        req = self.imp._request(utt_id, seq, sampling, int(seed), task, lengths)
+        self.imp._check_streamed(req)
+        self._rows.fits(utt_id, req[2], req[3])
         if sampling is not None:
             self._rows.use_per_row()
         self._live.add(utt_id)
-        self._queue.append((utt_id, seq, P, G, sampling, int(seed)))
+        self._queue.append(req)
 
     @property
     def pending(self) -> int:

@@ -27,6 +27,7 @@ utterance.
 from __future__ import annotations
 
 from contextlib import contextmanager
+from dataclasses import dataclass
 from typing import Dict, Iterable, Iterator, List, NamedTuple, Optional, Tuple
 
 import numpy as np
@@ -256,9 +257,7 @@ class InferenceImp(object):
             raise RstnetError("the sequence has no prompt frames")
         return prefix_len, L - prefix_len, L - prefix_len
 
-    def _request(self, utt, seq, sp, seed, task=None, lengths=None) -> tuple:
-        """an admission request (utt, seq, P, G, Sampling or None, seed, task, minlen, windowed): G = maxlen, the frames it
-        may run; windowed: its window can stop it (maxlen - 1 > minlen), so the device decides its status every frame"""
+    def _request(self, utt, seq, sp, seed, task=None, lengths=None) -> "_Request":
         task = self.task_name if task is None else task
         P, minlen, maxlen = self._layout(seq, task)
         if lengths is not None:
@@ -268,8 +267,7 @@ class InferenceImp(object):
             minlen, maxlen = int(lengths[0]), int(lengths[1])
             if not 1 <= maxlen < 2 ** 31 or not -2 ** 31 <= minlen < 2 ** 31:
                 raise RstnetError(f"lengths[{utt!r}]: max_frames must be in [1, 2^31) and min_frames an int32 (got {lengths!r})")
-        return utt, seq, P, maxlen, sp, seed, task, minlen, maxlen - 1 > minlen
-
+        return _Request(utt, seq, P, maxlen, sp, seed, task, minlen, maxlen - 1 > minlen)
 
     def _check_many(self, capacity: int, kv_pages: Optional[int], n_samples: int = 1, streamed: bool = False) -> None:
         """the argument checks of generate_many / stream_many / serve.TTSEngine"""
@@ -291,11 +289,10 @@ class InferenceImp(object):
                 raise RstnetError(f"{type(self.model).__name__} has no paged KV scope to fork a prompt into n_samples rows")
 
     @staticmethod
-    def _check_streamed(req: tuple) -> None:
+    def _check_streamed(req: "_Request") -> None:
         """streamed generation runs the audio tasks (their generated frames decode to audio)"""
-        utt, task = req[0], req[6]
-        if task not in AUDIO_TASKS:
-            raise RstnetError(f"utterance {utt!r}: task {task!r} generates text; streamed generation runs {AUDIO_TASKS}")
+        if req.task not in AUDIO_TASKS:
+            raise RstnetError(f"utterance {req.utt!r}: task {req.task!r} generates text; streamed generation runs {AUDIO_TASKS}")
 
     @staticmethod
     def _check_sampling(sampling: Optional[Dict[object, Sampling]]) -> None:
@@ -375,13 +372,11 @@ class InferenceImp(object):
         if n_samples > 1 and return_frames:
             raise RstnetError("return_frames is not available with n_samples > 1")
         m = self.model
-        stats = {} if stats is None else stats
-        stats.update(frames=0, row_frames=0, wait_frames=0)
         self._check_sampling(sampling)
         pull = self._puller(items, seeds, sampling, tasks, lengths)
         with _tts_scope(m, capacity, kv_pages):
-            rows = _TTSRows(self, capacity, sampling is not None, stats, n_samples=int(n_samples))
-            groups: Dict[object, list] = {}
+            rows = _TTSRows(self, capacity, sampling is not None, {} if stats is None else stats, n_samples=int(n_samples))
+            groups: Dict[int, list] = {}
             ready = []   # utterances whose candidates all finished in the last frame: their sums are still being copied
             while True:
                 rows.admit(pull)
@@ -393,15 +388,18 @@ class InferenceImp(object):
                     yield utt, _ranked(cands, rank)
                 ready = []
                 for utt, codes, raw, st in done:
-                    if n_samples == 1:
-                        if st["task"] != "TTS":
-                            yield utt, raw
-                        else:
-                            yield (utt, codes, raw) if return_frames else (utt, codes)
+                    result = codes if st.task == "TTS" else raw
+                    group = groups.setdefault(st.group, [])
+                    group.append((st, result))
+                    if len(group) < n_samples:
                         continue
-                    groups.setdefault(st["group"], []).append((st, codes if st["task"] == "TTS" else raw))
-                    if len(groups[st["group"]]) == n_samples:
-                        ready.append((utt, groups.pop(st["group"])))
+                    del groups[st.group]
+                    if n_samples > 1:
+                        ready.append((utt, group))
+                    elif return_frames and st.task == "TTS":
+                        yield utt, codes, raw
+                    else:
+                        yield utt, result
                 if last:
                     break
             for utt, cands in ready:
@@ -465,12 +463,55 @@ def _tts_scope(m, capacity: int, kv_pages: Optional[int]):
         yield
 
 
+class _Request(NamedTuple):
+    """An admission request of the batch loop (InferenceImp._request): the item's prompt of P frames, G = maxlen the
+    frames it may run, its Sampling (None: the instance's) and seed; windowed: its window can stop it (maxlen - 1 >
+    minlen), so the device decides its status every frame."""
+    utt: object
+    seq: torch.Tensor
+    P: int
+    G: int
+    sampling: Optional[Sampling]
+    seed: int
+    task: str
+    minlen: int
+    windowed: bool
+
+
+@dataclass(eq=False)
+class _Row:
+    """The state of one occupied row of the batch loop: what it was admitted with (`g` counts the frames it has run,
+    from frame `start` on; `cand` is its candidate index in request `group`), then its outcome, set when it finishes:
+    its result is frames start .. end - 1; stopped: its stop rule fired on frame `end` (`dropped`, not part of the
+    result); lp: (host sums, row, event or None) of its log-probability sums (best-of-N); codes: its codes (audio tasks)."""
+    utt: object
+    P: int
+    G: int
+    start: int
+    sampling: Optional[Sampling]
+    task: str
+    minlen: int
+    windowed: bool
+    cand: int
+    group: int
+    g: int = 0
+    end: Optional[int] = None
+    stopped: bool = False
+    dropped: Optional[torch.Tensor] = None
+    lp: Optional[tuple] = None
+    codes: Optional[torch.Tensor] = None
+
+    @property
+    def frames(self) -> int:
+        return self.end - self.start
+
+
 class _TTSRows:
     """The admission and frame loop of batch TTS, shared by generate_many, stream_many and serve.TTSEngine, inside one LM
-    scope of B rows (`_tts_scope`).  `admit(pull)` fills free rows in order with the requests pull() gives -- (utt, seq,
-    P, G, Sampling or None, seed), None when there is none -- and stops at the first one whose KV pages the pool cannot
-    give yet (it waits, in `pending`, for the next call); `frame()` runs one generated frame for every row and returns
-    the utterances it finished as (utt, codes [8, G-1], raw frames [G, 9]).  per_row: every row samples with its own
+    scope of B rows (`_tts_scope`).  `admit(pull)` fills free rows in order with the requests pull() gives (a _Request,
+    None when there is none), each as n_samples rows, and stops at the first one whose rows or KV pages are not free yet
+    (it waits, in `pending`, for the next call); `frame()` runs one generated frame for every row and returns the rows it
+    finished as (utt, codes [8, G-1] or None, raw frames [G, 9], row state).  per_row: every row samples with its own
     settings (a request's Sampling, else the InferenceImp's) from the per-row tables; False: the instance's scalar settings.
 
     With a codec (stream_step), every frame also runs, for all B rows, the acoustic-delay cache kernel
@@ -484,7 +525,7 @@ class _TTSRows:
         m = imp.model
         self.imp, self.m, self.B, self.stats = imp, m, B, stats
         self.n_samples = n_samples      # > 1: each request is that many candidates, forked from one prefill
-        self.groups = 0                 # requests admitted (a candidate's group id)
+        self.groups = 0                 # requests admitted (a row's group id)
         stats.update(frames=0, row_frames=0, wait_frames=0)
         self.default = None             # the instance's Sampling while rows sample with per-row settings
         if per_row:
@@ -493,7 +534,7 @@ class _TTSRows:
         self.pages = m._state.pages if self.paged else None   # the scope's allocator, read to decide admissions
         self.dev, n_cb = m.device, m.num_codebooks
         self.dep_q = n_cb - 1                 # text + dep_q audio codebooks per frame
-        self.rows: List[Optional[dict]] = [None] * B
+        self.rows: List[Optional[_Row]] = [None] * B
         self.history: Dict[int, torch.Tensor] = {}       # frame -> tokens [B, 9] of every row
         self.n = 0                                       # frames run
         self.cur = torch.zeros(B, n_cb, 1, dtype=torch.int64, device=self.dev)
@@ -501,14 +542,13 @@ class _TTSRows:
         self.active = np.zeros(B, dtype=np.int64)
         m.set_active_streams(self.active)
         self.init = m._get_initial_token()[0].to(self.dev)
-        self.pending = None   # the next request while it waits for pages
+        self.pending = None   # the next request while it waits for rows or pages
         self.dirty = set()    # rows whose pages changed on the host since the last upload
         self.admitted = False
-        # rows whose window can stop them (`win`) run with the device's generation records (forward_step(gen_rows=True)):
+        # rows whose window can stop them run with the device's generation records (forward_step(gen_rows=True)):
         self.gen = False      # the last frame ran them
         self.fresh = set()    # rows admitted since the last frame (their records are uploaded before it)
-        self.awaiting = []    # (row, state) of windowed rows that ran their last frame, until its status is read
-        self.lagged = None    # (frame, slot, event, {row: state}) of the last frame's statuses, copied, not yet read
+        self.lagged = None    # (frame, slot, event, {row: state}, sums) of the last windowed frame, copied, not yet read
         self.status = None    # two pinned host slots for the statuses [B] int32, allocated on the first windowed frame
         self.status_slot = 0
         self.lp_frames: Dict[int, torch.Tensor] = {}   # best-of-N: windowed frame -> every row's sums after it (host)
@@ -518,9 +558,8 @@ class _TTSRows:
             self.card = codec.codebook_size
             cuda = self.dev.type == "cuda"
             self.pcm = [torch.zeros(B, codec.frame_size, dtype=torch.float32, pin_memory=cuda) for _ in range(2)]
-            self.events = [torch.cuda.Event() for _ in range(2)] if cuda else None
             self.slot = 0
-            self.in_flight = None         # (slot, chunk records) of the last frame run, not yet handed out
+            self.in_flight = None         # (slot, event, chunk records) of the last frame run, not yet handed out
 
     def use_per_row(self) -> None:
         """from the next frame on, every row samples with its own settings (per-row tables)"""
@@ -529,6 +568,15 @@ class _TTSRows:
 
     def occupied(self) -> List[int]:
         return [r for r in range(self.B) if self.rows[r] is not None]
+
+    def _event(self):
+        """a CUDA event recorded on the current stream after the work enqueued so far; None on a CPU device, where that
+        work is done already"""
+        if self.dev.type != "cuda":
+            return None
+        ev = torch.cuda.Event()
+        ev.record()
+        return ev
 
     def pages_needed(self, P: int, G: int) -> int:
         """KV pages of one request: its P + G positions, and with n_samples > 1 the N - 1 forked candidates' own pages
@@ -546,106 +594,70 @@ class _TTSRows:
                               f"more than the whole pool of {self.pages.n_pages}")
 
     def admit(self, pull) -> None:
-        if self.n_samples > 1:
-            return self._admit_groups(pull)
-        m, dev, pages = self.m, self.dev, self.pages
-        admitted = {}
-        for r in range(self.B):
-            if self.rows[r] is not None:
-                continue
-            if self.pending is None:
-                req = pull()
-                if req is None:
-                    break
-                self.fits(req[0], req[2], req[3])
-                self.pending = req
-            utt, seq, P, G, sp, seed, task, minlen, win = self.pending
-            if self.paged:
-                if pages.pages_for(P + G) > pages.free:
-                    self.stats["wait_frames"] += 1
-                    break
-                # it writes P positions in the prompt feed (init token + all prompt frames but the last) and one
-                # per generated frame: at most P + G (G = maxlen; a row that stops runs one frame past its stop, at
-                # most frame maxlen - 1)
-                pages.reserve([r], P + G)
-                self.dirty.add(r)
-            self.pending = None
-            feed = torch.cat([self.init, seq[:, :P].to(device=dev, dtype=torch.int64)], dim=1)
-            admitted[r] = feed
-            self.rows[r] = dict(utt=utt, P=P, G=G, g=0, start=self.n, sp=sp, task=task, minlen=minlen, win=win)
-            self.keys[r] = seed
-            self.fresh.add(r)
-        if self.dirty:
-            # one upload of the table rows this frame's releases and admissions changed, before any launch
-            m._state.upload_pages(sorted(self.dirty))
-            self.dirty.clear()
-        self.admitted = bool(admitted)
-        if admitted:
-            # the init token + all prompt frames but the last only feed the KV rings; the step on the last prompt
-            # frame yields generated frame 0 (as generate)
-            m.reset_streaming(streams=sorted(admitted))
-            if self.codec is not None:
-                self.delay.reset(sorted(admitted))
-                self.codec.reset_streaming(streams=sorted(admitted))
-            m.prefill_streams({r: f[:, :-1] for r, f in admitted.items()})
-            for r, f in admitted.items():
-                self.cur[r, :, 0] = f[:, -1]
-
-    def _admit_groups(self, pull) -> None:
-        """admit with n_samples = N > 1: a request takes the N lowest free rows once they and its pages are free; its
-        prompt is prefilled into the first and forked into the others"""
-        m, dev, pages, N = self.m, self.dev, self.pages, self.n_samples
-        st = m._state
-        groups = []
-        forked = 0   # pages the forks of this call's groups will take (they run after the prefill)
+        """A request takes the n_samples lowest free rows once they and its pages are free; its prompt is prefilled into
+        the first, and with n_samples > 1 forked into the others (their log-probability sums start from zero)."""
+        m, pages, N = self.m, self.pages, self.n_samples
+        groups = []   # (rows, request, prompt feed) admitted by this call
+        taken = set()
+        forked = 0    # pages the forks of this call's groups will take (they run after the prefill)
         while True:
-            free = [r for r in range(self.B) if self.rows[r] is None and all(r not in g[0] for g in groups)]
+            free = [r for r in range(self.B) if self.rows[r] is None and r not in taken]
             if len(free) < N:
                 break
             if self.pending is None:
                 req = pull()
                 if req is None:
                     break
-                self.fits(req[0], req[2], req[3])
+                self.fits(req.utt, req.P, req.G)
                 self.pending = req
-            utt, seq, P, G, sp, seed, task, minlen, win = self.pending
-            if self.pages_needed(P, G) > pages.free - forked:
-                self.stats["wait_frames"] += 1
-                break
-            forked += self.pages_needed(P, G) - pages.pages_for(P + G)
-            rows = free[:N]
-            pages.reserve([rows[0]], P + G)
-            self.dirty.add(rows[0])
+            req, rows = self.pending, free[:N]
+            if self.paged:
+                need = self.pages_needed(req.P, req.G)
+                if need > pages.free - forked:
+                    self.stats["wait_frames"] += 1
+                    break
+                forked += need - pages.pages_for(req.P + req.G)
+                # it writes P positions in the prompt feed (init token + all prompt frames but the last) and one per
+                # generated frame: at most P + G (G = maxlen; a row that stops runs one frame past its stop, at most
+                # frame maxlen - 1)
+                pages.reserve([rows[0]], req.P + req.G)
+                self.dirty.add(rows[0])
             self.pending = None
-            groups.append((rows, utt, seq, P, G, sp, seed, (task, minlen, win)))
+            taken.update(rows)
+            groups.append((rows, req, torch.cat([self.init, req.seq[:, :req.P].to(device=self.dev, dtype=torch.int64)], dim=1)))
         if self.dirty:
-            st.upload_pages(sorted(self.dirty))
+            # one upload of the table rows this frame's releases and admissions changed, before any launch
+            m._state.upload_pages(sorted(self.dirty))
             self.dirty.clear()
         self.admitted = bool(groups)
         if not groups:
             return
-        all_rows = sorted(r for g in groups for r in g[0])
-        m.reset_streaming(streams=all_rows)
-        if st.lp_acc is None:
-            st.logprob_reset()
-        st.logprob_reset(all_rows)
-        feeds = {}
-        for rows, utt, seq, P, G, sp, seed, _ in groups:
-            feeds[rows[0]] = torch.cat([self.init, seq[:, :P].to(device=dev, dtype=torch.int64)], dim=1)
-        m.prefill_streams({r: f[:, :-1] for r, f in feeds.items()})
-        for rows, utt, seq, P, G, sp, seed, (task, minlen, win) in groups:
-            m.fork_kv(rows[0], rows[1:], P + G)
-            gid, self.groups = self.groups, self.groups + 1
+        # the init token + all prompt frames but the last only feed the KV rings; the step on the last prompt frame
+        # yields generated frame 0 (as generate)
+        admitted = sorted(taken)
+        m.reset_streaming(streams=admitted)
+        if self.codec is not None:
+            self.delay.reset(admitted)
+            self.codec.reset_streaming(streams=admitted)
+        if N > 1:
+            if m._state.lp_acc is None:
+                m._state.logprob_reset()
+            m._state.logprob_reset(admitted)
+        m.prefill_streams({rows[0]: feed[:, :-1] for rows, _, feed in groups})
+        for rows, req, feed in groups:
+            if N > 1:
+                m.fork_kv(rows[0], rows[1:], req.P + req.G)
             for i, r in enumerate(rows):
-                self.rows[r] = dict(utt=utt, P=P, G=G, g=0, start=self.n, sp=sp, cand=i, group=gid, task=task, minlen=minlen,
-                                    win=win)
+                self.rows[r] = _Row(req.utt, req.P, req.G, self.n, req.sampling, req.task, req.minlen, req.windowed,
+                                    cand=i, group=self.groups)
+                self.keys[r] = sample_seed(req.seed, i)
                 self.fresh.add(r)
-                self.keys[r] = sample_seed(seed, i)
-                self.cur[r, :, 0] = feeds[rows[0]][:, -1]
+                self.cur[r, :, 0] = feed[:, -1]
+            self.groups += 1
 
-    def _argmax(self, st: dict) -> bool:
+    def _argmax(self, st: _Row) -> bool:
         """the row's audio heads take the argmax (no candidate masks: the whole card)"""
-        sp = st["sp"] if st["sp"] is not None else (self.default or self.imp.sampling())
+        sp = st.sampling if st.sampling is not None else (self.default or self.imp.sampling())
         return sp.heads()[1][0] == 0
 
     def _upload_records(self, rows: List[int]) -> None:
@@ -654,23 +666,23 @@ class _TTSRows:
         for r in rows:
             st = self.rows[r]
             argmax = self._argmax(st)
-            kind = _lib.GEN_WINDOWED if st["win"] else _lib.GEN_FIXED
-            recs.append([st["P"], st["minlen"], st["G"], st["g"], kind | (_lib.GEN_ARGMAX if argmax else 0)])
+            kind = _lib.GEN_WINDOWED if st.windowed else _lib.GEN_FIXED
+            recs.append([st.P, st.minlen, st.G, st.g, kind | (_lib.GEN_ARGMAX if argmax else 0)])
             valid.append([self.m.config.audio_card] * self.dep_q if argmax else
-                         candidate_counts(st["P"], st["minlen"], st["g"], self.dep_q))
+                         candidate_counts(st.P, st.minlen, st.g, self.dep_q))
         self.m._state.gen_rows_set(rows, recs, valid)
 
     def frame(self, records: Optional[list] = None) -> List[Tuple]:
-        """One generated frame of every row (there must be an occupied row).  records: a list that receives the
-        frame's chunk records (row, utt, index, codes or None) when the codec runs.  -> the utterances finished:
-        (utt, codes or None, raw frames [G', 9], row state)."""
+        """One generated frame of every row (there must be an occupied row).  records: a list that receives a chunk
+        record (row, row state, frame, chunk index, has PCM) of every row the frame ran, when the codec runs.  -> the
+        rows finished: (utt, codes or None, raw frames [G', 9], row state)."""
         imp, m, B, rows = self.imp, self.m, self.B, self.rows
         occupied = self.occupied()
         mask = np.array([1 if rows[r] is not None else 0 for r in range(B)], dtype=np.int64)
         if not np.array_equal(mask, self.active):
             self.active = mask
             m.set_active_streams(self.active)
-        gen = any(rows[r]["win"] for r in occupied)
+        gen = any(rows[r].windowed for r in occupied)
         table = None
         if gen:
             # a row whose window can stop it is in the batch: the device keeps every row's window and candidate counts
@@ -681,13 +693,13 @@ class _TTSRows:
             table = torch.full((B, self.dep_q), 2048, dtype=torch.int32)
             for r in occupied:
                 st = rows[r]
-                table[r] = torch.tensor(candidate_counts(st["P"], st["minlen"], st["g"], self.dep_q), dtype=torch.int32)
+                table[r] = torch.tensor(candidate_counts(st.P, st.minlen, st.g, self.dep_q), dtype=torch.int32)
         self.gen = gen
         self.fresh.clear()
         per_row = None
         if self.default is not None:
             default = self.default
-            per_row = [default if rows[r] is None or rows[r]["sp"] is None else rows[r]["sp"] for r in range(B)]
+            per_row = [default if rows[r] is None or rows[r].sampling is None else rows[r].sampling for r in range(B)]
         extra = {"gen_rows": True} if gen else {}
         if self.n_samples > 1:
             extra["logprob"] = True
@@ -704,10 +716,7 @@ class _TTSRows:
             slot, self.status_slot = self.status_slot, self.status_slot ^ 1
             self.status[slot].copy_(m._state.gen_status[:B], non_blocking=True)
             lp = _to_host(m._state.logprob_sums()) if self.n_samples > 1 else None
-            ev = torch.cuda.Event() if self.dev.type == "cuda" else None
-            if ev is not None:
-                ev.record()
-            lagged = (self.n, slot, ev, {r: rows[r] for r in occupied if rows[r]["win"]}, lp)
+            lagged = (self.n, slot, self._event(), {r: rows[r] for r in occupied if rows[r].windowed}, lp)
         if self.codec is not None:
             self._decode(toks)
         self.history[self.n] = toks
@@ -718,40 +727,27 @@ class _TTSRows:
         # the statuses of the frame before this one: the device has this frame queued while the host waits for them
         done = self.settle(keep_open=True)
         self.lagged = lagged
-        lp = None
+        lp = {}
         if self.n_samples > 1:
-            last = [r for r in occupied if rows[r] is not None and not rows[r]["win"] and rows[r]["g"] + 1 == rows[r]["G"]]
+            last = [r for r in occupied if rows[r] is not None and not rows[r].windowed and rows[r].g + 1 == rows[r].G]
             if last:
-                # the log-probability sums of the candidates this frame finishes: one copy to pinned host memory, not
+                # the log-probability sums of the fixed rows this frame finishes: one copy to pinned host memory, not
                 # waited for here (generate_many reads it after the next frame is enqueued)
-                host = _to_host(m._state.logprob_sums()[last])
-                ev = torch.cuda.Event()
-                ev.record()
+                host, ev = _to_host(m._state.logprob_sums()[last]), self._event()
                 lp = {r: (host, i, ev) for i, r in enumerate(last)}
         for r in occupied:
             st = rows[r]
-            if st is None or st["start"] >= self.n:
+            if st is None or st.start >= self.n:
                 continue   # released above (it stopped at the frame before), or admitted after this frame
-            st["g"] += 1
-            last = st["g"] == st["G"]
-            codes = raw = None
-            if last:
+            st.g += 1
+            if st.g == st.G:
                 self._release(r)
-                if st["win"]:
-                    # its status of this frame (kept, or stopped and dropped) is read with the next frame's
-                    self.awaiting.append((r, st))
-                else:
-                    if lp is not None:
-                        st["lp"] = lp[r]
-                    st["frames"] = st["G"]
-                    raw, codes = self._result(st, r, self.n)
-                    done.append((st["utt"], codes, raw, st))
-            if records is not None and st["win"]:
-                # a windowed row's chunk is decided when it is handed out, once this frame's status has been read
-                records.append((r, st["utt"], max(st["g"] - 2, 0), st, st["g"] >= 2, self.n - 1))
-            elif records is not None and (st["g"] >= 2 or last):
+                # a windowed row's status of this frame (kept, or stopped and dropped) is read with the next frame's
+                if not st.windowed:
+                    done.append(self._finish(st, r, self.n, False, lp.get(r)))
+            if records is not None:
                 # step g - 1 >= 1 completes codec frame g - 2; an utterance of one frame has no audio
-                records.append((r, st["utt"], max(st["g"] - 2, 0), codes, st["g"] >= 2))
+                records.append((r, st, self.n - 1, max(st.g - 2, 0), st.g >= 2))
         freed = [r for r in occupied if rows[r] is None]
         if records is not None and freed:
             self.delay.reset(freed)   # a free row has no frame: the codec holds it
@@ -766,17 +762,26 @@ class _TTSRows:
             self.pages.release([r])
             self.dirty.add(r)
 
-    def _result(self, st: dict, r: int, end: int):
-        """(raw frames [G', 9] of frames start .. end - 1 of row r, codes [8, G' - 1] for the audio tasks else None)"""
-        if end > st["start"]:
-            raw = torch.stack([self.history[f][r] for f in range(st["start"], end)])
+    def _finish(self, st: _Row, r: int, end: int, stopped: bool, lp: Optional[tuple]) -> Tuple:
+        """Record the outcome of row r: frames st.start .. end - 1 kept (stopped: its stop rule fired on frame `end`), lp
+        its log-probability sums.  -> (utt, codes [8, G' - 1] for the audio tasks else None, raw frames [G', 9], st)"""
+        if end > st.start:
+            raw = torch.stack([self.history[f][r] for f in range(st.start, end)])
         else:
             raw = torch.zeros(0, self.dep_q + 1, dtype=torch.int64, device=self.dev)
-        return raw, (reverse_delay(raw[:, 1:]) if st["task"] in AUDIO_TASKS else None)
+        st.end, st.stopped, st.lp = end, stopped, lp
+        st.codes = reverse_delay(raw[:, 1:]) if st.task in AUDIO_TASKS else None
+        if stopped:
+            st.dropped = self.history[end][r]
+        return st.utt, st.codes, raw, st
 
     def _prune(self) -> None:
-        live = [st for st in self.rows if st is not None] + [st for _, st in self.awaiting]
-        first = min([st["start"] for st in live], default=self.n)
+        """drop the frames no running or unfinished row needs (a windowed row that ran its last frame is finished once
+        that frame's statuses are read)"""
+        live = [st for st in self.rows if st is not None]
+        if self.lagged is not None:
+            live += [st for st in self.lagged[3].values() if st.end is None]
+        first = min([st.start for st in live], default=self.n)
         for f in [f for f in self.history if f < first]:
             del self.history[f]
 
@@ -796,35 +801,25 @@ class _TTSRows:
             # best-of-N: each windowed frame's sums, kept while a row that ran it may still end there
             self.lp_frames = {k: v for k, v in self.lp_frames.items() if k >= f - 1}
             self.lp_frames[f] = lp
-        awaiting = {id(st): r for r, st in self.awaiting}
         for r, st in snap.items():
             stopped = int(status[r]) == _lib.GEN_STOPPED
             if self.rows[r] is st:
                 if not stopped:
                     continue
                 self._release(r)
-            elif id(st) not in awaiting:
-                continue
+            elif st.end is not None:
+                continue   # it stopped at the frame before
             end = f if stopped else f + 1
-            st["frames"] = end - st["start"]
-            st["stopped"] = stopped
-            if lp is not None:
-                # the sums after frame end - 1: this frame's copy if it is kept, else the one before (or none)
-                st["lp"] = self._lp_at(end - 1, st, r)
-            raw, codes = self._result(st, r, end)
-            st["end"], st["codes"] = end, codes
-            if stopped:
-                st["dropped"] = self.history[f][r]     # the frame its stop rule fired on (not part of the result)
-            done.append((st["utt"], codes, raw, st))
-        self.awaiting = [(r, st) for r, st in self.awaiting if "frames" not in st]
+            # the sums after frame end - 1: this frame's copy if it is kept, else the one before (or none)
+            done.append(self._finish(st, r, end, stopped, None if lp is None else self._lp_at(end - 1, st, r)))
         if not keep_open:
             self._prune()
         return done
 
-    def _lp_at(self, frame: int, st: dict, r: int):
+    def _lp_at(self, frame: int, st: _Row, r: int):
         """(host sums, row, event) of row r's log-probability sums after `frame` (zeros before its first frame); the
         copies were read by settle(), so no event is left to wait for"""
-        if frame < st["start"]:
+        if frame < st.start:
             return (torch.zeros(1, self.dep_q + 1, dtype=torch.float64), 0, None)
         return (self.lp_frames[frame], r, None)
 
@@ -842,42 +837,34 @@ class _TTSRows:
         prev, self.in_flight = self.in_flight, None
         if self.occupied():
             records = []
-            self.frame(records)
-            cuda = self.events is not None
-            records = [rec if len(rec) == 6 else rec[:3] + (None if rec[3] is None else _to_host(rec[3]), rec[4])
-                       for rec in records]
-            if cuda:
-                self.events[self.slot].record()
-            self.in_flight, self.slot = (self.slot, records), self.slot ^ 1
+            for _, _, _, st in self.frame(records):
+                if not st.windowed:
+                    st.codes = _to_host(st.codes)   # copied behind the slot's event; a windowed row's at hand-out
+            self.in_flight, self.slot = (self.slot, self._event(), records), self.slot ^ 1
         elif prev is None:
             return None
         else:
             self.settle()   # the last frame's statuses, which decide its windowed rows' chunks
         return [] if prev is None else self._hand_out(*prev)
 
-    def _hand_out(self, slot: int, records) -> List[TTSChunk]:
-        if self.events is not None:
-            self.events[slot].synchronize()
+    def _hand_out(self, slot: int, ev, records) -> List[TTSChunk]:
+        """The chunks of one frame's records, whose rows' outcomes are known by now (a windowed row's one frame late): a
+        frame before the row's last kept one gives its PCM (a row's first frame has none), the last kept frame its chunk
+        with the codes, and the frame a stop fired on (its chunk would decode the dropped frame) an empty chunk with the
+        codes instead.  Nothing comes of the frame a row ran after its stop."""
+        if ev is not None:
+            ev.synchronize()
         pcm = self.pcm[slot].numpy()
         empty = torch.zeros(0, dtype=torch.float32)
         out = []
-        for rec in records:
-            if len(rec) == 5:
-                r, utt, i, codes, has_pcm = rec
-                out.append(TTSChunk(utt, i, torch.from_numpy(pcm[r].copy()) if has_pcm else empty, codes))
-                continue
-            # a windowed row's frame f, whose status is known by now: kept (running, or its last frame, which carries the
-            # codes), the frame its stop fired on (its chunk would decode the dropped frame: an empty last chunk carries
-            # the codes instead), or the frame it ran after its stop (nothing)
-            r, utt, i, st, has_pcm, f = rec
-            end = st.get("end")
-            if end is None or f < end - 1:
+        for r, st, f, i, has_pcm in records:
+            if st.end is None or f < st.end - 1:
                 if has_pcm:
-                    out.append(TTSChunk(utt, i, torch.from_numpy(pcm[r].copy()), None))
-            elif f == end - 1:
-                out.append(TTSChunk(utt, i, torch.from_numpy(pcm[r].copy()) if has_pcm else empty, st["codes"].cpu()))
-            elif f == end:
-                out.append(TTSChunk(utt, i, empty, st["codes"].cpu()))
+                    out.append(TTSChunk(st.utt, i, torch.from_numpy(pcm[r].copy()), None))
+            elif f == st.end - 1:
+                out.append(TTSChunk(st.utt, i, torch.from_numpy(pcm[r].copy()) if has_pcm else empty, st.codes.cpu()))
+            elif f == st.end:
+                out.append(TTSChunk(st.utt, i, empty, st.codes.cpu()))
         return out
 
 
@@ -885,11 +872,11 @@ def _ranked(cands, rank: Optional[str]) -> List[Candidate]:
     """[(finished row state, codes)] of one utterance -> its Candidates ranked; waits for the copy of their sums"""
     out = []
     for st, codes in cands:
-        host, i, ev = st["lp"]
+        host, i, ev = st.lp
         if ev is not None:
             ev.synchronize()
         lp = host[i]
-        out.append(Candidate(st["cand"], codes, float(lp[1:].sum()), float(lp[0]), st["frames"]))
+        out.append(Candidate(st.cand, codes, float(lp[1:].sum()), float(lp[0]), st.frames))
     return rank_candidates(out, rank)
 
 

@@ -758,7 +758,7 @@ class TTSEngine:
             raise RstnetError(f"seq must be [{self._rows.dep_q + 1}, L], got {tuple(seq.shape)}")
         req = self.imp._request(utt_id, seq, sampling, int(seed), task, lengths)
         self.imp._check_streamed(req)
-        self._rows.fits(utt_id, req[2], req[3])
+        self._rows.fits(utt_id, req.P, req.G)
         if sampling is not None:
             self._rows.use_per_row()
         self._live.add(utt_id)

@@ -164,22 +164,22 @@ class _Pages:
             self.free += self.held.pop(r)
 
 
-def test_page_reservation_and_release_of_a_row_that_stops():
+def test_pages_of_a_stopped_row_released_when_its_status_is_read():
     """a windowed row reserves P + maxlen positions and gives them all back when its stop is learned, one frame late;
     the frames it ran after the stop are dropped from its result"""
     from rstnet_b200 import _lib
-    from rstnet_b200.infer import _TTSRows
+    from rstnet_b200.infer import _Row, _TTSRows
     rows = _TTSRows.__new__(_TTSRows)
     rows.B, rows.dep_q, rows.dev, rows.paged = 2, 8, torch.device("cpu"), True
     rows.pages = _Pages(8, 16)
     rows.m = type("M", (), {"reset_streaming": lambda self, streams: None})()
-    rows.dirty, rows.awaiting, rows.lp_frames = set(), [], {}
+    rows.dirty, rows.lp_frames = set(), {}
     imp = InferenceImp(None, None, "sampling", 0.7, 25, 0.8, 30, "TTS")
     req = imp._request("u", GT.task_sequence("ASR", 6, 14, 2, 41), None, 0, "ASR")
-    P, G = req[2], req[3]
+    P, G = req.P, req.G
     rows.pages.reserve([1], P + G)
     assert rows.pages.held[1] == rows.pages.pages_for(7 + 27)
-    st = dict(utt="u", P=P, G=G, g=4, start=3, sp=None, task="ASR", minlen=req[7], win=True)
+    st = _Row("u", P, G, 3, None, "ASR", req.minlen, True, cand=0, group=0, g=4)
     rows.rows = [None, st]
     # frames 3..8 ran (the host has enqueued frame 8); the statuses of frame 7 say row 1 stopped there
     rows.history = {f: torch.full((2, 9), f, dtype=torch.int64) for f in range(3, 9)}
@@ -189,7 +189,7 @@ def test_page_reservation_and_release_of_a_row_that_stops():
     done = rows.settle()
     assert rows.rows == [None, None] and rows.pages.free == 8 and 1 in rows.dirty
     (utt, codes, raw, fin), = done
-    assert utt == "u" and codes is None and fin["frames"] == 4 and fin["stopped"]
+    assert utt == "u" and codes is None and fin.frames == 4 and fin.stopped
     assert raw[:, 0].tolist() == [3, 4, 5, 6]      # frames 7 (stopped) and 8 (run after the stop) dropped
     assert not rows.history                        # nothing left to keep
 

@@ -434,6 +434,16 @@ int rstnet_lm_rope_pair_kv_append_paged_bf16(const void* qkv, const int64_t* off
 int rstnet_lm_rope_pair_kv_append_rows_bf16(const void* qkv, const int64_t* offset, const int32_t* row_stream, const int32_t* row_tl,
                                             void* q_out, void* kv, int32_t rows, int32_t B, int32_t H, int32_t hd, int32_t cap,
                                             const float* freqs, rstnet_stream_t stream);
+/* ---- the Kyutai pair-RoPE append with both a row map and a page table (a ragged prompt prefill of some rows of a live
+ * paged scope: LMGen.prefill_streams).  Rows, offsets and padding rows as rstnet_lm_rope_pair_kv_append_rows_bf16; the
+ * pool, table, its checks and the unmapped rule as rstnet_lm_rope_pair_kv_append_paged_bf16.  Every stored q and K/V byte
+ * equals the contiguous row-map form's for the same (stream, position); only addresses change.  Same kernel.
+ * Reference call site: moshi/models/lm.py LMGen.step's forward_text, run over the prompt's positions at once
+ * (models/model.py:364-389, modules/transformer.py:391-399). */
+int rstnet_lm_rope_pair_kv_append_paged_rows_bf16(const void* qkv, const int64_t* offset, const int32_t* row_stream,
+                                                  const int32_t* row_tl, void* q_out, void* kv, int32_t rows, int32_t B, int32_t H,
+                                                  int32_t hd, int32_t cap, const float* freqs, const int32_t* page_table,
+                                                  int32_t pages_stride, int32_t log2_page, rstnet_stream_t stream);
 /* ---- one query position per row over the ring with RingKVCache.complete's position labels and the
  * (pos_k>=0)&(delta>=0)&(delta<context) mask (llama_streaming.py:983-992), fp32 softmax. HBM-bound.  Rows and row map as
  * rstnet_lm_rope_kv_append_bf16 (padding rows write no output); every position of the launch must already be in the ring
@@ -527,6 +537,24 @@ int rstnet_lm_delay_cache_in(int64_t* cache, const int64_t* off, const int64_t* 
 int rstnet_lm_delay_cache_out(int64_t* cache, int64_t* off, const int64_t* active, const int64_t* delays,
                               const int64_t* tokens, int32_t tok_stride, int64_t* out, int32_t out_stride, int64_t* valid,
                               int32_t B, int32_t K, int32_t dep_q, int32_t CT, int32_t max_delay, rstnet_stream_t stream);
+
+/* prompt (LMGen.prefill_streams), n listed rows: row rows[i] runs lengths[i] steps of cache_in then cache_out from its
+ * current cache and off, active, with user[k - dep_q - 1] = prompt[(starts[i] + t) * prompt_stride + k] for k > dep_q and
+ * tokens[k] = the same entry for k <= dep_q at step t (the prompt in LMGen's step layout, [sum P][K] packed); the seq row
+ * cache_in forms at step t -> feed[(starts[i] + t) * feed_stride + k] (the temporal transformer's prefill input).  Then
+ * the row's cache columns, off += lengths[i] and valid = off > max_delay are written; `out` is not.  Every byte equals
+ * lengths[i] launch pairs of cache_in / cache_out on the row.  A row of length 0 is left untouched.  rows, starts and
+ * lengths are int32 HOST arrays, read at the call and carried in the launch's parameters (graph-capturable: a captured
+ * launch keeps the list).  Error returns before any launch: a null pointer, n outside [0, RSTNET_DELAY_PROMPT_MAX_ROWS],
+ * a bad shape (as cache_out; K * CT * 8 <= 48 KiB) or stride, a row outside [0, B), a row listed twice, a negative start
+ * or length.  One CTA per row of nonzero length; nothing is launched when there is none.
+ * Reference call site: moshi/models/lm.py LMGen.step (MLLM_v2/moshi/models/lm.py:398-455), P times with the sampled
+ * tokens replaced by the prompt's. */
+#define RSTNET_DELAY_PROMPT_MAX_ROWS 256
+int rstnet_lm_delay_cache_prompt(int64_t* cache, int64_t* off, int64_t* valid, const int64_t* delays, const int64_t* prompt,
+                                 int32_t prompt_stride, int64_t* feed, int32_t feed_stride, const int32_t* rows,
+                                 const int32_t* starts, const int32_t* lengths, int32_t n, int32_t B, int32_t K, int32_t dep_q,
+                                 int32_t CT, int32_t max_delay, int64_t text_init, int64_t audio_init, rstnet_stream_t stream);
 
 /* ---- segment gather / scatter: one batch row's streaming state <-> a packed staging blob (session suspend / resume).
  * A segment is `count` pieces of `bytes` at base + i * stride_bytes (device memory); in staging it occupies

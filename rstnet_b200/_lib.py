@@ -32,7 +32,8 @@ SYMBOLS = [
     "rstnet_lm_rope_kv_append_paged_bf16", "rstnet_lm_paged_decode_attention_bf16", "rstnet_lm_rope_pair_kv_append_paged_bf16",
     "rstnet_stft_loss_workspace", "rstnet_stft_loss_sums_f32", "rstnet_sisnr_moments_workspace", "rstnet_sisnr_moments_f32",
     "rstnet_segments_gather", "rstnet_segments_scatter", "rstnet_lm_rope_pair_kv_append_rows_bf16",
-    "rstnet_kv_pages_copy", "rstnet_lm_gen_rows_advance",
+    "rstnet_kv_pages_copy", "rstnet_lm_gen_rows_advance", "rstnet_lm_delay_cache_prompt",
+    "rstnet_lm_rope_pair_kv_append_paged_rows_bf16",
 ]
 
 KV_LOG2_PAGE_MIN, KV_LOG2_PAGE_MAX = 4, 12   # RSTNET_KV_LOG2_PAGE_MIN / _MAX: pages of 16 .. 4096 positions
@@ -40,6 +41,7 @@ KV_COPY_MAX_POOLS = 256                      # RSTNET_KV_COPY_MAX_POOLS
 GEN_REC = 5                                  # RSTNET_GEN_REC: int32 {pre_gen_len, minlen, maxlen, g_idx, mode} per row
 GEN_HELD, GEN_FIXED, GEN_WINDOWED, GEN_ARGMAX = 0, 1, 2, 4          # RSTNET_GEN_* row modes (mode & 3) and flag
 GEN_RUNNING, GEN_LAST, GEN_STOPPED, GEN_IDLE = 0, 1, 2, 3           # RSTNET_GEN_* frame statuses
+DELAY_PROMPT_MAX_ROWS = 256                  # RSTNET_DELAY_PROMPT_MAX_ROWS: rows of one rstnet_lm_delay_cache_prompt launch
 
 RESAMPLE_MAX_TABLE_BYTES = 48 * 1024   # RSTNET_RESAMPLE_MAX_TABLE_BYTES
 
@@ -190,6 +192,10 @@ def lib() -> C.CDLL:
     L.rstnet_segments_scatter.argtypes = [vp, i32, vp, i32, vp]
     L.rstnet_kv_pages_copy.argtypes = [vp, i32, vp, i32, i64, i32, vp]
     L.rstnet_lm_gen_rows_advance.argtypes = [vp, i32, vp, vp, i32, vp, i32, i32, i32, vp]
+    L.rstnet_lm_delay_cache_prompt.argtypes = [vp, vp, vp, vp, vp, i32, vp, i32, vp, vp, vp, i32, i32, i32, i32, i32, i32, i64, i64,
+                                               vp]
+    L.rstnet_lm_rope_pair_kv_append_paged_rows_bf16.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, i32, i32,
+                                                                vp]
     for name in SYMBOLS:
         fn = getattr(L, name)
         if fn.restype is C.c_int and name not in ("rstnet_version",):

@@ -1022,6 +1022,17 @@ extern "C" int rstnet_lm_rope_pair_kv_append_rows_bf16(const void* qkv, const in
   return rope_pair_kv_append(qkv, offset, 1, q_out, kv, rows, B, H, hd, cap, freqs, nullptr, 0, 0, row_stream, row_tl, stream);
 }
 
+extern "C" int rstnet_lm_rope_pair_kv_append_paged_rows_bf16(const void* qkv, const int64_t* offset, const int32_t* row_stream,
+                                                             const int32_t* row_tl, void* q_out, void* kv, int32_t rows, int32_t B,
+                                                             int32_t H, int32_t hd, int32_t cap, const float* freqs,
+                                                             const int32_t* page_table, int32_t pages_stride, int32_t log2_page,
+                                                             rstnet_stream_t stream) {
+  RSTNET_REQUIRE(row_stream && row_tl, "lm_rope_pair_kv_append_paged_rows: null row map");
+  if (check_pages("lm_rope_pair_kv_append_paged_rows", page_table, pages_stride, log2_page, cap)) return 1;
+  return rope_pair_kv_append(qkv, offset, 1, q_out, kv, rows, B, H, hd, cap, freqs, page_table, pages_stride, log2_page, row_stream,
+                             row_tl, stream);
+}
+
 static int ring_decode_attention(const void* q, const void* kv, const int64_t* offset, int32_t offset_stride,
                                  const int32_t* row_stream, const int32_t* row_tl, void* out, int32_t rows, int32_t B, int32_t n_head,
                                  int32_t n_kv, int32_t hs, int32_t cap, int32_t context, const int32_t* page_table,

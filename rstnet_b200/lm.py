@@ -1633,9 +1633,10 @@ class _LMState:
                 raise RstnetError(f"stream index {s} outside [0, {self.B})")
             if p.dim() != 2 or p.shape[0] != K:
                 raise RstnetError(f"the prompt of stream {s} must be [{K}, T], got {tuple(p.shape)}")
-            if p.shape[1] > self.m.max_seq_length:
+            # the GPT's length and RoPE-table limits (the Moshi twin computes its angles and has neither)
+            if self.cos is not None and p.shape[1] > self.m.max_seq_length:
                 raise ValueError(f"Cannot forward sequence of length {p.shape[1]}, max seq length is only {self.m.max_seq_length}.")
-            if int(self.pos_host[s]) + p.shape[1] > self.cos.shape[0]:
+            if self.cos is not None and int(self.pos_host[s]) + p.shape[1] > self.cos.shape[0]:
                 raise IndexError(f"position {int(self.pos_host[s]) + p.shape[1] - 1} of stream {s} is beyond block_size = "
                                  f"{self.cos.shape[0]} (RoPE table exhausted; reset the stream or raise Config.block_size)")
             if self.pages is not None:

@@ -84,13 +84,17 @@ class _MoshiState(_LMState):
         return 1   # the pair-RoPE and attention launches index the counters per stream, even with B == 1
 
     def _rope_kv(self, L, l: int, ost: int, rs, rt, pg, st) -> None:
-        """layer l's pair-RoPE at the positions' fp32 angles and the K/V append; a row-mapped chunk (row_chunk, contiguous
-        rings only) runs the row-map entry point"""
+        """layer l's pair-RoPE at the positions' fp32 angles and the K/V append; a row-mapped chunk (row_chunk) runs a
+        row-map entry point, the paged one on a paged scope"""
         c = self.c
-        if self.row_mapped:
+        if self.row_mapped and self.pages is None:
             _lib.check(L.rstnet_lm_rope_pair_kv_append_rows_bf16(self.qkv.data_ptr(), self.offset.data_ptr(), rs, rt, self.q.data_ptr(),
                                                                  self.kv[l].data_ptr(), self.M, self.B, c.n_head, c.head_size, self.cap,
                                                                  self.freqs.data_ptr(), st), "rope_pair_kv_rows")
+        elif self.row_mapped:
+            _lib.check(L.rstnet_lm_rope_pair_kv_append_paged_rows_bf16(
+                self.qkv.data_ptr(), self.offset.data_ptr(), rs, rt, self.q.data_ptr(), self.kv[l].data_ptr(), self.M, self.B, c.n_head,
+                c.head_size, self.cap, self.freqs.data_ptr(), *pg, st), "rope_pair_kv_paged_rows")
         else:
             rope = L.rstnet_lm_rope_pair_kv_append_bf16 if self.pages is None else L.rstnet_lm_rope_pair_kv_append_paged_bf16
             _lib.check(rope(self.qkv.data_ptr(), self.offset.data_ptr(), ost, self.q.data_ptr(), self.kv[l].data_ptr(), self.M, self.B,
@@ -235,6 +239,16 @@ class LMModel(_DecodeModel):
             raise RstnetError("streaming forward_text takes one frame per call")
         out, logits = self._st().forward_global(sequence)
         return out, logits[:, None]                                  # [B,1,dim], [B,1,1,text_card]
+
+    @torch.no_grad()
+    @on_own_device
+    def prefill_streams(self, feeds) -> None:
+        """Inside a streaming scope (contiguous or paged): feed each listed stream its own input frames, feeds {stream:
+        int64 [K, T_s]}, through the temporal transformer only (KV and position counter advance by T_s; no text head, no
+        depth steps).  The other streams are untouched.  The frames of all listed streams are packed into ragged chunks
+        of at most MAX_ROWS rows (GPT.prefill_streams' row map).  On a paged scope each stream must hold pages for the
+        positions it writes, or this raises before any launch."""
+        self._st().prefill_streams(feeds)
 
     @torch.no_grad()
     @on_own_device
@@ -456,6 +470,68 @@ class LMGen(nn.Module):
         return ("lmgen",) + key, step
 
     @torch.no_grad()
+    def prefill_streams(self, prompts) -> None:
+        """Extension: start rows from prompts {row: int64 [K, P]} in the step layout (`prompt_from_aligned`): rows 0..dep_q
+        the tokens the row takes as sampled at steps 0..P-1, rows dep_q+1..K-1 the user tokens of those steps.  Afterwards
+        the row is in the state P calls of `step` would leave it in had the sampler returned prompt[:dep_q + 1, t] at step
+        t: the KV of its positions, its position counter, its delay-cache columns, step count and valid flag, and its
+        per-row sampler step count (+P).  Nothing is reset: restart the rows first (reset_streaming(streams=...)) as for
+        any admission; a row is taken from wherever it is.  A row with P = 0 is left as it is; every row not listed --
+        live, held or mid-generation -- is untouched.  One rstnet_lm_delay_cache_prompt launch writes the cache and the
+        temporal transformer's inputs, then ragged prefill chunks (the row map of LMModel.prefill_streams) run them.  On a paged scope
+        each row must hold pages for min(P, context) more positions, or this raises before any launch."""
+        todo = self._prompt_begin(prompts)
+        while todo:
+            todo = self._prompt_chunk(todo)
+
+    def _prompt_begin(self, prompts) -> list:
+        """prefill_streams up to the ragged prefill: checks, the delay-cache prompt launch, the host mirrors and step
+        counts.  -> the prefill's work list for `_prompt_chunk` ([row, feed [P, K], positions fed]); until it is empty the
+        rows must not step."""
+        st = self._require()
+        lm, ms = self.lm_model, st.lm
+        K, dev = lm.num_codebooks, lm.device
+        rows, parts = [], []
+        for r, p in prompts.items():
+            r = int(r)
+            if not 0 <= r < st.B:
+                raise RstnetError(f"stream index {r} outside [0, {st.B})")
+            if not torch.is_tensor(p) or p.dim() != 2 or p.shape[0] != K or p.dtype.is_floating_point or p.dtype == torch.bool:
+                raise RstnetError(f"the prompt of row {r} must be an integer tensor [{K}, P], got "
+                                  f"{tuple(p.shape) if torch.is_tensor(p) else type(p).__name__}")
+            if r in rows:
+                raise RstnetError(f"row {r} is listed twice")
+            rows.append(r)
+            parts.append(p)
+        lens = np.array([p.shape[1] for p in parts], dtype=np.int64)
+        if ms.pages is not None:
+            for r, n in zip(rows, lens):
+                ms.pages.check([r], [ms.pos_host[r]], int(n))
+        keep = [i for i in range(len(rows)) if lens[i] > 0]
+        if not keep:
+            return []
+        rows, parts, lens = [rows[i] for i in keep], [parts[i] for i in keep], lens[keep]
+        prompt = torch.cat([p.to(device=dev, dtype=torch.int64).t() for p in parts]).contiguous()     # [sum P, K]
+        feed = torch.empty_like(prompt)
+        starts = np.concatenate([[0], np.cumsum(lens)[:-1]])
+        r32, s32, l32 = (np.ascontiguousarray(a, dtype=np.int32) for a in (rows, starts, lens))
+        _lib.check(_lib.lib().rstnet_lm_delay_cache_prompt(
+            st.cache.data_ptr(), st.off.data_ptr(), st.valid.data_ptr(), self.delays_cuda.data_ptr(), prompt.data_ptr(), K,
+            feed.data_ptr(), K, r32.ctypes.data, s32.ctypes.data, l32.ctypes.data, len(rows), st.B, K, lm.dep_q,
+            st.cache.shape[2], self.max_delay, lm.text_initial_token_id, lm.initial_token_id, ops._stream()), "delay_cache_prompt")
+        ms._cow(rows, ms.pos_host[rows], lens)
+        st.off_host[rows] += lens
+        idx = torch.tensor(rows, dtype=torch.int64, device=dev)
+        ms.row_step.index_add_(0, idx, torch.from_numpy(lens).to(dev))
+        return [[r, feed[int(a):int(a) + int(n)], 0] for r, a, n in zip(rows, starts, lens)]
+
+    def _prompt_chunk(self, todo) -> list:
+        """One ragged prefill chunk (at most MAX_ROWS rows, entries in order) of `_prompt_begin`'s work lists (several
+        may be concatenated).  -> the entries not yet complete."""
+        self._require().lm.row_chunk(todo)
+        return [it for it in todo if it[2] < it[1].shape[0]]
+
+    @torch.no_grad()
     def step(self, input_tokens: torch.Tensor) -> Optional[torch.Tensor]:
         """One step of every active row: -> [B, dep_q + 1, 1] in the delayed layout, or None while every row is still in
         its `max_delay` warm-up steps.  One input copy and one graph replay."""
@@ -483,6 +559,169 @@ class LMGen(nn.Module):
         if not (st.off_host > self.max_delay).any():
             return None
         return st.out[:, :, None].clone()
+
+
+# ------------------------------------------------------------------------------------------- prompted generation
+def prompt_from_aligned(seq: torch.Tensor, P: int, delays, dep_q: int, initial: int = -2) -> torch.Tensor:
+    """Aligned dialogue codes seq [K, L] (rows: text, Moshi's audio codebooks 1..dep_q, then the user's audio; frame t of
+    every row is time t) -> the prompt of its first P frames in LMGen's step layout, int64 [K, P], for
+    LMGen.prefill_streams: forced[k, t] = seq[k, t - delays[k]] for k <= dep_q and t >= delays[k] (the token the delayed
+    codebook k is sampled as at step t), `initial` where t < delays[k] (never read: LMGen feeds its initial token
+    there); user[k, t] = seq[k, t] for k > dep_q (LMGen delays them itself).  P may be any length from 0 to L.
+
+    The step layout lags codebook k by delays[k]: after the prompt, aligned frames P - max_delay .. P - 1 are only partly
+    in it (codebook k holds frames < P - delays[k]).  The first max_delay steps after the prompt return aligned frames
+    P - max_delay .. P - 1, whose codebooks with t + delays[k] >= P are newly sampled; steps P .. L - 1 return aligned
+    frames P - max_delay .. L - 1 - max_delay."""
+    if not torch.is_tensor(seq) or seq.dim() != 2 or seq.dtype.is_floating_point:
+        raise RstnetError("seq must be an integer tensor [K, L]")
+    K, L = seq.shape
+    delays = [int(d) for d in delays]
+    if len(delays) != K or min(delays) < 0:
+        raise RstnetError(f"{len(delays)} delays (each >= 0) for K = {K} codebooks")
+    if not 0 <= dep_q < K:
+        raise RstnetError(f"dep_q = {dep_q} outside [0, {K})")
+    P = int(P)
+    if not 0 <= P <= L:
+        raise RstnetError(f"P = {P} outside [0, {L}]")
+    out = torch.full((K, P), int(initial), dtype=torch.int64, device=seq.device)
+    for k in range(dep_q + 1):
+        d = delays[k]
+        if P > d:
+            out[k, d:] = seq[k, :P - d]
+    out[dep_q + 1:] = seq[dep_q + 1:, :P]
+    return out
+
+
+def _item(item, K: int):
+    try:
+        utt, seq, P = item
+    except (TypeError, ValueError):
+        raise RstnetError("an item is (utt_id, seq [K, L], P)") from None
+    if not torch.is_tensor(seq) or seq.dim() != 2 or seq.shape[0] != K or seq.dtype.is_floating_point:
+        raise RstnetError(f"item {utt!r}: seq must be an integer tensor [{K}, L], got "
+                          f"{tuple(seq.shape) if torch.is_tensor(seq) else type(seq).__name__}")
+    if isinstance(P, bool) or not isinstance(P, (int, np.integer)) or not 0 <= int(P) < seq.shape[1]:
+        raise RstnetError(f"item {utt!r}: P = {P!r} must be an int in [0, L = {seq.shape[1]})")
+    return utt, seq, int(P)
+
+
+@torch.no_grad()
+def generate_many(gen: LMGen, items, capacity: int, *, seeds=None, sampling=None, kv_pages: Optional[int] = None,
+                  stats: Optional[dict] = None):
+    """Continuous batching of prompted Moshi generation over (utt_id, seq [K, L], P) items, seq aligned dialogue codes
+    (prompt_from_aligned's layout), 0 <= P < L: yields (utt_id, out int64 [dep_q + 1, L - P]) in completion order, out
+    being the aligned frames `LMGen.step` returned at steps P .. L - 1 (column j: aligned frame P + j - max_delay;
+    the columns of steps below max_delay carry no frame).  An item's row is prefilled with its first P frames
+    (LMGen.prefill_streams; rows admitted together share ragged chunks), then steps once per frame, fed its own
+    recorded user tokens seq[dep_q + 1:, t] at step t, and finishes after step L - 1.
+
+    Up to `capacity` items are live, one row each of an `LMGen.streaming(capacity)` scope the call opens (the generator
+    must not be streaming) and closes; one graph replay per frame.  Every row samples with its own settings
+    (sampling {utt_id: Sampling}; default the generator's) and random stream (seeds {utt_id: int}; default 0): an item's
+    output depends on its seed and settings only, not on its row, its admission or the other items, at a given capacity.
+    kv_pages N: a paged scope of N pages of KV_PAGE positions; an item holds pages for min(L, context) positions while it
+    is live, and waits for them while a row is free (an item needing more than the pool raises).  Paged and contiguous
+    scopes give the same tokens.  stats: a dict that receives 'frames' (steps run), 'row_frames' (live rows summed over
+    steps) and 'prefill_rows' (prompt frames prefilled)."""
+    lm = gen.lm_model
+    K, dq = lm.num_codebooks, lm.dep_q
+    Ku = K - dq - 1
+    if isinstance(capacity, bool) or not isinstance(capacity, int) or not 1 <= capacity <= MAX_STREAMS:
+        raise RstnetError(f"capacity must be an int in [1, {MAX_STREAMS}] (got {capacity!r})")
+    if gen.is_streaming:
+        raise RstnetError("generate_many opens its own streaming scope: call it on a generator that is not streaming")
+    for name, d in (("seeds", seeds), ("sampling", sampling)):
+        if d is not None and not isinstance(d, dict):
+            raise RstnetError(f"{name} must be a dict keyed by utt_id")
+    for s in (sampling or {}).values():
+        if not isinstance(s, Sampling):
+            raise RstnetError(f"sampling values must be Sampling (got {type(s).__name__})")
+    seeds, sampling = seeds or {}, sampling or {}
+    dev = lm.device
+    counts = dict(frames=0, row_frames=0, prefill_rows=0)
+    it = iter(items)
+    nxt = None
+    gen.streaming_forever(capacity, kv_pages=kv_pages)
+    try:
+        st = gen._st
+        gen.set_stream_sampling([])                 # per-row settings and random streams from the start
+        pages = st.lm.pages
+        free = list(range(capacity))
+        live = {}                                    # row -> (utt_id, L, P, index of its first step in `hist`)
+        ubuf = torch.zeros(capacity, Ku, 1, dtype=torch.int64, device=dev)   # each row's user tokens by step
+        hist: List[torch.Tensor] = []                # st.out after each step, from global step `base` on
+        base = 0
+        mask = None
+        done = False
+        while True:
+            admitted = {}
+            while free and not done:
+                if nxt is None:
+                    try:
+                        nxt = _item(next(it), K)
+                    except StopIteration:
+                        done = True
+                        break
+                utt, seq, P = nxt
+                L = seq.shape[1]
+                if pages is not None:
+                    need = pages.pages_for(min(L, lm.context))
+                    if need > pages.n_pages:
+                        raise RstnetError(f"item {utt!r} needs {need} KV pages, the pool has {pages.n_pages}")
+                    if need > pages.free:
+                        break
+                r = free.pop(0)
+                gen.reset_streaming(streams=[r])
+                gen.set_stream_sampling([r], sampling.get(utt), seeds.get(utt, 0))
+                if pages is not None:
+                    gen.reserve_kv([r], L)
+                seq = seq.to(device=dev, dtype=torch.int64)
+                if L > ubuf.shape[2]:
+                    grown = torch.zeros(capacity, Ku, L, dtype=torch.int64, device=dev)
+                    grown[:, :, :ubuf.shape[2]] = ubuf
+                    ubuf = grown
+                ubuf[r, :, :L] = seq[dq + 1:]
+                admitted[r] = prompt_from_aligned(seq, P, lm.delays, dq)
+                live[r] = (utt, L, P, base + len(hist))
+                nxt = None
+            if admitted:
+                gen.prefill_streams(admitted)
+                counts["prefill_rows"] += sum(p.shape[1] for p in admitted.values())
+            if not live:
+                if not done:
+                    raise RstnetError("no item could be admitted into an empty scope")
+                break
+            rows = sorted(live)
+            want = np.zeros(capacity, dtype=np.int64)
+            want[rows] = 1
+            if mask is None or not np.array_equal(mask, want):
+                gen.set_active_streams(want)
+                mask = want
+            # each row's user tokens at its own step count (held rows read a clamped column and are not stepped)
+            idx = st.off.clamp(max=ubuf.shape[2] - 1)[:, None, None].expand(capacity, Ku, 1)
+            gen.step(ubuf.gather(2, idx))
+            hist.append(st.out.clone())
+            counts["frames"] += 1
+            counts["row_frames"] += len(rows)
+            for r in rows:
+                utt, L, P, first = live[r]
+                if int(st.off_host[r]) == L:
+                    del live[r]
+                    if pages is not None:
+                        gen.release_kv([r])
+                    free.append(r)
+                    free.sort()
+                    out = torch.stack(hist[first - base:], 2)[r]        # [dep_q + 1, L - P]
+                    yield utt, out.cpu()
+            first = min((v[3] for v in live.values()), default=base + len(hist))
+            del hist[:first - base]
+            base = first
+    finally:
+        gen._st = None
+        lm._state = None
+        if stats is not None:
+            stats.update(counts)
 
 
 # ------------------------------------------------------------------------------------------- teacher-forced scoring

@@ -26,6 +26,10 @@
     with a codec, one 24 kHz 16-bit wav per utterance (Mimi decode of equal-length groups, as main()'s detokenize).
     `synthesize_stream` / `synthesize --stream`: the same codes through InferenceImp.stream_many, each wav decoded frame by
     frame during generation and written when its utterance completes.
+  * `continue --model moshi` / `continue_corpus`: generation from a Moshi fine-tune over recorded dialogues (`torch.save`d
+    dict utt_id -> int64 [n_q + 1, L], aligned): each prompted with its first --prompt-frames frames, then fed its
+    recorded user channel, with moshi.generate_many; writes utt_id -> int64 [dep_q + 1, L - P] and, with a codec, the
+    wavs of Moshi's audio channel through MimiCodec.decode_many.
 
 Audio at any integer sample rate is resampled to 24 kHz on the GPU the way the reference does it,
 torchaudio.transforms.Resample(sr, 24000) with its defaults (mimi_tokenizer.py:40,67; inference.py:24-34 `convert_audio`:
@@ -262,6 +266,13 @@ def _positive_float(text: str) -> float:
     return v
 
 
+def _nonnegative_int(text: str) -> int:
+    v = int(text)
+    if v < 0:
+        raise argparse.ArgumentTypeError(f"must be an integer >= 0 (got {text})")
+    return v
+
+
 def _load_gpt(config_path: str, checkpoint: str, device: str):
     """GPT(Config from json) with the checkpoint's ['model'] weights, `module.` prefixes stripped
     (utils/train_utils.py:resume_for_inference), in bf16 on `device`."""
@@ -380,6 +391,49 @@ def _score_cli(args) -> int:
     return 0
 
 
+@torch.no_grad()
+def continue_corpus(gen, corpus: Dict[str, torch.Tensor], prompt_frames: int, capacity: int, kv_pages=None,
+                    seed: int = 0) -> Dict[str, torch.Tensor]:
+    """{utt: int64 [dep_q + 1, L - P]} of moshi.generate_many over `corpus` ({utt: int64 [K, L]} aligned dialogue codes),
+    every item prompted with its first P = prompt_frames frames and seeded with `seed`."""
+    from .moshi import generate_many
+    items = [(utt, torch.as_tensor(seq), prompt_frames) for utt, seq in corpus.items()]
+    seeds = {utt: seed for utt, _, _ in items}
+    return dict(generate_many(gen, items, capacity, seeds=seeds, kv_pages=kv_pages))
+
+
+def continuation_wavs(codec: MimiCodec, out: Dict[str, torch.Tensor], prompt_frames: int, max_delay: int, dep_q: int,
+                      capacity: int = 64):
+    """{utt: float32 wav} of Moshi's audio channel in `continue_corpus`'s outputs through MimiCodec.decode_many: the
+    columns that carry an aligned frame (step >= max_delay), audio codebooks 1..dep_q clamped to the codebook."""
+    j0 = max(0, max_delay - prompt_frames)
+    items = [(u, o[1:dep_q + 1, j0:].clamp(0, codec.codebook_size - 1)) for u, o in out.items() if o.shape[1] > j0]
+    return dict(codec.decode_many(items, capacity))
+
+
+def _continue_cli(args) -> int:
+    from .lm import kv_pages_for_budget
+    from .moshi import LMGen
+    model = _load_moshi(args.config, args.checkpoint, args.device)
+    gen = LMGen(model, use_sampling=args.use_sampling, temp=args.temp, temp_text=args.temp_text, top_k=args.top_k,
+                top_k_text=args.top_k_text)
+    corpus = torch.load(args.input, map_location="cpu")
+    kv_pages = None if args.kv_gb is None else kv_pages_for_budget(model.config, args.kv_gb)
+    out = continue_corpus(gen, corpus, args.prompt_frames, args.capacity, kv_pages=kv_pages, seed=args.seed)
+    torch.save(out, args.output_file)
+    print(f"continued {len(out)} dialogues -> {args.output_file}")
+    if args.wav_dir:
+        if not args.codec_checkpoint:
+            raise SystemExit("--wav-dir needs --codec-checkpoint")
+        codec = _load_codec(argparse.Namespace(weights=args.codec_checkpoint, config=args.codec_config, device=args.device))
+        os.makedirs(args.wav_dir, exist_ok=True)
+        wavs = continuation_wavs(codec, out, args.prompt_frames, max(model.delays), model.dep_q)
+        for utt, w in wavs.items():
+            write_wav(os.path.join(args.wav_dir, f"{utt}_sample.wav"), w, codec.sample_rate)
+        print(f"wrote {len(wavs)} wavs -> {args.wav_dir}")
+    return 0
+
+
 def _load_codec(args) -> MimiCodec:
     import json
     cfg = json.load(open(args.config)) if args.config else dict(encoder_rates=[8, 6, 5, 4], codebook_size=2048, codebook_dim=256, rvq_layers=8)
@@ -433,6 +487,8 @@ def main(argv=None) -> int:
         return _synthesize_cli(args)
     if args.cmd == "score":
         return _score_cli(args)
+    if args.cmd == "continue":
+        return _continue_cli(args)
     codec = _load_codec(args)
     if args.cmd == "tokenize":
         def items():
@@ -516,6 +572,28 @@ def build_parser() -> argparse.ArgumentParser:
                                                        "bare state_dict)")
     p.add_argument("--output-file", required=True, help="json file of per-utterance metrics")
     p.add_argument("--capacity", type=int, default=8, help="utterances packed into the same chunks (<= 256)")
+    p.add_argument("--device", default="cuda")
+    p = sub.add_parser("continue", help="continue recorded dialogues with a Moshi fine-tune: each prompted with its first "
+                                        "--prompt-frames frames, then fed its recorded user channel (moshi.generate_many)")
+    p.add_argument("--model", choices=("moshi",), required=True, help="the Moshi-style LMModel (--config: its kwargs)")
+    p.add_argument("--config", required=True, help="json with the LMModel constructor kwargs")
+    p.add_argument("--checkpoint", required=True, help="a state_dict or {'model': state_dict}")
+    p.add_argument("--input", required=True, help="torch.save'd dict utt_id -> int64 [n_q + 1, L], aligned (text, Moshi "
+                                                  "audio, user audio)")
+    p.add_argument("--prompt-frames", type=_nonnegative_int, required=True, help="P: frames of each dialogue taken as the prompt (< L)")
+    p.add_argument("--output-file", required=True, help="torch.save'd dict utt_id -> int64 [dep_q + 1, L - P]")
+    p.add_argument("--capacity", type=int, default=32, help="dialogues generated together (<= 256)")
+    p.add_argument("--kv-gb", type=_positive_float, default=None,
+                   help="KV cache budget in GiB (paged; default: a whole context ring per row)")
+    p.add_argument("--seed", type=int, default=0, help="every dialogue's random stream")
+    p.add_argument("--use-sampling", action=argparse.BooleanOptionalAction, default=True)
+    p.add_argument("--temp", type=float, default=0.8)
+    p.add_argument("--top-k", type=int, default=250)
+    p.add_argument("--temp-text", type=float, default=0.7)
+    p.add_argument("--top-k-text", type=int, default=25)
+    p.add_argument("--wav-dir", default=None, help="also write <utt_id>_sample.wav of Moshi's audio (needs --codec-checkpoint)")
+    p.add_argument("--codec-checkpoint", default=None)
+    p.add_argument("--codec-config", default=None, help="json with the MimiCodec constructor arguments")
     p.add_argument("--device", default="cuda")
     p = sub.add_parser("evaluate", help="multi-resolution STFT loss and SI-SNR of degraded wavs against references "
                                         "(Evaluation/codec/compute_ms_stft_loss.py, compute_sisnr.py)")

@@ -92,27 +92,42 @@ class FrameScheduler:
         self.ticks = 0
 
     # ---- session lifecycle
-    def admit(self, session: Hashable, sampling=None, seed: Optional[int] = None) -> int:
+    def admit(self, session: Hashable, sampling=None, seed: Optional[int] = None, prompt=None) -> int:
         """Lease the lowest free row to `session` and restart that row's streaming state (server.py:156-158 does
         `mimi.reset_streaming(); lm_gen.reset_streaming()` for its single session).  sampling (an lm.Sampling) / seed:
         the session's own settings and random stream, passed to the engine's reset_rows; None: the engine's defaults.
         Once any session brought settings, a session's random stream is its seed alone (None: 0): pass distinct seeds to
-        keep sessions with the same settings and input apart."""
+        keep sessions with the same settings and input apart.
+
+        prompt (a MoshiDuplexEngine only): int64 [K, P] in LMGen's step layout (moshi.prompt_from_aligned), the frames
+        the session starts from (MoshiDuplexEngine.reset_rows).  Its prefill is spread over the following ticks, one
+        ragged chunk of at most MAX_ROWS rows per tick (packing the pending prompts of every session admitted so), run
+        before the tick's step; until it is complete the session is held and its pushed frames queue.  A paged engine
+        needs kv_pages_for(P + 1) + kv_headroom free pages."""
         if session in self._row_of:
             raise RuntimeError(f"session {session!r} is already admitted")
         if not self._free:
             raise RuntimeError("no free row: the batch is full")
-        if self.paged and self.engine.kv_pages_free < 1 + self.kv_headroom:
+        P = 0
+        if prompt is not None:
+            if not hasattr(self.engine, "check_prompt"):
+                raise RstnetError("prompts are a MoshiDuplexEngine feature: this engine starts sessions empty")
+            P = self.engine.check_prompt(prompt)
+        need = (self.engine.kv_pages_for(P + 1) if prompt is not None and self.paged else 1) + self.kv_headroom
+        if self.paged and self.engine.kv_pages_free < need:
             raise RuntimeError(f"the KV pool is short: {self.engine.kv_pages_free} pages free, admission needs "
-                               f"1 + {self.kv_headroom} (kv_headroom)")
+                               f"{need - self.kv_headroom} + {self.kv_headroom} (kv_headroom)")
         self._free.sort()
-        row = self._free.pop(0)
-        self._row_of[session] = row
-        self._queue[session] = deque()
-        if sampling is None and seed is None:
+        row = self._free[0]
+        if prompt is not None:
+            self.engine.start_rows([row], sampling=sampling, seed=seed, prompts={row: prompt})
+        elif sampling is None and seed is None:
             self.engine.reset_rows([row])
         else:
             self.engine.reset_rows([row], sampling=sampling, seed=seed)
+        self._free.pop(0)
+        self._row_of[session] = row
+        self._queue[session] = deque()
         return row
 
     def release(self, session: Hashable) -> None:
@@ -123,6 +138,8 @@ class FrameScheduler:
         row = self._row_of.pop(session)
         self._queue.pop(session, None)
         self._free.append(row)
+        if row in self._prefilling():
+            self.engine.drop_prefill([row])
         if self.paged:
             self.engine.release_rows([row])
 
@@ -135,6 +152,8 @@ class FrameScheduler:
         """Pack the session's state into host memory (engine.suspend_rows) and free its row and pages; its queue stays.
         -> its SessionState."""
         row = self._row_of[session]
+        if row in self._prefilling():
+            raise RuntimeError(f"session {session!r} is still prefilling its prompt")
         state = self.engine.suspend_rows([row])[0]
         del self._row_of[session]
         self._free.append(row)
@@ -187,11 +206,18 @@ class FrameScheduler:
         """Queue one 80 ms frame (1920 samples) of the session's input audio."""
         self._queue[session].append(frame)
 
+    def _prefilling(self):
+        return getattr(self.engine, "prefilling", frozenset())
+
     def tick(self) -> Dict[Hashable, Tuple]:
-        """One scheduler period: step every session that has a frame queued; returns {session: (tokens, pcm)}."""
+        """One scheduler period: one chunk of the pending prompt prefills, if any, then step every session that has a
+        frame queued and no prefill left; returns {session: (tokens, pcm)}."""
         if self.on_short == "suspend" and self._suspended:
             self._resume_waiting()
-        ready = {s: r for s, r in self._row_of.items() if self._queue[s]}
+        if self._prefilling():
+            self.engine.prefill_chunk()
+        held = self._prefilling()
+        ready = {s: r for s, r in self._row_of.items() if self._queue[s] and r not in held}
         self.ticks += 1
         if self.paged and ready:
             short = set(self.engine.grow_kv(list(ready.values())))     # admission order: the oldest sessions grow first
@@ -350,6 +376,9 @@ class _DuplexCore(_PagedRows):
             raise RstnetError(f"sampling must be a Sampling (got {type(sampling).__name__})")
         self._wait_rows(rows)
         self._reserve_first_page(rows)
+        self._restart(rows, sampling, seed)
+
+    def _restart(self, rows, sampling, seed) -> None:
         self.codec.reset_streaming(streams=list(rows))
         self._reset_lm_rows(rows, sampling, seed)
         if self.up is not None:
@@ -615,6 +644,13 @@ class DuplexEngine(_DuplexCore):
         self.row_keys[r] = host["key"]
         self._keys_dirty = True
 
+    def reset_rows(self, rows, sampling=None, seed: Optional[int] = None, prompts=None) -> None:
+        """_DuplexCore.reset_rows; prompts are a Moshi engine's (MoshiDuplexEngine.reset_rows): here they raise and change
+        nothing."""
+        if prompts is not None:
+            raise RstnetError("prompts are a MoshiDuplexEngine feature: the GPT duplex engine starts sessions empty")
+        super().reset_rows(rows, sampling, seed)
+
     def _reset_lm_rows(self, rows, sampling, seed) -> None:
         if sampling is not None or seed is not None or self.row_sampling is not None:
             default = Sampling(*self._defaults)
@@ -664,6 +700,7 @@ class MoshiDuplexEngine(_DuplexCore):
             raise RstnetError(f"the codec emits {codec.n_q} codes per frame, the LM takes {n_user} user codebooks")
         super().__init__(codec, lm_gen, lm, capacity, sample_rate, kv_pages, kv_page, lm.dep_q)
         self.lm_gen = lm_gen
+        self._prefill: list = []      # LMGen._prompt_begin work lists of the rows still prefilling
         self.dec_mask_host = torch.zeros(capacity, dtype=torch.int64, pin_memory=self.dev.type == "cuda")
         self.dec_mask_dev = torch.zeros(capacity, dtype=torch.int64, device=self.dev)
 
@@ -686,6 +723,64 @@ class MoshiDuplexEngine(_DuplexCore):
         g._st.lm.pos_host[r] = host["pos"]
         g._st.off_host[r], g._st.stepped[r] = host["off"], host["stepped"]
         g._row_sampling[r] = host["sampling"] if host["sampling"] is not None else g.default_sampling()
+
+    # ---- prompted sessions
+    def check_prompt(self, prompt) -> int:
+        """-> P of a prompt int64 [K, P] in LMGen's step layout; raises RstnetError on another shape or dtype"""
+        K = self.lm_gen.lm_model.num_codebooks
+        if not torch.is_tensor(prompt) or prompt.dim() != 2 or prompt.shape[0] != K or prompt.dtype.is_floating_point \
+                or prompt.dtype == torch.bool:
+            raise RstnetError(f"a prompt is an integer tensor [{K}, P], got "
+                              f"{tuple(prompt.shape) if torch.is_tensor(prompt) else type(prompt).__name__}")
+        return int(prompt.shape[1])
+
+    def reset_rows(self, rows, sampling=None, seed: Optional[int] = None, prompts=None) -> None:
+        """Restart `rows` (_DuplexCore.reset_rows).  prompts {row: int64 [K, P]} (LMGen's step layout,
+        moshi.prompt_from_aligned) start those rows from their prompts: LMGen.prefill_streams after the restart, so their
+        first step is the one P steps of LMGen.step with the prompt's tokens forced would have reached.  On a paged engine
+        a prompted row is given pages for P + 1 positions first (all rows or none: a short pool raises and changes
+        nothing).  The codec rows start from a reset state, as for any new session: the prompt's audio does not prime
+        the decoder or the encoder."""
+        self.start_rows(rows, sampling, seed, prompts)
+        while self._prefill:
+            self.prefill_chunk()
+
+    def start_rows(self, rows, sampling=None, seed: Optional[int] = None, prompts=None) -> None:
+        """reset_rows without running the prefill: the prompted rows are `prefilling` until `prefill_chunk` calls have
+        run it (FrameScheduler runs one per tick); they must not step until then."""
+        if sampling is not None and not isinstance(sampling, Sampling):
+            raise RstnetError(f"sampling must be a Sampling (got {type(sampling).__name__})")
+        rows = [int(r) for r in rows]
+        prompts = {int(r): p for r, p in (prompts or {}).items()}
+        if any(r not in rows for r in prompts):
+            raise RstnetError("every prompted row must be one of the rows restarted")
+        lens = {r: self.check_prompt(p) for r, p in prompts.items()}
+        self._wait_rows(rows)
+        if self._kv_lm is not None and prompts:
+            # all or nothing, before anything changes: prompted rows hold P + 1 positions, the others their first page
+            page = self._kv_lm._paged().pages.page
+            self._kv_lm.reserve_kv(rows, [lens[r] + 1 if r in lens else page for r in rows])
+        self.drop_prefill(rows)
+        if not prompts:
+            self._reserve_first_page(rows)
+        self._restart(rows, sampling, seed)
+        if prompts:
+            self._prefill += self.lm_gen._prompt_begin(prompts)
+
+    @property
+    def prefilling(self) -> frozenset:
+        """Rows whose prompt prefill has chunks left to run."""
+        return frozenset(it[0] for it in self._prefill)
+
+    def prefill_chunk(self) -> None:
+        """Run one ragged chunk (at most MAX_ROWS rows) of the pending prompt prefills, oldest first."""
+        if self._prefill:
+            self._prefill = self.lm_gen._prompt_chunk(self._prefill)
+
+    def drop_prefill(self, rows) -> None:
+        """Forget the pending prefill of `rows` (a session released before its prompt was in)."""
+        rows = set(int(r) for r in rows)
+        self._prefill = [it for it in self._prefill if it[0] not in rows]
 
     def _reset_lm_rows(self, rows, sampling, seed) -> None:
         self.lm_gen.reset_streaming(streams=list(rows))

@@ -485,6 +485,8 @@ int rstnet_lm_depth_attention_bf16(const void* qkv, void* kvd, void* out, int32_
  *     Masses are summed in fixed point (2^-40): identical calls and graph replays give identical tokens.  top_p >= 1 is
  *     the top_k < 0 multinomial; top_p == 0 leaves the mode to top_k.  Unlike the reference's masked audio samplers (NaN
  *     with top_p > 0) the distribution is renormalised over the candidates.
+ *   In every mode -0 and +0 are equal logits, a NaN logit is never drawn and takes no top-k slot, and a row in which no
+ *   kept id scores above -inf (every candidate -inf or NaN, say) draws id 0: every token is an id in [0, n_valid).
  * Candidates per row (InferenceImp over a batch of utterances, each with its own candidate sets
  * infer_no_streaming.py:264-283): n_valid_rows given, row r samples ids < n_valid_rows[r * n_valid_stride] (<= 0 or > V:
  * all V) in place of the scalar n_valid, with top_k clamped per row.

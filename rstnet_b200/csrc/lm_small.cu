@@ -501,8 +501,12 @@ __device__ __forceinline__ uint32_t hash_u32(uint32_t a, uint32_t b, uint32_t c,
 constexpr int SAMPLE_CAND = 1024;
 constexpr int SAMPLE_HISTS = 16;
 
+// The one order key of every path: monotone in the bf16 value under float comparison, so -0 and +0 share a key (equal
+// logits tie, and ties go lowest index first), and NaN takes key 0, below -inf (0x7F): no path counts a NaN id.
 __device__ __forceinline__ uint32_t bf16_order_key(bf16 v) {
-  const uint32_t u = (uint32_t)__bfloat16_as_ushort(v);
+  uint32_t u = (uint32_t)__bfloat16_as_ushort(v);
+  if ((u & 0x7FFFu) > 0x7F80u) return 0u;
+  if (u == 0x8000u) u = 0u;
   return (u & 0x8000u) ? (~u & 0xFFFFu) : (u | 0x8000u);
 }
 
@@ -546,19 +550,15 @@ __device__ __forceinline__ float multinomial_score(float l, float inv_t, uint32_
   return l * inv_t + gumbel_of(seed, stepc, row, i);
 }
 
-// Nucleus: the order key with -0 folded onto +0 (equal logits take the same key, so ties go lowest index first), and
-// the weight exp((l - max) / temp) in 2^-40 fixed point (<= 2^40 per id, < 2^58 for 152 064 ids).  Integer sums give
-// the same mass whatever the order of the atomics.  NaN logits and weights below 2^-40 weigh 0.
+// Nucleus: bf16_order_key, and the weight exp((l - max) / temp) in 2^-40 fixed point (<= 2^40 per id, < 2^58 for
+// 152 064 ids).  Integer sums give the same mass whatever the order of the atomics.  NaN logits and weights below 2^-40
+// weigh 0.
 constexpr int SAMPLE_MHISTS = 4;
-__device__ __forceinline__ uint32_t nucleus_key(bf16 v) {
-  const unsigned short u = __bfloat16_as_ushort(v);
-  return bf16_order_key(__ushort_as_bfloat16(u == 0x8000u ? (unsigned short)0 : u));
-}
 __device__ __forceinline__ unsigned long long nucleus_weight(float l, float mx, float inv_t) {
   const float w = expf((l - mx) * inv_t);
   return w > 0.f ? (unsigned long long)(w * 1099511627776.0f) : 0ull;
 }
-__device__ __forceinline__ float key_value(uint32_t k) {   // inverse of bf16_order_key
+__device__ __forceinline__ float key_value(uint32_t k) {   // inverse of bf16_order_key (key 0: a NaN)
   const unsigned short u = (k & 0x8000u) ? (unsigned short)(k & 0x7FFFu) : (unsigned short)(~k & 0xFFFFu);
   return b2f(__ushort_as_bfloat16(u));
 }
@@ -574,6 +574,16 @@ __device__ __forceinline__ float key_value(uint32_t k) {   // inverse of bf16_or
 // whenever every id is kept).  The cut: two 256-bin passes over the order key with counts and fixed-point masses.
 // Deviation: the reference's masked audio samplers (sample_token_audio[_2048] with top_p > 0) give NaN, because they mask
 // with -inf before the cumulative sum; here the distribution is restricted to the ids < n_valid and renormalised.
+//
+// Order and edges, the same in every mode and on every path (full scan, candidate list, tie walk):
+// - The order is (value desc, index asc) under float comparison: -0 and +0 are equal logits.
+// - A NaN logit is never a candidate: it takes no top-k slot and is never drawn.  With fewer than top_k other ids, the
+//   top-k keeps them all.
+// - A +inf logit scores +inf wherever the score is l / temp + Gumbel noise (equal scores: the lowest id), as it wins the
+//   argmax; top_k <= 64 weighs each +inf id 1 and every other id 0.
+// - If no kept id scores above -inf (in particular when every id < n_valid is -inf or NaN), the draw is id 0.  So every
+//   draw is an id in [0, n_valid).
+// tests/sampler_restatement.py restates every draw on the host.
 // All threads of the block call it (any block size that is a multiple of 32, <= 1024); writes *token_out.
 __device__ __noinline__ void sample_row(const bf16* __restrict__ lr, int n_valid, int top_k, float temp, float top_p, uint32_t seed,
                                         uint32_t stepc, int row, long long* __restrict__ token_out) {
@@ -595,7 +605,7 @@ __device__ __noinline__ void sample_row(const bf16* __restrict__ lr, int n_valid
     int mi = 0;
     for (int i = tid; i < n_valid; i += nthr) mx = fmaxf(mx, b2f(lr[i]));
     block_argmax(mx, mi, s_val, s_idx);
-    if (mx > -INFINITY) {   // (all -inf: the multinomial path below)
+    if (mx > -INFINITY) {   // (no id above -inf: the top_k paths below, which draw id 0)
       int* myh = hist[(tid / 32) % SAMPLE_HISTS];
       unsigned long long* mym = mhist[(tid / 32) % SAMPLE_MHISTS];
       for (int pass = 0; pass < 2; ++pass) {
@@ -612,8 +622,8 @@ __device__ __noinline__ void sample_row(const bf16* __restrict__ lr, int n_valid
           unsigned long long w = 0;
           if (i < n_valid) {
             const bf16 v = lr[i];
-            const uint32_t k = nucleus_key(v);
-            if (pass == 0 || (k >> 8) == b1) {
+            const uint32_t k = bf16_order_key(v);
+            if (k && (pass == 0 || (k >> 8) == b1)) {
               bin = pass ? (k & 255u) : (k >> 8);
               w = nucleus_weight(b2f(v), mx, inv_t);
             }
@@ -682,7 +692,7 @@ __device__ __noinline__ void sample_row(const bf16* __restrict__ lr, int n_valid
           if (tid == 0) s_sel[0] = 0;
           __syncthreads();
           for (int i = tid; i < n_valid; i += nthr)
-            if (nucleus_key(lr[i]) == thr) cand_i[atomicAdd(&s_sel[0], 1)] = i;
+            if (bf16_order_key(lr[i]) == thr) cand_i[atomicAdd(&s_sel[0], 1)] = i;
           __syncthreads();
           for (int t = tid; t < cnt; t += nthr) {
             const int id = cand_i[t];
@@ -695,7 +705,7 @@ __device__ __noinline__ void sample_row(const bf16* __restrict__ lr, int n_valid
           if (tid == 0) s_sel[0] = 0;
           for (int base = 0; base < n_valid; base += nthr) {
             const int i = base + tid;
-            const bool tie = i < n_valid && nucleus_key(lr[i]) == thr;
+            const bool tie = i < n_valid && bf16_order_key(lr[i]) == thr;
             const unsigned bal = __ballot_sync(0xffffffffu, tie);
             const int wpre = __popc(bal & ((1u << (tid % 32)) - 1u));
             __syncthreads();
@@ -717,14 +727,14 @@ __device__ __noinline__ void sample_row(const bf16* __restrict__ lr, int n_valid
       int bi = 0x7fffffff;
       for (int i = tid; i < n_valid; i += nthr) {
         const bf16 v = lr[i];
-        const uint32_t k = nucleus_key(v);
+        const uint32_t k = bf16_order_key(v);
         if (k > thr || (k == thr && i <= last)) {
           const float sc = multinomial_score(b2f(v), inv_t, seed, stepc, (uint32_t)row, (uint32_t)i);
           if (sc > bv) { bv = sc; bi = i; }
         }
       }
       block_argmax(bv, bi, s_val, s_idx);
-      if (tid == 0) *token_out = bi;
+      if (tid == 0) *token_out = bv > -INFINITY ? bi : 0;   // no kept id scores above -inf: id 0
       return;
     }
   }
@@ -738,7 +748,7 @@ __device__ __noinline__ void sample_row(const bf16* __restrict__ lr, int n_valid
       if (sc > bv) { bv = sc; bi = i; }
     }
     block_argmax(bv, bi, s_val, s_idx);
-    if (tid == 0) *token_out = bi;
+    if (tid == 0) *token_out = bv > -INFINITY ? bi : 0;
     return;
   }
 
@@ -754,6 +764,7 @@ __device__ __noinline__ void sample_row(const bf16* __restrict__ lr, int n_valid
       const int b1 = pass ? s_sel[0] : 0;
       for (int i = tid; i < n_valid; i += nthr) {
         const uint32_t k = bf16_order_key(lr[i]);
+        if (!k) continue;   // NaN
         if (pass == 0) atomicAdd(&myh[k >> 8], 1);
         else if ((int)(k >> 8) == b1) atomicAdd(&myh[k & 255u], 1);
       }
@@ -776,7 +787,8 @@ __device__ __noinline__ void sample_row(const bf16* __restrict__ lr, int n_valid
     const uint32_t thr = (uint32_t)s_sel[2];
     for (int i = tid; i < n_valid; i += nthr) {
       const bf16 v = lr[i];
-      if (bf16_order_key(v) >= thr) {
+      const uint32_t k = bf16_order_key(v);
+      if (k && k >= thr) {
         const int slot = atomicAdd(&s_sel[3], 1);
         if (slot < SAMPLE_CAND) { cand_v[slot] = b2f(v); cand_i[slot] = i; }
       }
@@ -812,7 +824,7 @@ __device__ __noinline__ void sample_row(const bf16* __restrict__ lr, int n_valid
       for (int base = 0; base < n_valid; base += nthr) {
         const int i = base + tid;
         const uint32_t k = i < n_valid ? bf16_order_key(lr[i]) : 0u;
-        const bool tie = i < n_valid && k == thr;
+        const bool tie = i < n_valid && k && k == thr;
         const unsigned bal = __ballot_sync(0xffffffffu, tie);
         const int wpre = __popc(bal & ((1u << (tid % 32)) - 1u));
         __syncthreads();
@@ -831,7 +843,7 @@ __device__ __noinline__ void sample_row(const bf16* __restrict__ lr, int n_valid
       }
     }
     block_argmax(bv, bi, s_val, s_idx);
-    if (tid == 0) *token_out = bi;
+    if (tid == 0) *token_out = bv > -INFINITY ? bi : 0;
     return;
   }
 
@@ -853,11 +865,12 @@ __device__ __noinline__ void sample_row(const bf16* __restrict__ lr, int n_valid
     last_i = bi;
   }
   if (tid == 0) {
-    int pick = top_i[0];
-    if (top_k > 0) {
+    int pick = top_v[0] > -INFINITY ? top_i[0] : 0;   // no id above -inf (or none but NaN): id 0
+    if (top_k > 0 && top_v[0] > -INFINITY) {
       float best = -INFINITY;
-      for (int r = 0; r < kk; ++r) {
-        const float w = expf((top_v[r] - top_v[0]) / temp);
+      for (int r = 0; r < kk && top_i[r] < n_valid; ++r) {   // (fewer than kk ids that are not NaN: the rest are empty)
+        // a +inf logit weighs 1 (its difference to the top +inf would be NaN); then every other id weighs 0
+        const float w = top_v[r] == INFINITY ? 1.f : expf((top_v[r] - top_v[0]) / temp);
         const uint32_t u = hash_u32(seed, stepc, (uint32_t)row, (uint32_t)r);
         const float uni = ((float)(u >> 8) + 0.5f) * (1.0f / 16777216.0f);  // (0,1)
         const float e = -logf(uni);                                        // Exp(1)

@@ -610,6 +610,14 @@ enum { RSTNET_GEN_RUNNING = 0, RSTNET_GEN_LAST = 1, RSTNET_GEN_STOPPED = 2, RSTN
 int rstnet_lm_gen_rows_advance(const int64_t* tokens, int32_t tok_stride, int32_t* rec, int32_t* row_valid, int32_t valid_stride,
                                int32_t* status, int32_t B, int32_t dep_q, int32_t card, rstnet_stream_t stream);
 
+/* ---- forced tokens (added in version 206): run after the sampler of head `col` (graph-capturable).  For every row
+ * r < rows, tokens[r * tok_stride + col] = force[r * force_stride + col] where that id is >= 0; a negative id keeps the
+ * sampled token.  An id >= V (the head's vocabulary) is not written and sets the sticky device error bit 1
+ * (rstnet_device_error_flags).  tokens int64 and force int32, device memory.  Checked before any launch, each an error
+ * return: a null pointer, rows < 1, V < 1, col < 0, col >= tok_stride or col >= force_stride.  One thread per row. */
+int rstnet_lm_force_tokens(int64_t* tokens, int32_t tok_stride, int32_t col, const int32_t* force, int32_t force_stride,
+                           int32_t rows, int32_t V, rstnet_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -33,7 +33,7 @@ SYMBOLS = [
     "rstnet_stft_loss_workspace", "rstnet_stft_loss_sums_f32", "rstnet_sisnr_moments_workspace", "rstnet_sisnr_moments_f32",
     "rstnet_segments_gather", "rstnet_segments_scatter", "rstnet_lm_rope_pair_kv_append_rows_bf16",
     "rstnet_kv_pages_copy", "rstnet_lm_gen_rows_advance", "rstnet_lm_delay_cache_prompt",
-    "rstnet_lm_rope_pair_kv_append_paged_rows_bf16",
+    "rstnet_lm_rope_pair_kv_append_paged_rows_bf16", "rstnet_lm_force_tokens",
 ]
 
 KV_LOG2_PAGE_MIN, KV_LOG2_PAGE_MAX = 4, 12   # RSTNET_KV_LOG2_PAGE_MIN / _MAX: pages of 16 .. 4096 positions
@@ -196,6 +196,7 @@ def lib() -> C.CDLL:
                                                vp]
     L.rstnet_lm_rope_pair_kv_append_paged_rows_bf16.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, i32, i32,
                                                                 vp]
+    L.rstnet_lm_force_tokens.argtypes = [vp, i32, i32, vp, i32, i32, i32, vp]
     for name in SYMBOLS:
         fn = getattr(L, name)
         if fn.restype is C.c_int and name not in ("rstnet_version",):

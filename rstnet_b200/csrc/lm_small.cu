@@ -1109,6 +1109,34 @@ extern "C" int rstnet_lm_depth_attention_bf16(const void* qkv, void* kvd, void* 
   return check_launch("lm_depth_attention");
 }
 
+// ---------------------------------------------------------------- forced tokens (generation with given ids)
+// tokens[r, col] = force[r, col] where that id is >= 0; a negative id keeps the sample.  An id >= V is not written: it
+// sets error bit 0 (1), as an out-of-range embedding id does.  One thread per row.
+__global__ void force_tokens_kernel(long long* __restrict__ tokens, int tok_stride, int col, const int* __restrict__ force,
+                                    int force_stride, int rows, int V) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= rows) return;
+  const int id = force[(long long)r * force_stride + col];
+  if (id < 0) return;
+  if (id >= V) {
+    atomicOr(&g_lm_dev_err, 1u);
+    return;
+  }
+  tokens[(long long)r * tok_stride + col] = id;
+}
+
+extern "C" int rstnet_lm_force_tokens(int64_t* tokens, int32_t tok_stride, int32_t col, const int32_t* force, int32_t force_stride,
+                                      int32_t rows, int32_t V, rstnet_stream_t stream) {
+  RSTNET_REQUIRE(tokens && force, "lm_force_tokens: null pointer");
+  RSTNET_REQUIRE(rows > 0 && V > 0 && col >= 0 && col < tok_stride && col < force_stride,
+                 "lm_force_tokens: bad shape (rows=%d, V=%d, col=%d, tok_stride=%d, force_stride=%d)", rows, V, col, tok_stride,
+                 force_stride);
+  force_tokens_kernel<<<dim3(ceil_div(rows, 256)), dim3(256), 0, (cudaStream_t)stream>>>((long long*)tokens, tok_stride, col, force,
+                                                                                          force_stride, rows, V);
+  count_launch();
+  return check_launch("lm_force_tokens");
+}
+
 extern "C" int rstnet_lm_sample_params_bf16(const void* logits, int32_t rows, int32_t V, int32_t n_valid, const int32_t* n_valid_rows,
                                             int32_t n_valid_stride, int32_t top_k, float temp, float top_p, const int32_t* top_k_rows,
                                             const float* temp_rows, const float* top_p_rows, int32_t param_stride, uint32_t seed,

@@ -269,6 +269,21 @@ class InferenceImp(object):
                 raise RstnetError(f"lengths[{utt!r}]: max_frames must be in [1, 2^31) and min_frames an int32 (got {lengths!r})")
         return _Request(utt, seq, P, maxlen, sp, seed, task, minlen, maxlen - 1 > minlen)
 
+    def _check_forced(self, utt, forced, G: int) -> np.ndarray:
+        """forced[utt]: int64 [dep_q + 1, G] over the item's G generated frames, each id -1 (sample) or inside its head's
+        vocabulary -> the host int32 table the frame loop reads"""
+        c = self.model.config
+        n_cb = self.model.num_codebooks
+        if not torch.is_tensor(forced) or forced.dtype != torch.int64 or tuple(forced.shape) != (n_cb, G):
+            raise RstnetError(f"forced[{utt!r}] must be an int64 tensor [{n_cb}, {G}] (its generated frames; -1: sample), got "
+                              f"{(tuple(forced.shape), forced.dtype) if torch.is_tensor(forced) else type(forced).__name__}")
+        f = forced.cpu().numpy()
+        vocab = np.array([c.padded_vocab_size] + [c.audio_card] * (n_cb - 1))[:, None]
+        if ((f < -1) | (f >= vocab)).any():
+            raise RstnetError(f"forced[{utt!r}]: every id is -1 or inside its head's vocabulary (text < {c.padded_vocab_size}, "
+                              f"audio < {c.audio_card})")
+        return f.astype(np.int32)
+
     def _check_many(self, capacity: int, kv_pages: Optional[int], n_samples: int = 1, streamed: bool = False) -> None:
         """the argument checks of generate_many / stream_many / serve.TTSEngine"""
         self._check_task()
@@ -295,17 +310,29 @@ class InferenceImp(object):
             raise RstnetError(f"utterance {req.utt!r}: task {req.task!r} generates text; streamed generation runs {AUDIO_TASKS}")
 
     @staticmethod
+    def _check_forced_keys(forced: dict, utts) -> None:
+        unknown = [u for u in forced if u not in utts]
+        if unknown:
+            raise RstnetError(f"forced names utterance(s) that are not among the items: {unknown[:5]!r}")
+
+    @staticmethod
     def _check_sampling(sampling: Optional[Dict[object, Sampling]]) -> None:
         if sampling is not None:
             for utt, sp in sampling.items():
                 if not isinstance(sp, Sampling):
                     raise RstnetError(f"sampling[{utt!r}] must be a Sampling (got {type(sp).__name__})")
 
-    def _puller(self, items, seeds, sampling, tasks=None, lengths=None, streamed=False):
+    def _puller(self, items, seeds, sampling, tasks=None, lengths=None, streamed=False, forced=None, tables=None):
         """-> pull(): the next item of `items` as an admission request (_request), or None once they are exhausted; items
-        are read one at a time, when a row can take them.  streamed: the text tasks raise (their frames are no audio)."""
+        are read one at a time, when a row can take them.  streamed: the text tasks raise (their frames are no audio).
+        forced: each request's forced table is checked (_check_forced) into `tables` {utt_id: int32 [9, G]}; a table for
+        an utterance that is not among the items raises, before any launch when `items` is a list or tuple, else once they
+        are exhausted."""
         source, seeds, done = iter(items), seeds or {}, []
-        tasks, lengths = tasks or {}, lengths or {}
+        tasks, lengths, forced = tasks or {}, lengths or {}, forced or {}
+        if forced and isinstance(items, (list, tuple)):
+            self._check_forced_keys(forced, {it[0] for it in items})
+        seen = set()
 
         def pull():
             if done:
@@ -314,9 +341,15 @@ class InferenceImp(object):
                 utt, seq = next(source)
             except StopIteration:
                 done.append(True)
+                if forced:
+                    self._check_forced_keys(forced, seen)
                 return None
+            if forced:
+                seen.add(utt)
             req = self._request(utt, seq, None if sampling is None else sampling.get(utt), int(seeds.get(utt, 0)),
                                 tasks.get(utt, self.task_name), lengths.get(utt))
+            if utt in forced:
+                tables[utt] = self._check_forced(utt, forced[utt], req.G)
             if streamed:
                 self._check_streamed(req)
             return req
@@ -328,7 +361,8 @@ class InferenceImp(object):
                       sampling: Optional[Dict[object, Sampling]] = None, kv_pages: Optional[int] = None,
                       stats: Optional[dict] = None, n_samples: int = 1, rank: Optional[str] = "logprob",
                       tasks: Optional[Dict[object, str]] = None,
-                      lengths: Optional[Dict[object, Tuple[int, int]]] = None) -> Iterator[Tuple]:
+                      lengths: Optional[Dict[object, Tuple[int, int]]] = None,
+                      forced: Optional[Dict[object, torch.Tensor]] = None) -> Iterator[Tuple]:
         """Continuous batching over (utt_id, seq [9, L]) items, each in its own TTS layout: yields (utt_id, codes [8, G-1])
         in completion order.  Up to `capacity` utterances decode together, one graph replay per frame; a finished row is
         held until the next utterance is admitted into it (its prompt fed through GPT.prefill_streams while the other
@@ -365,17 +399,30 @@ class InferenceImp(object):
         >= 2048 in audio codebooks 3..7; that frame is dropped).  A row whose window can stop is decided on the device
         (rstnet_lm_gen_rows_advance in the frame graph); the host reads frame n's statuses after it has enqueued frame
         n + 1, so such a row runs one frame past its stop before it is released.  It reserves KV pages for P + max_frames
-        positions: that extra frame is at most frame max_frames - 1.  With no such row in the batch, no status is read."""
+        positions: that extra frame is at most frame max_frames - 1.  With no such row in the batch, no status is read.
+
+        forced: {utt_id: int64 [9, G]} fixes tokens of an utterance's generated frames, G its maxlen: column g is generated
+        frame g (text token, audio codebooks 0..7, the layout of return_frames' frames, before reverse_delay), -1 where the
+        head samples.  A forced token is the frame's token everywhere: the next depth step, the next frame's input, the
+        log-probability sums and the stop rule (e.g. fix the semantic codebook 0 and sample the others).  It need not lie
+        in the frame's candidate set, only in its head's vocabulary.  The candidates of one utterance (n_samples > 1)
+        share its table.  Each frame the loop fills every forced row's slice of a pinned [B, 9] table from the host and
+        uploads it without a synchronise; the frames run the forced graph (with -1 everywhere else, it draws what the plain
+        frame draws).  Shape, dtype and ids are checked at admission, before the item is launched."""
         self._check_many(capacity, kv_pages, n_samples)
+        if forced is not None and not isinstance(forced, dict):
+            raise RstnetError("forced must be a dict keyed by utt_id")
         if rank not in ("logprob", None):
             raise RstnetError(f"rank is 'logprob' or None (got {rank!r})")
         if n_samples > 1 and return_frames:
             raise RstnetError("return_frames is not available with n_samples > 1")
         m = self.model
         self._check_sampling(sampling)
-        pull = self._puller(items, seeds, sampling, tasks, lengths)
+        tables = {} if forced else None
+        pull = self._puller(items, seeds, sampling, tasks, lengths, forced=forced, tables=tables)
         with _tts_scope(m, capacity, kv_pages):
-            rows = _TTSRows(self, capacity, sampling is not None, {} if stats is None else stats, n_samples=int(n_samples))
+            rows = _TTSRows(self, capacity, sampling is not None, {} if stats is None else stats, n_samples=int(n_samples),
+                            forced=tables)
             groups: Dict[int, list] = {}
             ready = []   # utterances whose candidates all finished in the last frame: their sums are still being copied
             while True:
@@ -483,7 +530,8 @@ class _Row:
     """The state of one occupied row of the batch loop: what it was admitted with (`g` counts the frames it has run,
     from frame `start` on; `cand` is its candidate index in request `group`), then its outcome, set when it finishes:
     its result is frames start .. end - 1; stopped: its stop rule fired on frame `end` (`dropped`, not part of the
-    result); lp: (host sums, row, event or None) of its log-probability sums (best-of-N); codes: its codes (audio tasks)."""
+    result); lp: (host sums, row, event or None) of its log-probability sums (best-of-N); codes: its codes (audio tasks);
+    forced: the request's forced table."""
     utt: object
     P: int
     G: int
@@ -500,6 +548,7 @@ class _Row:
     dropped: Optional[torch.Tensor] = None
     lp: Optional[tuple] = None
     codes: Optional[torch.Tensor] = None
+    forced: Optional[np.ndarray] = None
 
     @property
     def frames(self) -> int:
@@ -521,10 +570,12 @@ class _TTSRows:
     frame's copy before it hands that frame's chunks out.  No eager torch arithmetic runs on this path, except the clamp of
     the codes to the codebook (ids 2048 / 2049 are LM samples, which the codec's gather clamps alike but flags as errors)."""
 
-    def __init__(self, imp: InferenceImp, B: int, per_row: bool, stats: dict, codec=None, n_samples: int = 1):
+    def __init__(self, imp: InferenceImp, B: int, per_row: bool, stats: dict, codec=None, n_samples: int = 1,
+                 forced: Optional[dict] = None):
         m = imp.model
         self.imp, self.m, self.B, self.stats = imp, m, B, stats
         self.n_samples = n_samples      # > 1: each request is that many candidates, forked from one prefill
+        self.forced = forced            # {utt: int32 [9, G]} (generate_many(forced=)): every frame runs the forced graph
         self.groups = 0                 # requests admitted (a row's group id)
         stats.update(frames=0, row_frames=0, wait_frames=0)
         self.default = None             # the instance's Sampling while rows sample with per-row settings
@@ -649,7 +700,8 @@ class _TTSRows:
                 m.fork_kv(rows[0], rows[1:], req.P + req.G)
             for i, r in enumerate(rows):
                 self.rows[r] = _Row(req.utt, req.P, req.G, self.n, req.sampling, req.task, req.minlen, req.windowed,
-                                    cand=i, group=self.groups)
+                                    cand=i, group=self.groups,
+                                    forced=None if self.forced is None else self.forced.get(req.utt))
                 self.keys[r] = sample_seed(req.seed, i)
                 self.fresh.add(r)
                 self.cur[r, :, 0] = feed[:, -1]
@@ -703,6 +755,12 @@ class _TTSRows:
         extra = {"gen_rows": True} if gen else {}
         if self.n_samples > 1:
             extra["logprob"] = True
+        if self.forced is not None:
+            force = np.full((B, self.dep_q + 1), -1, dtype=np.int32)
+            for r in occupied:
+                if rows[r].forced is not None:
+                    force[r] = rows[r].forced[:, rows[r].g]
+            extra["force"] = torch.from_numpy(force).pin_memory() if self.dev.type == "cuda" else torch.from_numpy(force)
         toks = m.forward_step(self.cur, use_sampling=imp.use_sampling, temp_text=imp.temp_text, top_k_text=imp.top_k_text,
                               temp=imp.temp, top_k=imp.top_k, audio_valid=table,
                               sample_key=self.keys if self.admitted else None, depth_ring_quirk=False,

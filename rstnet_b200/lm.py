@@ -881,7 +881,7 @@ class GPT(_DecodeModel):
     def forward_step(self, sequence: torch.Tensor, *, use_sampling: bool = True, temp_text: float = 0.7, top_k_text: int = 25,
                      temp: float = 0.8, top_k: int = 30, audio_valid=2049, depth_ring_quirk: bool = True, sample_key=None,
                      sample_step=None, top_p_text: float = 0.0, top_p: float = 0.0, sampling=None,
-                     logprob: bool = False, gen_rows: bool = False) -> torch.Tensor:
+                     logprob: bool = False, gen_rows: bool = False, force: Optional[torch.Tensor] = None) -> torch.Tensor:
         """One generated frame: temporal step on sequence[B,9,1], text token, then the 8 depth steps, each sampled
         on the device (sample_token / sample_token_audio[_2048], utils/sampling.py:85-154: use_sampling False ->
         argmax over the whole card; True -> temperature + top-k (top_k == 0: plain multinomial) over ids <
@@ -910,13 +910,21 @@ class GPT(_DecodeModel):
         gen_rows (with audio_valid=None): the per-row candidate counts are the scope's device table row_valid, kept by the
         rows' generation windows (`_LMState.gen_rows_set`): after the last depth sample, rstnet_lm_gen_rows_advance decides
         each row's status for this frame (running, last, stopped by the reference's stop rule, idle) into
-        `_state.gen_status` and writes the next frame's counts.  A graph of its own."""
+        `_state.gen_status` and writes the next frame's counts.  A graph of its own.
+
+        force: an integer tensor [B, dep_q + 1] (text, audio_0..): where an id is >= 0 the row takes it in place of that
+        head's sample (-1: the head samples).  The forced id is the frame's token everywhere downstream: the next depth
+        step's input, the returned tokens (the next frame's input), the log-probability sums and the stop rule.  It need
+        not lie inside the row's candidate counts; an id outside the head's vocabulary is not taken and sets the device
+        error flag.  Every draw's noise is keyed by the row and head, not by the tokens, so forcing a head to the token it
+        would have drawn changes nothing.  A graph of its own, next to the one without; the table is copied to the device
+        before the replay."""
         if self._state is None:
             raise RstnetError("forward_step is a streaming call: use it inside `with gpt.streaming(B):`")
         if sampling is None and (top_p_text or top_p):
             Sampling(use_sampling, temp_text, top_k_text, top_p_text, temp, top_k, top_p)   # validates a nucleus frame's settings
         return self._state.forward_step(sequence, use_sampling, temp_text, top_k_text, temp, top_k, audio_valid, depth_ring_quirk,
-                                        sample_key, sample_step, top_p_text, top_p, sampling, logprob, gen_rows)
+                                        sample_key, sample_step, top_p_text, top_p, sampling, logprob, gen_rows, force)
 
     @torch.no_grad()
     @on_own_device
@@ -1260,6 +1268,8 @@ class _LMState:
             self.row_temp = z(M, 2, dtype=torch.float32)
             self.row_topp = z(M, 2, dtype=torch.float32)
             self._row_params = None   # (the Sampling list last uploaded to the three tables, its argmax rows)
+            # forced frames (forward_step(force=...)): each row's given ids, -1 where the head samples
+            self.force_rows = torch.full((M, c.dep_q + 1), -1, dtype=torch.int32, device=dev)
             hd = D // c.codecformer_heads
             self.dkv_all = z(c.codecformer_layers, 2, M, c.codecformer_heads, c.dep_q, hd)
             self.dkv = [self.dkv_all[l] for l in range(c.codecformer_layers)]
@@ -1436,6 +1446,24 @@ class _LMState:
         _lib.check(_lib.lib().rstnet_lm_sample_params_bf16(
             logits.data_ptr(), self.M, V, V if n_valid is None else n_valid, nv, c.dep_q, tk, float(temp), float(tp), *tabs, 2,
             self.seed + col, *rng, self.tokens.data_ptr() + 8 * col, c.dep_q + 1, ops._stream()), "sample")
+
+    def _force(self, col: int) -> None:
+        """column col of self.tokens takes each row's id in force_rows where it is >= 0 (an id outside the head's
+        vocabulary is not taken and sets the device error flag)"""
+        c = self.c
+        V = c.padded_vocab_size if col == 0 else c.audio_card
+        _lib.check(_lib.lib().rstnet_lm_force_tokens(self.tokens.data_ptr(), c.dep_q + 1, col, self.force_rows.data_ptr(),
+                                                     c.dep_q + 1, self.M, V, ops._stream()), "force_tokens")
+
+    def set_force(self, force: torch.Tensor) -> None:
+        """force, an integer tensor [B, dep_q + 1] (text, audio heads; a negative id: the head samples) -> the scope's
+        force_rows, read by the next forced frame: one copy, no synchronise for a device or pinned source"""
+        c = self.c
+        if (not torch.is_tensor(force) or tuple(force.shape) != (self.B, c.dep_q + 1) or force.dtype.is_floating_point
+                or force.dtype.is_complex or force.dtype == torch.bool):
+            raise RstnetError(f"force is an integer tensor [{self.B}, {c.dep_q + 1}] (-1: sample), got "
+                              f"{tuple(force.shape) if torch.is_tensor(force) else type(force).__name__}")
+        self.force_rows[:self.B].copy_(force, non_blocking=True)
 
     def set_row_sampling(self, sampling):
         """sampling: B `Sampling` -> the scope's per-row tables, uploaded from pinned memory without a synchronise, and
@@ -1725,10 +1753,12 @@ class _LMState:
             out[:, k].copy_(self.dlogits)
 
     def forward_step(self, sequence, use_sampling, temp_text, top_k_text, temp, top_k, audio_valid, quirk=True, sample_key=None,
-                     sample_step=None, top_p_text=0.0, top_p=0.0, sampling=None, logprob=False, gen_rows=False):
+                     sample_step=None, top_p_text=0.0, top_p=0.0, sampling=None, logprob=False, gen_rows=False, force=None):
         c = self.c
         if sequence.shape[0] != self.B or sequence.shape[2] != 1:
             raise RstnetError(f"forward_step takes sequence [{self.B}, {c.n_q + 1}, 1], got {tuple(sequence.shape)}")
+        if force is not None:
+            self.set_force(force)
         if gen_rows:
             if audio_valid is not None:
                 raise RstnetError("gen_rows=True reads the candidate counts the device keeps in row_valid: pass audio_valid=None")
@@ -1764,7 +1794,7 @@ class _LMState:
                                                    _head_mode(use_sampling, temp, top_k, top_p))
         if logprob and self.lp_acc is None:
             self.logprob_reset()
-        self._replay(*self._frame(modes, valid, per_row, quirk, bool(logprob), bool(gen_rows)))
+        self._replay(*self._frame(modes, valid, per_row, quirk, bool(logprob), bool(gen_rows), force is not None))
         return self.tokens.clone()
 
     # ---- per-row generation windows (forward_step(gen_rows=True))
@@ -1814,14 +1844,16 @@ class _LMState:
         self.lp_lab[col].copy_(self.tokens[:, col])
         cross_entropy_sums(logits, self.lp_lab[col], self.lp_w, 1, None, self.lp_slot, self.lp_acc[col], self.lp_nll, self.lp_pred)
 
-    def _frame(self, modes, valid, per_row_rng: bool, quirk, logprob: bool = False, gen: bool = False):
+    def _frame(self, modes, valid, per_row_rng: bool, quirk, logprob: bool = False, gen: bool = False, force: bool = False):
         """(graph key, launch sequence) of one generated frame from the ids in self.seq to the tokens in self.tokens.
         modes: ((top_k, temp, top_p) of the text head, (...) of the audio heads) for every row, as _head_mode gives them, or
         None: each row's own from the row_topk / row_temp / row_topp tables.  valid: the dep_q audio heads' candidate
         counts for every row, or None: each row's own from row_valid.  per_row_rng: the RNG keyed by (row_step, row_key)
         in place of (frame_counter, row); the frame advances the counter it keys by.  logprob: after each head's sampler,
         add the log-probability of the sampled tokens into the rows' sums (logprob_sums); a graph of its own.  gen: then
-        advance the rows' generation windows (gen_rows): status, next frame's row_valid; a graph of its own."""
+        advance the rows' generation windows (gen_rows): status, next frame's row_valid; a graph of its own.  force: right
+        after each head's sampler, the rows' ids in force_rows replace the samples (set_force), so the forced ids feed the
+        next depth step, the log-probability sums and the window's stop rule; a graph of its own."""
         c = self.c
         if modes is not None and modes[1][0] == 0:
             valid = (c.audio_card,) * c.dep_q   # the 2048 / 2049 masks exist on the sampling path only (sampling.py:107-154)
@@ -1830,12 +1862,16 @@ class _LMState:
         def frame():
             self._temporal()
             self._sample(0, text, c.padded_vocab_size, per_row_rng)
+            if force:
+                self._force(0)
             if logprob:
                 self._logprob(0)
             self.tout.copy_(self.out)
             for k in range(c.dep_q):
                 self._depth(k, self.tokens[:, k], c.dep_q + 1, quirk=quirk)
                 self._sample(k + 1, audio, None if valid is None else min(valid[k], c.audio_card), per_row_rng)
+                if force:
+                    self._force(k + 1)
                 if logprob:
                     self._logprob(k + 1)
             if per_row_rng:
@@ -1845,6 +1881,7 @@ class _LMState:
 
         key = ("frame", "tables" if modes is None else modes, "rows" if valid is None else valid, per_row_rng, bool(quirk))
         key = key + ("logprob",) if logprob else key
+        key = key + ("force",) if force else key
         if not gen:
             return key, frame
 

@@ -444,17 +444,18 @@ class LMGen(nn.Module):
         self._st = st
         self.lm_model._state = None if st is None else st.lm
 
-    def _frame(self, st: _GenState):
+    def _frame(self, st: _GenState, force: bool = False):
         """(graph key, launch sequence): cache_in -> temporal step + text sampling + dep_q depth steps with sampling
-        (sample_token over the whole card: LMGen uses plain `sample_token`, models/model.py:528-533, 581-586) -> cache_out."""
+        (sample_token over the whole card: LMGen uses plain `sample_token`, models/model.py:528-533, 581-586) -> cache_out.
+        force: each sampler is followed by the forced ids of the scope's force_rows (_LMState._frame)."""
         lm, ms, L = self.lm_model, st.lm, _lib.lib()
         if self._row_sampling is not None:
             ms.set_row_sampling(self._row_sampling)     # row_valid stays 0: every row samples over the whole card
-            key, frame = ms._frame(None, None, True, True)
+            key, frame = ms._frame(None, None, True, True, force=force)
         else:
             modes = (_head_mode(self.use_sampling, self.temp_text, self.top_k_text, self.top_p_text),
                      _head_mode(self.use_sampling, self.temp, self.top_k, self.top_p))
-            key, frame = ms._frame(modes, (lm.card,) * ms.c.dep_q, False, True)
+            key, frame = ms._frame(modes, (lm.card,) * ms.c.dep_q, False, True, force=force)
         K, CT = lm.num_codebooks, st.cache.shape[2]
 
         def step():
@@ -532,9 +533,15 @@ class LMGen(nn.Module):
         return [it for it in todo if it[2] < it[1].shape[0]]
 
     @torch.no_grad()
-    def step(self, input_tokens: torch.Tensor) -> Optional[torch.Tensor]:
+    def step(self, input_tokens: torch.Tensor, force: Optional[torch.Tensor] = None) -> Optional[torch.Tensor]:
         """One step of every active row: -> [B, dep_q + 1, 1] in the delayed layout, or None while every row is still in
-        its `max_delay` warm-up steps.  One input copy and one graph replay."""
+        its `max_delay` warm-up steps.  One input copy and one graph replay.
+
+        Extension: force, an integer tensor [B, dep_q + 1, 1] (input_tokens' convention), gives the (text, audio) tokens
+        the rows take at this step instead of their samples where an id is >= 0 (-1: sample), as the reference's
+        depformer takes teacher-forced tokens: the forced ids feed the next depth step and the delay cache, so the next
+        steps condition on them.  An id outside the head's vocabulary is not taken and sets the device error flag.  A
+        graph of its own; one more copy before the replay."""
         st = self._st
         if st is None:
             raise RuntimeError("You should wrap those calls with a `with lm_gen.streaming(): ...`.")
@@ -547,9 +554,14 @@ class LMGen(nn.Module):
         if B != st.B:
             raise RstnetError(f"streaming batch size is {st.B}, got {B}")
         ms = st.lm
+        if force is not None:
+            if not torch.is_tensor(force) or force.dim() != 3 or force.shape[2] != 1:
+                raise RstnetError(f"force is an integer tensor [{st.B}, {lm.dep_q + 1}, 1] (-1: sample), got "
+                                  f"{tuple(force.shape) if torch.is_tensor(force) else type(force).__name__}")
+            ms.set_force(force[:, :, 0])
         ms._advance_host(1)
         st.user.copy_(input_tokens[:, :, 0])
-        ms._replay(*self._frame(st))
+        ms._replay(*self._frame(st, force is not None))
         act = ms.active_host != 0
         if self.check:
             seq = ms.seq.cpu()[torch.from_numpy(act)]
@@ -584,13 +596,44 @@ def prompt_from_aligned(seq: torch.Tensor, P: int, delays, dep_q: int, initial: 
     P = int(P)
     if not 0 <= P <= L:
         raise RstnetError(f"P = {P} outside [0, {L}]")
-    out = torch.full((K, P), int(initial), dtype=torch.int64, device=seq.device)
-    for k in range(dep_q + 1):
-        d = delays[k]
-        if P > d:
-            out[k, d:] = seq[k, :P - d]
+    out = torch.empty((K, P), dtype=torch.int64, device=seq.device)
+    out[:dep_q + 1] = _to_steps(seq[:dep_q + 1], delays, P, initial)
     out[dep_q + 1:] = seq[dep_q + 1:, :P]
     return out
+
+
+def _to_steps(x: torch.Tensor, delays, n: int, fill: int) -> torch.Tensor:
+    """Moshi's channels x [dep_q + 1, L] in the aligned layout -> their first n steps in LMGen's step layout, int64
+    [dep_q + 1, n]: out[k, t] = x[k, t - delays[k]] for delays[k] <= t < L + delays[k], `fill` elsewhere (the steps that
+    sample codebook k before its first aligned frame, or after the recording's last)."""
+    out = torch.full((x.shape[0], n), int(fill), dtype=torch.int64, device=x.device)
+    for k in range(x.shape[0]):
+        d = int(delays[k])
+        m = min(n - d, x.shape[1])
+        if m > 0:
+            out[k, d:d + m] = x[k, :m]
+    return out
+
+
+def force_from_aligned(seq: torch.Tensor, mask: torch.Tensor, delays, dep_q: int) -> torch.Tensor:
+    """Aligned dialogue codes seq [K, L] and a bool mask [dep_q + 1, L] over Moshi's channels (text, audio codebooks
+    1..dep_q; True: take seq's token at that aligned frame instead of sampling it) -> the forced ids of steps 0..L-1 in
+    LMGen's step layout, int64 [dep_q + 1, L], -1 where the step samples: forced[k, t] = seq[k, t - delays[k]] where
+    mask[k, t - delays[k]], the mapping prompt_from_aligned applies to the prompt.  Column t is LMGen.step's `force` at
+    the row's step t; steps inside a prompt are fixed by it already."""
+    if not torch.is_tensor(seq) or seq.dim() != 2 or seq.dtype.is_floating_point:
+        raise RstnetError("seq must be an integer tensor [K, L]")
+    K, L = seq.shape
+    delays = [int(d) for d in delays]
+    if len(delays) != K or min(delays) < 0:
+        raise RstnetError(f"{len(delays)} delays (each >= 0) for K = {K} codebooks")
+    if not 0 <= dep_q < K:
+        raise RstnetError(f"dep_q = {dep_q} outside [0, {K})")
+    if not torch.is_tensor(mask) or mask.dtype != torch.bool or tuple(mask.shape) != (dep_q + 1, L):
+        raise RstnetError(f"a force mask is a bool tensor [{dep_q + 1}, {L}] (the item's aligned frames), got "
+                          f"{(tuple(mask.shape), mask.dtype) if torch.is_tensor(mask) else type(mask).__name__}")
+    vals = torch.where(mask.to(seq.device), seq[:dep_q + 1].to(torch.int64), -1)
+    return _to_steps(vals, delays, L, -1)
 
 
 def _item(item, K: int):
@@ -608,7 +651,7 @@ def _item(item, K: int):
 
 @torch.no_grad()
 def generate_many(gen: LMGen, items, capacity: int, *, seeds=None, sampling=None, kv_pages: Optional[int] = None,
-                  stats: Optional[dict] = None):
+                  stats: Optional[dict] = None, force=None):
     """Continuous batching of prompted Moshi generation over (utt_id, seq [K, L], P) items, seq aligned dialogue codes
     (prompt_from_aligned's layout), 0 <= P < L: yields (utt_id, out int64 [dep_q + 1, L - P]) in completion order, out
     being the aligned frames `LMGen.step` returned at steps P .. L - 1 (column j: aligned frame P + j - max_delay;
@@ -623,7 +666,15 @@ def generate_many(gen: LMGen, items, capacity: int, *, seeds=None, sampling=None
     kv_pages N: a paged scope of N pages of KV_PAGE positions; an item holds pages for min(L, context) positions while it
     is live, and waits for them while a row is free (an item needing more than the pool raises).  Paged and contiguous
     scopes give the same tokens.  stats: a dict that receives 'frames' (steps run), 'row_frames' (live rows summed over
-    steps) and 'prefill_rows' (prompt frames prefilled)."""
+    steps) and 'prefill_rows' (prompt frames prefilled).
+
+    force: {utt_id: bool mask [dep_q + 1, L]} over the item's aligned frames of Moshi's channels: where True the row
+    takes seq's token at that frame instead of sampling it (force_from_aligned maps the mask to the steps; frames inside
+    the prompt are fixed by it already), so every forced position of `out` equals the recording.  Forcing the audio
+    codebooks and sampling the text transcribes the recording's Moshi channel; forcing the text re-voices it.  The
+    per-row step tables stay on the device and are gathered by each row's step count, as the user tokens are.  Items
+    without an entry run exactly as without `force` (the forced frame with nothing forced draws what the plain frame
+    draws).  A mask of the wrong shape or a forced id outside its head's vocabulary raises at the item's admission."""
     lm = gen.lm_model
     K, dq = lm.num_codebooks, lm.dep_q
     Ku = K - dq - 1
@@ -631,14 +682,15 @@ def generate_many(gen: LMGen, items, capacity: int, *, seeds=None, sampling=None
         raise RstnetError(f"capacity must be an int in [1, {MAX_STREAMS}] (got {capacity!r})")
     if gen.is_streaming:
         raise RstnetError("generate_many opens its own streaming scope: call it on a generator that is not streaming")
-    for name, d in (("seeds", seeds), ("sampling", sampling)):
+    for name, d in (("seeds", seeds), ("sampling", sampling), ("force", force)):
         if d is not None and not isinstance(d, dict):
             raise RstnetError(f"{name} must be a dict keyed by utt_id")
     for s in (sampling or {}).values():
         if not isinstance(s, Sampling):
             raise RstnetError(f"sampling values must be Sampling (got {type(s).__name__})")
-    seeds, sampling = seeds or {}, sampling or {}
+    seeds, sampling, force = seeds or {}, sampling or {}, force or {}
     dev = lm.device
+    vocab = (lm.config.padded_vocab_size,) + (lm.card,) * dq   # the heads' vocabularies: text, then audio
     counts = dict(frames=0, row_frames=0, prefill_rows=0)
     it = iter(items)
     nxt = None
@@ -650,6 +702,7 @@ def generate_many(gen: LMGen, items, capacity: int, *, seeds=None, sampling=None
         free = list(range(capacity))
         live = {}                                    # row -> (utt_id, L, P, index of its first step in `hist`)
         ubuf = torch.zeros(capacity, Ku, 1, dtype=torch.int64, device=dev)   # each row's user tokens by step
+        fbuf = torch.full((capacity, dq + 1, 1), -1, dtype=torch.int32, device=dev) if force else None   # ... forced ids
         hist: List[torch.Tensor] = []                # st.out after each step, from global step `base` on
         base = 0
         mask = None
@@ -665,6 +718,7 @@ def generate_many(gen: LMGen, items, capacity: int, *, seeds=None, sampling=None
                         break
                 utt, seq, P = nxt
                 L = seq.shape[1]
+                steps = _forced_steps(utt, seq, force.get(utt), lm.delays, dq, vocab) if utt in force else None
                 if pages is not None:
                     need = pages.pages_for(min(L, lm.context))
                     if need > pages.n_pages:
@@ -681,7 +735,15 @@ def generate_many(gen: LMGen, items, capacity: int, *, seeds=None, sampling=None
                     grown = torch.zeros(capacity, Ku, L, dtype=torch.int64, device=dev)
                     grown[:, :, :ubuf.shape[2]] = ubuf
                     ubuf = grown
+                    if fbuf is not None:
+                        grown = torch.full((capacity, dq + 1, L), -1, dtype=torch.int32, device=dev)
+                        grown[:, :, :fbuf.shape[2]] = fbuf
+                        fbuf = grown
                 ubuf[r, :, :L] = seq[dq + 1:]
+                if fbuf is not None:
+                    fbuf[r] = -1
+                    if steps is not None:
+                        fbuf[r, :, :L] = steps.to(device=dev, dtype=torch.int32)
                 admitted[r] = prompt_from_aligned(seq, P, lm.delays, dq)
                 live[r] = (utt, L, P, base + len(hist))
                 nxt = None
@@ -699,8 +761,9 @@ def generate_many(gen: LMGen, items, capacity: int, *, seeds=None, sampling=None
                 gen.set_active_streams(want)
                 mask = want
             # each row's user tokens at its own step count (held rows read a clamped column and are not stepped)
-            idx = st.off.clamp(max=ubuf.shape[2] - 1)[:, None, None].expand(capacity, Ku, 1)
-            gen.step(ubuf.gather(2, idx))
+            off = st.off.clamp(max=ubuf.shape[2] - 1)[:, None, None]
+            frc = None if fbuf is None else fbuf.gather(2, off.expand(capacity, dq + 1, 1))
+            gen.step(ubuf.gather(2, off.expand(capacity, Ku, 1)), force=frc)
             hist.append(st.out.clone())
             counts["frames"] += 1
             counts["row_frames"] += len(rows)
@@ -722,6 +785,20 @@ def generate_many(gen: LMGen, items, capacity: int, *, seeds=None, sampling=None
         lm._state = None
         if stats is not None:
             stats.update(counts)
+
+
+def _forced_steps(utt, seq: torch.Tensor, mask, delays, dep_q: int, vocab) -> torch.Tensor:
+    """generate_many's admission check and step table of one forced item: force_from_aligned, with every forced id
+    inside its head's vocabulary"""
+    try:
+        steps = force_from_aligned(seq, mask, delays, dep_q)
+    except RstnetError as e:
+        raise RstnetError(f"item {utt!r}: {e}") from None
+    for k, V in enumerate(vocab):
+        row = seq[k][mask[k].to(seq.device)]
+        if row.numel() and (int(row.min()) < 0 or int(row.max()) >= V):
+            raise RstnetError(f"item {utt!r}: a forced id of channel {k} lies outside [0, {V})")
+    return steps
 
 
 # ------------------------------------------------------------------------------------------- teacher-forced scoring

@@ -29,7 +29,8 @@
   * `continue --model moshi` / `continue_corpus`: generation from a Moshi fine-tune over recorded dialogues (`torch.save`d
     dict utt_id -> int64 [n_q + 1, L], aligned): each prompted with its first --prompt-frames frames, then fed its
     recorded user channel, with moshi.generate_many; writes utt_id -> int64 [dep_q + 1, L - P] and, with a codec, the
-    wavs of Moshi's audio channel through MimiCodec.decode_many.
+    wavs of Moshi's audio channel through MimiCodec.decode_many.  --force audio takes Moshi's recorded audio at every
+    frame and samples its text (row 0 of each output: a time-aligned transcript as token ids); --force text the reverse.
 
 Audio at any integer sample rate is resampled to 24 kHz on the GPU the way the reference does it,
 torchaudio.transforms.Resample(sr, 24000) with its defaults (mimi_tokenizer.py:40,67; inference.py:24-34 `convert_audio`:
@@ -393,13 +394,25 @@ def _score_cli(args) -> int:
 
 @torch.no_grad()
 def continue_corpus(gen, corpus: Dict[str, torch.Tensor], prompt_frames: int, capacity: int, kv_pages=None,
-                    seed: int = 0) -> Dict[str, torch.Tensor]:
+                    seed: int = 0, force: Optional[str] = None) -> Dict[str, torch.Tensor]:
     """{utt: int64 [dep_q + 1, L - P]} of moshi.generate_many over `corpus` ({utt: int64 [K, L]} aligned dialogue codes),
-    every item prompted with its first P = prompt_frames frames and seeded with `seed`."""
+    every item prompted with its first P = prompt_frames frames and seeded with `seed`.  force 'text': every item's text
+    channel is taken from the recording at every frame and its audio sampled (re-voicing); 'audio': its audio codebooks
+    1..dep_q are taken and its text sampled, so row 0 of the output is a time-aligned transcript (as token ids)."""
     from .moshi import generate_many
     items = [(utt, torch.as_tensor(seq), prompt_frames) for utt, seq in corpus.items()]
     seeds = {utt: seed for utt, _, _ in items}
-    return dict(generate_many(gen, items, capacity, seeds=seeds, kv_pages=kv_pages))
+    masks = None
+    if force is not None:
+        if force not in ("text", "audio"):
+            raise ValueError(f"force is 'text' or 'audio' (got {force!r})")
+        dq = gen.lm_model.dep_q
+        masks = {}
+        for utt, seq, _ in items:
+            m = torch.zeros(dq + 1, seq.shape[1], dtype=torch.bool)
+            m[slice(0, 1) if force == "text" else slice(1, dq + 1)] = True
+            masks[utt] = m
+    return dict(generate_many(gen, items, capacity, seeds=seeds, kv_pages=kv_pages, force=masks))
 
 
 def continuation_wavs(codec: MimiCodec, out: Dict[str, torch.Tensor], prompt_frames: int, max_delay: int, dep_q: int,
@@ -419,7 +432,7 @@ def _continue_cli(args) -> int:
                 top_k_text=args.top_k_text)
     corpus = torch.load(args.input, map_location="cpu")
     kv_pages = None if args.kv_gb is None else kv_pages_for_budget(model.config, args.kv_gb)
-    out = continue_corpus(gen, corpus, args.prompt_frames, args.capacity, kv_pages=kv_pages, seed=args.seed)
+    out = continue_corpus(gen, corpus, args.prompt_frames, args.capacity, kv_pages=kv_pages, seed=args.seed, force=args.force)
     torch.save(out, args.output_file)
     print(f"continued {len(out)} dialogues -> {args.output_file}")
     if args.wav_dir:
@@ -586,6 +599,9 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--kv-gb", type=_positive_float, default=None,
                    help="KV cache budget in GiB (paged; default: a whole context ring per row)")
     p.add_argument("--seed", type=int, default=0, help="every dialogue's random stream")
+    p.add_argument("--force", choices=("text", "audio"), default=None,
+                   help="take this channel of Moshi's side from the recording at every frame and sample only the other: "
+                        "'audio' writes a time-aligned transcript (row 0, token ids), 'text' re-voices the recorded text")
     p.add_argument("--use-sampling", action=argparse.BooleanOptionalAction, default=True)
     p.add_argument("--temp", type=float, default=0.8)
     p.add_argument("--top-k", type=int, default=250)
